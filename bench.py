@@ -1,16 +1,18 @@
 #!/usr/bin/env python
-"""bench.py -- query-points/sec of the DINO-Tracker inference hot path on B200 (BASELINE.json metric).
+"""bench.py -- query-points/sec of the DINO-Tracker inference hot path on H100 (BASELINE.json metric).
 
 One "step" = one ``ModelInference.infer`` over one synthetic 854x476, T=50 video with 256 query points
 (BASELINE.json configs[1]): trajectories, cos-sims, anchor re-tracking, occlusion.  1 query-point = one
 row of ``infer`` output (T-frame trajectory + T-frame occlusion mask), SURVEY.md 8d.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 * ``value``  : whole-job query-points/s, inputs resident in HBM, device-timed (CUDA events), max over ranks.
 * ``e2e``    : same metric through the public API with HOST buffers: pinned query points H2D, result D2H
                inside the timed region.
 * ``roofline``: dominant kernel of the step (per-kernel CUDA-event times recorded inside the timed region).
+* ``--dump-outputs DIR``: after the timed steps, the last timed step's result (rank 0) as DIR/traj.npy (float32,
+  [nq][T][2] pixels) and DIR/occ.npy (float32 0 / 1, [nq][T]); the inputs are seeded, so two builds can be compared.
 * ``cpu_baseline`` / ``--impl reference``: the oracle's faithful restatement of the reference's PyTorch
   path (same einsum / gathers per model() call) on the host cores, on a bounded sample of the workload.
 
@@ -49,7 +51,7 @@ def parse():
     ap.add_argument("--noise", type=float, default=0.25)
     ap.add_argument("--chunk-maps", type=int, default=32768)
     ap.add_argument("--precision", default="fp16x3", choices=["fp16x3", "fp32"],
-                    help="wide correlation groups: tcgen05 3xTF32 tensor cores, or the exact-fp32 FFMA GEMM")
+                    help="wide correlation groups: split-precision fp16 (3 passes) wgmma tensor cores, or the exact-fp32 FFMA GEMM")
     ap.add_argument("--cpu-baseline", type=int, default=1, help="0: skip the cpu_baseline leg")
     ap.add_argument("--stream-probe", type=int, default=1, help="0: skip the dedicated corr_stream HBM probe")
     ap.add_argument("--stages", type=int, default=1, help="0: skip the ViT / delta-DINO / best-buddies stage timings")
@@ -59,6 +61,8 @@ def parse():
     ap.add_argument("--second-head", type=int, default=1, help="0: skip the extra timing with the mixed-sign head")
     ap.add_argument("--multi", type=int, default=1, help="0: skip the config 3 / 4 / 5 blocks (bench_multi.py)")
     ap.add_argument("--config3-vit", type=int, default=1, help="0: config 3 without the ViT stage (tracker + delta-DINO only)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's trajectories and occlusion as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -91,7 +95,7 @@ def query_lattice(nq, seed):
 
 
 class ClockSampler:
-    """SM clock and clock-event (throttle) reasons sampled DURING the timed region (B200_PROFILING.md's clocks line):
+    """SM clock and clock-event (throttle) reasons sampled DURING the timed region (the clocks line of the result):
     NVML from a Python thread every 20 ms; `nvidia-smi -lms` as the fallback when pynvml is missing."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -175,7 +179,8 @@ def measured_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "which": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "which": "fallback (B200_PROFILING.md)"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- upper bounds, not measured rates
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "which": "fallback (H100 SXM data sheet)"}
 
 
 # ------------------------------------------------------------------------------------------ reference arm
@@ -381,8 +386,9 @@ def run_b200(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t_wall0 = time.perf_counter()
     e0.record()
+    out = None
     for _ in range(args.steps):
-        step_resident()
+        out = step_resident()
     e1.record()
     torch.cuda.synchronize()
     t_wall1 = time.perf_counter()
@@ -393,6 +399,11 @@ def run_b200(args):
     prof = _lib.profile_collect()
     _lib.profile_enable(False)
     clocks = sampler.stop(t_wall0, t_wall1)
+    if args.dump_outputs and rank == 0 and out is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "traj.npy"), out[0].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "occ.npy"), out[1].float().cpu().numpy())
 
     # ---- e2e: host buffers, H2D + D2H inside the timed region
     torch.cuda.synchronize()
@@ -574,10 +585,10 @@ def kernel_roofline(name, stat, args, maps_per_step, peaks, clocks, path_stats=N
                 "traffic_note": "DRAM read + write bytes per launch from the committed ncu --set full capture of this kernel "
                                 "(profiles/ncu_r2_xw_coarse.csv), null until captured; algorithmic bytes per map: fp16 operands "
                                 "(descriptor 2 KB + its share of the frame's 16.6 MB) + 384 B of tile keys -- no map is stored",
-                "note": "single kind::f16 pass over the hi halves: executed MMA FLOPs = algorithmic 2*maps*P*C; " + tensor_note,
+                "note": "single fp16 wgmma pass over the hi halves: executed MMA FLOPs = algorithmic 2*maps*P*C; " + tensor_note,
                 "maps_per_launch": maps_per_launch, "ms_per_launch": avg_s * 1e3}
     if name == "xw_exact_gemm":
-        cell = max(args.T if args.T <= 128 else 125, 1)                 # maps per cell; UMMA N = 64 or 128 columns
+        cell = max(args.T if args.T <= 128 else 125, 1)                 # maps per cell; wgmma N = 64 or 128 columns
         flops_exec = 2.0 * maps_per_launch * 512 * args.C * 3 * ((64.0 if cell <= 64 else 128.0) / cell)
         flops_alg = 2.0 * maps_per_launch * 225 * args.C
         ach = flops_alg / avg_s / 1e12
@@ -585,7 +596,7 @@ def kernel_roofline(name, stat, args, maps_per_step, peaks, clocks, path_stats=N
                 "frac": ach / peaks["tf_sustained"], "traffic": ncu_traffic("ncu_r2_final_xw.csv"),
                 "executed_mma_tflops": flops_exec / avg_s / 1e12,
                 "note": "algorithmic = the 15 x 15 window the head needs per map (2*225*C FLOPs); executed = 3 split-precision "
-                        "passes x 512 box-token rows (4 parts of 128, 441 used) x 64 UMMA columns per cell of T <= 64 maps; "
+                        "passes x 512 box-token rows (4 parts of 128, 441 used) x 64 wgmma columns per cell of T <= 64 maps; "
                         "traffic: profiles/ncu_r2_final_xw.csv, first kernel; " + tensor_note,
                 "maps_per_launch": maps_per_launch, "ms_per_launch": avg_s * 1e3}
     if name in ("corr_gemm", "best_buddies", "vit_gemm", "delta_conv"):
@@ -595,7 +606,7 @@ def kernel_roofline(name, stat, args, maps_per_step, peaks, clocks, path_stats=N
                 "frac": ach / peaks["tf_sustained"],
                 "traffic": None,
                 "note": ("algorithmic FLOPs = 2*maps*P*C per launch; %s. precision=%s: "
-                         "fp16x3 executes 3 kind::f16 MMA passes (lo*hi, hi*lo, hi*hi) per algorithmic FLOP, so the tensor "
+                         "fp16x3 executes 3 fp16 MMA passes (lo*hi, hi*lo, hi*hi) per algorithmic FLOP, so the tensor "
                          "pipe is busy ~3x this fraction; fp32 = exact FFMA GEMM on the CUDA cores") % (tensor_note, args.precision),
                 "executed_mma_tflops": ach * 3 if args.precision == "fp16x3" else None,
                 "maps_per_launch": maps_per_launch, "ms_per_launch": avg_s * 1e3}
@@ -610,7 +621,7 @@ def kernel_roofline(name, stat, args, maps_per_step, peaks, clocks, path_stats=N
                 "reference_formulation_tflops": 4.67e6 * maps_per_launch / avg_s / 1e12,
                 "note": ("exact-fp32 CUDA-core work of the windowed refiner (83.5 kFLOP per map; the full-map formulation the "
                          "reference evaluates is 4.67 MFLOP per map and is only run for uncertified maps); "
-                         "peak = 148 SMs x 128 lanes x 2 x max SM clock")}
+                         "peak = SMs x 128 lanes x 2 x max SM clock")}
     return {"kernel": name, "bound": "hbm", "achieved": None, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": None,
             "traffic": None, "note": "see roofline_other.corr_stream_probe"}
 
@@ -656,7 +667,7 @@ def stage_timings(args, dev, _lib, peaks, vit_only=False):
     flops = 2.0 * (12 * dim * dim * (P + 1) + 2 * (P + 1) ** 2 * dim) * (layer + 1) * frames.shape[0]
     out["vit"] = {"model": f"{name}@block{layer}", "frames_per_s": frames.shape[0] / (ms / 1000), "ms_per_frame": ms / frames.shape[0],
                   "tflops": flops / (ms / 1000) / 1e12, "frac_of_bf16_peak": flops / (ms / 1000) / 1e12 / peaks["tf_sustained"],
-                  "kernel_ms_per_call": prof, "math": "kind::f16 tcgen05 GEMMs (fp16 operands, fp32 accumulate, fp32 residual stream) + fused tcgen05 attention"}
+                  "kernel_ms_per_call": prof, "math": "fp16 wgmma GEMMs (fp16 operands, fp32 accumulate, fp32 residual stream) + fused wgmma attention"}
     del ex, sd
     if vit_only:
         return out
@@ -669,7 +680,7 @@ def stage_timings(args, dev, _lib, peaks, vit_only=False):
     ms, prof = timed(lambda: dd.refine_tpc(fr4, dino, geom), 2)
     out["delta_dino"] = {"frames_per_s": 4 / (ms / 1000), "ms_per_frame": ms / 4, "tflops": 171.4e9 * 4 / (ms / 1000) / 1e12,
                          "kernel_ms_per_call": prof,
-                         "math": "convs = im2col (fp16 hi/lo split) + tcgen05 split-precision GEMMs, fp32-faithful"}
+                         "math": "convs = im2col (fp16 hi/lo split) + wgmma split-precision GEMMs, fp32-faithful"}
     del dd
     # pixels -> tracks for one video of the bench shape: ViT + delta-DINO once per video, then the tracker step
     per_video_s = (out["vit"]["ms_per_frame"] + out["delta_dino"]["ms_per_frame"]) * args.T / 1000.0
@@ -681,7 +692,7 @@ def stage_timings(args, dev, _lib, peaks, vit_only=False):
     ms, prof = timed(lambda: nearest_neighbours(feats, norms, geom, pairs), 2)
     out["best_buddies"] = {"ordered_pairs_per_s": len(pairs) / (ms / 1000), "ms_per_ordered_pair": ms / len(pairs),
                            "tflops": 2.0 * P * P * args.C * len(pairs) / (ms / 1000) / 1e12, "kernel_ms_per_call": prof,
-                           "math": "tcgen05 3xTF32 GEMM + top-2 epilogue + exact fp32 resolve"}
+                           "math": "split-precision fp16 wgmma GEMM + top-2 epilogue + exact fp32 resolve"}
     return out
 
 
@@ -739,8 +750,8 @@ def train_step_stage(args, dev, _lib, torch_baseline):
 
 
 def fp32_peak_tflops(clocks):
-    mhz = (clocks or {}).get("sm_max_mhz") or 1965.0
-    return 148 * 128 * 2 * mhz * 1e6 / 1e12
+    mhz = (clocks or {}).get("sm_max_mhz") or 1980.0   # H100 SXM maximum boost clock
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count * 128 * 2 * mhz * 1e6 / 1e12
 
 
 def stream_probe(model, mi, lib, _lib, args, peaks):

@@ -1,4 +1,4 @@
-"""dino_tracker_b200 -- B200 (sm_100a) implementation of the DINO-Tracker inference hot path.
+"""dino_tracker_b200 -- H100 (sm_90a) implementation of the DINO-Tracker inference hot path.
 
 Host side mirrors the reference's ``models/tracker.py`` + ``models/model_inference.py`` call surface
 (SURVEY.md 8b); all arithmetic runs in hand-written CUDA kernels behind the C ABI of

@@ -155,7 +155,7 @@ def on_device(fn):
 
 def require_cuda(device):
     if not torch.cuda.is_available():
-        raise DinotrkError("dino_tracker_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise DinotrkError("dino_tracker_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     dev = torch.device(device)
     if dev.type != "cuda":
         raise DinotrkError(f"dino_tracker_b200 runs on CUDA only, got device={device!r}")

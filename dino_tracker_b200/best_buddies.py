@@ -2,7 +2,7 @@
 
 ``run(args)`` keeps the reference script's contract (``--dino-emb-path --h --w --stride --out-path``;
 output ``dict['s_t'] -> {source_coords, target_coords, cos_sims}``, rows in ascending source-token
-order).  The affinity matrices never reach HBM: every ordered pair runs through the tcgen05 split-fp16
+order).  The affinity matrices never reach HBM: every ordered pair runs through the wgmma split-fp16
 GEMM with a fused top-2 epilogue, candidates are re-evaluated in exact fp32, and the mutual check
 works on index vectors (``dinotrk_best_buddies_pairs`` / ``dinotrk_bb_mutual``).
 

@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libdinotrk.so for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""In-tree nvcc build of libdinotrk.so for sm_90a (no JIT cache: the .so travels with the repo)."""
 import glob
 import os
 import subprocess
@@ -8,7 +8,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG_DIR)
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libdinotrk.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -27,7 +27,8 @@ def needs_build():
     if not os.path.exists(LIB_PATH):
         return True
     t = os.path.getmtime(LIB_PATH)
-    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(ROOT, "include", "*.h"))
+    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(ROOT, "include", "*.h")) + \
+        [os.path.join(ROOT, "tools", "gen_wgmma_ops.py")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -36,8 +37,11 @@ def build(force=False, verbose=False):
     if not force and not needs_build():
         return LIB_PATH
     objdir = os.path.join(ROOT, "build")
-    os.makedirs(objdir, exist_ok=True)
-    inc = ["-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
+    gendir = os.path.join(objdir, "generated")
+    os.makedirs(gendir, exist_ok=True)
+    subprocess.run([sys.executable, os.path.join(ROOT, "tools", "gen_wgmma_ops.py"), os.path.join(gendir, "wgmma_ops.cuh")],
+                   check=True)
+    inc = ["-I" + os.path.join(ROOT, "include"), "-I" + CSRC, "-I" + gendir]
     objs, procs = [], []
     for src in sources():
         obj = os.path.join(objdir, os.path.basename(src)[:-3] + ".o")

@@ -3,8 +3,8 @@
 //
 // The reference materialises the 8107 x 8107 cosine-affinity matrix per ordered pair (263 MB), divides it,
 // and runs two arg-max passes over it.  Here, per ordered pair (s, t):
-//   1. tcgen05 split-fp16 (hi/lo, 3-pass) GEMM  Fs x Ft^T  with a fused epilogue that keeps, per source token and 256-token
-//      column tile, the best and second-best cosine (value + index) -- the matrix never leaves TMEM;
+//   1. wgmma split-fp16 (hi/lo, 3-pass) GEMM  Fs x Ft^T  with a fused epilogue that keeps, per source token and 256-token
+//      column tile, the best and second-best cosine (value + index) -- the matrix never leaves the SM;
 //   2. a warp per source token merges the 32 tile partials, and re-evaluates its (one or two) candidates in
 //      exact fp32 so that the arg-max and the reported cosine do not depend on tensor-core rounding;
 //   3. mutual check  nn_ts[nn_st[n]] == n  on the index vectors.
@@ -249,9 +249,7 @@ int dinotrk_best_buddies_pairs(const dinotrk_features* feat, const dinotrk_geom*
   }
   TcProblem pb{pair_tgt, row0, m, tile_start, n_pairs, P, C};
   BBEpi epi{feat->norms, pair_src, pair_tgt, part, P, n_tiles};
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   {
     ProfRange pr(PROF_BB, st);
     tc_gemm_kernel<TcMode::F16X3, BBEpi><<<sms, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
@@ -273,7 +271,7 @@ int dinotrk_bb_nms(const float* maps, int n_maps, const dinotrk_geom* g, float b
   if (n_maps == 0) return DINOTRK_OK;
   const int P = g->h * g->w;
   DTK_CHECK_ARG(topk <= P, "bb_nms: topk %d exceeds the %d tokens of a map (torch.topk would fail too)", topk, P);
-  int grid = n_maps < 148 * 8 ? n_maps : 148 * 8;
+  int grid = n_maps < num_sms() * 8 ? n_maps : num_sms() * 8;
   ProfRange pr(PROF_BB, (cudaStream_t)stream);
   bb_nms_kernel<<<grid, NMS_THREADS, 0, (cudaStream_t)stream>>>(maps, n_maps, dinotrk_map_stride(g), P, g->w, g->stride, g->patch / 2,
                                                                 box_size, iou_thresh, topk, peak_affs, r);

@@ -1,4 +1,4 @@
-// Shared helpers for libdinotrk (sm_100a).  Not part of the C ABI.
+// Shared helpers for libdinotrk (sm_90a).  Not part of the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -74,6 +74,9 @@ struct NvtxRange {
   ~NvtxRange() { nvtxRangePop(); }
 };
 
+// multiprocessors of the current device (cached per device; corr_tc.cu)
+int num_sms();
+
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
@@ -91,6 +94,11 @@ struct Arena {
   }
   bool ok() const { return off <= size; }
 };
+
+// element-wise IEEE fp32 operations on pairs (two FFMA / FMUL / FADD: bit for bit what a packed instruction would give)
+__device__ __forceinline__ float2 f2fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 f2mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f2add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -35,7 +35,7 @@ struct CorrAssist {
 };
 
 size_t corr_plan_bytes(int n_groups);
-int corr_tc_tile_rows();   // 256: CTA-pair (cta_group::2) kernel, the default; 128: single-CTA kernel (DTK_CORR_PAIRS=0)
+int corr_tc_tile_rows();   // 256: CTA-pair (two-CTA cluster) kernel, the default; 128: single-CTA kernel (DTK_CORR_PAIRS=0)
 size_t corr_tc_workspace_bytes(int total_rows, int C);
 // desc_rows = number of rows of the desc array (bounds of its tensor map); split_ws: corr_tc_workspace_bytes
 // (only touched when fv.tensor()).

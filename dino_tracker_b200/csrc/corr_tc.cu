@@ -1,18 +1,28 @@
-// Tensor-core correlation GEMM (tcgen05, split-precision fp16 hi/lo) + operand splitting + TMA tensor-map helpers.
+// Tensor-core correlation GEMM (wgmma, split-precision fp16 hi/lo) + operand splitting + TMA tensor-map helpers.
 //
 //   corr[j][p] = relu( <d_j, F[frame][p]> / max(|d_j| |F[frame][p]|, 1e-8) )     (models/tracker.py:158-173)
 //
-// The contraction runs as lo*hi + hi*lo + hi*hi on the kind::f16 tensor pipe with fp32 accumulation in TMEM
+// The contraction runs as lo*hi + hi*lo + hi*hi on the f16 tensor pipe with fp32 accumulation in registers
 // (operands pre-split into fp16 hi + fp16 lo, x = hi + lo up to 2^-22 |x|), which keeps the products
-// faithful to ~2^-21; the cosine normalisation and ReLU are the epilogue on the accumulator as it leaves TMEM.
+// faithful to ~2^-21; the cosine normalisation and ReLU are the epilogue on the accumulator.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "corr.cuh"
 #include "tcgemm.cuh"
-#include "tcgemm2.cuh"
 
 namespace dtk {
+
+int num_sms() {
+  static PerDev<int> sms_dev;
+  int& sms = sms_dev.get();
+  if (sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 1;
+  }
+  return sms;
+}
 
 // ---- driver entry point for cuTensorMapEncodeTiled (resolved once; no link-time libcuda dependency) ----
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -99,7 +109,7 @@ int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t 
   DTK_CHECK_ARG(n % 4 == 0, "split_fp16: length must be a multiple of 4");
   size_t n4 = n / 4;
   unsigned grid = (unsigned)((n4 + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > (unsigned)num_sms() * 16) grid = num_sms() * 16;
   ProfRange pr(PROF_MISC, st);
   split_f16_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(hi),
                                          reinterpret_cast<uint2*>(lo), n4);
@@ -183,7 +193,7 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
   if (rc) return rc;
   const bool pairs = (tile_rows > 0 ? tile_rows : corr_tc_tile_rows()) == TC2_BM;   // tile_start was planned with this M tile
   CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
-  const uint32_t b_box = pairs ? TC2_BN / 2 : TC_BN;   // a CTA of a pair stages half of the B tile
+  const uint32_t b_box = pairs ? TC_BN / 2 : TC_BN;    // a CTA of a pair loads half of the B tile (multicast to both)
   if ((rc = make_tmap_2d(&tmA_hi, d_hi, desc_rows, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
   if ((rc = make_tmap_2d(&tmA_lo, d_lo, desc_rows, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
   if ((rc = make_tmap_3d(&tmB_hi, tpc_hi, T, P, C, b_box, Cfg::kBK, TMAP_F16))) return rc;
@@ -193,22 +203,19 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
   if (!attr) {
     DTK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TcMode::F16X3, CorrEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   Cfg::kSmem));
-    DTK_CUDA(cudaFuncSetAttribute(tc_gemm2_kernel<TcMode::F16X3, CorrEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  Tc2Cfg<TcMode::F16X3>::kSmem));
+    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  Cfg::kSmem));
     attr = true;
   }
   TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
   CorrEpi epi{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, tkeys, cdiv(P, CORR_TILE)};
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   int tiles_bound = max_tiles * cdiv(P, TC_BN);
   ProfRange pr(PROF_CORR_GEMM, st);
   if (pairs) {
     int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
     if (grid < 2) grid = 2;
-    tc_gemm2_kernel<TcMode::F16X3, CorrEpi><<<grid, TC_THREADS, Tc2Cfg<TcMode::F16X3>::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi,
-                                                                                                   tmB_lo, pb, epi);
+    tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
     DTK_LAUNCHED();
     return DINOTRK_OK;
   }

@@ -229,7 +229,7 @@ __global__ void align_add_kernel(const float* __restrict__ cnn, const float* __r
 }
 
 
-// ---- tensor-core path: explicit im2col (fp16 hi/lo split on the fly) + tcgen05 split-precision GEMM ------------------
+// ---- tensor-core path: explicit im2col (fp16 hi/lo split on the fly) + wgmma split-precision GEMM --------------------
 // A[m][k] = in[b][reflect(y + (ky-2) d)][reflect(x + (kx-2) d)][ci],  k = (ky*5 + kx)*Cin + ci, zero padded to Kp
 __global__ void im2col_split_kernel(const float* __restrict__ in, __half* __restrict__ hi, __half* __restrict__ lo,
                                     int H, int W, int Cin, int dil, int Kp, size_t m0, size_t m_count) {
@@ -299,9 +299,7 @@ static int conv_gemm(const __half* a_hi, const __half* a_lo, int rows, int Kp, c
     attr = true;
   }
   TcProblem pb{plan, plan + 4, plan + 8, plan + 12, 1, Cout, Kp};
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   int tiles = cdiv(rows, TC_BM) * cdiv(Cout, BN);
   ProfRange pr(PROF_CONV, st);
   kern<<<tiles < sms ? tiles : sms, TC_THREADS, Cfg::kSmem, st>>>(tA_hi, tA_lo, tB_hi, tB_lo, pb, epi);

@@ -1,23 +1,13 @@
-// Fused attention for the ViT (sm_100a, tcgen05):  O = softmax(Q K^T) V  per (frame, head).  Q arrives pre-scaled by
+// Fused attention for the ViT (sm_90a, wgmma):  O = softmax(Q K^T) V  per (frame, head).  Q arrives pre-scaled by
 // head_dim^-1/2 * log2(e), so the softmax is exp2(s - max).
 //
-// One CTA per (frame*head, 128-query tile), two CTAs per SM; 192 threads:
-//   warp 0     : TMA producer (Q once; K_j [64 keys][64] and V^T_j [64][64 keys] through a 4-stage ring)
-//   warp 1     : TMEM alloc + MMA issue.  S_j = Q K_j^T (kind::f16, M128 N64 K64) goes to one of TWO TMEM score buffers
-//                and is issued as soon as the softmax warps have READ S_{j-2} out of that buffer (s_free) -- two tiles
-//                ahead of its consumer, independent of the P V chain;  O += P_j V_j (M128 N64 K64, A = P_j read FROM
-//                TENSOR MEMORY) accumulates IN TMEM across all key tiles.
-//   warps 2..5 : softmax, thread = query row = TMEM lane.  Per key tile: the 64 scores (requested from TMEM one tile
-//                ahead), row max (FMNMX3), p = exp2(s - m), row sum in registers, fp16 P into one of two 32-column TMEM
-//                buffers (one tcgen05.st; no shared-memory tile, no generic->async proxy fence), published one tile
-//                later (the store has the next tile's score read and max phase to land).  The running max m is LAZY:
-//                it only moves (and the TMEM accumulator is only rescaled, tcgen05.ld -> multiply -> tcgen05.st) when
-//                some row of the warp would exceed it by 2^8, so after the first few tiles there is no per-tile
-//                accumulator traffic at all; p <= 256 keeps fp16 P in range, and the final O / l is independent of
-//                which m was used.  The exponentials are MUFU-bound (16/clk/SM against 4 x 128 x 64-wide MMAs), so a
-//                share of them (POLY) is evaluated on the FMA pipe instead (Cody-Waite split + cubic on packed fp32
-//                instructions, relative error 1.1e-4 < fp16 rounding of P).
-// The score matrix (8108 x 8108 per head) never leaves the SM.
+// One CTA per (frame*head, 128-query tile); 384 threads:
+//   warpgroup 0     : TMA producer (Q once; K_j [64 keys][64] and V^T_j [64][64 keys] through a 4-stage ring)
+//   warpgroups 1, 2 : 64 query rows each.  Per key tile: S = Q K_j^T (m64n64k16 x 4, both operands from shared memory)
+//                     into registers, online softmax on the accumulator fragment (a row lives in the 4 lanes of a quad),
+//                     p = exp2(s - m) packed to fp16 pairs that ARE the A fragments of O += P V_j (m64n64k16 x 4, A from
+//                     registers, V^T from shared memory).  O and the row sums stay in registers across all key tiles.
+// The score matrix (N1 x N1 per head) never leaves the SM.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -26,52 +16,22 @@
 
 namespace dtk {
 
-// POLY (template parameter of the kernel): bit k set -> the k-th fp16 pair of every 8 pairs takes the FMA-pipe exp2
-constexpr int FA_POLY_DEFAULT = 0x88;   // 25 %
-constexpr int FA_BQ = 128, FA_BKV = 64, FA_D = 64, FA_THREADS = 192;
-constexpr int FA_NV = 64;                          // V^T tile rows = MMA N: the 64 head dims
+constexpr int FA_BQ = 128, FA_BKV = 64, FA_D = 64, FA_THREADS = 384;
 constexpr int FA_KV_STAGES = 4;
 constexpr int FA_SQ = FA_BQ * 128;                 // Q tile bytes (128 rows x 64 fp16)
 constexpr int FA_SK = FA_BKV * 128;                // K tile bytes
-constexpr int FA_SVT = FA_D * 128;                 // TMA-written part of the V^T tile
-constexpr int FA_SV = FA_NV * 128;                 // whole V^T tile
+constexpr int FA_SV = FA_D * 128;                  // V^T tile bytes
 constexpr int FA_STAGE = FA_SK + FA_SV;
-constexpr int FA_TMEM = 256;                       // S0 [0,64) S1 [64,128) O [128,192) P0 [192,224) P1 [224,256)
-constexpr int FA_SMEM = FA_SQ + FA_KV_STAGES * FA_STAGE + 256;   // extern smem is declared 1024-byte aligned
-constexpr float FA_RESCALE_STEP = 8.f;             // log2 units
+constexpr int FA_SMEM = 1024 + FA_SQ + FA_KV_STAGES * FA_STAGE + 256;
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// exp2 on the FMA pipe for x <= 0: n = round(x), 2^(x-n) by a cubic on [-0.5, 0.5], exponent patched in by integer add
-__device__ __forceinline__ float poly_exp2(float x) {
-  x = fmaxf(x, -125.f);
-  const float t = x + 12582912.f;                  // 1.5 * 2^23: low mantissa bits of t hold n
-  const float f = x - (t - 12582912.f);
-  float p = fmaf(0.055268917f, f, 0.24221092f);
-  p = fmaf(p, f, 0.6932298f);
-  p = fmaf(p, f, 1.f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-// the same for two values at once on packed fp32 instructions (FADD2 / FFMA2: one issue slot per pair)
-__device__ __forceinline__ float2 poly_exp2x2(float2 x) {
-  x.x = fmaxf(x.x, -125.f); x.y = fmaxf(x.y, -125.f);
-  const float2 magic = make_float2(12582912.f, 12582912.f), neg_magic = make_float2(-12582912.f, -12582912.f);
-  const float2 t = __fadd2_rn(x, magic);
-  const float2 r = __fadd2_rn(t, neg_magic);
-  const float2 f = __ffma2_rn(r, make_float2(-1.f, -1.f), x);
-  float2 p = __ffma2_rn(make_float2(0.055268917f, 0.055268917f), f, make_float2(0.24221092f, 0.24221092f));
-  p = __ffma2_rn(p, f, make_float2(0.6932298f, 0.6932298f));
-  p = __ffma2_rn(p, f, make_float2(1.f, 1.f));
-  return make_float2(__int_as_float(__float_as_int(p.x) + (__float_as_int(t.x) << 23)),
-                     __int_as_float(__float_as_int(p.y) + (__float_as_int(t.y) << 23)));
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
 }
 
 struct FlashParams {
@@ -82,237 +42,126 @@ struct FlashParams {
   int out_f16;
 };
 
-template <int POLY>
-__global__ void __launch_bounds__(FA_THREADS, 2)
+__global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                   const __grid_constant__ CUtensorMap tmV, FlashParams fp) {
-  extern __shared__ __align__(1024) uint8_t fa_smem[];
-  uint8_t* sQ = fa_smem;
+  extern __shared__ uint8_t fa_smem_raw[];
+  uint8_t* sQ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(fa_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sKV = sQ + FA_SQ;                 // stage s: K at sKV + s*FA_STAGE, V^T at + FA_SK
   uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + FA_KV_STAGES * FA_STAGE);
-  uint64_t* q_full = bars;           // 1
+  uint64_t* q_full = bars;                                    // 1
   uint64_t* kv_full = bars + 1;                               // [FA_KV_STAGES]
-  uint64_t* kv_empty = kv_full + FA_KV_STAGES;                // [FA_KV_STAGES]
-  uint64_t* s_full = kv_empty + FA_KV_STAGES;                 // [2]
-  uint64_t* p_ready = s_full + 2;    // [2] (4 arrivals: one per softmax warp)
-  uint64_t* pv_done = p_ready + 2;   // [2] P V_j retired: P buffer j&1 reusable, accumulator quiescent until the next p_ready
-  uint64_t* s_free = pv_done + 2;    // [2] (4 arrivals) S_j is in the softmax warps' registers: its buffer may be overwritten
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_free + 2);
-  static_assert((1 + 2 * FA_KV_STAGES + 8) * 8 + 4 <= 256, "barrier block");
+  uint64_t* kv_empty = kv_full + FA_KV_STAGES;                // [FA_KV_STAGES] (one arrival per consumer warpgroup)
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int bh = blockIdx.y, q0 = blockIdx.x * FA_BQ;
   const int N1 = fp.N1;
   const int n_kv = (N1 + FA_BKV - 1) / FA_BKV;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&tmQ); tc::prefetch_tmap(&tmK); tc::prefetch_tmap(&tmV);
     tc::mbar_init(q_full, 1);
-    for (int s = 0; s < FA_KV_STAGES; ++s) { tc::mbar_init(&kv_full[s], 1); tc::mbar_init(&kv_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) {
-      tc::mbar_init(&s_full[s], 1); tc::mbar_init(&p_ready[s], 4); tc::mbar_init(&pv_done[s], 1); tc::mbar_init(&s_free[s], 4);
-    }
+    for (int s = 0; s < FA_KV_STAGES; ++s) { tc::mbar_init(&kv_full[s], 1); tc::mbar_init(&kv_empty[s], 2); }
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, FA_TMEM);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_O = tmem_base + 2 * FA_BKV, tmem_P = tmem_O + FA_D;
-  constexpr uint32_t kIdescS = tc::make_idesc(0, 128, FA_BKV);   // f16 inputs, fp32 accumulate
-  constexpr uint32_t kIdescO = tc::make_idesc(0, 128, FA_NV);
 
-  if (warp == 0) {
-    if (tc::elect_one()) {
+  if (wg == 0) {
+    if (warp == 0 && tc::elect_one()) {
       tc::mbar_expect_tx(q_full, FA_SQ);
       tc::tma_load_2d(&tmQ, q_full, sQ, 0, bh * N1 + q0);
       int s = 0, ph = 0;
       for (int j = 0; j < n_kv; ++j) {
         tc::mbar_wait(&kv_empty[s], ph ^ 1);
-        tc::mbar_expect_tx(&kv_full[s], FA_SK + FA_SVT);
+        tc::mbar_expect_tx(&kv_full[s], FA_STAGE);
         uint8_t* st = sKV + s * FA_STAGE;
         tc::tma_load_3d(&tmK, &kv_full[s], st, 0, j * FA_BKV, bh);
         tc::tma_load_3d(&tmV, &kv_full[s], st + FA_SK, j * FA_BKV, 0, bh);
         if (++s == FA_KV_STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    auto mma_S = [&](int s, int buf) {   // S = Q K^T : 4 k-steps of 16 over d = 64
-      const uint32_t a = tc::smem_u32(sQ), b = tc::smem_u32(sKV + s * FA_STAGE);
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-        tc::mma_ss<false>(tmem_base + buf * FA_BKV, tc::smem_desc_sw128(a + ks * 32), tc::smem_desc_sw128(b + ks * 32), kIdescS,
-                          ks ? 1u : 0u);
-    };
-    auto mma_O = [&](int s, int buf, bool acc) {   // O (+)= P V : 4 k-steps over 64 keys, P from tensor memory
-      const uint32_t b = tc::smem_u32(sKV + s * FA_STAGE + FA_SK);
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-        tc::mma_ts_f16(tmem_O, tmem_P + buf * 32 + ks * 8, tc::smem_desc_sw128(b + ks * 32), kIdescO, (acc || ks) ? 1u : 0u);
-    };
-    tc::mbar_wait(q_full, 0);
-    for (int t = 0; t < 2 && t < n_kv; ++t) {          // S_0, S_1: both score buffers start empty
-      tc::mbar_wait(&kv_full[t], 0);
-      tc::fence_after_sync();
-      if (tc::elect_one()) { mma_S(t, t); tc::mma_commit(&s_full[t]); }
-      __syncwarp();
-    }
-    for (int j = 0; j < n_kv; ++j) {
-      if (j + 2 < n_kv) {
-        // S_{j+2} -> buffer j&1 the moment the softmax warps hold S_j in registers: two tiles before it is consumed
-        const int t = j + 2, st = t % FA_KV_STAGES;
-        tc::mbar_wait(&s_free[j & 1], (j >> 1) & 1);
-        tc::mbar_wait(&kv_full[st], (t / FA_KV_STAGES) & 1);
-        tc::fence_after_sync();
-        if (tc::elect_one()) { mma_S(st, j & 1); tc::mma_commit(&s_full[j & 1]); }
-        __syncwarp();
-      }
-      tc::mbar_wait(&p_ready[j & 1], (j >> 1) & 1);
-      tc::fence_after_sync();
-      if (tc::elect_one()) {
-        mma_O(j % FA_KV_STAGES, j & 1, j > 0);
-        tc::mma_commit(&pv_done[j & 1]);
-        tc::mma_commit(&kv_empty[j % FA_KV_STAGES]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ---------------- softmax: thread = query row ----------------
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;                 // row inside the Q tile = TMEM lane
-    const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-    float m_run = -INFINITY;
-    float2 l2 = make_float2(0.f, 0.f);                // row sum of p (two partial sums), rescaled with the accumulator
-    // The scores of tile j + 1 are requested from TMEM BEFORE the P tile of tile j is stored and published: the softmax
-    // warps are nearly alone on their schedulers (two per SMSP), so the TMEM read latency was fully exposed at the top
-    // of every tile (long-scoreboard stalls: 1.6 cycles per issued instruction in the capture of the unrotated loop).
-    uint32_t v[FA_BKV];
-    uint32_t (&v0)[32] = *reinterpret_cast<uint32_t (*)[32]>(&v[0]);
-    uint32_t (&v1)[32] = *reinterpret_cast<uint32_t (*)[32]>(&v[32]);
-    auto request_scores = [&](int jj) {
-      tc::mbar_wait(&s_full[jj & 1], (jj >> 1) & 1);
-      tc::fence_after_sync();
-      tc::tmem_ld32(tmem_base + lane_addr + (jj & 1) * FA_BKV, v0);
-      tc::tmem_ld32(tmem_base + lane_addr + (jj & 1) * FA_BKV + 32, v1);
-    };
-    request_scores(0);
-    for (int j = 0; j < n_kv; ++j) {
-      const int buf = j & 1, kbase = j * FA_BKV;
-      tc::tmem_ld_wait(v0);
-      tc::tmem_ld_wait(v1);
-      tc::fence_before_sync();                        // S_j is in registers: the MMA warp may overwrite its buffer (S_{j+2})
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s_free[buf]);
-      if (kbase + FA_BKV > N1) {                      // only the last key tile needs masking
-#pragma unroll
-        for (int i = 0; i < FA_BKV; ++i)
-          if (kbase + i >= N1) v[i] = 0xff800000u;    // -inf: ignored by the max, exp2 -> 0
-      }
-      float mx;
-      {   // four independent FMNMX3 chains (the SMSP holds only two softmax warps: latency matters)
-        float m4[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          m4[k] = fmax3(__uint_as_float(v[16 * k]), __uint_as_float(v[16 * k + 1]), __uint_as_float(v[16 * k + 2]));
-#pragma unroll
-          for (int i = 3; i + 1 < 16; i += 2) m4[k] = fmax3(m4[k], __uint_as_float(v[16 * k + i]), __uint_as_float(v[16 * k + i + 1]));
-          m4[k] = fmaxf(m4[k], __uint_as_float(v[16 * k + 15]));
-        }
-        mx = fmaxf(fmax3(m4[0], m4[1], m4[2]), m4[3]);
-      }
-      // publish P_{j-1}: its tcgen05.st was issued at the end of the previous iteration and had the score read and the
-      // max phase of this tile to land (the wait right behind the store cost its full latency on every tile).  S_{j+1} does
-      // not depend on this arrival (it is issued before P_{j-1} V_{j-1}), and the rescale below needs it to have happened.
-      if (j > 0) {
-        tc::tmem_st_wait();
-        tc::fence_before_sync();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&p_ready[(j - 1) & 1]);
-      }
-      // lazy running max: move it (and rescale the TMEM accumulator, row sums included) only on a 2^8 overshoot
-      if (__any_sync(0xffffffffu, mx > m_run + FA_RESCALE_STEP)) {
-        const float m_new = fmaxf(m_run, mx);
-        if (j > 0) {
-          tc::mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);   // accumulator quiescent: PV_j waits for our p_ready
-          tc::fence_after_sync();
-          const float alpha = fast_exp2(m_run - m_new);
-#pragma unroll
-          for (int c = 0; c < FA_D; c += 32) {
-            uint32_t o[32];
-            tc::tmem_ld32(tmem_O + lane_addr + c, o);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tc::tmem_st32(tmem_O + lane_addr + c, o);
-          }
-          l2.x *= alpha; l2.y *= alpha;
-          tc::tmem_st_wait();
-        }
-        m_run = m_new;
-      }
-      // p = exp2(s - m) as fp16 pairs
-      uint32_t packed[FA_BKV / 2];
-      const float2 neg_m = make_float2(-m_run, -m_run);
-#pragma unroll
-      for (int i = 0; i < FA_BKV; i += 2) {
-        const float2 x = __fadd2_rn(make_float2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])), neg_m);   // one packed add
-        float2 pp;
-        if ((POLY >> ((i / 2) & 7)) & 1) pp = poly_exp2x2(x);
-        else pp = make_float2(fast_exp2(x.x), fast_exp2(x.y));
-        l2 = __fadd2_rn(l2, pp);
-        __half2 h = __floats2half2_rn(pp.x, pp.y);
-        packed[i >> 1] = *reinterpret_cast<uint32_t*>(&h);
-      }
-      if (j + 1 < n_kv) request_scores(j + 1);   // S_{j+1} was issued before PV_{j-1}: never waits on our own p_ready
-      if (j >= 2) tc::mbar_wait(&pv_done[buf], ((j - 2) >> 1) & 1);   // P buffer `buf` was the A operand of PV_{j-2}
-      tc::tmem_st32(tmem_P + lane_addr + buf * 32, packed);
-    }
-    tc::tmem_st_wait();
-    tc::fence_before_sync();
-    __syncwarp();
-    if (lane == 0) tc::mbar_arrive(&p_ready[(n_kv - 1) & 1]);
-    // accumulator complete: normalise by the row sum and store
-    tc::mbar_wait(&pv_done[(n_kv - 1) & 1], ((n_kv - 1) >> 1) & 1);
-    tc::fence_after_sync();
-    const float inv = 1.f / (l2.x + l2.y);
-    const int qrow = q0 + row;
-    const int b = bh / fp.heads, hd = bh - b * fp.heads;
-    const size_t off = ((size_t)b * N1 + qrow) * fp.D + hd * FA_D;
-#pragma unroll
-    for (int c = 0; c < FA_D; c += 32) {
-      uint32_t v[32];
-      tc::tmem_ld32(tmem_O + lane_addr + c, v);
-      tc::tmem_ld_wait();
-      if (qrow < N1) {
-        if (fp.out_f16) {
-          __half* dst = reinterpret_cast<__half*>(fp.out) + off + c;
-#pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            uint32_t w[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              __half2 h = __floats2half2_rn(__uint_as_float(v[i + 2 * k]) * inv, __uint_as_float(v[i + 2 * k + 1]) * inv);
-              w[k] = *reinterpret_cast<uint32_t*>(&h);
-            }
-            *reinterpret_cast<uint4*>(dst + i) = make_uint4(w[0], w[1], w[2], w[3]);
-          }
-        } else {
-          float* dst = reinterpret_cast<float*>(fp.out) + off + c;
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            *reinterpret_cast<float4*>(dst + i) = make_float4(__uint_as_float(v[i]) * inv, __uint_as_float(v[i + 1]) * inv,
-                                                              __uint_as_float(v[i + 2]) * inv, __uint_as_float(v[i + 3]) * inv);
-        }
-      }
-    }
+    return;
   }
 
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, FA_TMEM);
+  // ---------------- consumer warpgroup cw: query rows [64 cw, 64 cw + 64) of the tile ----------------
+  const int cw = wg - 1;
+  const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);   // fragment rows fr, fr + 8; columns 8 i + fc (+1)
+  const uint32_t qa = tc::smem_u32(sQ) + cw * 64 * 128;
+  float o[FA_D / 2];
+#pragma unroll
+  for (int i = 0; i < FA_D / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // per fragment row; l_run is this lane's partial sum
+  tc::mbar_wait(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int s = j % FA_KV_STAGES, kbase = j * FA_BKV;
+    tc::mbar_wait(&kv_full[s], (j / FA_KV_STAGES) & 1);
+    const uint32_t kb = tc::smem_u32(sKV + s * FA_STAGE), vb = kb + FA_SK;
+    float sc[FA_BKV / 2];
+#pragma unroll
+    for (int i = 0; i < FA_BKV / 2; ++i) sc[i] = 0.f;
+    tc::wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < FA_D / 16; ++ks)
+      tc::wgmma_ss<false, FA_BKV>(sc, tc::smem_desc_sw128(qa + ks * 32), tc::smem_desc_sw128(kb + ks * 32), 1u);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(sc);
+    if (kbase + FA_BKV > N1) {                      // only the last key tile needs masking
+#pragma unroll
+      for (int i = 0; i < FA_BKV / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (kbase + 8 * i + fc + (e & 1) >= N1) sc[4 * i + e] = -INFINITY;   // ignored by the max, exp2 -> 0
+    }
+    uint32_t pa[FA_BKV / 16][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < FA_BKV / 8; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * h], sc[4 * i + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);      // finite: every key tile holds at least one key
+      const float alpha = fast_exp2(m_run[h] - m_new);
+      m_run[h] = m_new;
+      float sum = 0.f;
+#pragma unroll
+      for (int i = 0; i < FA_BKV / 8; ++i) {
+        const float p0 = fast_exp2(sc[4 * i + 2 * h] - m_new), p1 = fast_exp2(sc[4 * i + 2 * h + 1] - m_new);
+        sum += p0 + p1;
+        // S columns 16 kk + {fc, fc + 1} (i = 2 kk) and 16 kk + 8 + {fc, fc + 1} (i = 2 kk + 1) of rows fr / fr + 8 are
+        // registers {0, 2} / {1, 3} of the A fragment of K step kk
+        pa[i >> 1][(i & 1) * 2 + h] = pack_half2(p0, p1);
+      }
+      l_run[h] = l_run[h] * alpha + sum;
+#pragma unroll
+      for (int i = 0; i < FA_D / 8; ++i) { o[4 * i + 2 * h] *= alpha; o[4 * i + 2 * h + 1] *= alpha; }
+    }
+    tc::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < FA_BKV / 16; ++kk) tc::wgmma_rs_f16<FA_D>(o, pa[kk], tc::smem_desc_sw128(vb + kk * 32), 1u);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(o);
+    if (t == 0) tc::mbar_arrive(&kv_empty[s]);
+  }
+  // normalise by the row sums and store
+  const int b = bh / fp.heads, hd = bh - b * fp.heads;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    const int qrow = q0 + cw * 64 + fr + 8 * h;
+    if (qrow >= N1) continue;
+    const size_t off = ((size_t)b * N1 + qrow) * fp.D + hd * FA_D + fc;
+#pragma unroll
+    for (int i = 0; i < FA_D / 8; ++i) {
+      const float v0 = o[4 * i + 2 * h] * inv, v1 = o[4 * i + 2 * h + 1] * inv;
+      if (fp.out_f16) *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(fp.out) + off + 8 * i) = pack_half2(v0, v1);
+      else *reinterpret_cast<float2*>(reinterpret_cast<float*>(fp.out) + off + 8 * i) = make_float2(v0, v1);
+    }
   }
 }
 

@@ -680,9 +680,7 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
     for (int k = 0; k < 9; ++k) { p1 += hw.w1[o][k] > 0.f ? hw.w1[o][k] : 0.f; p2 += hw.w2[o][k] > 0.f ? hw.w2[o][k] : 0.f; }
     hp.P1[o] = p1 * (1.f + 1e-6f); hp.P2[o] = p2 * (1.f + 1e-6f);   // rounded up: the bound must stay a bound
   }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   const int lin_elems = (map_stride + 3) & ~3;
   // the window fast path needs the disc inside the 11 x 11 box and a scratch list for the uncertified maps
   const bool window_ok = scratch != nullptr && g.radius <= 5 * g.stride && g.w <= HEAD_MAX_W;

@@ -19,7 +19,7 @@
 
 namespace dtk {
 
-constexpr int TC2_BM_ROWS = 256;   // M tile of the CTA-pair GEMM (tcgemm2.cuh: TC2_BM)
+constexpr int TC2_BM_ROWS = 256;   // M tile of the CTA-pair GEMM (tcgemm.cuh: TC2_BM)
 
 // ---------------------------------------------------------------------------------- phase A helpers
 // descriptors of the query points: frames_set = [t_q, s..e-1], set index 0 (model_inference.py:8-34)

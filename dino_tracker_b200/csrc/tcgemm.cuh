@@ -1,16 +1,20 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:   D[m][n] = sum_k A[m][k] * B[n][k]
-// (both operands K-major: A = [rows][K], B = [batch][N][K]), 128 x 256 output tiles, accumulators in
-// TMEM (two 256-column buffers so the epilogue of tile i overlaps the MMAs of tile i+1), operands
-// staged by TMA into 128B-swizzled shared memory through an mbarrier ring.
+// Persistent, warp-specialised wgmma GEMM for sm_90a:   D[m][n] = sum_k A[m][k] * B[n][k]
+// (both operands K-major: A = [rows][K], B = [batch][N][K]), 128 x BN output tiles, operands staged by TMA into
+// 128B-swizzled shared memory through an mbarrier ring, accumulators in registers.
 //
-//   warp 0      : TMA producer (one elected lane)
-//   warp 1      : TMEM allocation + MMA issue (one elected lane), tcgen05.commit -> barriers
-//   warps 2..5  : epilogue (tcgen05.ld of the warp's 32-lane quadrant -> Epi functor -> global)
+//   warpgroup 0     : TMA producer (one elected lane; its registers are handed to the consumers)
+//   warpgroups 1, 2 : wgmma on 64 rows each (m64nBN), then the epilogue of those rows: 32-column blocks of the
+//                     accumulator go through shared memory so that the Epi functor sees one row per thread (or, for
+//                     coalesced epilogues, 4 consecutive columns per thread with lanes running along the rows)
+// The producer runs ahead into the next tile while the consumers are in the epilogue.
+//
+// Pair variant (tc_gemm_pair_kernel, a cluster of two CTAs): the two CTAs compute the two 128-row halves of a 256 x BN
+// tile; each loads half of the B tile and multicasts it to both, which halves the B operand traffic from L2 per CTA.
 //
 // Modes:
 //   F16X3  : fp32-faithful split-precision: operands pre-split into fp16 hi + fp16 lo (x = hi + lo up to 2^-22),
-//            lo*hi + hi*lo + hi*hi on the kind::f16 pipe (K = 16 per MMA: twice the TF32 rate), fp32 accumulation
-//   TF32X3 : the same scheme with TF32 parts (fp32 storage, K = 8 per MMA)
+//            lo*hi + hi*lo + hi*hi on the f16 tensor pipe (twice the TF32 rate), fp32 accumulation
+//   TF32X3 : the same scheme with TF32 parts (fp32 storage)
 //   TF32   : single pass on fp32 data (the tensor core reads the top 19 bits)
 //   BF16   : single pass on bf16 data
 //   F16    : single pass on fp16 data (11-bit significand like TF32, twice its rate)
@@ -24,12 +28,13 @@
 
 namespace dtk {
 
-constexpr int TC_EPI_SCRATCH = 4 * 32 * 36 * 4;   // bytes: one 32 x 36 fp32 block per epilogue warp
-
 enum class TcMode { TF32X3 = 0, TF32 = 1, BF16 = 2, F16X3 = 3, F16 = 4 };
 
 constexpr int TC_BM = 128, TC_BN = 256;   // TC_BN: default N tile (template parameter BN overrides it)
-constexpr int TC_THREADS = 192;
+constexpr int TC2_BM = 256;               // M tile of a CTA pair
+constexpr int TC_THREADS = 384;
+constexpr int TC_EPI_PITCH = 36;          // floats per row of a consumer warpgroup's 64 x 32 epilogue block
+constexpr int TC_SMEM_MAX = 227 * 1024;
 
 template <TcMode MODE, int BN = TC_BN>
 struct TcCfg {
@@ -37,28 +42,25 @@ struct TcCfg {
   static constexpr int kElem = (MODE == TcMode::BF16 || MODE == TcMode::F16X3 || MODE == TcMode::F16) ? 2 : 4;
   static constexpr int kBK = 128 / kElem;                         // elements per 128-byte swizzle row
   static constexpr int kOps = (MODE == TcMode::TF32X3 || MODE == TcMode::F16X3) ? 2 : 1;   // hi (+ lo) tiles per operand
-  static constexpr int kUmmaK = 32 / kElem;                       // K per tcgen05.mma
+  static constexpr int kMmaK = 32 / kElem;                        // K per wgmma
   static constexpr int kABytes = TC_BM * 128, kBBytes = BN * 128;
   static constexpr int kStageBytes = kOps * (kABytes + kBBytes);
-  static constexpr int kStages = (kOps == 2) ? 2 : 4;
-  static constexpr int kSmem = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ +
-                               (kOps == 1 ? TC_EPI_SCRATCH : 0) /*epilogue transpose (single-pass modes)*/;
+  static constexpr int kEpiBytes = 2 * 64 * TC_EPI_PITCH * 4;
+  static constexpr int kFixed = kEpiBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kStages = (TC_SMEM_MAX - kFixed) / kStageBytes > 6 ? 6 : (TC_SMEM_MAX - kFixed) / kStageBytes;
+  static_assert(kStages >= 2, "shared memory ring too shallow");
+  static constexpr int kSmem = kStages * kStageBytes + kFixed;
   static constexpr bool kTF32 = (MODE == TcMode::TF32X3 || MODE == TcMode::TF32);
-  static constexpr int kFmt = kTF32 ? 2 : (MODE == TcMode::BF16 ? 1 : 0);   // 0 f16, 1 bf16, 2 tf32
-  static constexpr uint32_t kIdesc = tc::make_idesc(kFmt, TC_BM, BN);
-  static constexpr uint32_t kTmemCols = 2 * BN;   // two accumulator buffers (power of two >= 32)
 };
 
-// Epilogues that declare `static constexpr bool kCoalesced = true` get their accumulator block transposed through shared
-// memory (see the epilogue loop) and are called as vec4(g, row, col, float4) with lanes running along a row; they also
-// provide `bool direct(int col0)` to keep the thread-per-row call for selected column ranges.
+// Epilogues that declare `static constexpr bool kCoalesced = true` are called as vec4(g, row, col, float4) with lanes
+// running along a row; they also provide `bool direct(int col0)` to keep the thread-per-row call for selected column ranges.
 template <class E, class = void> struct EpiCoalesced { static constexpr bool value = false; };
 template <class E> struct EpiCoalesced<E, std::enable_if_t<E::kCoalesced>> { static constexpr bool value = true; };
 
 // Read-modify-write epilogues (`static constexpr bool kPrefetch = true`) additionally provide
-// `float4 fetch(g, row, col)` and `vec4(g, row, col, acc, fetched)`: the coalesced loop then issues the 8 reads of a warp's
-// block before the first write (through one pointer the compiler must otherwise keep every load behind the previous
-// store, and each of the 64 round trips of a tile costs a full memory latency on warps that are alone on their scheduler).
+// `float4 fetch(g, row, col)` and `vec4(g, row, col, acc, fetched)`: the coalesced loop then issues a thread's reads of a
+// block before its first write (through one pointer the compiler must otherwise keep every load behind the previous store).
 template <class E, class = void> struct EpiPrefetch { static constexpr bool value = false; };
 template <class E> struct EpiPrefetch<E, std::enable_if_t<E::kPrefetch>> { static constexpr bool value = true; };
 
@@ -66,7 +68,7 @@ struct TcProblem {
   const int* grp_batch;    // [n_groups] B batch item (frame) of each group
   const int* grp_row0;     // [n_groups] first A row
   const int* grp_m;        // [n_groups] number of A rows
-  const int* tile_start;   // [n_groups + 1] prefix of ceil(m / 128)
+  const int* tile_start;   // [n_groups + 1] prefix of ceil(m / M tile)  (M tile: TC_BM, or TC2_BM for the pair kernel)
   int n_groups;
   int N, K;                // B rows per batch item, reduction length
 };
@@ -74,42 +76,35 @@ struct TcProblem {
 // Epi must provide a per-thread `State` plus
 //   tile_begin(State&)                                                      once per (row, tile)
 //   operator()(State&, int g, int r_in_group, int col0, const float (&v)[32], int ncols_valid)
-//                                                                           per 32 consecutive columns
+//                                                                           per 32 consecutive columns, in column order
 //   tile_end(State&, int g, int r_in_group, int n_tile)                     once per (row, tile)
-template <TcMode MODE, class Epi, int BN = TC_BN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-               const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, TcProblem pb,
-               Epi epi) {
+template <TcMode MODE, class Epi, int BN, bool PAIR>
+__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi,
+                                             const CUtensorMap& tmB_lo, const TcProblem& pb, const Epi& epi) {
   using Cfg = TcCfg<MODE, BN>;
+  constexpr int TM = PAIR ? TC2_BM : TC_BM;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* full = bars;                       // [kStages]
-  uint64_t* empty = bars + Cfg::kStages;       // [kStages]
-  uint64_t* tfull = bars + 2 * Cfg::kStages;   // [2]
-  uint64_t* tempty = tfull + 2;                // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);   // [kStages]
+  uint64_t* empty = full + Cfg::kStages;                                                    // [kStages]
   float* epi_scratch = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + 256);
-  static_assert(!EpiCoalesced<Epi>::value || Cfg::kOps == 1, "coalesced epilogues need the scratch of the single-pass modes");
+  static_assert(2 * Cfg::kStages * 8 <= 256, "barrier block");
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const uint32_t rank = PAIR ? tc::cluster_ctarank() : 0u;
+  const int unit = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, n_units = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   const int n_tiles_n = (pb.N + BN - 1) / BN;
   const int total_tiles = pb.tile_start[pb.n_groups] * n_tiles_n;
   const int KB = (pb.K + Cfg::kBK - 1) / Cfg::kBK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&tmA_hi); tc::prefetch_tmap(&tmB_hi);
     if (Cfg::kOps == 2) { tc::prefetch_tmap(&tmA_lo); tc::prefetch_tmap(&tmB_lo); }
-    for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { tc::mbar_init(&tfull[b], 1); tc::mbar_init(&tempty[b], 4); }
+    // empty: one arrival per consumer warpgroup of every CTA whose B half lands in this CTA's slot
+    for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], PAIR ? 4 : 2); }
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+  if (PAIR) tc::cluster_sync_all(); else __syncthreads();
 
   // tile id -> (group, m0, n0): m-tile index is the slow dimension so that CTAs that run together share
   // the same B rows (frame) in L2
@@ -122,14 +117,15 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       if (pb.tile_start[mid] <= mt) lo = mid; else hi = mid - 1;
     }
     g = lo;
-    m0 = (mt - pb.tile_start[g]) * TC_BM;
+    m0 = (mt - pb.tile_start[g]) * TM + (int)rank * TC_BM;
   };
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (tc::elect_one()) {
+    tc::regs_dealloc<40>();
+    if (warp == 0 && tc::elect_one()) {
       int stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      for (int tile = unit; tile < total_tiles; tile += n_units) {
         int g, m0, n0;
         decode(tile, g, m0, n0);
         const int arow = pb.grp_row0[g] + m0, batch = pb.grp_batch[g];
@@ -141,114 +137,147 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           tc::tma_load_2d(&tmA_hi, &full[stage], st, k0, arow);
           if (Cfg::kOps == 2) tc::tma_load_2d(&tmA_lo, &full[stage], st + Cfg::kABytes, k0, arow);
           uint8_t* sb = st + Cfg::kOps * Cfg::kABytes;
-          tc::tma_load_3d(&tmB_hi, &full[stage], sb, k0, n0, batch);
-          if (Cfg::kOps == 2) tc::tma_load_3d(&tmB_lo, &full[stage], sb + Cfg::kBBytes, k0, n0, batch);
+          if constexpr (PAIR) {   // this CTA's half of the B rows, into both CTAs
+            const int off = (int)rank * (BN / 2);
+            tc::tma_load_3d_mc(&tmB_hi, &full[stage], sb + off * 128, k0, n0 + off, batch, 3);
+            if (Cfg::kOps == 2) tc::tma_load_3d_mc(&tmB_lo, &full[stage], sb + Cfg::kBBytes + off * 128, k0, n0 + off, batch, 3);
+          } else {
+            tc::tma_load_3d(&tmB_hi, &full[stage], sb, k0, n0, batch);
+            if (Cfg::kOps == 2) tc::tma_load_3d(&tmB_lo, &full[stage], sb + Cfg::kBBytes, k0, n0, batch);
+          }
           if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    int stage = 0, phase = 0, it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1, aphase = (it >> 1) & 1;
-      tc::mbar_wait(&tempty[buf], aphase ^ 1);
-      tc::fence_after_sync();
-      const uint32_t tmem_d = tmem_base + buf * BN;
-      for (int kb = 0; kb < KB; ++kb) {
-        tc::mbar_wait(&full[stage], phase);
-        tc::fence_after_sync();
-        if (tc::elect_one()) {
-          const uint32_t sa = tc::smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kOps * Cfg::kABytes;
-#pragma unroll
-          for (int ks = 0; ks < Cfg::kBK / Cfg::kUmmaK; ++ks) {
-            const uint32_t koff = ks * 32;  // bytes inside the 128-byte swizzle row
-            const uint64_t a_hi = tc::smem_desc_sw128(sa + koff), b_hi = tc::smem_desc_sw128(sb + koff);
-            const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
-            if (Cfg::kOps == 2) {
-              const uint64_t a_lo = tc::smem_desc_sw128(sa + Cfg::kABytes + koff);
-              const uint64_t b_lo = tc::smem_desc_sw128(sb + Cfg::kBBytes + koff);
-              // small terms first, then the dominant hi*hi
-              tc::mma_ss<Cfg::kTF32>(tmem_d, a_lo, b_hi, Cfg::kIdesc, first);
-              tc::mma_ss<Cfg::kTF32>(tmem_d, a_hi, b_lo, Cfg::kIdesc, 1u);
-              tc::mma_ss<Cfg::kTF32>(tmem_d, a_hi, b_hi, Cfg::kIdesc, 1u);
-            } else {
-              tc::mma_ss<Cfg::kTF32>(tmem_d, a_hi, b_hi, Cfg::kIdesc, first);
-            }
-          }
-          tc::mma_commit(&empty[stage]);                 // smem slot reusable once these MMAs have read it
-          if (kb == KB - 1) tc::mma_commit(&tfull[buf]);  // accumulator complete
-        }
-        __syncwarp();
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-      }
-    }
   } else {
-    // ===================== epilogue (warps 2..5 -> TMEM lane quadrants 2,3,0,1) =====================
-    const int quad = warp & 3;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1, aphase = (it >> 1) & 1;
+    // ===================== MMA + epilogue: warpgroup cw owns rows [64 cw, 64 cw + 64) of the tile =====================
+    tc::regs_alloc<232>();
+    const int cw = wg - 1;
+    float* sw = epi_scratch + cw * 64 * TC_EPI_PITCH;
+    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);   // accumulator fragment: rows fr, fr + 8
+    auto release = [&](int s) {
+      if (t == 0) {
+        if constexpr (PAIR) { tc::mbar_arrive_cluster(&empty[s], 0); tc::mbar_arrive_cluster(&empty[s], 1); }
+        else tc::mbar_arrive(&empty[s]);
+      }
+    };
+    int stage = 0, phase = 0;
+    float acc[BN / 2];
+    for (int tile = unit; tile < total_tiles; tile += n_units) {
       int g, m0, n0;
       decode(tile, g, m0, n0);
-      const int r = m0 + quad * 32 + lane;       // row inside the group
-      const bool row_ok = r < pb.grp_m[g];
-      typename Epi::State est;
-      epi.tile_begin(est);
-      tc::mbar_wait(&tfull[buf], aphase);
-      tc::fence_after_sync();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + buf * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        uint32_t v[32];
-        tc::tmem_ld32(taddr + c, v);
-        tc::tmem_ld_wait();
-        const int ncols = min(32, pb.N - (n0 + c));
-        if constexpr (EpiCoalesced<Epi>::value) {
-          if (!epi.direct(n0 + c)) {
-            // transpose the warp's 32 x 32 block through shared memory so that global accesses run along rows:
-            // lane (r4, c4) then owns 4 consecutive columns of rows it*4 + r4 -> 8 lanes cover 128 contiguous bytes
-            float* sw = epi_scratch + (warp - 2) * (32 * 36);
 #pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              *reinterpret_cast<float4*>(sw + lane * 36 + i) =
-                  make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-            __syncwarp();
-            const int c4 = (lane & 7) * 4, r4 = lane >> 3;
-            const int row_base = m0 + quad * 32;
-            if (c4 < ncols) {
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < KB; ++kb) {
+        tc::mbar_wait(&full[stage], phase);
+        tc::wgmma_fence();
+        const uint32_t sa = tc::smem_u32(smem + stage * Cfg::kStageBytes) + cw * 64 * 128;
+        const uint32_t sb = tc::smem_u32(smem + stage * Cfg::kStageBytes) + Cfg::kOps * Cfg::kABytes;
 #pragma unroll
-              for (int it = 0; it < 8; ++it) {
-                const int rr = it * 4 + r4;
-                if (row_base + rr < pb.grp_m[g])
-                  epi.vec4(g, row_base + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * 36 + c4));
-              }
-            }
-            __syncwarp();
-            continue;
+        for (int ks = 0; ks < Cfg::kBK / Cfg::kMmaK; ++ks) {
+          const uint32_t koff = ks * 32;  // bytes inside the 128-byte swizzle row
+          const uint64_t a_hi = tc::smem_desc_sw128(sa + koff), b_hi = tc::smem_desc_sw128(sb + koff);
+          if (Cfg::kOps == 2) {
+            const uint64_t a_lo = tc::smem_desc_sw128(sa + Cfg::kABytes + koff);
+            const uint64_t b_lo = tc::smem_desc_sw128(sb + Cfg::kBBytes + koff);
+            // small terms first, then the dominant hi*hi
+            tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_lo, b_hi, 1u);
+            tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_lo, 1u);
+            tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_hi, 1u);
+          } else {
+            tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_hi, 1u);
           }
         }
-        if (row_ok && ncols > 0) {
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();            // the previous K-block's MMAs are done: its slot may be refilled
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
+      tc::wgmma_wait<0>();
+      tc::reg_fence(acc);
+      if (prev >= 0) release(prev);
+
+      // ---- epilogue: 32-column blocks through shared memory ----
+      const int rbase = m0 + cw * 64;        // row (inside the group) of the warpgroup's first row
+      const int r = rbase + t;
+      const bool row_ok = t < 64 && r < pb.grp_m[g];
+      typename Epi::State est;
+      epi.tile_begin(est);
+#pragma unroll
+      for (int c = 0; c < BN; c += 32) {
+#pragma unroll
+        for (int ii = 0; ii < 4; ++ii) {
+          const int i = c / 8 + ii;
+          *reinterpret_cast<float2*>(sw + fr * TC_EPI_PITCH + ii * 8 + fc) = make_float2(acc[4 * i], acc[4 * i + 1]);
+          *reinterpret_cast<float2*>(sw + (fr + 8) * TC_EPI_PITCH + ii * 8 + fc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        }
+        tc::named_sync(1 + cw, 128);
+        const int ncols = min(32, pb.N - (n0 + c));
+        bool done = false;
+        if constexpr (EpiCoalesced<Epi>::value) {
+          if (!epi.direct(n0 + c)) {
+            // thread (r4, c4) owns 4 consecutive columns of rows it * 16 + r4 -> 8 threads cover 128 contiguous bytes
+            const int c4 = (t & 7) * 4, r4 = t >> 3;
+            if (c4 < ncols) {
+              if constexpr (EpiPrefetch<Epi>::value) {
+                float4 pre[4];
+#pragma unroll
+                for (int it = 0; it < 4; ++it) {
+                  const int rr = it * 16 + r4;
+                  pre[it] = rbase + rr < pb.grp_m[g] ? epi.fetch(g, rbase + rr, n0 + c + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+                }
+#pragma unroll
+                for (int it = 0; it < 4; ++it) {
+                  const int rr = it * 16 + r4;
+                  if (rbase + rr < pb.grp_m[g])
+                    epi.vec4(g, rbase + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * TC_EPI_PITCH + c4), pre[it]);
+                }
+              } else {
+#pragma unroll
+                for (int it = 0; it < 4; ++it) {
+                  const int rr = it * 16 + r4;
+                  if (rbase + rr < pb.grp_m[g])
+                    epi.vec4(g, rbase + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * TC_EPI_PITCH + c4));
+                }
+              }
+            }
+            done = true;
+          }
+        }
+        if (!done && row_ok && ncols > 0) {
           float f[32];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
+          for (int i = 0; i < 32; i += 4) {
+            const float4 v = *reinterpret_cast<const float4*>(sw + t * TC_EPI_PITCH + i);
+            f[i] = v.x; f[i + 1] = v.y; f[i + 2] = v.z; f[i + 3] = v.w;
+          }
           epi(est, g, r, n0 + c, f, ncols);
         }
+        tc::named_sync(1 + cw, 128);
       }
       if (row_ok) epi.tile_end(est, g, r, n0 / BN);
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tempty[buf]);
     }
   }
+  if (PAIR) tc::cluster_sync_all();   // no CTA may exit while its peer can still multicast into it or arrive on its barriers
+}
 
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
+template <TcMode MODE, class Epi, int BN = TC_BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+               const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, TcProblem pb,
+               Epi epi) {
+  tc_gemm_body<MODE, Epi, BN, false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
+}
+
+// pb.tile_start: prefix of ceil(m / TC2_BM) per group; B tensor maps with boxes of BN / 2 rows; even grid.
+template <TcMode MODE, class Epi, int BN = TC_BN>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
+tc_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, TcProblem pb,
+                    Epi epi) {
+  tc_gemm_body<MODE, Epi, BN, true>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
 }
 
 }  // namespace dtk

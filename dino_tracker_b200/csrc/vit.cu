@@ -5,7 +5,7 @@
 // facebookresearch/dinov2's -- parity unpinned, see DESIGN.md).
 //
 // Default path (gemm_f16 = 1, attn_materialized = 0): fp16 operands / fp32 accumulation everywhere.  The linear layers
-// (patch embedding, qkv, proj, fc1, fc2) run on the tcgen05 GEMMs of tcgemm.cuh / tcgemm2.cuh (CTA pairs when gemm_pair = 1)
+// (patch embedding, qkv, proj, fc1, fc2) run on the wgmma GEMMs of tcgemm.cuh (two-CTA clusters when gemm_pair = 1)
 // with bias / position embedding / GELU / LayerScale + residual / head scatter as coalesced epilogues on the accumulator;
 // the residual stream stays fp32.  Attention is the fused kernel of flash.cuh (scores never leave the SM).
 // Validation path (attn_materialized = 1): TF32 GEMMs, attention scores materialised per (frame, row chunk) in a workspace
@@ -14,7 +14,6 @@
 #include "corr.cuh"
 #include "tcgemm.cuh"
 #include "flash.cuh"
-#include "tcgemm2.cuh"
 
 namespace dtk {
 
@@ -387,9 +386,7 @@ static int run_gemm(const void* A, uint64_t a_rows, const void* Bm, uint64_t b_b
     attr = true;
   }
   TcProblem pb{pl.batch, pl.row0, pl.m, pl.tile_start, n_groups, (int)b_rows, K};
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   int tiles = max_tiles * cdiv((int)b_rows, BN);
   int grid = tiles < sms ? tiles : sms;
   ProfRange pr(prof_cls, st);
@@ -407,21 +404,17 @@ static int plan(const Plan& pl, int n_groups, int rows, int row_stride, int row_
   return DINOTRK_OK;
 }
 
-// CTA-pair variant (cta_group::2, 256 x 256 tiles) for the single-pass fp16 linear layers; the plan must be in
-// 256-row tiles.
+// CTA-pair variant (a cluster of two CTAs sharing the B tile by multicast, 256 x 256 tiles) for the single-pass fp16
+// linear layers; the plan must be in 256-row tiles.
 template <class Epi>
 static int run_gemm_pair(const void* A, uint64_t a_rows, const void* Bm, uint64_t b_rows, int K, const Plan& pl,
                          int max_tiles, const Epi& epi, int prof_cls, cudaStream_t st) {
-  // 8 epilogue warps (two per TMEM lane quadrant): the fused epilogues (GELU, LayerScale + residual, head scatter) run on
-  // warps that have their scheduler to themselves, so their latency chains, not the MMAs, paced these GEMMs with 4 warps
-  constexpr int kEpiWarps = 8;
-  using Base = TcCfg<TcMode::F16, TC2_BN>;
-  using Cfg = Tc2Cfg<TcMode::F16, kEpiWarps, true>;
+  using Cfg = TcCfg<TcMode::F16, TC_BN>;
   CUtensorMap tmA, tmB;
   int rc;
-  if ((rc = make_tmap_2d(&tmA, A, a_rows, K, 128, Base::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB, Bm, 1, b_rows, K, TC2_BN / 2, Base::kBK, TMAP_F16))) return rc;
-  auto kern = tc_gemm2_kernel<TcMode::F16, Epi, kEpiWarps>;
+  if ((rc = make_tmap_2d(&tmA, A, a_rows, K, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
+  if ((rc = make_tmap_3d(&tmB, Bm, 1, b_rows, K, TC_BN / 2, Cfg::kBK, TMAP_F16))) return rc;
+  auto kern = tc_gemm_pair_kernel<TcMode::F16, Epi, TC_BN>;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
@@ -429,13 +422,11 @@ static int run_gemm_pair(const void* A, uint64_t a_rows, const void* Bm, uint64_
     attr = true;
   }
   TcProblem pb{pl.batch, pl.row0, pl.m, pl.tile_start, 1, (int)b_rows, K};
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int pairs = max_tiles * cdiv((int)b_rows, TC2_BN);
+  const int sms = num_sms();
+  int pairs = max_tiles * cdiv((int)b_rows, TC_BN);
   int grid = 2 * (pairs < sms / 2 ? pairs : sms / 2);
   ProfRange pr(prof_cls, st);
-  kern<<<grid, 64 + 32 * kEpiWarps, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
+  kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -451,25 +442,16 @@ static int launch_flash(const __half* q16, const __half* k16, const __half* v16,
   if ((rc = make_tmap_2d(&tmQ, q16, (uint64_t)B * heads * N1, HD, FA_BQ, HD, TMAP_F16))) return rc;
   if ((rc = make_tmap_3d(&tmK, k16, (uint64_t)B * heads, N1, HD, FA_BKV, HD, TMAP_F16))) return rc;
   if ((rc = make_tmap_3d(&tmV, v16, (uint64_t)B * heads, HD, N1, HD, 64, TMAP_F16, (uint64_t)N1p))) return rc;
-  // share of the exponentials evaluated on the FMA pipe (DTK_FA_POLY = 0 / 25 / 37 / 50 %, default 25)
-  static int poly = -1;
-  if (poly < 0) {
-    const char* e = getenv("DTK_FA_POLY");
-    // measured on ViT-L (8108 tokens, 2 frames x 16 blocks): 0 % 11.3 ms, 25 % 10.2 ms, 37 % 10.3 ms, 50 % 10.9 ms -- since
-    // P goes through tensor memory the softmax warps are MUFU-bound enough for the packed polynomial to pay
-    poly = e ? atoi(e) : 25;
-    DTK_CUDA(cudaFuncSetAttribute(flash_attn_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-    DTK_CUDA(cudaFuncSetAttribute(flash_attn_kernel<0x88>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-    DTK_CUDA(cudaFuncSetAttribute(flash_attn_kernel<0xA8>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-    DTK_CUDA(cudaFuncSetAttribute(flash_attn_kernel<0xAA>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
+  static PerDev<bool> attr_dev;
+  bool& attr = attr_dev.get();
+  if (!attr) {
+    DTK_CUDA(cudaFuncSetAttribute(flash_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
+    attr = true;
   }
   FlashParams fpar{N1, D, heads, out, out_f16 ? 1 : 0};
   ProfRange pr(PROF_VIT_ATTN, st);
   const dim3 fgrid(cdiv(N1, FA_BQ), B * heads);
-  if (poly <= 0) flash_attn_kernel<0><<<fgrid, FA_THREADS, FA_SMEM, st>>>(tmQ, tmK, tmV, fpar);
-  else if (poly <= 25) flash_attn_kernel<0x88><<<fgrid, FA_THREADS, FA_SMEM, st>>>(tmQ, tmK, tmV, fpar);
-  else if (poly <= 37) flash_attn_kernel<0xA8><<<fgrid, FA_THREADS, FA_SMEM, st>>>(tmQ, tmK, tmV, fpar);
-  else flash_attn_kernel<0xAA><<<fgrid, FA_THREADS, FA_SMEM, st>>>(tmQ, tmK, tmV, fpar);
+  flash_attn_kernel<<<fgrid, FA_THREADS, FA_SMEM, st>>>(tmQ, tmK, tmV, fpar);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -537,7 +519,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   // significand like TF32, twice the tensor rate, half the operand traffic).  The validation path
   // (attn_materialized) keeps every operand fp32 / TF32.
   const bool f16 = c->gemm_f16 != 0 && c->attn_materialized == 0;
-  const bool pairs = f16 && c->gemm_pair != 0;   // linear layers on CTA pairs (cta_group::2)
+  const bool pairs = f16 && c->gemm_pair != 0;   // linear layers on two-CTA clusters
   const int pair_tiles = cdiv((int)((size_t)B * (g->h * g->w + 1)), TC2_BM);
   __half* y16 = reinterpret_cast<__half*>(y);
   __half* h16 = reinterpret_cast<__half*>(hbuf);
@@ -577,7 +559,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
     if ((rc = layernorm(w[0], w[1]))) return rc;
     if ((rc = plan(pl, 1, (int)rows, 0, 0, 0, st, pairs ? TC2_BM : TC_BM))) return rc;
     if (c->attn_materialized == 0) {
-      // fused attention: fp16 q / k / v^T, scores stay in TMEM / shared memory
+      // fused attention: fp16 q / k / v^T, scores stay in registers
       __half* q16 = reinterpret_cast<__half*>(q);
       __half* k16 = reinterpret_cast<__half*>(k);
       __half* v16 = reinterpret_cast<__half*>(vT);
@@ -624,7 +606,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
     if ((rc = layernorm(w[7], w[8]))) return rc;
     if (pairs) {
       EpiGelu<__half> eg{{}, h16, w[10], 4 * D};
-      static const int epi_direct2 = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;  // bit 1: fp16 GELU rows written thread-per-row (64 B per thread, whole sectors; measured 6.46 -> 6.32 ms per 2 x 16 blocks)
+      static const int epi_direct2 = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;  // bit 1: fp16 GELU rows written thread-per-row (64 B per thread, whole sectors)
       eg.all_direct = (epi_direct2 & 2) ? 1 : 0;
       if ((rc = run_gemm_pair<EpiGelu<__half>>(y16, rows, w[9], 4 * D, D, pl, pair_tiles, eg, PROF_VIT_GEMM, st))) return rc;
       if ((rc = run_gemm_pair<EpiResidual>(h16, rows, w[11], D, 4 * D, pl, pair_tiles, EpiResidual{{}, x, w[12], w[13], D},

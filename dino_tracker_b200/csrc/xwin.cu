@@ -4,7 +4,6 @@
 #include "common.cuh"
 #include "corr.cuh"
 #include "tcgemm.cuh"
-#include "tcgemm2.cuh"
 #include "xwin.cuh"
 
 namespace dtk {
@@ -13,7 +12,7 @@ int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], con
                  const uint32_t box[4], int elem);   // corr_tc.cu
 
 // ====================================================================================================== 1. coarse GEMM
-// Epilogue of the single-pass kind::f16 GEMM over the `hi` halves: nothing is stored per token.  Per (map, 256-token tile):
+// Epilogue of the single-pass fp16 GEMM over the `hi` halves: nothing is stored per token.  Per (map, 128-token tile):
 // key1 = bits(max) << 32 | (0x7fffffff - first token holding it), max2 = second largest value (>= 0).  Values are the same
 // expression as the exact path, relu(acc / max(|d| |F|, 1e-8)), with a fast division (its error is part of XW_EPS).
 struct CoarseEpi {
@@ -86,7 +85,7 @@ int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cuda
   const size_t n = (size_t)fv.T * fv.P;
   DTK_CUDA(cudaMemsetAsync(min_bits, 0x7f, sizeof(unsigned), st));   // 0x7f7f7f7f: a huge positive float
   ProfRange pr(PROF_XW_PLAN, st);
-  xw_rnorm_kernel<<<148 * 4, 256, 0, st>>>(fv.norms, rnorms, n, min_bits);
+  xw_rnorm_kernel<<<num_sms() * 4, 256, 0, st>>>(fv.norms, rnorms, n, min_bits);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -94,14 +93,13 @@ int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cuda
 int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
                      const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                      int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms) {
-  using Cfg = Tc2Cfg<TcMode::F16, 8, false>;
-  using Base = TcCfg<TcMode::F16, TC2_BN>;
-  static_assert(TC2_BN == 2 * XW_TILE, "coarse keys are per half GEMM tile (8 epilogue warps)");
+  using Cfg = TcCfg<TcMode::F16, XW_TILE>;
+  static_assert(XW_TILE == 128, "coarse keys are per GEMM N tile");
   CUtensorMap tmA, tmB;
   int rc;
-  if ((rc = make_tmap_2d(&tmA, desc_hi, desc_rows, fv.C, 128, Base::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB, fv.hi, fv.T, fv.P, fv.C, TC2_BN / 2, Base::kBK, TMAP_F16))) return rc;
-  auto kern = tc_gemm2_kernel<TcMode::F16, CoarseEpi, 8>;
+  if ((rc = make_tmap_2d(&tmA, desc_hi, desc_rows, fv.C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
+  if ((rc = make_tmap_3d(&tmB, fv.hi, fv.T, fv.P, fv.C, XW_TILE / 2, Cfg::kBK, TMAP_F16))) return rc;
+  auto kern = tc_gemm_pair_kernel<TcMode::F16, CoarseEpi, XW_TILE>;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
@@ -110,14 +108,12 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
   }
   TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, fv.P, fv.C};
   CoarseEpi epi{rnorms, desc_norm, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int tiles_bound = max_tiles * cdiv(fv.P, TC2_BN);
+  const int sms = num_sms();
+  const int tiles_bound = max_tiles * cdiv(fv.P, XW_TILE);
   int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
   if (grid < 2) grid = 2;
   ProfRange pr(PROF_XW_COARSE, st);
-  kern<<<grid, 64 + 32 * 8, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
+  kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -249,49 +245,36 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
   if (cells.n_cells <= 0 || n_maps <= 0) return DINOTRK_OK;
   ProfRange pr(PROF_XW_PLAN, st);
   int grid = cdiv(n_maps, PLAN_WARPS);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
   xw_cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, n_groups, n_tiles, xc.key1, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
   DTK_LAUNCHED();
   grid = cdiv(cells.n_cells, PLAN_WARPS);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
   xw_cell_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(cells, g.w, xc.cand, xc.pinfo, xc.stat, xc.cell_of, xc.box_org);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
 
 // ====================================================================================================== 3. exact box GEMM
-// Persistent, warp-specialised (same roles as tc_gemm_kernel).  One "tile" = one cell.  The BOX TOKENS are the UMMA M
-// operand (4 parts of 6 box rows = 126 of 128 rows) and the cell's descriptors the N operand (64 or 128 columns): a cell
-// of T = 50 maps fills 50 of 64 columns, where descriptors-as-rows filled 50 of 128 rows.  D[part][token][map] in TMEM
-// (4 x NB columns; two cells in flight for NB = 64), split precision (lo*hi + hi*lo + hi*hi per K step, in the full-map
-// GEMM's order).  A K-block of the descriptors (hi, lo) is loaded once and used by the four parts; the box rows arrive as
-// 4-D TMA boxes {64 channels, 21 columns, 6 rows, 1 frame} of the [T][h][w][C] feature video, zero-filled outside the
-// token grid.  Epilogue: TMEM lane = box token, so for every map the 32 lanes of a warp write 32 consecutive floats of
-// its accumulator row -- coalesced without a transpose.
+// Persistent, warp-specialised (same roles as tc_gemm_kernel).  One tile = one part of a cell's box: the BOX TOKENS are the
+// wgmma M operand (4 parts of 6 box rows = 126 of 128 rows, 64 per consumer warpgroup) and the cell's descriptors the N
+// operand (64 or 128 columns): a cell of T = 50 maps fills 50 of 64 columns, where descriptors-as-rows filled 50 of 128
+// rows.  Split precision (lo*hi + hi*lo + hi*hi per K step, in the full-map GEMM's order).  The box rows arrive as 4-D TMA
+// boxes {64 channels, 21 columns, 6 rows, 1 frame} of the [T][h][w][C] feature video, zero-filled outside the token grid;
+// the descriptor K-block travels in the same stage.  Epilogue: straight from the accumulator fragment to xbox[map][token]
+// (4 lanes of a quad hold 8 consecutive maps of one token, 8 quads 8 consecutive tokens: 32-byte runs).
 template <int NB>
 struct XwCfg {
   static constexpr int kBK = 64;                            // fp16 elements per 128-byte swizzle row
   static constexpr int kTokBytes = 128 * 128;               // one operand half (hi or lo) of a token tile: 128 rows, 126 written
-  static constexpr int kTokStage = 2 * kTokBytes, kTokStages = NB == 64 ? 5 : 4;
   static constexpr int kTokTx = 2 * XW_PART_TOK * 128;
   static constexpr int kLastRows = XW_BOX - (XW_PARTS - 1) * XW_PART_ROWS;     // the last part holds 3 box rows, not 6
   static constexpr int kTokTxLast = 2 * kLastRows * XW_BOX * 128;
   static constexpr int kDescBytes = NB * 128;               // one operand half of the descriptor K-block
-  static constexpr int kDescStage = 2 * kDescBytes, kDescStages = 2;
-  static constexpr int kSmem = kDescStages * kDescStage + kTokStages * kTokStage + 256;
-  static constexpr int kAccCols = XW_PARTS * NB, kAccBufs = 512 / kAccCols;
-  static constexpr uint32_t kIdesc = tc::make_idesc(0, 128, NB);
+  static constexpr int kStageBytes = 2 * kTokBytes + 2 * kDescBytes;
+  static constexpr int kStages = NB == 64 ? 4 : 3;
+  static constexpr int kSmem = kStages * kStageBytes + 1024 + 256;
 };
-
-namespace tc {
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];\n" ::"r"(
-          smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-}  // namespace tc
 
 template <int NB>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -301,151 +284,100 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
                const int2* __restrict__ box_org, float* __restrict__ xbox, int K) {
   using Cfg = XwCfg<NB>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if (tc::smem_u32(smem) & 1023u) __trap();   // no static shared memory in this kernel: the window starts 1 KB-aligned
-  uint8_t* t_ring = smem;                                           // token tiles (UMMA A)
-  uint8_t* d_ring = smem + Cfg::kTokStages * Cfg::kTokStage;        // descriptor K-blocks (UMMA B)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(d_ring + Cfg::kDescStages * Cfg::kDescStage);
-  uint64_t* d_full = bars;                          // [2]
-  uint64_t* d_empty = d_full + Cfg::kDescStages;    // [2]
-  uint64_t* t_full = d_empty + Cfg::kDescStages;    // [kTokStages]
-  uint64_t* t_empty = t_full + Cfg::kTokStages;     // [kTokStages]
-  uint64_t* tfull = t_empty + Cfg::kTokStages;      // [2]
-  uint64_t* tempty = tfull + 2;                     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  static_assert((2 * Cfg::kDescStages + 2 * Cfg::kTokStages + 4) * 8 + 4 <= 256, "barrier block");
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);   // [kStages]
+  uint64_t* empty = full + Cfg::kStages;                                                    // [kStages]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int KB = (K + Cfg::kBK - 1) / Cfg::kBK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo); tc::prefetch_tmap(&tmT_hi); tc::prefetch_tmap(&tmT_lo);
     tc::prefetch_tmap(&tmL_hi); tc::prefetch_tmap(&tmL_lo);
-    for (int s = 0; s < Cfg::kDescStages; ++s) { tc::mbar_init(&d_full[s], 1); tc::mbar_init(&d_empty[s], 1); }
-    for (int s = 0; s < Cfg::kTokStages; ++s) { tc::mbar_init(&t_full[s], 1); tc::mbar_init(&t_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc::mbar_init(&tfull[s], 1); tc::mbar_init(&tempty[s], 4); }
+    for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 2); }
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (tc::elect_one()) {
-      int ds = 0, dph = 0, ts = 0, tph = 0;
+    tc::regs_dealloc<40>();
+    if (warp == 0 && tc::elect_one()) {
+      int stage = 0, phase = 0;
       for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
         const int2 org = box_org[cell];
         if (org.y == INT_MIN) continue;            // every map of the cell takes the full-map path
         const int drow = cells.row0[cell], frame = cells.frame[cell];
-        for (int kb = 0; kb < KB; ++kb) {
-          const int k0 = kb * Cfg::kBK;
-          tc::mbar_wait(&d_empty[ds], dph ^ 1);
-          uint8_t* sd = d_ring + ds * Cfg::kDescStage;
-          tc::mbar_expect_tx(&d_full[ds], Cfg::kDescStage);
-          tc::tma_load_2d(&tmD_hi, &d_full[ds], sd, k0, drow);
-          tc::tma_load_2d(&tmD_lo, &d_full[ds], sd + Cfg::kDescBytes, k0, drow);
-          if (++ds == Cfg::kDescStages) { ds = 0; dph ^= 1; }
-          for (int part = 0; part < XW_PARTS; ++part) {
-            tc::mbar_wait(&t_empty[ts], tph ^ 1);
-            uint8_t* st = t_ring + ts * Cfg::kTokStage;
-            if (part < XW_PARTS - 1) {
-              tc::mbar_expect_tx(&t_full[ts], Cfg::kTokTx);
-              tc::tma_load_4d(&tmT_hi, &t_full[ts], st, k0, org.y, org.x + part * XW_PART_ROWS, frame);
-              tc::tma_load_4d(&tmT_lo, &t_full[ts], st + Cfg::kTokBytes, k0, org.y, org.x + part * XW_PART_ROWS, frame);
-            } else {   // only the box rows that exist (this kernel runs at the L2 -> shared-memory bandwidth)
-              tc::mbar_expect_tx(&t_full[ts], Cfg::kTokTxLast);
-              tc::tma_load_4d(&tmL_hi, &t_full[ts], st, k0, org.y, org.x + part * XW_PART_ROWS, frame);
-              tc::tma_load_4d(&tmL_lo, &t_full[ts], st + Cfg::kTokBytes, k0, org.y, org.x + part * XW_PART_ROWS, frame);
-            }
-            if (++ts == Cfg::kTokStages) { ts = 0; tph ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    int ds = 0, dph = 0, ts = 0, tph = 0, it = 0;
-    for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
-      if (box_org[cell].y == INT_MIN) continue;
-      const int buf = it % Cfg::kAccBufs, use = it / Cfg::kAccBufs;
-      tc::mbar_wait(&tempty[buf], (use & 1) ^ 1);
-      tc::fence_after_sync();
-      for (int kb = 0; kb < KB; ++kb) {
-        tc::mbar_wait(&d_full[ds], dph);
-        const uint32_t sd = tc::smem_u32(d_ring + ds * Cfg::kDescStage);
         for (int part = 0; part < XW_PARTS; ++part) {
-          tc::mbar_wait(&t_full[ts], tph);
-          tc::fence_after_sync();
-          if (tc::elect_one()) {
-            const uint32_t st = tc::smem_u32(t_ring + ts * Cfg::kTokStage);
-            const uint32_t tmem_d = tmem_base + buf * Cfg::kAccCols + part * NB;
-#pragma unroll
-            for (int ks = 0; ks < Cfg::kBK / 16; ++ks) {
-              const uint32_t koff = ks * 32;
-              const uint64_t t_hi = tc::smem_desc_sw128(st + koff), t_lo = tc::smem_desc_sw128(st + Cfg::kTokBytes + koff);
-              const uint64_t d_hi = tc::smem_desc_sw128(sd + koff), d_lo = tc::smem_desc_sw128(sd + Cfg::kDescBytes + koff);
-              const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
-              tc::mma_ss<false>(tmem_d, t_hi, d_lo, Cfg::kIdesc, first);   // desc_lo * tok_hi, desc_hi * tok_lo, desc_hi * tok_hi:
-              tc::mma_ss<false>(tmem_d, t_lo, d_hi, Cfg::kIdesc, 1u);      // the product order of tc_gemm_kernel (F16X3)
-              tc::mma_ss<false>(tmem_d, t_hi, d_hi, Cfg::kIdesc, 1u);
-            }
-            tc::mma_commit(&t_empty[ts]);
-            if (part == XW_PARTS - 1) {
-              tc::mma_commit(&d_empty[ds]);
-              if (kb == KB - 1) tc::mma_commit(&tfull[buf]);
-            }
+          const bool last = part == XW_PARTS - 1;   // only the box rows that exist
+          for (int kb = 0; kb < KB; ++kb) {
+            const int k0 = kb * Cfg::kBK;
+            tc::mbar_wait(&empty[stage], phase ^ 1);
+            uint8_t* st = smem + stage * Cfg::kStageBytes;
+            uint8_t* sd = st + 2 * Cfg::kTokBytes;
+            tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + (last ? Cfg::kTokTxLast : Cfg::kTokTx));
+            tc::tma_load_4d(last ? &tmL_hi : &tmT_hi, &full[stage], st, k0, org.y, org.x + part * XW_PART_ROWS, frame);
+            tc::tma_load_4d(last ? &tmL_lo : &tmT_lo, &full[stage], st + Cfg::kTokBytes, k0, org.y, org.x + part * XW_PART_ROWS, frame);
+            tc::tma_load_2d(&tmD_hi, &full[stage], sd, k0, drow);
+            tc::tma_load_2d(&tmD_lo, &full[stage], sd + Cfg::kDescBytes, k0, drow);
+            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
           }
-          __syncwarp();
-          if (++ts == Cfg::kTokStages) { ts = 0; tph ^= 1; }
         }
-        if (++ds == Cfg::kDescStages) { ds = 0; dph ^= 1; }
       }
-      ++it;
     }
   } else {
-    // ===================== epilogue: TMEM lane = box token -> xbox[map][token], coalesced along the tokens =====================
-    const int quad = warp & 3;
-    int it = 0;
+    // ===================== MMA + epilogue: warpgroup cw owns box tokens [64 cw, 64 cw + 64) of a part =====================
+    tc::regs_alloc<232>();
+    const int cw = wg - 1;
+    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+    int stage = 0, phase = 0;
+    float acc[NB / 2];
     for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
       if (box_org[cell].y == INT_MIN) continue;
       const int m = cells.m[cell], map0 = cells.row0[cell];
-      const int buf = it % Cfg::kAccBufs, use = it / Cfg::kAccBufs;
-      tc::mbar_wait(&tfull[buf], use & 1);
-      tc::fence_after_sync();
-      const int tok = quad * 32 + lane;
-#pragma unroll 1
       for (int part = 0; part < XW_PARTS; ++part) {
-        const int col = part * XW_PART_TOK + tok;
-        const bool ok = tok < XW_PART_TOK && col < XW_BOX * XW_BOX;
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + buf * Cfg::kAccCols + part * NB;
-        float* dst = xbox + (size_t)map0 * XW_COLS + col;
-#pragma unroll 1
-        for (int c = 0; c < NB && c < m; c += 32) {
-          uint32_t v[32];
-          tc::tmem_ld32(taddr + c, v);
-          tc::tmem_ld_wait();
-          if (ok) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c + i < m) dst[(size_t)(c + i) * XW_COLS] = __uint_as_float(v[i]);
+        for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < KB; ++kb) {
+          tc::mbar_wait(&full[stage], phase);
+          tc::wgmma_fence();
+          const uint32_t st = tc::smem_u32(smem + stage * Cfg::kStageBytes) + cw * 64 * 128;
+          const uint32_t sd = tc::smem_u32(smem + stage * Cfg::kStageBytes) + 2 * Cfg::kTokBytes;
+#pragma unroll
+          for (int ks = 0; ks < Cfg::kBK / 16; ++ks) {
+            const uint32_t koff = ks * 32;
+            const uint64_t t_hi = tc::smem_desc_sw128(st + koff), t_lo = tc::smem_desc_sw128(st + Cfg::kTokBytes + koff);
+            const uint64_t d_hi = tc::smem_desc_sw128(sd + koff), d_lo = tc::smem_desc_sw128(sd + Cfg::kDescBytes + koff);
+            tc::wgmma_ss<false, NB>(acc, t_hi, d_lo, 1u);   // desc_lo * tok_hi, desc_hi * tok_lo, desc_hi * tok_hi:
+            tc::wgmma_ss<false, NB>(acc, t_lo, d_hi, 1u);   // the product order of tc_gemm_kernel (F16X3)
+            tc::wgmma_ss<false, NB>(acc, t_hi, d_hi, 1u);
+          }
+          tc::wgmma_commit();
+          tc::wgmma_wait<1>();
+          if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
+          prev = stage;
+          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+        }
+        tc::wgmma_wait<0>();
+        tc::reg_fence(acc);
+        if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int tok = cw * 64 + fr + 8 * h;
+          const int col = part * XW_PART_TOK + tok;
+          if (tok < XW_PART_TOK && col < XW_BOX * XW_BOX) {
+            float* dst = xbox + (size_t)map0 * XW_COLS + col;
+#pragma unroll
+            for (int i = 0; i < NB / 8; ++i) {
+              const int c = 8 * i + fc;
+              if (c < m) dst[(size_t)c * XW_COLS] = acc[4 * i + 2 * h];
+              if (c + 1 < m) dst[(size_t)(c + 1) * XW_COLS] = acc[4 * i + 2 * h + 1];
+            }
           }
         }
       }
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tempty[buf]);
-      ++it;
     }
-  }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -474,9 +406,7 @@ int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_h
     DTK_CUDA(cudaFuncSetAttribute(xw_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, XwCfg<128>::kSmem));
     attr = true;
   }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   const int grid = cells.n_cells < sms ? cells.n_cells : sms;
   ProfRange pr(PROF_XW_GEMM, st);
   if (small)
@@ -519,7 +449,7 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
   const int h = hp.h, w = hp.w;
   const int cp = lane & 7, pg = lane >> 3;
   // ---- input window (15 x 15 exact values, zero outside the map; extracted by xw_window_kernel, 16-float rows), every
-  // value as the pair (v, v): the packed FMAs below take it straight from one 64-bit shared-memory load ----
+  // value as the pair (v, v): the pair FMAs below take it straight from one 64-bit shared-memory load ----
 #pragma unroll
   for (int q = 0; q < 8; ++q) {
     const int i = lane + 32 * q;
@@ -527,11 +457,11 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
     if (y < XWM && x < XWM) mm2[y * XH_MP + x] = make_float2(wv[q], wv[q]);
   }
   __syncwarp();
-  // ---- refiner on packed fp32 FMAs (FFMA2: two IEEE fp32 FMAs per issue slot; this kernel is issue-bound).  Lane =
+  // ---- refiner on fp32 FMA pairs (f2fma: the lane's two channels share every operand load).  Lane =
   // (channel pair cp = channels (cp, cp + 8), row group pg).  Hidden layer: the lane's two channels on the rows pg, pg + 4,
   // ... of the 13 x 13 window, a 3 x 3 input window sliding along the row (weights in registers), stored [position][pair].
   // Output layer: the SAME lane layout -- the lane forms its two channels' contribution to the logits of box rows pg,
-  // pg + 4, pg + 8 (again sliding along the row: 3 new 64-bit shared-memory words per 9 packed FMAs); the pair is folded
+  // pg + 4, pg + 8 (again sliding along the row: 3 new 64-bit shared-memory words per 9 pair FMAs); the pair is folded
   // and the 8 pair lanes of a row group are summed by shuffles.
   {
     float2 w1r[9];
@@ -556,10 +486,10 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
 #pragma unroll
       for (int x = 0; x < XWH; ++x) {
         // three short chains per output (one per input row) instead of one chain of nine dependent FMAs
-        float2 a0 = __ffma2_rn(w1r[0], in0[x], b1r), a1 = __fmul2_rn(w1r[3], in1[x]), a2 = __fmul2_rn(w1r[6], in2[x]);
-        a0 = __ffma2_rn(w1r[1], in0[x + 1], a0); a1 = __ffma2_rn(w1r[4], in1[x + 1], a1); a2 = __ffma2_rn(w1r[7], in2[x + 1], a2);
-        a0 = __ffma2_rn(w1r[2], in0[x + 2], a0); a1 = __ffma2_rn(w1r[5], in1[x + 2], a1); a2 = __ffma2_rn(w1r[8], in2[x + 2], a2);
-        const float2 a = __fadd2_rn(__fadd2_rn(a0, a1), a2);
+        float2 a0 = f2fma(w1r[0], in0[x], b1r), a1 = f2mul(w1r[3], in1[x]), a2 = f2mul(w1r[6], in2[x]);
+        a0 = f2fma(w1r[1], in0[x + 1], a0); a1 = f2fma(w1r[4], in1[x + 1], a1); a2 = f2fma(w1r[7], in2[x + 1], a2);
+        a0 = f2fma(w1r[2], in0[x + 2], a0); a1 = f2fma(w1r[5], in1[x + 2], a1); a2 = f2fma(w1r[8], in2[x + 2], a2);
+        const float2 a = f2add(f2add(a0, a1), a2);
         const int c = acol - 6 + x;
         const bool in = INTERIOR || (row_in && c >= 0 && c < w);
         hh2[(y * XWH + x) * 8 + cp] = in ? make_float2(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f)) : make_float2(0.f, 0.f);
@@ -584,10 +514,10 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
 #pragma unroll
       for (int x = 0; x < XWB; ++x) {
         const float2 i02 = h0[(x + 2) * 8], i12 = h0[(XWH + x + 2) * 8], i22 = h0[(2 * XWH + x + 2) * 8];
-        float2 a0 = __fmul2_rn(w2r[0], i00), a1 = __fmul2_rn(w2r[3], i10), a2 = __fmul2_rn(w2r[6], i20);
-        a0 = __ffma2_rn(w2r[1], i01, a0); a1 = __ffma2_rn(w2r[4], i11, a1); a2 = __ffma2_rn(w2r[7], i21, a2);
-        a0 = __ffma2_rn(w2r[2], i02, a0); a1 = __ffma2_rn(w2r[5], i12, a1); a2 = __ffma2_rn(w2r[8], i22, a2);
-        const float2 a = __fadd2_rn(__fadd2_rn(a0, a1), a2);
+        float2 a0 = f2mul(w2r[0], i00), a1 = f2mul(w2r[3], i10), a2 = f2mul(w2r[6], i20);
+        a0 = f2fma(w2r[1], i01, a0); a1 = f2fma(w2r[4], i11, a1); a2 = f2fma(w2r[7], i21, a2);
+        a0 = f2fma(w2r[2], i02, a0); a1 = f2fma(w2r[5], i12, a1); a2 = f2fma(w2r[8], i22, a2);
+        const float2 a = f2add(f2add(a0, a1), a2);
         v[x] = a.x + a.y;
         i00 = i01; i01 = i02; i10 = i11; i11 = i12; i20 = i21; i21 = i22;
       }
@@ -814,9 +744,7 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
     for (int k = 0; k < 9; ++k) { p1 += hw.w1[o][k] > 0.f ? hw.w1[o][k] : 0.f; p2 += hw.w2[o][k] > 0.f ? hw.w2[o][k] : 0.f; }
     hp.P1[o] = p1 * (1.f + 1e-6f); hp.P2[o] = p2 * (1.f + 1e-6f);
   }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   int grid = cdiv(n_maps, XH_WARPS);
   if (grid > sms * 2) grid = sms * 2;
   static PerDev<bool> attr_dev;

@@ -6,9 +6,9 @@
 //   (ii) the map values on the 15 x 15 window around it (11 x 11 logits <- 13 x 13 hidden <- 15 x 15 inputs) and (iii) an
 //   upper bound on everything else (certificate that the stability branch, tracker_head.py:87-94, stays off).
 //
-//   1. coarse GEMM   one kind::f16 pass over the fp16 `hi` halves (1/3 of the split-precision work), epilogue keeps per
+//   1. coarse GEMM   one fp16 wgmma pass over the `hi` halves (1/3 of the split-precision work), epilogue keeps per
 //                    map and 256-token tile only (largest value, its first token, second largest value); |coarse - exact|
-//                    <= XW_EPS for every token (fp16 rounding of both operands + TMEM accumulation, see DESIGN.md).
+//                    <= XW_EPS for every token (fp16 rounding of both operands + fp32 accumulation, see DESIGN.md).
 //   2. plan          per map: the tokens that can be the exact arg-max (coarse >= max - 2 XW_EPS); a map whose candidates
 //                    are not all tile maxima is "ambiguous".  Maps come in CELLS = the <= 128 source frames of one (query,
 //                    anchor frame) pair: their arg-maxes cluster around the query's position in the anchor frame, so one
@@ -30,15 +30,15 @@ namespace dtk {
 constexpr float XW_EPS = 1.1e-3f;     // bound on |coarse - exact| in cosine units (2^-10 + accumulation, rounded up)
 constexpr int XW_BOX = 21;            // box side (tokens); windows of maps whose arg-max lies within +-3 of the centre fit
 constexpr int XW_SLACK = 3;
-constexpr int XW_PARTS = 4, XW_PART_ROWS = 6;                    // 4 M-parts of 6 box rows (126 tokens = 126 UMMA rows of 128)
+constexpr int XW_PARTS = 4, XW_PART_ROWS = 6;                    // 4 M-parts of 6 box rows (126 tokens = 126 wgmma rows of 128)
 constexpr int XW_PART_TOK = XW_PART_ROWS * XW_BOX;
 constexpr int XW_COLS = 448;                                     // accumulator row pitch per map (441 box tokens, row-major)
-constexpr int XW_MAX_CELL = 128;      // maps (source frames) per cell = UMMA N (64 or 128)
+constexpr int XW_MAX_CELL = 128;      // maps (source frames) per cell = wgmma N (64 or 128)
 constexpr int XW_MAX_CAND = 4;
 constexpr float XW_MIN_NORM = 1e-4f;  // the coarse pass forms acc / (|d| |F|) without the reference's max(|d| |F|, 1e-8) clamp: both
                                       // norms must be >= 1e-4 (smaller descriptor norms -> ambiguous map, smaller token norms
                                       // anywhere in the video -> the whole call takes the full-map pipeline)
-constexpr int XW_TILE = 128;          // tokens per coarse key (the coarse GEMM's 8 epilogue warps cover 128 columns each)
+constexpr int XW_TILE = 128;          // tokens per coarse key (= the coarse GEMM's N tile)
 
 // column of box token (by, bx) in a map's accumulator row
 __host__ __device__ inline int xw_col(int by, int bx) { return by * XW_BOX + bx; }

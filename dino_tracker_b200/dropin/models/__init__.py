@@ -1,6 +1,6 @@
 """Drop-in ``models`` package: put ``dino_tracker_b200/dropin`` in front of the reference root on
 ``PYTHONPATH`` and the reference's ``inference_grid.py`` / ``inference_benchmark.py`` /
-``dino_tracker.py`` pick up the B200 ``models.tracker`` and ``models.model_inference`` unchanged
+``dino_tracker.py`` pick up this project's ``models.tracker`` and ``models.model_inference`` unchanged
 (INTEGRATION.md).  Every other ``models.*`` module (``models.utils``, ``models.networks``,
 ``models.extractor``) falls through to the reference tree: its ``models`` directory is appended to this
 package's search path when it is importable."""

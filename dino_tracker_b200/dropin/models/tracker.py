@@ -1,2 +1,2 @@
-"""``models.tracker`` drop-in: the B200 Tracker under the reference's module path."""
+"""``models.tracker`` drop-in: the CUDA Tracker under the reference's module path."""
 from dino_tracker_b200.tracker import EPS, Tracker  # noqa: F401

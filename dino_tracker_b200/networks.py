@@ -115,7 +115,7 @@ class DeltaDINO(nn.Module):
                 layers.append(_BlurPoolParams(channels[i + 1]))
         self.layers = nn.ModuleList(layers)
         self._folded = (None, None)
-        # "fp16x3": convolutions as im2col + tcgen05 split-precision GEMMs (needs channel counts % 8 == 0);
+        # "fp16x3": convolutions as im2col + wgmma split-precision GEMMs (needs channel counts % 8 == 0);
         # "fp32": exact-fp32 implicit GEMM on the CUDA cores
         ok8 = all(c % 8 == 0 for c in channels[1:])
         self.conv_precision = conv_precision or ("fp16x3" if ok8 else "fp32")

@@ -30,7 +30,8 @@ def query_shard(N: int, world: int, rank: int):
 def video_cost(T: int, n_query_points: int, c_map: float = 2.5e-8, c_frame: float = 1.55e-2) -> float:
     """Seconds one video costs on one GPU: every query point is tracked into every frame (T maps) and, from each of its T
     track points, re-tracked into every anchor frame (<= T * T maps) -> N_q * T * (T + 1) correlation maps; the feature
-    stage (ViT + delta-DINO) is per frame.  Defaults: measured on B200 (exact-window pipeline; ViT-L/14@15)."""
+    stage (ViT + delta-DINO) is per frame.  Defaults: relative weights of the two terms for the exact-window pipeline with ViT-L/14@15
+    features; only their ratio matters to the assignment."""
     return n_query_points * T * (T + 1) * c_map + T * c_frame
 
 

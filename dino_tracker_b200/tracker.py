@@ -52,7 +52,7 @@ class Tracker(nn.Module):
         t, c, h, w = video.shape
         self._geom = _lib.make_geom(h, w, dino_patch_size, stride, 35)
         assert corr_precision in ("fp16x3", "fp32")
-        # "fp16x3": wide correlation groups on tcgen05 tensor cores (fp16 hi/lo split, 3 passes, fp32-faithful);
+        # "fp16x3": wide correlation groups on wgmma tensor cores (fp16 hi/lo split, 3 passes, fp32-faithful);
         # "fp32"  : exact-fp32 FFMA GEMM on the CUDA cores (validation path)
         self.corr_precision = corr_precision
         self._refined_tpc = None

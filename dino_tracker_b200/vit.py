@@ -65,7 +65,7 @@ class DinoV2Features(torch.nn.Module):
         self.attention = attention
         self.cta_pairs = cta_pairs
         self._sd = sd
-        # fused mode: weight matrices in fp16 (kind::f16 MMAs); materialized (validation) mode: fp32 / TF32
+        # fused mode: weight matrices in fp16 (fp16 MMAs); materialized (validation) mode: fp32 / TF32
         self._f16 = attention == "fused"
         wdt = torch.float16 if self._f16 else torch.float32
         mats = ("attn.qkv.weight", "attn.proj.weight", "mlp.fc1.weight", "mlp.fc2.weight")

@@ -1,5 +1,5 @@
 /*
- * dinotrk.h -- C ABI of libdinotrk.so, the B200 (sm_100a) implementation of the
+ * dinotrk.h -- C ABI of libdinotrk.so, the H100 (sm_90a) implementation of the
  * DINO-Tracker inference hot path.
  *
  * The reference (AssafSinger94/dino-tracker) has no FFI layer: its boundary is the Python
@@ -53,7 +53,7 @@ typedef struct dinotrk_head_weights {
 
 /* A cached feature video.  tpc [T][P][C] and norms [T][P] are required.  hi / lo (optional, both or
  * neither): the fp16 split of tpc ([T][P][C] halves each, x = hi + lo) produced by dinotrk_split_fp16; when
- * present the wide correlation groups run on the tcgen05 tensor cores (3-pass split precision,
+ * present the wide correlation groups run on the wgmma tensor cores (3-pass split precision,
  * fp32-faithful), otherwise on the exact-fp32 FFMA GEMM.  C must then be a multiple of 8. */
 typedef struct dinotrk_features {
   const float* tpc;
@@ -219,7 +219,7 @@ int dinotrk_delta_refine_allgather(const float* frames, int B, int H, int W, con
                                    const float* ixs, const float* iys, int h, int w, float* refined_tpc,
                                    float* norms, void* workspace, size_t workspace_bytes,
                                    float* const* peer_bases, int n_peers, size_t first_frame, void* stream);
-/* Tensor-core variant: the four convolutions run as explicit-im2col (fp16 hi/lo split on the fly) + tcgen05
+/* Tensor-core variant: the four convolutions run as explicit-im2col (fp16 hi/lo split on the fly) + wgmma
  * split-precision GEMMs (fp32-faithful).  wgt_hi[l] / wgt_lo[l]: fp16 split (dinotrk_split_fp16) of the folded K-major
  * weights [C_out][Kp], Kp = 25 * C_in_pad rounded up to 8; channel counts multiples of 8.  peer_bases / n_peers /
  * first_frame as in dinotrk_delta_refine_allgather (n_peers = 0: single GPU). */
@@ -239,13 +239,13 @@ typedef struct dinotrk_vit_config {
   int depth, dim, heads;   /* ViT-L/14: 24, 1024, 16; ViT-B/14: 12, 768, 12 (head dim 64) */
   int tap_layer;           /* 0-based block whose output (before the final norm) is returned; 15 in the shipped config */
   int patch, stride;       /* 14, 7 */
-  int attn_materialized;   /* 0: fused tcgen05 attention (fp16 q/k/v/p, scores stay on the SM); 1: TF32 scores through a
+  int attn_materialized;   /* 0: fused wgmma attention (fp16 q/k/v/p, scores stay on the SM); 1: TF32 scores through a
                               workspace (tensor-core GEMM -> softmax -> tensor-core GEMM), validation path */
-  int gemm_f16;            /* 1: linear layers on the kind::f16 pipe -- patch_w and the qkv / proj / fc1 / fc2 weight matrices
+  int gemm_f16;            /* 1: linear layers on the fp16 tensor pipe -- patch_w and the qkv / proj / fc1 / fc2 weight matrices
                               are passed as fp16 arrays, activations are written in fp16 by the producing epilogue;
                               0 (or attn_materialized): fp32 arrays, TF32 MMAs */
-  int gemm_pair;           /* with gemm_f16: 1 = linear layers on CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles, each SM
-                              stages half of the weight tile), 0 = single-CTA 128 x 256 tiles */
+  int gemm_pair;           /* with gemm_f16: 1 = linear layers on CTA pairs (two-CTA clusters, 256 x 256 tiles, each CTA
+                              loads half of the weight tile and multicasts it to both), 0 = single-CTA 128 x 256 tiles */
 } dinotrk_vit_config;
 /* Device fp32 (weight matrices fp16 when gemm_f16).  patch_w: patch-embedding conv weight flattened K-major
  * [dim][Kp], Kp = 3*patch*patch zero-padded to a multiple of 4 (fp32) / 8 (fp16) elements; cls_pos [dim] =
@@ -261,7 +261,7 @@ size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_ge
 int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const dinotrk_vit_config* c,
                         const dinotrk_vit_weights* wt, float* out_tpc, void* workspace,
                         size_t workspace_bytes, void* stream);
-/* The attention of one ViT block on its own (the fused tcgen05 kernel of dinotrk_vit_forward; head dim 64):
+/* The attention of one ViT block on its own (the fused wgmma kernel of dinotrk_vit_forward; head dim 64):
  * q16 [B*heads][N1][64] fp16 ALREADY multiplied by 64^-1/2 * log2(e), k16 [B*heads][N1][64] fp16,
  * vT16 [B*heads][64][N1p] fp16 (v transposed, row pitch N1p >= N1, a multiple of 8);
  * out [B*N1][heads*64] fp32 = softmax(q k^T) v with head h in columns [64 h, 64 h + 64)
@@ -272,8 +272,8 @@ int dinotrk_vit_attention(const void* q16, const void* k16, const void* vT16, in
 /* ---- best buddies (preprocessing_dino_bb/extract_dino_best_buddies.py:12-54) ------------------------ */
 /* For every ordered pair k (source frame pair_src[k], target frame pair_tgt[k]; device int32[n_pairs]):
  * nn_idx[k][n] = argmax_m cos(F_src[n], F_tgt[m]) (first maximum), nn_cos[k][n] = that cosine (exact fp32,
- * clamp 1e-8 on the norm product).  The affinity matrix runs through the tcgen05 split-fp16 GEMM and never
- * leaves TMEM; candidates are re-evaluated in exact fp32.  feat->hi / lo are required. */
+ * clamp 1e-8 on the norm product).  The affinity matrix runs through the wgmma split-fp16 GEMM and never
+ * leaves the SM; candidates are re-evaluated in exact fp32.  feat->hi / lo are required. */
 size_t dinotrk_best_buddies_workspace_bytes(int n_pairs, int P);
 int dinotrk_best_buddies_pairs(const dinotrk_features* feat, const dinotrk_geom* g, const int* pair_src,
                                const int* pair_tgt, int n_pairs, int* nn_idx, float* nn_cos,

@@ -1,4 +1,4 @@
-"""GPU parity: best-buddies (tcgen05 GEMM + top-2 epilogue + exact resolve) against the reference vectors
+"""GPU parity: best-buddies (wgmma GEMM + top-2 epilogue + exact resolve) against the reference vectors
 and the oracle."""
 import os
 

@@ -69,7 +69,7 @@ def test_state_dict_keys_match_reference_checkpoint_format():
 
 @gpu
 def test_tensor_core_convs_match_exact_path_and_oracle():
-    """delta-DINO with the convolutions on tcgen05 (im2col + split-fp16 GEMM) vs the exact-fp32 CUDA-core path and
+    """delta-DINO with the convolutions on wgmma (im2col + split-fp16 GEMM) vs the exact-fp32 CUDA-core path and
     the oracle, at a shape with ragged tiles (channels 16/24/40/72)."""
     from dino_tracker_b200 import Tracker
     channels = [3, 16, 24, 40, 72]

@@ -1,15 +1,12 @@
 """CPU: the surface the reference's own entry points touch (inference_grid.py, inference_benchmark.py,
 dino_tracker.py::get_model / train_setup, models/model_inference.py) exists on the drop-in classes.  The surface is
 extracted from the reference sources by tools/dropin_surface.py (AST walk) and committed as
-tests/golden/dropin_surface.json; when the reference tree is present the extraction is repeated and must match."""
-import importlib.util
+tests/golden/dropin_surface.json."""
 import inspect
 import json
 import os
 import re
 import sys
-
-import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SURFACE = json.load(open(os.path.join(ROOT, "tests", "golden", "dropin_surface.json")))
@@ -22,16 +19,6 @@ def _instance_attributes(cls):
     for c in cls.__mro__:
         names |= set(vars(c).keys())
     return names
-
-
-def test_surface_fixture_matches_the_reference_tree():
-    ref = os.environ.get("DINOTRK_REFERENCE_ROOT", "/root/reference")
-    if not os.path.isfile(os.path.join(ref, "inference_grid.py")):
-        pytest.skip("reference tree not present")
-    spec = importlib.util.spec_from_file_location("dropin_surface", os.path.join(ROOT, "tools", "dropin_surface.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    assert mod.surface(ref) == SURFACE
 
 
 def test_tracker_offers_everything_the_reference_touches():

@@ -20,7 +20,7 @@ XY_TOL = 1e-3
 DEV = "cuda:0"
 
 
-PRECISIONS = ["fp16x3", "fp32"]  # tcgen05 3xTF32 tensor-core GEMM / exact-fp32 FFMA GEMM
+PRECISIONS = ["fp16x3", "fp32"]  # split-fp16 wgmma tensor-core GEMM / exact-fp32 FFMA GEMM
 
 
 def make_model(geo, feats, head, precision="fp16x3"):
@@ -126,8 +126,8 @@ def test_corr_gemm_error_vs_float64(precision):
     ref = torch.relu((desc.double() @ f) / (desc.double().norm(dim=1)[:, None] * f.norm(dim=0)[None]).clamp_min(1e-8))
     err = (maps - ref).abs().max().item()
     print(f"[{precision}] max |corr - float64| = {err:.3e}")
-    # measured on B200: fp32 FFMA 1.1e-6 (sequential fp32 accumulation over K=1024), tcgen05 3xTF32 1.8e-5
-    # (TMEM accumulation truncates; the bias is coherent across tokens, see DESIGN.md "Precision")
+    # fp32 FFMA: sequential fp32 accumulation over K=1024; split fp16: three tensor-core passes whose accumulation
+    # truncates (the bias is coherent across tokens, see DESIGN.md "Precision")
     assert err <= (3e-6 if precision == "fp32" else 4e-5)
 
 

@@ -1,4 +1,4 @@
-"""GPU tests: tcgen05 ViT (fp16-operand GEMMs on CTA pairs or single CTAs + fused attention; TF32 GEMMs + materialised
+"""GPU tests: wgmma ViT (fp16-operand GEMMs on CTA pairs or single CTAs + fused attention; TF32 GEMMs + materialised
 attention as the validation path) against the fp32 oracle restatement (itself pinned to the live reference pipeline and to
 transformers' DINOv2 block, see oracle/vit.py), and the attention kernel on its own against float64."""
 import numpy as np
@@ -64,9 +64,9 @@ def _attention_reference(q, k, v):
 
 @pytest.mark.parametrize("case", ["random-small", "random-large", "ramp", "late-spike", "tail-1", "tail-63"])
 def test_fused_attention_against_float64(case):
-    """The attention kernel on its own (dinotrk_vit_attention): accumulator kept in TMEM across key tiles with a LAZY
-    running maximum -- 'ramp' and 'late-spike' make the row maxima jump by far more than 2^8 between key tiles, so the
-    tcgen05.ld / multiply / tcgen05.st rescale of the accumulator (row sums included) runs many times; the tail cases
+    """The attention kernel on its own (dinotrk_vit_attention): accumulator kept in registers across key tiles with an
+    online running maximum -- 'ramp' and 'late-spike' make the row maxima jump by far more than 2^8 between key tiles, so
+    the rescale of the accumulator (row sums included) matters on many tiles; the tail cases
     end the keys 1 / 63 columns into the last 64-key tile."""
     from dino_tracker_b200 import _lib
     lib = _lib.load()

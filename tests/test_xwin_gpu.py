@@ -145,7 +145,7 @@ def test_uncertifiable_head_switches_pipeline():
 
 
 def test_long_video_cells_split_into_blocks():
-    """T > 128: the source frames of a (query, anchor frame) pair are split into cells of <= 128 rows (UMMA M = 128)."""
+    """T > 128: the source frames of a (query, anchor frame) pair are split into cells of <= 128 rows (wgmma N <= 128)."""
     geo = Geometry(H=98, W=126)
     T, C = 150, 32
     feats, _ = synth.shifted_field_features(T, C, geo.h, geo.w, seed=5, noise=0.15, max_shift=2)

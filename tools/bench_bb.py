@@ -54,7 +54,7 @@ def main():
         print(json.dumps({"config": f"best-buddies T={a.T} C={a.C} 854x476", "n_gpus": world, "ordered_pairs": n_ordered,
                           "seconds": s, "ordered_pairs_per_s": n_ordered / s,
                           "algorithmic_tflops": 2.0 * bench.P ** 2 * a.C * n_ordered / s / 1e12,
-                          "note": "each ordered pair = one 8107x8107xC affinity GEMM (tcgen05 split-fp16) + top-2 epilogue + exact resolve"}))
+                          "note": "each ordered pair = one 8107x8107xC affinity GEMM (wgmma split-fp16) + top-2 epilogue + exact resolve"}))
     if world > 1:
         dist.destroy_process_group()
 

@@ -1,4 +1,4 @@
-"""Bench-scale A/B of the two correlation-GEMM precisions (tcgen05 split-fp16, three passes, vs exact-fp32 FFMA):
+"""Bench-scale A/B of the two correlation-GEMM precisions (wgmma split-fp16, three passes, vs exact-fp32 FFMA):
 max trajectory difference, occlusion mismatches, anchor-track differences, timing.  GPU only."""
 import argparse
 import sys
