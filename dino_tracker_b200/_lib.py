@@ -2,6 +2,7 @@
 missing or fails to load, importing the product path raises."""
 import ctypes
 import os
+import warnings
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_size_t, c_ulonglong, c_void_p
 
 import torch
@@ -50,6 +51,8 @@ SIGNATURES = {
     "dinotrk_token_norms": (c_int, [_P, _P, c_int, c_int, c_int, _P]),
     "dinotrk_sample_descriptors": (c_int, [_P, c_int, c_int, POINTER(Geom), _P, c_int, _P, c_int, c_int, _P, _P, _P]),
     "dinotrk_split_fp16": (c_int, [_P, _P, _P, c_size_t, _P]),
+    "dinotrk_split_range": (c_int, [_P, c_size_t, _P, c_size_t, _P, _P]),
+    "dinotrk_split_faithful": (c_int, [c_float, c_float, c_int]),
     "dinotrk_corr_track_workspace_bytes": (c_size_t, [c_int, c_int, c_int, POINTER(Geom)]),
     "dinotrk_corr_track": (c_int, [POINTER(Features), POINTER(Geom), POINTER(HeadWeights), _P, _P, _P, _P, _P, _P,
                                    c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_size_t, _P]),
@@ -172,6 +175,35 @@ def make_features(tpc, norms, hi=None, lo=None):
     return f
 
 
+def split_range(tpc, norms, stream):
+    """(max |x|, smallest non-zero token norm, in the fp16 split's faithful range?) of a [T][P][C] feature video
+    (include/dinotrk.h: dinotrk_split_range).  Reads two floats back: syncs the stream."""
+    lib = load()
+    rng = torch.empty(2, device=tpc.device, dtype=torch.float32)
+    check(lib.dinotrk_split_range(ptr(tpc), tpc.numel(), ptr(norms), norms.numel(), ptr(rng), stream), "split_range")
+    max_abs, min_norm = rng.tolist()
+    return max_abs, min_norm, bool(lib.dinotrk_split_faithful(max_abs, min_norm, tpc.shape[-1]))
+
+
+def split_fp16(x, stream):
+    hi = torch.empty(x.shape, device=x.device, dtype=torch.float16)
+    lo = torch.empty(x.shape, device=x.device, dtype=torch.float16)
+    check(load().dinotrk_split_fp16(ptr(x), ptr(hi), ptr(lo), x.numel(), stream), "split_fp16")
+    return hi, lo
+
+
+def split_features(tpc, norms, stream):
+    """fp16 hi / lo halves of a feature video for the tensor-core contractions, or (None, None) -- the exact-fp32 path,
+    with a RuntimeWarning -- when the video lies outside the split's faithful range."""
+    max_abs, min_norm, ok = split_range(tpc, norms, stream)
+    if not ok:
+        warnings.warn(f"feature video outside the fp16 split's faithful range (max |x| = {max_abs:.3g}, smallest token "
+                      f"norm = {min_norm:.3g}, C = {tpc.shape[-1]}): its contractions run on the exact-fp32 path",
+                      RuntimeWarning, stacklevel=3)
+        return None, None
+    return split_fp16(tpc, stream)
+
+
 def make_geom(H, W, patch=14, stride=7, radius=35):
     g = Geom()
     check(load().dinotrk_make_geom(H, W, patch, stride, radius, ctypes.byref(g)), "make_geom")
@@ -193,11 +225,12 @@ def profile_collect():
 
 
 def infer_stats():
-    """{anchor-phase maps, finished by the exact-window path, re-done by the full-map path, pipeline} of the last infer."""
-    a = (ctypes.c_longlong * 5)()
-    check(load().dinotrk_infer_last_stats(a, 5), "infer_last_stats")
+    """{anchor-phase maps, finished by the exact-window path, re-done by the full-map path, pipeline, contraction} of the
+    last infer."""
+    a = (ctypes.c_longlong * 6)()
+    check(load().dinotrk_infer_last_stats(a, 6), "infer_last_stats")
     return {"anchor_maps": int(a[0]), "exact_window": int(a[1]), "full_map": int(a[2]), "pipeline": "exact-window" if a[3] else "full-map",
-            "full_map_by_certificate": int(a[4])}
+            "full_map_by_certificate": int(a[4]), "contraction": "fp16x3" if a[5] else "fp32"}
 
 
 def launch_count():

@@ -9,7 +9,9 @@ works on index vectors (``dinotrk_best_buddies_pairs`` / ``dinotrk_bb_mutual``).
 Pairs shard trivially over ranks (``rank`` / ``world`` arguments): SURVEY.md 8e config 5.
 """
 import ctypes
+import math
 import os
+import warnings
 
 import torch
 
@@ -37,9 +39,20 @@ def _nearest_neighbours(tpc, norms, geom, pairs, hi, lo, pairs_per_launch):
     dev = tpc.device
     T, P, C = tpc.shape
     if hi is None:
-        hi = torch.empty(tpc.shape, device=dev, dtype=torch.float16)
-        lo = torch.empty(tpc.shape, device=dev, dtype=torch.float16)
-        _lib.check(lib.dinotrk_split_fp16(_lib.ptr(tpc), _lib.ptr(hi), _lib.ptr(lo), tpc.numel(), _lib.stream_ptr()))
+        max_abs, min_norm, ok = _lib.split_range(tpc, norms, _lib.stream_ptr())
+        if not ok and 0.0 < max_abs < math.inf:
+            # Outside the split's faithful range the GEMM's ranking error can exceed the resolve margin.  Best buddies are
+            # cosines only, so run on a copy scaled by 2^e (max |x| in (2^13, 2^14]): an exact scaling of every product,
+            # sum and norm, so the exact-fp32 cosines of the copy are bit-identical to the video's own (wherever the video's
+            # own products do not underflow and |d| |F| stays above the 1e-8 clamp).
+            s = 2.0 ** (14 - math.ceil(math.log2(max_abs)))
+            tpc, norms = tpc * s, norms * s
+            max_abs, min_norm, ok = _lib.split_range(tpc, norms, _lib.stream_ptr())
+        if not ok:   # a spread of token norms wider than the range (or non-finite features): no scale brings it inside
+            warnings.warn(f"best buddies: feature video outside the fp16 split's faithful range even after rescaling (max |x| = "
+                          f"{max_abs:.3g}, smallest token norm = {min_norm:.3g}, C = {C}): the affinity GEMM's ranking is not "
+                          f"bounded by the exact-fp32 resolve margin", RuntimeWarning, stacklevel=3)
+        hi, lo = _lib.split_fp16(tpc, _lib.stream_ptr())
     feat = _lib.make_features(tpc, norms, hi, lo)
     n = len(pairs)
     nn_idx = torch.empty(n, P, device=dev, dtype=torch.int32)
@@ -115,9 +128,7 @@ class PackedFeatures:
             _lib.check(lib.dinotrk_pack_features(_lib.ptr(chw), _lib.ptr(self.tpc), _lib.ptr(self.norms), T, C, h * w, _lib.stream_ptr()))
             self.hi = self.lo = None
             if C % 8 == 0:
-                self.hi = torch.empty(self.tpc.shape, device=self.dev, dtype=torch.float16)
-                self.lo = torch.empty(self.tpc.shape, device=self.dev, dtype=torch.float16)
-                _lib.check(lib.dinotrk_split_fp16(_lib.ptr(self.tpc), _lib.ptr(self.hi), _lib.ptr(self.lo), self.tpc.numel(), _lib.stream_ptr()))
+                self.hi, self.lo = _lib.split_features(self.tpc, self.norms, _lib.stream_ptr())
         self.feat = _lib.make_features(self.tpc, self.norms, self.hi, self.lo)
 
 

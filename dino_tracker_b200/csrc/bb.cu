@@ -68,30 +68,27 @@ __global__ void bb_resolve_kernel(const float* __restrict__ tpc, const float* __
   const size_t wid = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (wid >= (size_t)n_pairs * P) return;
   const int g = (int)(wid / P), r = (int)(wid - (size_t)g * P);
-  unsigned long long k1 = 0ull; float v2 = -INFINITY; int i2 = -1;
+  // top-2 as (value, first index) keys: every lane ends with the same two candidates even when values tie (the exact
+  // re-evaluation below sums the lanes' partial dot products, so all lanes must evaluate the same token)
+  unsigned long long k1 = 0ull, k2 = 0ull;
+  auto push = [&](unsigned long long k) {
+    if (k > k1) { k2 = k1; k1 = k; } else if (k > k2) { k2 = k; }
+  };
   for (int t = lane; t < n_tiles; t += 32) {
     BBPartial p = part[((size_t)g * n_tiles + t) * P + r];
-    if (p.key1 > k1) {
-      if (k1 != 0ull) { float o = ord2f((unsigned)(k1 >> 32)); if (o > v2) { v2 = o; i2 = 0x7fffffff - (int)(k1 & 0xffffffffu); } }
-      k1 = p.key1;
-    } else if (p.key1 != 0ull) {
-      float o = ord2f((unsigned)(p.key1 >> 32));
-      if (o > v2) { v2 = o; i2 = 0x7fffffff - (int)(p.key1 & 0xffffffffu); }
-    }
-    if (p.v2 > v2) { v2 = p.v2; i2 = p.i2; }
+    push(p.key1);
+    if (p.i2 >= 0) push(((unsigned long long)f2ord(p.v2) << 32) | (unsigned)(0x7fffffff - p.i2));
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    unsigned long long ok1 = __shfl_xor_sync(0xffffffffu, k1, o);
-    float ov2 = __shfl_xor_sync(0xffffffffu, v2, o);
-    int oi2 = __shfl_xor_sync(0xffffffffu, i2, o);
-    unsigned long long lo = ok1 < k1 ? ok1 : k1, hi = ok1 < k1 ? k1 : ok1;
-    if (lo != 0ull) { float lv = ord2f((unsigned)(lo >> 32)); if (lv > v2) { v2 = lv; i2 = 0x7fffffff - (int)(lo & 0xffffffffu); } }
-    if (ov2 > v2) { v2 = ov2; i2 = oi2; }
-    k1 = hi;
+  for (int o = 16; o > 0; o >>= 1) {   // the two lanes of a step hold disjoint token sets: no key arrives twice
+    const unsigned long long ok1 = __shfl_xor_sync(0xffffffffu, k1, o), ok2 = __shfl_xor_sync(0xffffffffu, k2, o);
+    push(ok1);
+    push(ok2);
   }
   int i1 = 0x7fffffff - (int)(k1 & 0xffffffffu);
   const float v1 = ord2f((unsigned)(k1 >> 32));
+  const int i2 = k2 ? 0x7fffffff - (int)(k2 & 0xffffffffu) : -1;
+  const float v2 = k2 ? ord2f((unsigned)(k2 >> 32)) : -INFINITY;
   const int fs = grp_src[g], ft = grp_tgt[g];
   const float4* a = reinterpret_cast<const float4*>(tpc + ((size_t)fs * P + r) * C);
   auto exact = [&](int col) {

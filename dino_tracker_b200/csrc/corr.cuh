@@ -50,6 +50,15 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
                         unsigned long long* tkeys = nullptr, bool split_ready = false, int tile_rows = 0 /* 0: default */);
 int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t st);
 
+// Faithful range of the fp16 hi/lo split (DESIGN.md 3.1).  Per element, x - hi - lo is at most 2^-22 |x| while lo is an fp16
+// normal and at most 2^-25 (half the smallest subnormal step) otherwise, so the split contraction's cosine error is
+//   <= 2^-21 + 2^-25 sqrt(C) (1 / |d| + 1 / |F|).
+// Norms >= 2^-3 sqrt(C) keep the absolute part <= 2^-22 per operand.  Elements above the largest fp16 (65504) make hi = inf.
+// A video is in range when every |x| <= SPLIT_MAX_ABS and every token norm is 0 (an exact zero splits exactly) or
+// >= split_min_norm(C).
+constexpr float SPLIT_MAX_ABS = 65504.f;
+__host__ __device__ inline float split_min_norm(int C) { return 0.125f * sqrtf((float)C); }
+
 int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geom& g,
                 const dinotrk_head_weights& hw, const int* out_index, float* out, int out_stride, int out_mode,
                 int* aux, int* scratch /* n_maps + 1 ints, or NULL: full-map kernel for every map */, cudaStream_t st,

@@ -117,6 +117,28 @@ int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t 
   return DINOTRK_OK;
 }
 
+// range[0] = max |x| (NaN counts as above every bound), range[1] = smallest non-zero norm; both as float bits, which order like
+// the values for non-negative floats.  range[1] stays 0x7f7f7f7f (3.4e38) when every norm is zero.
+__global__ void split_range_kernel(const float* __restrict__ x, size_t n, const float* __restrict__ norms, size_t n_tok,
+                                   unsigned* __restrict__ range) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  unsigned mx = 0u, mn = 0x7f7f7f7fu;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const unsigned b = __float_as_uint(x[i]) & 0x7fffffffu;
+    mx = b > mx ? b : mx;
+  }
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_tok; i += stride) {
+    const float v = norms[i];
+    if (v > 0.f && __float_as_uint(v) < mn) mn = __float_as_uint(v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+  }
+  if ((threadIdx.x & 31) == 0) { atomicMax(range, mx); atomicMin(range + 1, mn); }
+}
+
 struct CorrEpi {
   const float* norms;      // [T][P]
   const float* desc_norm;  // [rows]
@@ -233,4 +255,24 @@ using namespace dtk;
 extern "C" int dinotrk_split_fp16(const float* x, void* hi, void* lo, size_t n, void* stream) {
   DTK_CHECK_ARG(x && hi && lo, "split_fp16: null pointer");
   return launch_split_f16(x, hi, lo, n, (cudaStream_t)stream);
+}
+
+extern "C" int dinotrk_split_range(const float* x, size_t n, const float* norms, size_t n_tok, float* range, void* stream) {
+  DTK_CHECK_ARG(x && norms && range, "split_range: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned* r = reinterpret_cast<unsigned*>(range);
+  DTK_CUDA(cudaMemsetAsync(r, 0, sizeof(unsigned), st));
+  DTK_CUDA(cudaMemsetAsync(r + 1, 0x7f, sizeof(unsigned), st));
+  size_t m = n > n_tok ? n : n_tok;
+  unsigned grid = (unsigned)((m + 255) / 256);
+  if (grid > (unsigned)num_sms() * 8) grid = num_sms() * 8;
+  if (grid == 0) return DINOTRK_OK;
+  ProfRange pr(PROF_MISC, st);
+  split_range_kernel<<<grid, 256, 0, st>>>(x, n, norms, n_tok, r);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
+extern "C" int dinotrk_split_faithful(float max_abs, float min_norm, int C) {
+  return (max_abs <= SPLIT_MAX_ABS && min_norm >= split_min_norm(C)) ? 1 : 0;
 }

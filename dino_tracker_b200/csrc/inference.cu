@@ -441,7 +441,7 @@ static XwAsync* xw_async() {
   return xa.state == 1 ? &xa : nullptr;
 }
 static int g_xw_path = -1;                     // -1: automatic (DTK_XW or on), 0: full-map path only, 1: exact-window path
-static long long g_infer_stats[5] = {0, 0, 0, 0, 0};   // anchor-phase maps | on the exact-window path | queued | path used | queued by the certificate
+static long long g_infer_stats[6] = {0, 0, 0, 0, 0, 0};   // anchor-phase maps | on the exact-window path | queued | path used | queued by the certificate | tensor-core contraction
 
 }  // namespace dtk
 
@@ -457,7 +457,7 @@ int dinotrk_infer_set_path(int path) {
 
 int dinotrk_infer_last_stats(long long* out, int n) {
   DTK_CHECK_ARG(out && n >= 4, "infer_last_stats: need at least 4 slots");
-  for (int i = 0; i < (n < 5 ? n : 5); ++i) out[i] = g_infer_stats[i];
+  for (int i = 0; i < (n < 6 ? n : 6); ++i) out[i] = g_infer_stats[i];
   return DINOTRK_OK;
 }
 
@@ -792,10 +792,10 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING, d_cntA, (size_t)n_chunks_A * sizeof(int), cudaMemcpyDeviceToHost, st));
     DTK_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
     DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: sizes of the anchor work lists
-    if (use_xw) {   // a (near-)zero token anywhere voids the coarse pass's error bound (xwin.cuh: XW_MIN_NORM)
+    if (use_xw) {   // a token below the split's faithful range (a zero one included) voids the coarse pass's error bound
       float mn;
       memcpy(&mn, xa->host_cnt + 2 * XW_RING + 16, sizeof(float));
-      if (!(mn >= XW_MIN_NORM)) use_xw = false;
+      if (!(mn >= split_min_norm(C))) use_xw = false;
     }
     if (use_xw && pathsel < 0 && n_chunks_A > 0) {
       // head weights the certificate cannot handle send (almost) every map to the full-map kernels anyway: the trajectory
@@ -807,6 +807,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     long long maps_C = 0;
     for (int a = 0; a < T; ++a) maps_C += (long long)cnt[a] * T;
     g_infer_stats[0] = maps_C; g_infer_stats[1] = 0; g_infer_stats[2] = 0; g_infer_stats[3] = use_xw ? 1 : 0; g_infer_stats[4] = 0;
+    g_infer_stats[5] = tensor ? 1 : 0;
     size_t k0 = 0;            // first chunk of the full-map pipeline (> 0 after an exact-window probe)
     bool planned = false;
     if (use_xw) {
@@ -916,7 +917,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, xa->sample[k % XW_RING], 0));
         if ((rc = launch_xw_coarse(fv, hi_of(x, cm.used), cm.used, x.norm, gp.f, gp.r, gp.m, gp.map0, d_tiles + k * (gcap + 1),
                                    cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, d_rnorms))) return rc;
-        if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used))) return rc;
+        if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used, split_min_norm(C)))) return rc;
         if ((rc = launch_xw_gemm(fv, *g, hi_of(x, cm.used), lo_of(x, cm.used), cm.used, cells, x.xc, st))) return rc;
         if ((rc = launch_xw_head(fv, *g, *hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups)))
           return rc;

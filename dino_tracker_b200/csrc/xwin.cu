@@ -126,7 +126,8 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
 //     fits if every candidate lies within +-XW_SLACK of it.
 constexpr int PLAN_WARPS = 8;
 __global__ void __launch_bounds__(PLAN_WARPS * 32)
-xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, int n_groups, int n_tiles, const unsigned long long* __restrict__ key1,
+xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, int n_groups, int n_tiles,
+               const unsigned long long* __restrict__ key1,
                const float* __restrict__ max2, int* __restrict__ cand, int* __restrict__ pinfo, int* __restrict__ slow_cnt) {
   const int lane = threadIdx.x & 31;
   const int gw = blockIdx.x * PLAN_WARPS + (threadIdx.x >> 5), nw = gridDim.x * PLAN_WARPS;
@@ -161,8 +162,8 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, int n_groups, in
       if (isc && rank < XW_MAX_CAND) cand[(size_t)map * XW_MAX_CAND + rank] = 0x7fffffff - (int)(kk[q] & 0xffffffffu);
       ncand += __popc(cm);
     }
-    // a (near-)zero map has no meaningful arg-max candidates; a tiny descriptor norm voids the error bound
-    amb = amb || ncand > XW_MAX_CAND || !(gmax > 4.f * XW_EPS) || !(desc_norm[map] >= XW_MIN_NORM);
+    // a (near-)zero map has no meaningful arg-max candidates; a descriptor below the split's faithful range voids the bound
+    amb = amb || ncand > XW_MAX_CAND || !(gmax > 4.f * XW_EPS) || !(desc_norm[map] >= min_norm);
     if (lane >= ncand && lane < XW_MAX_CAND) cand[(size_t)map * XW_MAX_CAND + lane] = -1;
     if (lane == 0) pinfo[map] = amb ? -1 - ptok : ptok;
   }
@@ -237,7 +238,7 @@ xw_cell_kernel(XwCells cells, int w, const int* __restrict__ cand, const int* __
 }
 
 int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, const dinotrk_geom& g, const XwChunk& xc,
-                   cudaStream_t st, int n_maps) {
+                   cudaStream_t st, int n_maps, float min_norm) {
   static_assert(XW_MAX_CAND == 4, "candidates are read as one int4");
   const int n_tiles = cdiv(g.h * g.w, XW_TILE);
   DTK_CHECK_ARG(n_tiles <= 64, "exact-window path: token grid too large (%d tiles)", n_tiles);
@@ -246,7 +247,7 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
   ProfRange pr(PROF_XW_PLAN, st);
   int grid = cdiv(n_maps, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;
-  xw_cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, n_groups, n_tiles, xc.key1, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
+  xw_cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, min_norm, n_groups, n_tiles, xc.key1, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
   DTK_LAUNCHED();
   grid = cdiv(cells.n_cells, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;

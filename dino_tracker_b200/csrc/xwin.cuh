@@ -35,9 +35,9 @@ constexpr int XW_PART_TOK = XW_PART_ROWS * XW_BOX;
 constexpr int XW_COLS = 448;                                     // accumulator row pitch per map (441 box tokens, row-major)
 constexpr int XW_MAX_CELL = 128;      // maps (source frames) per cell = wgmma N (64 or 128)
 constexpr int XW_MAX_CAND = 4;
-constexpr float XW_MIN_NORM = 1e-4f;  // the coarse pass forms acc / (|d| |F|) without the reference's max(|d| |F|, 1e-8) clamp: both
-                                      // norms must be >= 1e-4 (smaller descriptor norms -> ambiguous map, smaller token norms
-                                      // anywhere in the video -> the whole call takes the full-map pipeline)
+constexpr float XW_MIN_NORM = 1e-4f;  // guard of the coarse epilogue's reciprocal norms only.  XW_EPS holds when both norms are
+                                      // >= split_min_norm(C) (corr.cuh): a smaller descriptor norm makes the map ambiguous, a
+                                      // smaller token norm anywhere in the video sends the whole call to the full-map pipeline
 constexpr int XW_TILE = 128;          // tokens per coarse key (= the coarse GEMM's N tile)
 
 // column of box token (by, bx) in a map's accumulator row
@@ -74,7 +74,7 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
 // rnorms = 1 / |F| for the coarse epilogue; *min_bits = bit pattern of the smallest token norm of the video
 int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cudaStream_t st);
 int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, const dinotrk_geom& g, const XwChunk& xc,
-                   cudaStream_t st, int n_maps);
+                   cudaStream_t st, int n_maps, float min_norm);
 int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_hi, const void* desc_lo, int desc_rows,
                    const XwCells& cells, const XwChunk& xc, cudaStream_t st);
 int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head_weights& hw, const XwCells& cells,

@@ -100,7 +100,8 @@ class Tracker(nn.Module):
 
     @_lib.on_device
     def features_struct(self, tpc, norms):
-        """C struct for a [T][P][C] feature video (+ its cached fp16 hi/lo split in fp16x3 mode)."""
+        """C struct for a [T][P][C] feature video (+ its cached fp16 hi/lo split in fp16x3 mode).  A video outside the
+        split's faithful range gets no split: its contractions run on the exact-fp32 path (with a RuntimeWarning)."""
         if self.corr_precision != "fp16x3" or tpc.shape[-1] % 8:
             return _lib.make_features(tpc, norms)
         # The split lives ON the tensor object it was computed from: a fresh feature tensor (uncached forward,
@@ -108,10 +109,7 @@ class Tracker(nn.Module):
         # Feature tensors are written once by the kernel that creates them; _version guards torch-level in-place edits.
         split = getattr(tpc, "_dtk_split", None)
         if split is None or split[0] != tpc._version:
-            hi = torch.empty(tpc.shape, device=tpc.device, dtype=torch.float16)
-            lo = torch.empty(tpc.shape, device=tpc.device, dtype=torch.float16)
-            _lib.check(self._lib.dinotrk_split_fp16(_lib.ptr(tpc), _lib.ptr(hi), _lib.ptr(lo), tpc.numel(),
-                                                     _lib.stream_ptr(self._dev)), "split_fp16")
+            hi, lo = _lib.split_features(tpc, norms, _lib.stream_ptr(self._dev))
             split = (tpc._version, hi, lo)
             tpc._dtk_split = split
         return _lib.make_features(tpc, norms, split[1], split[2])

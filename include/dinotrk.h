@@ -77,6 +77,12 @@ int dinotrk_unpack_features(const float* tpc, float* chw, int T, int C, int P, v
 int dinotrk_token_norms(const float* tpc, float* norms, int T, int C, int P, void* stream);
 /* x = hi + lo with hi = rn_fp16(x), lo = rn_fp16(x - hi) (fp16 arrays of n elements); n % 4 == 0. */
 int dinotrk_split_fp16(const float* x, void* hi, void* lo, size_t n, void* stream);
+/* The numbers the split's faithful range is stated in: range (device float[2]) = {max |x| over the n elements of x,
+ * smallest non-zero value of the n_tok token norms (3.4e38 if there is none)}.  dinotrk_split_faithful (host only) is 1
+ * when they are in range for C channels: the split contraction is then fp32-faithful (max |x| <= 65504, every non-zero
+ * token norm >= 2^-3 sqrt(C)).  Outside it, give the features without hi / lo: the exact-fp32 GEMM runs instead. */
+int dinotrk_split_range(const float* x, size_t n, const float* norms, size_t n_tok, float* range, void* stream);
+int dinotrk_split_faithful(float max_abs, float min_norm, int C);
 
 /* ---- descriptor sampling (models/tracker.py:77-111, utils.py:75-101) ------------------- */
 /* points [B][3] = (x_px, y_px, set_index) ; frames_set [N] int32 = frame of each set slot.
@@ -179,8 +185,8 @@ int dinotrk_infer_set_overlap(int mode);
  *      showed that the head's certificate fails for more than a quarter of the maps (ill-conditioned refiner weights);
  *      the DTK_XW environment variable (0 / 1) overrides.
  * dinotrk_infer_last_stats (n >= 4 slots): {anchor-phase maps, maps finished by the exact-window path, maps re-done by the
- * full-map path, pipeline used[, of the re-done maps: those queued by the head's certificate rather than by the plan]} of
- * the last dinotrk_infer call that ran the anchor phase. */
+ * full-map path, pipeline used[, of the re-done maps: those queued by the head's certificate rather than by the plan[,
+ * contraction: 1 = split fp16 tensor cores, 0 = exact fp32]]} of the last dinotrk_infer call that ran the anchor phase. */
 int dinotrk_infer_set_path(int path);
 int dinotrk_infer_last_stats(long long* out, int n);
 int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
