@@ -70,6 +70,9 @@ SIGNATURES = {
     "dinotrk_infer_set_path": (c_int, [c_int]),
     "dinotrk_infer_last_stats": (c_int, [POINTER(ctypes.c_longlong), c_int]),
     "dinotrk_infer_max_chunks": (c_size_t, [c_int, c_int, c_int]),
+    "dinotrk_xw_coarse_keys_workspace_bytes": (c_size_t, [c_int, c_int, POINTER(Geom)]),
+    "dinotrk_xw_coarse_keys": (c_int, [POINTER(Features), POINTER(Geom), _P, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, c_size_t,
+                                       _P]),
     "dinotrk_infer_plan": (c_int, [c_int, c_int, c_int, _P, c_int, _P, _P, c_int, _P]),
     "dinotrk_infer": (c_int, [POINTER(Features), POINTER(Geom), POINTER(HeadWeights), _P, c_int, c_float, c_float,
                               c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),

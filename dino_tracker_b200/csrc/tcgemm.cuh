@@ -5,7 +5,8 @@
 //   warpgroup 0     : TMA producer (one elected lane; its registers are handed to the consumers)
 //   warpgroups 1, 2 : wgmma on 64 rows each (m64nBN), then the epilogue of those rows: 32-column blocks of the
 //                     accumulator go through shared memory so that the Epi functor sees one row per thread (or, for
-//                     coalesced epilogues, 4 consecutive columns per thread with lanes running along the rows)
+//                     coalesced epilogues, 4 consecutive columns per thread with lanes running along the rows); fragment
+//                     epilogues take the accumulator registers directly
 // The producer runs ahead into the next tile while the consumers are in the epilogue.
 //
 // Pair variant (tc_gemm_pair_kernel, a cluster of two CTAs): the two CTAs compute the two 128-row halves of a 256 x BN
@@ -63,6 +64,15 @@ template <class E> struct EpiCoalesced<E, std::enable_if_t<E::kCoalesced>> { sta
 // block before its first write (through one pointer the compiler must otherwise keep every load behind the previous store).
 template <class E, class = void> struct EpiPrefetch { static constexpr bool value = false; };
 template <class E> struct EpiPrefetch<E, std::enable_if_t<E::kPrefetch>> { static constexpr bool value = true; };
+
+// Fragment epilogues (`static constexpr bool kFragment = true`) skip the shared-memory round trip: right after the tile's
+// last wgmma has completed, every consumer thread calls
+//   fragment(g, r, m, n0, fc, acc)
+// with its own accumulator registers: acc[4 i + {0, 1}] are row r, acc[4 i + {2, 3}] row r + 8 (rows inside group g, which
+// has m rows: rows >= m are padding), columns n0 + 8 i + fc + {0, 1}.  The 4 lanes of a quad (lane & 3) hold the same
+// two rows.  No barrier, no shared memory.
+template <class E, class = void> struct EpiFragment { static constexpr bool value = false; };
+template <class E> struct EpiFragment<E, std::enable_if_t<E::kFragment>> { static constexpr bool value = true; };
 
 struct TcProblem {
   const int* grp_batch;    // [n_groups] B batch item (frame) of each group
@@ -199,65 +209,69 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
       tc::reg_fence(acc);
       if (prev >= 0) release(prev);
 
-      // ---- epilogue: 32-column blocks through shared memory ----
       const int rbase = m0 + cw * 64;        // row (inside the group) of the warpgroup's first row
-      const int r = rbase + t;
-      const bool row_ok = t < 64 && r < pb.grp_m[g];
-      typename Epi::State est;
-      epi.tile_begin(est);
+      if constexpr (EpiFragment<Epi>::value) {
+        epi.fragment(g, rbase + fr, pb.grp_m[g], n0, fc, acc);
+      } else {
+        // ---- epilogue: 32-column blocks through shared memory ----
+        const int r = rbase + t;
+        const bool row_ok = t < 64 && r < pb.grp_m[g];
+        typename Epi::State est;
+        epi.tile_begin(est);
 #pragma unroll
-      for (int c = 0; c < BN; c += 32) {
+        for (int c = 0; c < BN; c += 32) {
 #pragma unroll
-        for (int ii = 0; ii < 4; ++ii) {
-          const int i = c / 8 + ii;
-          *reinterpret_cast<float2*>(sw + fr * TC_EPI_PITCH + ii * 8 + fc) = make_float2(acc[4 * i], acc[4 * i + 1]);
-          *reinterpret_cast<float2*>(sw + (fr + 8) * TC_EPI_PITCH + ii * 8 + fc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-        }
-        tc::named_sync(1 + cw, 128);
-        const int ncols = min(32, pb.N - (n0 + c));
-        bool done = false;
-        if constexpr (EpiCoalesced<Epi>::value) {
-          if (!epi.direct(n0 + c)) {
-            // thread (r4, c4) owns 4 consecutive columns of rows it * 16 + r4 -> 8 threads cover 128 contiguous bytes
-            const int c4 = (t & 7) * 4, r4 = t >> 3;
-            if (c4 < ncols) {
-              if constexpr (EpiPrefetch<Epi>::value) {
-                float4 pre[4];
+          for (int ii = 0; ii < 4; ++ii) {
+            const int i = c / 8 + ii;
+            *reinterpret_cast<float2*>(sw + fr * TC_EPI_PITCH + ii * 8 + fc) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2*>(sw + (fr + 8) * TC_EPI_PITCH + ii * 8 + fc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+          }
+          tc::named_sync(1 + cw, 128);
+          const int ncols = min(32, pb.N - (n0 + c));
+          bool done = false;
+          if constexpr (EpiCoalesced<Epi>::value) {
+            if (!epi.direct(n0 + c)) {
+              // thread (r4, c4) owns 4 consecutive columns of rows it * 16 + r4 -> 8 threads cover 128 contiguous bytes
+              const int c4 = (t & 7) * 4, r4 = t >> 3;
+              if (c4 < ncols) {
+                if constexpr (EpiPrefetch<Epi>::value) {
+                  float4 pre[4];
 #pragma unroll
-                for (int it = 0; it < 4; ++it) {
-                  const int rr = it * 16 + r4;
-                  pre[it] = rbase + rr < pb.grp_m[g] ? epi.fetch(g, rbase + rr, n0 + c + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
+                  for (int it = 0; it < 4; ++it) {
+                    const int rr = it * 16 + r4;
+                    pre[it] = rbase + rr < pb.grp_m[g] ? epi.fetch(g, rbase + rr, n0 + c + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+                  }
 #pragma unroll
-                for (int it = 0; it < 4; ++it) {
-                  const int rr = it * 16 + r4;
-                  if (rbase + rr < pb.grp_m[g])
-                    epi.vec4(g, rbase + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * TC_EPI_PITCH + c4), pre[it]);
-                }
-              } else {
+                  for (int it = 0; it < 4; ++it) {
+                    const int rr = it * 16 + r4;
+                    if (rbase + rr < pb.grp_m[g])
+                      epi.vec4(g, rbase + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * TC_EPI_PITCH + c4), pre[it]);
+                  }
+                } else {
 #pragma unroll
-                for (int it = 0; it < 4; ++it) {
-                  const int rr = it * 16 + r4;
-                  if (rbase + rr < pb.grp_m[g])
-                    epi.vec4(g, rbase + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * TC_EPI_PITCH + c4));
+                  for (int it = 0; it < 4; ++it) {
+                    const int rr = it * 16 + r4;
+                    if (rbase + rr < pb.grp_m[g])
+                      epi.vec4(g, rbase + rr, n0 + c + c4, *reinterpret_cast<const float4*>(sw + rr * TC_EPI_PITCH + c4));
+                  }
                 }
               }
+              done = true;
             }
-            done = true;
           }
-        }
-        if (!done && row_ok && ncols > 0) {
-          float f[32];
+          if (!done && row_ok && ncols > 0) {
+            float f[32];
 #pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            const float4 v = *reinterpret_cast<const float4*>(sw + t * TC_EPI_PITCH + i);
-            f[i] = v.x; f[i + 1] = v.y; f[i + 2] = v.z; f[i + 3] = v.w;
+            for (int i = 0; i < 32; i += 4) {
+              const float4 v = *reinterpret_cast<const float4*>(sw + t * TC_EPI_PITCH + i);
+              f[i] = v.x; f[i + 1] = v.y; f[i + 2] = v.z; f[i + 3] = v.w;
+            }
+            epi(est, g, r, n0 + c, f, ncols);
           }
-          epi(est, g, r, n0 + c, f, ncols);
+          tc::named_sync(1 + cw, 128);
         }
-        tc::named_sync(1 + cw, 128);
+        if (row_ok) epi.tile_end(est, g, r, n0 / BN);
       }
-      if (row_ok) epi.tile_end(est, g, r, n0 / BN);
     }
   }
   if (PAIR) tc::cluster_sync_all();   // no CTA may exit while its peer can still multicast into it or arrive on its barriers

@@ -12,10 +12,21 @@ int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], con
                  const uint32_t box[4], int elem);   // corr_tc.cu
 
 // ====================================================================================================== 1. coarse GEMM
-// Epilogue of the single-pass fp16 GEMM over the `hi` halves: nothing is stored per token.  Per (map, 128-token tile):
-// key1 = bits(max) << 32 | (0x7fffffff - first token holding it), max2 = second largest value (>= 0).  Values are the same
-// expression as the exact path, relu(acc / max(|d| |F|, 1e-8)), with a fast division (its error is part of XW_EPS).
+// Epilogue of the single-pass fp16 GEMM over the `hi` halves: nothing is stored per token.  Per (map, 128-token tile), two
+// per 256-column GEMM tile: key1 = bits(max) << 32 | (0x7fffffff - first token holding it), max2 = second largest value
+// (>= 0).  Values are the same expression as the exact path, relu(acc / max(|d| |F|, 1e-8)), with a fast division (its
+// error is part of XW_EPS).
+//
+// A fragment epilogue (tcgemm.cuh): it works on the accumulator registers of all eight consumer warps, with no shared
+// memory and no barrier.  Per element only u = acc * (1 / |F|) is formed; the row's positive factor 1 / |d| (and the ReLU)
+// are applied to the two statistics at the end -- multiplication by a positive constant does not change which token holds
+// the maximum.  The statistics -- the maximum, the first token holding it, the second largest value of the multiset -- do
+// not depend on the order the values are folded in: a thread folds its 32 values per (row, key tile) in increasing column
+// order, then the 4 lanes of the quad merge theirs by shuffles.
+constexpr int XW_GEMM_BN = 2 * XW_TILE;   // N tile of the coarse GEMM (m64n256 per consumer warpgroup)
+
 struct CoarseEpi {
+  static constexpr bool kFragment = true;
   const float* rnorms;     // [T][P] 1 / |F[t][p]| (xw_rnorm_kernel; every norm is >= XW_MIN_NORM on this path)
   const float* desc_norm;
   const int* grp_frame;
@@ -24,47 +35,62 @@ struct CoarseEpi {
   unsigned long long* key1;
   float* max2;
   int n_tiles, P;
-  // The epilogue warps have their schedulers (almost) to themselves, so every dependent instruction costs its full latency:
-  // the 32 values of a column block are formed as 32 independent chains (all loads first), and the (max, first token, second
-  // value) statistics run in four interleaved branch-free accumulators (columns = accumulator mod 4), merged per tile.
-  // Per element only u = acc * (1 / |F|) is formed; the row's positive factor 1 / |d| (and the ReLU) are applied to the two
-  // statistics at the end of the tile -- multiplication by a positive constant does not change which token holds the maximum.
-  struct State { float m1[4], m2[4]; int tok[4]; };
-  __device__ __forceinline__ void tile_begin(State& s) const {
-#pragma unroll
-    for (int a = 0; a < 4; ++a) { s.m1[a] = -INFINITY; s.m2[a] = -INFINITY; s.tok[a] = 0x7fffffff; }
+
+  struct Top2 { float m1, m2; int tok; };
+  static __device__ __forceinline__ void push(Top2& s, float v, int tok) {
+    s.m2 = fmaxf(s.m2, fminf(s.m1, v));
+    s.tok = v > s.m1 ? tok : s.tok;      // strict: tokens come in increasing order, the first one holding the maximum stays
+    s.m1 = fmaxf(s.m1, v);
   }
-  __device__ __forceinline__ void tile_end(State& s, int g, int r, int nt) const {
-    if (nt >= n_tiles) return;   // second half of the last GEMM tile lies completely past the end of the map
-    float m1 = s.m1[0], m2 = s.m2[0];
-    int tok = s.tok[0];
-#pragma unroll
-    for (int a = 1; a < 4; ++a) {   // top-2 of the union; equal maxima -> the smaller token (first arg-max)
-      m2 = fmaxf(fmaxf(m2, s.m2[a]), fminf(m1, s.m1[a]));
-      const bool take = s.m1[a] > m1 || (s.m1[a] == m1 && s.tok[a] < tok);
-      tok = take ? s.tok[a] : tok;
-      m1 = fmaxf(m1, s.m1[a]);
-    }
-    const float rdn = __fdividef(1.f, fmaxf(desc_norm[grp_row0[g] + r], XW_MIN_NORM));
-    const size_t o = (size_t)(grp_map0[g] + r) * n_tiles + nt;
-    key1[o] = ((unsigned long long)__float_as_uint(fmaxf(m1 * rdn, 0.f)) << 32) | (unsigned)(0x7fffffff - tok);
-    max2[o] = fmaxf(m2 * rdn, 0.f);
+  static __device__ __forceinline__ void merge(Top2& s, float m1, float m2, int tok) {   // equal maxima -> the smaller token
+    s.m2 = fmaxf(fmaxf(s.m2, m2), fminf(s.m1, m1));
+    const bool take = m1 > s.m1 || (m1 == s.m1 && tok < s.tok);
+    s.tok = take ? tok : s.tok;
+    s.m1 = fmaxf(s.m1, m1);
   }
-  __device__ __forceinline__ void operator()(State& s, int g, int r, int col0, const float (&f)[32], int ncols) const {
-    const float* rn = rnorms + (size_t)grp_frame[g] * P + col0;
-    float t[32];
+  // folds key tile kh of the thread's two rows into s[0], s[1].  EDGE: the GEMM tile reaches past the end of the map
+  template <bool EDGE>
+  __device__ __forceinline__ void fold(Top2 (&s)[2], int kh, const float* rn, int n0, int fc,
+                                       const float (&acc)[XW_GEMM_BN / 2]) const {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) t[i] = __ldg(rn + (i < ncols ? i : 0));
+    for (int ii = 0; ii < XW_TILE / 8; ++ii) {   // (constant trip count: acc must stay in registers)
+      const int i = kh * XW_TILE / 8 + ii;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) t[i] = i < ncols ? f[i] * t[i] : -INFINITY;      // columns past the end of the map never win
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int a = i & 3;
-      const float v = t[i];
-      s.m2[a] = fmaxf(s.m2[a], fminf(s.m1[a], v));
-      s.tok[a] = v > s.m1[a] ? col0 + i : s.tok[a];      // strict: the first token of this accumulator holding its maximum
-      s.m1[a] = fmaxf(s.m1[a], v);
+      for (int j = 0; j < 2; ++j) {
+        const int col = n0 + 8 * i + fc + j;
+        const bool ok = !EDGE || col < P;                // columns past the end of the map never win
+        const float rnv = __ldg(rn + (ok ? col : 0));
+        push(s[0], ok ? acc[4 * i + j] * rnv : -INFINITY, col);
+        push(s[1], ok ? acc[4 * i + 2 + j] * rnv : -INFINITY, col);
+      }
     }
+  }
+  __device__ __forceinline__ void fragment(int g, int r, int m, int n0, int fc, const float (&acc)[XW_GEMM_BN / 2]) const {
+    const float* rn = rnorms + (size_t)grp_frame[g] * P;
+    // after the quad's merge every lane holds all four results; lane q keeps and writes row r + 8 (q >> 1) of key tile
+    // 2 (n0 / 256) + (q & 1)
+    const int q = threadIdx.x & 3;
+    const bool edge = n0 + XW_GEMM_BN > P;
+    Top2 o;
+#pragma unroll
+    for (int kh = 0; kh < 2; ++kh) {
+      Top2 s[2] = {{-INFINITY, -INFINITY, 0x7fffffff}, {-INFINITY, -INFINITY, 0x7fffffff}};   // rows r, r + 8
+      if (edge) fold<true>(s, kh, rn, n0, fc, acc);
+      else fold<false>(s, kh, rn, n0, fc, acc);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int sh = 1; sh <= 2; sh <<= 1)
+          merge(s[h], __shfl_xor_sync(0xffffffffu, s[h].m1, sh), __shfl_xor_sync(0xffffffffu, s[h].m2, sh),
+                __shfl_xor_sync(0xffffffffu, s[h].tok, sh));
+      if ((q & 1) == kh) o = (q >> 1) ? s[1] : s[0];
+    }
+    const int rr = r + 8 * (q >> 1), nt = n0 / XW_TILE + (q & 1);
+    if (rr >= m || nt >= n_tiles) return;   // padding row, or a key tile lying completely past the end of the map
+    const float rdn = __fdividef(1.f, fmaxf(desc_norm[grp_row0[g] + rr], XW_MIN_NORM));
+    const size_t off = (size_t)(grp_map0[g] + rr) * n_tiles + nt;
+    key1[off] = ((unsigned long long)__float_as_uint(fmaxf(o.m1 * rdn, 0.f)) << 32) | (unsigned)(0x7fffffff - o.tok);
+    max2[off] = fmaxf(o.m2 * rdn, 0.f);
   }
 };
 
@@ -93,13 +119,13 @@ int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cuda
 int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
                      const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                      int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms) {
-  using Cfg = TcCfg<TcMode::F16, XW_TILE>;
-  static_assert(XW_TILE == 128, "coarse keys are per GEMM N tile");
+  using Cfg = TcCfg<TcMode::F16, XW_GEMM_BN>;
+  static_assert(XW_GEMM_BN == 256 && XW_TILE == 128, "one m64n256 GEMM N tile = two 128-token key tiles (CoarseEpi::fragment)");
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_tmap_2d(&tmA, desc_hi, desc_rows, fv.C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB, fv.hi, fv.T, fv.P, fv.C, XW_TILE / 2, Cfg::kBK, TMAP_F16))) return rc;
-  auto kern = tc_gemm_pair_kernel<TcMode::F16, CoarseEpi, XW_TILE>;
+  if ((rc = make_tmap_3d(&tmB, fv.hi, fv.T, fv.P, fv.C, XW_GEMM_BN / 2, Cfg::kBK, TMAP_F16))) return rc;
+  auto kern = tc_gemm_pair_kernel<TcMode::F16, CoarseEpi, XW_GEMM_BN>;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
@@ -109,7 +135,7 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
   TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, fv.P, fv.C};
   CoarseEpi epi{rnorms, desc_norm, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
   const int sms = num_sms();
-  const int tiles_bound = max_tiles * cdiv(fv.P, XW_TILE);
+  const int tiles_bound = max_tiles * cdiv(fv.P, XW_GEMM_BN);
   int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
   if (grid < 2) grid = 2;
   ProfRange pr(PROF_XW_COARSE, st);
@@ -834,4 +860,64 @@ size_t xw_chunk_bytes(int chunk_maps, int max_cells, int n_tiles, int gcap) {
   return b + 2048;
 }
 
+// tile_start[g] = sum over groups before g of ceil(m / TC2_BM) (one warp; the coarse GEMM's M-tile prefix)
+__global__ void xw_tile_prefix_kernel(const int* __restrict__ grp_m, int n_groups, int* __restrict__ tile_start) {
+  const int lane = threadIdx.x;
+  int base = 0;
+  for (int g0 = 0; g0 < n_groups; g0 += 32) {
+    const int g = g0 + lane;
+    const int v = g < n_groups ? (grp_m[g] + TC2_BM - 1) / TC2_BM : 0;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += u;
+    }
+    if (g < n_groups) tile_start[g] = base + inc - v;
+    base += __shfl_sync(0xffffffffu, inc, 31);
+  }
+  if (lane == 0) tile_start[n_groups] = base;
+}
+
 }  // namespace dtk
+
+using namespace dtk;
+
+extern "C" {
+
+size_t dinotrk_xw_coarse_keys_workspace_bytes(int T, int n_groups, const dinotrk_geom* g) {
+  const size_t P = g ? (size_t)g->h * g->w : 0;
+  return align_up((size_t)T * P * 4, 256) + align_up((size_t)(n_groups + 1) * 4, 256) + 256 + 1024;
+}
+
+int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, int desc_rows,
+                           const float* desc_norm, const int* grp_frame, const int* grp_row0, const int* grp_m, int n_groups,
+                           unsigned long long* key1, float* max2, void* workspace, size_t workspace_bytes, void* stream) {
+  DTK_CHECK_ARG(feat && feat->norms && feat->hi && g && desc_hi && desc_norm && grp_frame && grp_row0 && grp_m && key1 && max2,
+                "xw_coarse_keys: null pointer (the fp16 split of the features is required)");
+  DTK_CHECK_ARG(feat->T > 0 && feat->C > 0 && feat->C % 8 == 0 && desc_rows > 0 && n_groups >= 0,
+                "xw_coarse_keys: bad sizes (C must be a multiple of 8)");
+  DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_xw_coarse_keys_workspace_bytes(feat->T, n_groups, g),
+                "xw_coarse_keys: workspace too small");
+  if (n_groups == 0) return DINOTRK_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const FeatView fv = make_view(*feat, *g);
+  Arena ar(workspace, workspace_bytes);
+  float* rnorms = ar.take<float>((size_t)fv.T * fv.P);
+  int* tile_start = ar.take<int>(n_groups + 1);
+  unsigned* min_bits = ar.take<unsigned>(1);
+  int rc = launch_xw_rnorms(fv, rnorms, min_bits, st);
+  if (rc) return rc;
+  {
+    ProfRange pr(PROF_MISC, st);
+    xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, tile_start);
+    DTK_LAUNCHED();
+  }
+  XwChunk xc{};
+  xc.key1 = key1;
+  xc.max2 = max2;
+  return launch_xw_coarse(fv, desc_hi, desc_rows, desc_norm, grp_frame, grp_row0, grp_m, grp_row0, tile_start, n_groups,
+                          desc_rows / TC2_BM + n_groups, xc, st, rnorms);
+}
+
+}  // extern "C"

@@ -7,7 +7,7 @@
 //   upper bound on everything else (certificate that the stability branch, tracker_head.py:87-94, stays off).
 //
 //   1. coarse GEMM   one fp16 wgmma pass over the `hi` halves (1/3 of the split-precision work), epilogue keeps per
-//                    map and 256-token tile only (largest value, its first token, second largest value); |coarse - exact|
+//                    map and 128-token tile only (largest value, its first token, second largest value); |coarse - exact|
 //                    <= XW_EPS for every token (fp16 rounding of both operands + fp32 accumulation, see DESIGN.md).
 //   2. plan          per map: the tokens that can be the exact arg-max (coarse >= max - 2 XW_EPS); a map whose candidates
 //                    are not all tile maxima is "ambiguous".  Maps come in CELLS = the <= 128 source frames of one (query,
@@ -38,7 +38,7 @@ constexpr int XW_MAX_CAND = 4;
 constexpr float XW_MIN_NORM = 1e-4f;  // guard of the coarse epilogue's reciprocal norms only.  XW_EPS holds when both norms are
                                       // >= split_min_norm(C) (corr.cuh): a smaller descriptor norm makes the map ambiguous, a
                                       // smaller token norm anywhere in the video sends the whole call to the full-map pipeline
-constexpr int XW_TILE = 128;          // tokens per coarse key (= the coarse GEMM's N tile)
+constexpr int XW_TILE = 128;          // tokens per coarse key (half of the coarse GEMM's N tile: two keys per tile)
 
 // column of box token (by, bx) in a map's accumulator row
 __host__ __device__ inline int xw_col(int by, int bx) { return by * XW_BOX + bx; }

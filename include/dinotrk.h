@@ -175,7 +175,7 @@ int dinotrk_infer_plan(int kind, int T, int N, const int* anchor_counts, int chu
  * process (one process per GPU): with mode >= 1 do not run dinotrk_infer from two host threads at once. */
 int dinotrk_infer_set_overlap(int mode);
 /* Pipeline of the anchor re-tracking phase (process-wide):
- *  1 = coarse pass + exact window: one single-pass fp16 GEMM keeps per map and 256-token tile only (max, its token, second
+ *  1 = coarse pass + exact window: one single-pass fp16 GEMM keeps per map and 128-token tile only (max, its token, second
  *      value); the fp32-faithful split-precision contraction is then evaluated only on a 21 x 21 token box around the
  *      arg-max of each (query, anchor frame) cell, and a warp-per-map head consumes those values -- no correlation map is
  *      ever written.  Maps whose arg-max cannot be resolved from the coarse pass (near ties), that leave their cell's box
@@ -189,6 +189,16 @@ int dinotrk_infer_set_overlap(int mode);
  * contraction: 1 = split fp16 tensor cores, 0 = exact fp32]]} of the last dinotrk_infer call that ran the anchor phase. */
 int dinotrk_infer_set_path(int path);
 int dinotrk_infer_last_stats(long long* out, int n);
+/* The coarse pass of pipeline 1 on its own (for testing its keys): the single-pass fp16 GEMM of desc_hi [desc_rows][C]
+ * (fp16, the `hi` half of the descriptors) against feat->hi, group k correlating rows [grp_row0[k], grp_row0[k] + grp_m[k])
+ * with frame grp_frame[k] (device int32[n_groups]).  For descriptor row j and 128-token tile t (n_tiles = ceil(h*w / 128)):
+ * key1[j][t] = bits(max) << 32 | (0x7fffffff - first token holding it) and max2[j][t] = the second largest value of the
+ * tile, both of relu(coarse dot / max(|d| |F|)) with |d| = desc_norm[j], |F| = feat->norms (clamped at 1e-4).  Rows
+ * outside every group are not written.  feat->hi is required. */
+size_t dinotrk_xw_coarse_keys_workspace_bytes(int T, int n_groups, const dinotrk_geom* g);
+int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, int desc_rows,
+                           const float* desc_norm, const int* grp_frame, const int* grp_row0, const int* grp_m, int n_groups,
+                           unsigned long long* key1, float* max2, void* workspace, size_t workspace_bytes, void* stream);
 int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
                   const dinotrk_head_weights* hw, const float* query_points, int N,
                   float anchor_th, float cos_th, int frame_batch, int start_phase, int stop_after,
