@@ -13,8 +13,11 @@ from .model_inference import (ModelInference, generate_trajectory_input, generat
                               generate_trajectories)
 
 from .vit import DinoV2Features, get_dino_features_video  # noqa: F401
-from .pipeline import build_tracker_from_video, track_video, save_dino_embed_video  # noqa: F401
+from .pipeline import build_tracker_from_video, track_video, save_dino_embed_video, preprocess_best_buddies  # noqa: F401
 from .benchmark import infer_query_frames, save_predictions, run_videos  # noqa: F401
+from .trajectories import extract_trajectories, save_trajectories  # noqa: F401
+from .best_buddies import of_filter, run_of_filter  # noqa: F401
 
-__all__ = ["infer_query_frames", "save_predictions", "run_videos", "DinoV2Features", "get_dino_features_video", "build_tracker_from_video", "track_video", "save_dino_embed_video","Tracker", "ModelInference", "RangeNormalizer", "generate_trajectory_input", "generate_trajectory",
+__all__ = ["extract_trajectories", "save_trajectories", "of_filter", "run_of_filter", "preprocess_best_buddies",
+           "infer_query_frames", "save_predictions", "run_videos", "DinoV2Features", "get_dino_features_video", "build_tracker_from_video", "track_video", "save_dino_embed_video","Tracker", "ModelInference", "RangeNormalizer", "generate_trajectory_input", "generate_trajectory",
            "generate_trajectories"]

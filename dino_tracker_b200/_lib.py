@@ -35,6 +35,10 @@ class VitWeights(Structure):
                 ("blocks", POINTER(c_void_p))]
 
 
+class FlowVideo(Structure):
+    _fields_ = [("fwd", c_void_p), ("bwd", c_void_p), ("T", c_int), ("H", c_int), ("W", c_int)]
+
+
 class DinotrkError(RuntimeError):
     pass
 
@@ -101,6 +105,13 @@ SIGNATURES = {
     "dinotrk_peer_close": (c_int, [_P]),
     "dinotrk_peer_free": (c_int, [_P]),
     "dinotrk_occlusion": (c_int, [_P, _P, _P, c_int, c_int, c_float, c_float, _P, _P]),
+    "dinotrk_flow_masks": (c_int, [POINTER(FlowVideo), c_float, _P, _P]),
+    "dinotrk_traj_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "dinotrk_traj_chain": (c_int, [POINTER(FlowVideo), _P, c_int, c_float, c_int, _P, _P, c_float, _P, _P, c_size_t, _P]),
+    "dinotrk_traj_emit": (c_int, [POINTER(FlowVideo), c_int, _P, _P, c_size_t, _P]),
+    "dinotrk_traj_nearest_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "dinotrk_traj_nearest": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, c_float, _P, _P, c_size_t, _P]),
+    "dinotrk_of_filter": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, c_int, _P, _P]),
 }
 
 

@@ -186,11 +186,8 @@ def compute_max_r(bb, bb_rev):
     return bb, bb_rev
 
 
-def run_nms(args):
-    """Drop-in for ``compute_dino_bb_nms.run`` (same argparse namespace: dino_bb_path, dino_emb_path, out_path, stride,
-    box_size, iou_thresh)."""
-    dino_bb = torch.load(args.dino_bb_path)
-    pk = PackedFeatures(torch.load(args.dino_emb_path, map_location="cpu"), stride=args.stride)
+def nms_dict(dino_bb, pk, stride=7, box_size=50, iou_thresh=0.2):
+    """The loop of ``compute_dino_bb_nms.run`` over a best-buddy dict (in place; returns it).  ``pk``: PackedFeatures."""
     for key in list(dino_bb.keys()):
         if dino_bb[key]["source_coords"] is None:
             dino_bb[key]["peak_coords"] = dino_bb[key]["peak_affs"] = dino_bb[key]["r"] = None
@@ -198,12 +195,97 @@ def run_nms(args):
         if dino_bb[key].get("r", None) is not None:
             continue
         sf, tf = int(key.split("_")[0]), int(key.split("_")[1])
-        bb = compute_bb_nms(dino_bb[f"{sf}_{tf}"], sf, tf, pk, None, args.stride, args.box_size, args.iou_thresh)
-        bb_rev = compute_bb_nms(dino_bb[f"{tf}_{sf}"], tf, sf, pk, None, args.stride, args.box_size, args.iou_thresh)
+        bb = compute_bb_nms(dino_bb[f"{sf}_{tf}"], sf, tf, pk, None, stride, box_size, iou_thresh)
+        bb_rev = compute_bb_nms(dino_bb[f"{tf}_{sf}"], tf, sf, pk, None, stride, box_size, iou_thresh)
         bb, bb_rev = compute_max_r(bb, bb_rev)
         dino_bb[key], dino_bb[f"{tf}_{sf}"] = bb, bb_rev
+    return dino_bb
+
+
+def run_nms(args):
+    """Drop-in for ``compute_dino_bb_nms.run`` (same argparse namespace: dino_bb_path, dino_emb_path, out_path, stride,
+    box_size, iou_thresh)."""
+    dino_bb = torch.load(args.dino_bb_path)
+    pk = PackedFeatures(torch.load(args.dino_emb_path, map_location="cpu"), stride=args.stride)
+    nms_dict(dino_bb, pk, args.stride, args.box_size, args.iou_thresh)
     os.makedirs(os.path.dirname(args.out_path), exist_ok=True)
     torch.save(dino_bb, args.out_path)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Optical-flow filter of the best-buddy pairs: preprocessing_dino_bb/of_filter_dino_best_buddies.py (SURVEY.md 8f-3)
+_BB_FIELDS = ("source_coords", "target_coords", "cos_sims", "peak_coords", "peak_affs", "r")
+
+
+@torch.no_grad()
+def nearest_trajectories(traj, h, w, stride=7):
+    """of_filter_dino_best_buddies.py:51-56: [T][rows][columns] int64 index of the trajectory nearest to every token
+    centre of create_meshgrid(h, w, stride) at every frame (``dinotrk_traj_nearest``)."""
+    lib = _lib.load()
+    dev = _lib.require_cuda(traj.device)
+    traj = traj.to(dev, torch.float32).contiguous()
+    M, T = traj.shape[:2]
+    if M == 0:
+        raise ValueError("no trajectories: the nearest trajectory is undefined (torch.argmin over an empty dimension)")
+    gh, gw = len(range(7, h, stride)), len(range(7, w, stride))
+    with torch.cuda.device(dev):
+        out = torch.empty(T, gh, gw, device=dev, dtype=torch.int32)
+        nb = lib.dinotrk_traj_nearest_workspace_bytes(M, T, gh, gw)
+        ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+        _lib.check(lib.dinotrk_traj_nearest(_lib.ptr(traj), M, T, gh, gw, 7.0, float(stride), _lib.ptr(out), _lib.ptr(ws), nb,
+                                            _lib.stream_ptr()), "traj_nearest")
+    return out.long()
+
+
+@torch.no_grad()
+def of_filter(bb_dict, traj, h, w, stride=7):
+    """of_filter_dino_best_buddies.run (:45-108) on in-memory inputs.  ``bb_dict``: 's_t' -> {source_coords,
+    target_coords, cos_sims[, peak_coords, peak_affs, r]} for every ordered pair of the T = traj.shape[1] frames;
+    ``traj`` [M][T][2].  Keeps the pairs whose points' nearest trajectories do not reach the other frame.  Returns the
+    reference's dict: every field None for a pair with nothing kept, the optional fields None when absent."""
+    lib = _lib.load()
+    dev = _lib.require_cuda(traj.device if traj.is_cuda else "cuda:0")
+    traj = traj.to(dev, torch.float32).contiguous()
+    M, T = traj.shape[:2]
+    keys = [f"{s}_{t}" for s in range(T) for t in range(T) if s != t]
+    counts = [int(bb_dict[k]["source_coords"].shape[0]) for k in keys]
+    with torch.cuda.device(dev):
+        nearest = nearest_trajectories(traj, h, w, stride).int()
+        src = torch.cat([bb_dict[k]["source_coords"].to(dev, torch.float32) for k in keys]).reshape(-1, 2).contiguous()
+        tgt = torch.cat([bb_dict[k]["target_coords"].to(dev, torch.float32) for k in keys]).reshape(-1, 2).contiguous()
+        pairs = torch.tensor([[int(x) for x in k.split("_")] for k in keys], dtype=torch.int32).reshape(-1, 2)
+        pair_src, pair_tgt = pairs[:, 0].contiguous().to(dev), pairs[:, 1].contiguous().to(dev)
+        offsets = torch.tensor([0] + counts, dtype=torch.int64).cumsum(0).to(torch.int32).to(dev)
+        n = int(src.shape[0])
+        keep = torch.zeros(n, device=dev, dtype=torch.uint8)
+        _lib.check(lib.dinotrk_of_filter(_lib.ptr(traj), M, T, _lib.ptr(nearest), nearest.shape[1], nearest.shape[2], int(stride),
+                                         _lib.ptr(src), _lib.ptr(tgt), _lib.ptr(pair_src), _lib.ptr(pair_tgt), _lib.ptr(offsets),
+                                         len(keys), n, _lib.ptr(keep), _lib.stream_ptr()), "of_filter")
+        keep = keep.bool().cpu()                                   # one read-back for all pairs
+    out, i0 = {}, 0
+    for k, c in zip(keys, counts):
+        kp = keep[i0:i0 + c]
+        i0 += c
+        f = dict.fromkeys(_BB_FIELDS)
+        if bool(kp.any()):
+            bb = bb_dict[k]
+            for name in _BB_FIELDS:
+                v = bb.get(name, None)
+                if v is not None:
+                    f[name] = v[kp.to(v.device)]
+        out[k] = f
+    return out
+
+
+def run_of_filter(args):
+    """Drop-in for ``of_filter_dino_best_buddies.run`` (same argparse namespace: dino_bb_path, traj_path, out_path,
+    dino_bb_stride, h, w)."""
+    bb = torch.load(args.dino_bb_path)
+    traj = torch.load(args.traj_path, map_location="cpu")
+    out = of_filter(bb, traj, args.h, args.w, args.dino_bb_stride)
+    os.makedirs(os.path.dirname(args.out_path), exist_ok=True)
+    torch.save(out, args.out_path)
+    print(f"Saved filtered best buddies to {args.out_path}")
 
 
 def run(args):

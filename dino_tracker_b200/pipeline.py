@@ -38,6 +38,29 @@ def track_video(video01, vit: DinoV2Features, query_points, head_state_dict=None
 
 
 @torch.no_grad()
+def preprocess_best_buddies(features_chw, video01, dino_bb_dir, traj_path, h, w, stride=7, flow_fn=None, threshold=1.0,
+                            min_trajectory_length=2, box_size=50, iou_thresh=0.2, device="cuda:0"):
+    """preprocessing_dino_bb/main_dino_bb_preprocessing.py in one process: best buddies of the features (T x C x h' x w'),
+    optical-flow trajectories of the video (T x 3 x h x w in [0, 1], no direct-flow filtering), the flow filter of the
+    best buddies, then their NMS.  Features and trajectories stay on the GPU.  Writes the reference's three files:
+    ``dino_bb_dir``/dino_best_buddies.pt, ``traj_path`` and ``dino_bb_dir``/dino_best_buddies_filtered.pt.  Returns
+    (best buddies, trajectories, filtered best buddies)."""
+    from . import best_buddies as bbm
+    from .trajectories import extract_trajectories
+    dev = torch.device(device)
+    pk = bbm.PackedFeatures(features_chw, stride=stride, device=dev)
+    bb = bbm.best_buddies(features_chw, h, w, stride=stride, device=dev)
+    os.makedirs(dino_bb_dir, exist_ok=True)
+    torch.save(bb, os.path.join(dino_bb_dir, "dino_best_buddies.pt"))
+    traj = extract_trajectories(video01, flow_fn, threshold, min_trajectory_length, device=dev)
+    os.makedirs(os.path.dirname(traj_path) or ".", exist_ok=True)
+    torch.save(traj.cpu(), traj_path)
+    filtered = bbm.nms_dict(bbm.of_filter(bb, traj, h, w, stride), pk, stride, box_size, iou_thresh)
+    torch.save(filtered, os.path.join(dino_bb_dir, "dino_best_buddies_filtered.pt"))
+    return bb, traj, filtered
+
+
+@torch.no_grad()
 def save_dino_embed_video(video01, vit: DinoV2Features, path):
     """preprocessing/save_dino_embed_video.py:9-25: writes T x C x h x w fp32 (CPU tensor) to ``path``."""
     os.makedirs(os.path.dirname(path) or ".", exist_ok=True)

@@ -303,6 +303,48 @@ int dinotrk_bb_mutual(const int* nn_st, const int* nn_ts, int n_pairs, int P, ui
 int dinotrk_bb_nms(const float* maps, int n_maps, const dinotrk_geom* g, float box_size, float iou_thresh, int topk,
                    float* peak_affs, float* r, void* stream);
 
+/* ---- optical-flow trajectories (preprocessing/extract_trajectories.py) ------------------------------------------ */
+/* The flows of a T-frame H x W video: fwd[i] / bwd[i] = flow from frame i to i+1 / from i+1 to i, [T-1][2][H][W]
+ * fp32 (channel 0 = x).  Flows are sampled as data/data_utils.py bilinear_sampler does (grid_sample, zeros padding,
+ * align_corners), norms are fp32 sqrt(dx*dx + dy*dy). */
+typedef struct dinotrk_flow_video {
+  const float* fwd;
+  const float* bwd;
+  int T, H, W;
+} dinotrk_flow_video;
+/* get_flows_with_masks (extract_trajectories.py:61-95): masks [T+1][H][W] uint8; masks[i+1] = 1 where the round trip
+ * frame i+1 -> i -> i+1 returns within `threshold` px AND some pixel of frame i warps (rounded) onto the pixel.
+ * masks[0] = masks[T] = 0. */
+int dinotrk_flow_masks(const dinotrk_flow_video* fv, float threshold, uint8_t* masks, void* stream);
+/* Chaining of one start frame s (extract_trajectories.py:203-266).  dinotrk_traj_chain walks every pixel of frame s
+ * that starts a trajectory (masks[s] == 0, or no trajectory kept from an earlier start frame passes through it) through
+ * frames s+1.. while the cycle check (< threshold), the bounds check and, when direct flows are given, the direct-flow
+ * check (< direct_threshold, :98-160 and :222-255) hold; direct_fwd / direct_bwd = [T-1-s][2][H][W] flows s -> s+1+k /
+ * s+1+k -> s.  It writes the number of trajectories of at least min_len frames to *n_kept (device int).
+ * dinotrk_traj_emit then writes them to out [n_kept][T][2] (NaN outside their frames), in row-major pixel order, and
+ * records their rounded positions for the look-behind of later start frames.  Run s = 0, 1, ... in order, chain then
+ * emit, on one workspace zeroed before s = 0. */
+size_t dinotrk_traj_workspace_bytes(int T, int H, int W);
+int dinotrk_traj_chain(const dinotrk_flow_video* fv, const uint8_t* masks, int s, float threshold, int min_len,
+                       const float* direct_fwd, const float* direct_bwd, float direct_threshold, int* n_kept,
+                       void* workspace, size_t workspace_bytes, void* stream);
+int dinotrk_traj_emit(const dinotrk_flow_video* fv, int s, float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- optical-flow filter of the best buddies (preprocessing_dino_bb/of_filter_dino_best_buddies.py) ------------- */
+/* nearest [T][gh][gw] int32 = argmin_n |traj[n][t] - g| over trajectories traj [M][T][2] for the grid points
+ * g = (start + step j, start + step i) (create_meshgrid); a NaN position is never nearest, ties -> lowest n, a frame
+ * without any valid position -> 0 (torch.argmin over +inf).  Exact: distances are fp32 sqrt(dx*dx + dy*dy). */
+size_t dinotrk_traj_nearest_workspace_bytes(int M, int T, int gh, int gw);
+int dinotrk_traj_nearest(const float* traj, int M, int T, int gh, int gw, float start, float step, int* nearest,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/* The pair filter (:86-97) over all ordered pairs at once.  Pair k (frames pair_src[k] -> pair_tgt[k]) owns points
+ * [offsets[k], offsets[k+1]) of src_xy / tgt_xy [n_pts][2] (pixel coordinates).  keep[i] = 1 when the nearest
+ * trajectory of the source point's grid cell ((p - 7) // stride) is NaN at the target frame AND that of the target point
+ * is NaN at the source frame: the pairs the flow does not cover. */
+int dinotrk_of_filter(const float* traj, int M, int T, const int* nearest, int gh, int gw, int stride, const float* src_xy,
+                      const float* tgt_xy, const int* pair_src, const int* pair_tgt, const int* offsets, int n_pairs, int n_pts,
+                      uint8_t* keep, void* stream);
+
 /* ---- per-kernel-class device timing (CUDA events on the launching stream; bench.py roofline) ------ */
 int dinotrk_profile_classes(void);
 const char* dinotrk_profile_class_name(int cls);
