@@ -77,6 +77,7 @@ SIGNATURES = {
     "dinotrk_xw_coarse_keys_workspace_bytes": (c_size_t, [c_int, c_int, POINTER(Geom)]),
     "dinotrk_xw_coarse_keys": (c_int, [POINTER(Features), POINTER(Geom), _P, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, c_size_t,
                                        _P]),
+    "dinotrk_xw_box_gemm": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P]),
     "dinotrk_infer_plan": (c_int, [c_int, c_int, c_int, _P, c_int, _P, _P, c_int, _P]),
     "dinotrk_infer": (c_int, [POINTER(Features), POINTER(Geom), POINTER(HeadWeights), _P, c_int, c_float, c_float,
                               c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),

@@ -40,27 +40,31 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
+static CUtensorMapSwizzle swizzle_of(int bytes) {
+  return bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+}
+
 static int encode(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
-                  const cuuint32_t* box, int elem) {
+                  const cuuint32_t* box, int elem, int swizzle = 128) {
   EncodeTiledFn fn = get_encode();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return DINOTRK_ECUDA; }
   cuuint32_t estr[3] = {1, 1, 1};
   CUtensorMapDataType dt = elem == TMAP_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
                          : elem == TMAP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUresult r = fn(map, dt, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  swizzle_of(swizzle), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return DINOTRK_ECUDA; }
   return DINOTRK_OK;
 }
 
 int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols,
-                 int elem, uint64_t ld) {
+                 int elem, uint64_t ld, int swizzle) {
   const int elem_bytes = elem == TMAP_F32 ? 4 : 2;
   if (ld == 0) ld = cols;
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {ld * (uint64_t)elem_bytes};
   cuuint32_t box[2] = {box_cols, box_rows};
-  return encode(map, base, 2, dims, strides, box, elem);
+  return encode(map, base, 2, dims, strides, box, elem, swizzle);
 }
 int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t batch, uint64_t rows, uint64_t cols, uint32_t box_rows,
                  uint32_t box_cols, int elem, uint64_t ld) {
@@ -72,9 +76,8 @@ int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t batch, uint64_t ro
   return encode(map, base, 3, dims, strides, box, elem);
 }
 
-// rank-4 map over a [d3][d2][d1][d0] tensor (d0 contiguous): used for {channels, w, h, T} boxes of the feature video
 int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3],
-                 const uint32_t box[4], int elem) {
+                 const uint32_t box[4], int elem, int swizzle) {
   EncodeTiledFn fn = get_encode();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return DINOTRK_ECUDA; }
   cuuint64_t d[4] = {dims[0], dims[1], dims[2], dims[3]};
@@ -84,7 +87,7 @@ int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], con
   CUtensorMapDataType dt = elem == TMAP_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
                          : elem == TMAP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUresult r = fn(map, dt, 4, const_cast<void*>(base), d, s, b, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  swizzle_of(swizzle), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (4-d) failed (%d)", (int)r); return DINOTRK_ECUDA; }
   return DINOTRK_OK;
 }

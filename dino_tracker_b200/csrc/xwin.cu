@@ -8,9 +8,6 @@
 
 namespace dtk {
 
-int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3],
-                 const uint32_t box[4], int elem);   // corr_tc.cu
-
 // ====================================================================================================== 1. coarse GEMM
 // Epilogue of the single-pass fp16 GEMM over the `hi` halves: nothing is stored per token.  Per (map, 128-token tile), two
 // per 256-column GEMM tile: key1 = bits(max) << 32 | (0x7fffffff - first token holding it), max2 = second largest value
@@ -283,45 +280,108 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
 }
 
 // ====================================================================================================== 3. exact box GEMM
-// Persistent, warp-specialised (same roles as tc_gemm_kernel).  One tile = one part of a cell's box: the BOX TOKENS are the
-// wgmma M operand (4 parts of 6 box rows = 126 of 128 rows, 64 per consumer warpgroup) and the cell's descriptors the N
-// operand (64 or 128 columns): a cell of T = 50 maps fills 50 of 64 columns, where descriptors-as-rows filled 50 of 128
-// rows.  Split precision (lo*hi + hi*lo + hi*hi per K step, in the full-map GEMM's order).  The box rows arrive as 4-D TMA
-// boxes {64 channels, 21 columns, 6 rows, 1 frame} of the [T][h][w][C] feature video, zero-filled outside the token grid;
-// the descriptor K-block travels in the same stage.  Epilogue: straight from the accumulator fragment to xbox[map][token]
-// (4 lanes of a quad hold 8 consecutive maps of one token, 8 quads 8 consecutive tokens: 32-byte runs).
-template <int NB>
+// Persistent, warp-specialised (same roles as tc_gemm_kernel).  The cell's DESCRIPTORS are the wgmma M operand (64 rows per
+// consumer warpgroup) and the BOX TOKENS the N operand, in two parts: box rows 0-11 (252 tokens, m64n256k16) and rows 12-20
+// (189 tokens, m64n192k16), 448 columns for 441 tokens.  Large-N shapes read the fewest shared-memory operand bytes per FMA,
+// and shared-memory bandwidth is what bounds this kernel (DESIGN.md 4.3).  Two layouts:
+//   MB = 64   every cell of the call has <= 64 maps: both consumer warpgroups work on the same cell, warpgroup 1 on part 0
+//             and warpgroup 2 on part 1.  A ring stage holds the descriptor K-block and both parts, so the descriptors are
+//             loaded once per cell and each warpgroup drains its pipeline once per cell.
+//   MB = 128  cells of up to 128 maps: warpgroup 1 takes descriptor rows 0-63 and warpgroup 2 rows 64-127 of the same part;
+//             the two parts run one after the other, a stage holding the descriptor K-block and one part.
+// K blocks of 32 channels in 64-byte-swizzled rows (a MB = 64 stage is 64 KiB: three fit).  Split precision: lo*hi + hi*lo
+// + hi*hi per K step of 16, K ascending -- the full-map GEMM's sequence of products.  The box rows arrive as 4-D TMA boxes
+// {32 channels, 21 columns, 12 or 9 rows, 1 frame} of the [T][h][w][C] feature video, zero-filled outside the token grid.
+// Epilogue: straight from the accumulator fragment to xbox[map][token] (a quad holds 8 consecutive tokens of one map).
+template <int MB>
 struct XwCfg {
-  static constexpr int kBK = 64;                            // fp16 elements per 128-byte swizzle row
-  static constexpr int kTokBytes = 128 * 128;               // one operand half (hi or lo) of a token tile: 128 rows, 126 written
-  static constexpr int kTokTx = 2 * XW_PART_TOK * 128;
-  static constexpr int kLastRows = XW_BOX - (XW_PARTS - 1) * XW_PART_ROWS;     // the last part holds 3 box rows, not 6
-  static constexpr int kTokTxLast = 2 * kLastRows * XW_BOX * 128;
-  static constexpr int kDescBytes = NB * 128;               // one operand half of the descriptor K-block
-  static constexpr int kStageBytes = 2 * kTokBytes + 2 * kDescBytes;
-  static constexpr int kStages = NB == 64 ? 4 : 3;
+  static constexpr int kBK = 32;                                  // fp16 channels per 64-byte swizzle row
+  static constexpr int kRow = 2 * kBK;                            // bytes per operand row
+  static constexpr int kDescBytes = MB * kRow;                    // one operand half (hi or lo) of the descriptor K-block
+  static constexpr int kTok0Bytes = XW_N0 * kRow, kTok1Bytes = XW_N1 * kRow;   // one half of a part's token tile
+  static constexpr int kTok0Tx = XW_ROWS0 * XW_BOX * kRow, kTok1Tx = XW_ROWS1 * XW_BOX * kRow;   // bytes the TMA box lands
+  // stage: [desc hi | desc lo | part 0 hi | part 0 lo (| part 1 hi | part 1 lo, MB = 64)]; with MB = 128 either part uses
+  // the part 0 slots
+  static constexpr int kTokOff = 2 * kDescBytes;
+  static constexpr int kStageBytes = MB == 64 ? 2 * (kDescBytes + kTok0Bytes + kTok1Bytes) : 2 * (kDescBytes + kTok0Bytes);
+  static constexpr int kStages = MB == 64 ? 3 : 4;
   static constexpr int kSmem = kStages * kStageBytes + 1024 + 256;
+  static_assert(kStages * kStageBytes + 1024 + 256 <= 227 * 1024, "shared-memory ring too large");
 };
 
-template <int NB>
+// One part of a cell on one consumer warpgroup: the K loop over the ring, then rows [r0, r0 + 64) of the cell x the part's
+// tokens into xbox.  d_off / t_off: byte offsets of the warpgroup's descriptor rows / the part's token tile in a stage,
+// t_half: distance from a token tile's hi half to its lo half.
+template <int MB, int N>
+__device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t* empty, int& stage, int& phase, int KB,
+                                        uint32_t d_off, uint32_t t_off, uint32_t t_half, float* __restrict__ xbox, int map0,
+                                        int r0, int m) {
+  using Cfg = XwCfg<MB>;
+  constexpr int kTok = (N == XW_N0 ? XW_ROWS0 : XW_ROWS1) * XW_BOX;   // tokens of the part
+  constexpr int kCol0 = N == XW_N0 ? 0 : XW_ROWS0 * XW_BOX;           // its first column in xbox
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = threadIdx.x & 127;
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  int prev = -1;
+  for (int kb = 0; kb < KB; ++kb) {
+    tc::mbar_wait(&full[stage], phase);
+    tc::wgmma_fence();
+    const uint32_t sd = tc::smem_u32(smem + stage * Cfg::kStageBytes) + d_off;
+    const uint32_t st = tc::smem_u32(smem + stage * Cfg::kStageBytes) + t_off;
+#pragma unroll
+    for (int ks = 0; ks < Cfg::kBK / 16; ++ks) {
+      const uint32_t koff = ks * 32;
+      const uint64_t d_hi = tc::smem_desc_sw64(sd + koff), d_lo = tc::smem_desc_sw64(sd + Cfg::kDescBytes + koff);
+      const uint64_t t_hi = tc::smem_desc_sw64(st + koff), t_lo = tc::smem_desc_sw64(st + t_half + koff);
+      tc::wgmma_ss<false, N>(acc, d_lo, t_hi, 1u);   // desc_lo * tok_hi, desc_hi * tok_lo, desc_hi * tok_hi:
+      tc::wgmma_ss<false, N>(acc, d_hi, t_lo, 1u);   // the product order of tc_gemm_kernel (F16X3)
+      tc::wgmma_ss<false, N>(acc, d_hi, t_hi, 1u);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<1>();
+    if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
+    prev = stage;
+    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+  }
+  tc::wgmma_wait<0>();
+  tc::reg_fence(acc);
+  if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
+  // fragment rows are maps, columns box tokens: acc[4 i + 2 h + {0, 1}] = map r0 + fr + 8 h, tokens 8 i + fc + {0, 1}
+  const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + fr + 8 * h;
+    if (r >= m) continue;
+    float* dst = xbox + (size_t)(map0 + r) * XW_COLS + kCol0;
+#pragma unroll
+    for (int i = 0; i < N / 8; ++i) {
+      const int j = 8 * i + fc;
+      if (j + 1 < kTok) *reinterpret_cast<float2*>(dst + j) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      else if (j < kTok) dst[j] = acc[4 * i + 2 * h];
+    }
+  }
+}
+
+template <int MB>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant__ CUtensorMap tmD_lo,
-               const __grid_constant__ CUtensorMap tmT_hi, const __grid_constant__ CUtensorMap tmT_lo,
-               const __grid_constant__ CUtensorMap tmL_hi, const __grid_constant__ CUtensorMap tmL_lo, XwCells cells,
+               const __grid_constant__ CUtensorMap tm0_hi, const __grid_constant__ CUtensorMap tm0_lo,
+               const __grid_constant__ CUtensorMap tm1_hi, const __grid_constant__ CUtensorMap tm1_lo, XwCells cells,
                const int2* __restrict__ box_org, float* __restrict__ xbox, int K) {
-  using Cfg = XwCfg<NB>;
+  using Cfg = XwCfg<MB>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);   // [kStages]
   uint64_t* empty = full + Cfg::kStages;                                                    // [kStages]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int warp = threadIdx.x >> 5, wg = threadIdx.x >> 7;
   const int KB = (K + Cfg::kBK - 1) / Cfg::kBK;
 
   if (threadIdx.x == 0) {
-    tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo); tc::prefetch_tmap(&tmT_hi); tc::prefetch_tmap(&tmT_lo);
-    tc::prefetch_tmap(&tmL_hi); tc::prefetch_tmap(&tmL_lo);
-    for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 2); }
+    tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo); tc::prefetch_tmap(&tm0_hi); tc::prefetch_tmap(&tm0_lo);
+    tc::prefetch_tmap(&tm1_hi); tc::prefetch_tmap(&tm1_lo);
+    for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 2); }   // 2 consumer warpgroups
     tc::mbar_fence_init();
   }
   __syncthreads();
@@ -335,74 +395,50 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
         const int2 org = box_org[cell];
         if (org.y == INT_MIN) continue;            // every map of the cell takes the full-map path
         const int drow = cells.row0[cell], frame = cells.frame[cell];
-        for (int part = 0; part < XW_PARTS; ++part) {
-          const bool last = part == XW_PARTS - 1;   // only the box rows that exist
+        for (int part = 0; part < (MB == 64 ? 1 : 2); ++part) {
           for (int kb = 0; kb < KB; ++kb) {
             const int k0 = kb * Cfg::kBK;
             tc::mbar_wait(&empty[stage], phase ^ 1);
             uint8_t* st = smem + stage * Cfg::kStageBytes;
-            uint8_t* sd = st + 2 * Cfg::kTokBytes;
-            tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + (last ? Cfg::kTokTxLast : Cfg::kTokTx));
-            tc::tma_load_4d(last ? &tmL_hi : &tmT_hi, &full[stage], st, k0, org.y, org.x + part * XW_PART_ROWS, frame);
-            tc::tma_load_4d(last ? &tmL_lo : &tmT_lo, &full[stage], st + Cfg::kTokBytes, k0, org.y, org.x + part * XW_PART_ROWS, frame);
-            tc::tma_load_2d(&tmD_hi, &full[stage], sd, k0, drow);
-            tc::tma_load_2d(&tmD_lo, &full[stage], sd + Cfg::kDescBytes, k0, drow);
+            uint8_t* s0 = st + Cfg::kTokOff;
+            if constexpr (MB == 64) {   // the descriptors and both parts
+              tc::mbar_expect_tx(&full[stage], 2 * (Cfg::kDescBytes + Cfg::kTok0Tx + Cfg::kTok1Tx));
+              uint8_t* s1 = s0 + 2 * Cfg::kTok0Bytes;
+              tc::tma_load_4d(&tm0_hi, &full[stage], s0, k0, org.y, org.x, frame);
+              tc::tma_load_4d(&tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, k0, org.y, org.x, frame);
+              tc::tma_load_4d(&tm1_hi, &full[stage], s1, k0, org.y, org.x + XW_ROWS0, frame);
+              tc::tma_load_4d(&tm1_lo, &full[stage], s1 + Cfg::kTok1Bytes, k0, org.y, org.x + XW_ROWS0, frame);
+            } else {                    // the descriptors and part `part`
+              tc::mbar_expect_tx(&full[stage], 2 * (Cfg::kDescBytes + (part ? Cfg::kTok1Tx : Cfg::kTok0Tx)));
+              const int by = org.x + (part ? XW_ROWS0 : 0);
+              tc::tma_load_4d(part ? &tm1_hi : &tm0_hi, &full[stage], s0, k0, org.y, by, frame);
+              tc::tma_load_4d(part ? &tm1_lo : &tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, k0, org.y, by, frame);
+            }
+            tc::tma_load_2d(&tmD_hi, &full[stage], st, k0, drow);
+            tc::tma_load_2d(&tmD_lo, &full[stage], st + Cfg::kDescBytes, k0, drow);
             if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
   } else {
-    // ===================== MMA + epilogue: warpgroup cw owns box tokens [64 cw, 64 cw + 64) of a part =====================
+    // ===================== MMA + epilogue =====================
     tc::regs_alloc<232>();
     const int cw = wg - 1;
-    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
     int stage = 0, phase = 0;
-    float acc[NB / 2];
     for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
       if (box_org[cell].y == INT_MIN) continue;
       const int m = cells.m[cell], map0 = cells.row0[cell];
-      for (int part = 0; part < XW_PARTS; ++part) {
-#pragma unroll
-        for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;
-        int prev = -1;
-        for (int kb = 0; kb < KB; ++kb) {
-          tc::mbar_wait(&full[stage], phase);
-          tc::wgmma_fence();
-          const uint32_t st = tc::smem_u32(smem + stage * Cfg::kStageBytes) + cw * 64 * 128;
-          const uint32_t sd = tc::smem_u32(smem + stage * Cfg::kStageBytes) + 2 * Cfg::kTokBytes;
-#pragma unroll
-          for (int ks = 0; ks < Cfg::kBK / 16; ++ks) {
-            const uint32_t koff = ks * 32;
-            const uint64_t t_hi = tc::smem_desc_sw128(st + koff), t_lo = tc::smem_desc_sw128(st + Cfg::kTokBytes + koff);
-            const uint64_t d_hi = tc::smem_desc_sw128(sd + koff), d_lo = tc::smem_desc_sw128(sd + Cfg::kDescBytes + koff);
-            tc::wgmma_ss<false, NB>(acc, t_hi, d_lo, 1u);   // desc_lo * tok_hi, desc_hi * tok_lo, desc_hi * tok_hi:
-            tc::wgmma_ss<false, NB>(acc, t_lo, d_hi, 1u);   // the product order of tc_gemm_kernel (F16X3)
-            tc::wgmma_ss<false, NB>(acc, t_hi, d_hi, 1u);
-          }
-          tc::wgmma_commit();
-          tc::wgmma_wait<1>();
-          if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
-          prev = stage;
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        tc::wgmma_wait<0>();
-        tc::reg_fence(acc);
-        if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int tok = cw * 64 + fr + 8 * h;
-          const int col = part * XW_PART_TOK + tok;
-          if (tok < XW_PART_TOK && col < XW_BOX * XW_BOX) {
-            float* dst = xbox + (size_t)map0 * XW_COLS + col;
-#pragma unroll
-            for (int i = 0; i < NB / 8; ++i) {
-              const int c = 8 * i + fc;
-              if (c < m) dst[(size_t)c * XW_COLS] = acc[4 * i + 2 * h];
-              if (c + 1 < m) dst[(size_t)(c + 1) * XW_COLS] = acc[4 * i + 2 * h + 1];
-            }
-          }
-        }
+      if constexpr (MB == 64) {   // warpgroup 1: part 0, warpgroup 2: part 1, all 64 descriptor rows
+        if (cw == 0)
+          xw_part<MB, XW_N0>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 0, m);
+        else
+          xw_part<MB, XW_N1>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff + 2 * Cfg::kTok0Bytes, Cfg::kTok1Bytes,
+                             xbox, map0, 0, m);
+      } else {                    // warpgroup cw: descriptor rows [64 cw, 64 cw + 64) of both parts
+        const uint32_t d_off = cw * 64 * Cfg::kRow;
+        xw_part<MB, XW_N0>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
+        xw_part<MB, XW_N1>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
       }
     }
   }
@@ -413,19 +449,18 @@ int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_h
   if (cells.n_cells <= 0) return DINOTRK_OK;
   DTK_CHECK_ARG(fv.C % 8 == 0 && cells.max_m <= XW_MAX_CELL, "exact-window GEMM: bad sizes");
   const bool small = cells.max_m <= 64;
-  const int nb = small ? 64 : 128;
-  CUtensorMap tD_hi, tD_lo, tT_hi, tT_lo, tL_hi, tL_lo;
+  constexpr int BK = XwCfg<64>::kBK, SW = 2 * BK;   // 32-channel K blocks, 64-byte swizzle
+  CUtensorMap tD_hi, tD_lo, t0_hi, t0_lo, t1_hi, t1_lo;
   int rc;
-  if ((rc = make_tmap_2d(&tD_hi, desc_hi, desc_rows, fv.C, nb, 64, TMAP_F16))) return rc;
-  if ((rc = make_tmap_2d(&tD_lo, desc_lo, desc_rows, fv.C, nb, 64, TMAP_F16))) return rc;
+  if ((rc = make_tmap_2d(&tD_hi, desc_hi, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
+  if ((rc = make_tmap_2d(&tD_lo, desc_lo, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
   const uint64_t dims[4] = {(uint64_t)fv.C, (uint64_t)g.w, (uint64_t)g.h, (uint64_t)fv.T};
   const uint64_t strides[3] = {(uint64_t)fv.C * 2, (uint64_t)g.w * fv.C * 2, (uint64_t)fv.P * fv.C * 2};
-  const uint32_t box[4] = {64, XW_BOX, XW_PART_ROWS, 1};
-  if ((rc = make_tmap_4d(&tT_hi, fv.hi, dims, strides, box, TMAP_F16))) return rc;
-  if ((rc = make_tmap_4d(&tT_lo, fv.lo, dims, strides, box, TMAP_F16))) return rc;
-  const uint32_t box_last[4] = {64, XW_BOX, (uint32_t)XwCfg<64>::kLastRows, 1};
-  if ((rc = make_tmap_4d(&tL_hi, fv.hi, dims, strides, box_last, TMAP_F16))) return rc;
-  if ((rc = make_tmap_4d(&tL_lo, fv.lo, dims, strides, box_last, TMAP_F16))) return rc;
+  const uint32_t box0[4] = {BK, XW_BOX, XW_ROWS0, 1}, box1[4] = {BK, XW_BOX, XW_ROWS1, 1};
+  if ((rc = make_tmap_4d(&t0_hi, fv.hi, dims, strides, box0, TMAP_F16, SW))) return rc;
+  if ((rc = make_tmap_4d(&t0_lo, fv.lo, dims, strides, box0, TMAP_F16, SW))) return rc;
+  if ((rc = make_tmap_4d(&t1_hi, fv.hi, dims, strides, box1, TMAP_F16, SW))) return rc;
+  if ((rc = make_tmap_4d(&t1_lo, fv.lo, dims, strides, box1, TMAP_F16, SW))) return rc;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
@@ -437,9 +472,9 @@ int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_h
   const int grid = cells.n_cells < sms ? cells.n_cells : sms;
   ProfRange pr(PROF_XW_GEMM, st);
   if (small)
-    xw_gemm_kernel<64><<<grid, TC_THREADS, XwCfg<64>::kSmem, st>>>(tD_hi, tD_lo, tT_hi, tT_lo, tL_hi, tL_lo, cells, xc.box_org, xc.xbox, fv.C);
+    xw_gemm_kernel<64><<<grid, TC_THREADS, XwCfg<64>::kSmem, st>>>(tD_hi, tD_lo, t0_hi, t0_lo, t1_hi, t1_lo, cells, xc.box_org, xc.xbox, fv.C);
   else
-    xw_gemm_kernel<128><<<grid, TC_THREADS, XwCfg<128>::kSmem, st>>>(tD_hi, tD_lo, tT_hi, tT_lo, tL_hi, tL_lo, cells, xc.box_org, xc.xbox, fv.C);
+    xw_gemm_kernel<128><<<grid, TC_THREADS, XwCfg<128>::kSmem, st>>>(tD_hi, tD_lo, t0_hi, t0_lo, t1_hi, t1_lo, cells, xc.box_org, xc.xbox, fv.C);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -918,6 +953,22 @@ int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, 
   xc.max2 = max2;
   return launch_xw_coarse(fv, desc_hi, desc_rows, desc_norm, grp_frame, grp_row0, grp_m, grp_row0, tile_start, n_groups,
                           desc_rows / TC2_BM + n_groups, xc, st, rnorms);
+}
+
+int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
+                        int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
+                        int n_cells, int max_m, float* xbox, void* stream) {
+  DTK_CHECK_ARG(feat && feat->hi && feat->lo && g && desc_hi && desc_lo && cell_row0 && cell_m && cell_frame && box_org && xbox,
+                "xw_box_gemm: null pointer (the fp16 split of the features is required)");
+  DTK_CHECK_ARG(feat->T > 0 && feat->C > 0 && feat->C % 8 == 0 && desc_rows > 0 && n_cells >= 0 && max_m > 0 &&
+                max_m <= XW_MAX_CELL, "xw_box_gemm: bad sizes (C must be a multiple of 8, cells of 1..%d rows)", XW_MAX_CELL);
+  DTK_CHECK_ARG(reinterpret_cast<uintptr_t>(box_org) % 8 == 0, "xw_box_gemm: box_org must be 8-byte aligned");
+  const FeatView fv = make_view(*feat, *g);
+  const XwCells cells{cell_row0, cell_m, cell_frame, nullptr, n_cells, max_m};
+  XwChunk xc{};
+  xc.box_org = reinterpret_cast<int2*>(const_cast<int*>(box_org));
+  xc.xbox = xbox;
+  return launch_xw_gemm(fv, *g, desc_hi, desc_lo, desc_rows, cells, xc, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -30,10 +30,10 @@ namespace dtk {
 constexpr float XW_EPS = 1.1e-3f;     // bound on |coarse - exact| in cosine units (2^-10 + accumulation, rounded up)
 constexpr int XW_BOX = 21;            // box side (tokens); windows of maps whose arg-max lies within +-3 of the centre fit
 constexpr int XW_SLACK = 3;
-constexpr int XW_PARTS = 4, XW_PART_ROWS = 6;                    // 4 M-parts of 6 box rows (126 tokens = 126 wgmma rows of 128)
-constexpr int XW_PART_TOK = XW_PART_ROWS * XW_BOX;
+constexpr int XW_ROWS0 = 12, XW_ROWS1 = XW_BOX - XW_ROWS0;       // box rows of the two wgmma N parts (252 and 189 tokens)
+constexpr int XW_N0 = 256, XW_N1 = 192;                          // their wgmma N (448 columns for 441 tokens)
 constexpr int XW_COLS = 448;                                     // accumulator row pitch per map (441 box tokens, row-major)
-constexpr int XW_MAX_CELL = 128;      // maps (source frames) per cell = wgmma N (64 or 128)
+constexpr int XW_MAX_CELL = 128;      // maps (source frames) per cell = wgmma M rows (64 or 128)
 constexpr int XW_MAX_CAND = 4;
 constexpr float XW_MIN_NORM = 1e-4f;  // guard of the coarse epilogue's reciprocal norms only.  XW_EPS holds when both norms are
                                       // >= split_min_norm(C) (corr.cuh): a smaller descriptor norm makes the map ambiguous, a
@@ -50,7 +50,7 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
   int* pinfo;                 // [maps] coarse arg-max token, or -1 - token for an ambiguous map (plan scratch)
   int* stat;                  // [maps] 0: exact-window path, 1: full-map path
   int* cell_of;               // [maps] cell index
-  int2* box_org;              // [cells] (first box row, first box column); x = INT_MIN: skip the cell
+  int2* box_org;              // [cells] (first box row, first box column); y = INT_MIN: skip the cell
   float* xbox;                // [maps][XW_COLS] raw split-precision accumulators of the box tokens
   float* win;                 // [maps][256] exact 15 x 15 windows ([15][16] floats, zero outside the map)
   int2* hin;                  // [maps] (exact first arg-max token or -1, bits of m_out)

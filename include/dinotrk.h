@@ -199,6 +199,16 @@ size_t dinotrk_xw_coarse_keys_workspace_bytes(int T, int n_groups, const dinotrk
 int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, int desc_rows,
                            const float* desc_norm, const int* grp_frame, const int* grp_row0, const int* grp_m, int n_groups,
                            unsigned long long* key1, float* max2, void* workspace, size_t workspace_bytes, void* stream);
+/* The exact box GEMM of pipeline 1 on its own (for testing and timing it): per cell k (device int32[n_cells] arrays), the
+ * split-precision contraction (lo*hi + hi*lo + hi*hi, the full-map GEMM's sequence) of descriptor rows
+ * [cell_row0[k], cell_row0[k] + cell_m[k]) (desc_hi / desc_lo: fp16 [desc_rows][C], dinotrk_split_fp16 of the fp32 rows)
+ * against the 21 x 21 token box of frame cell_frame[k] whose first row / column is box_org[k] = {row, column} (int32
+ * [n_cells][2]; tokens outside the grid count as zero; column INT_MIN: skip the cell).  Writes the raw accumulators
+ * xbox[row][by * 21 + bx] (fp32, [desc_rows][448]); columns 441..447, rows outside every cell and the rows of skipped cells
+ * are not written.  max_m = the largest cell_m (<= 128).  feat->hi and feat->lo are required.  Syncs: no. */
+int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
+                        int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
+                        int n_cells, int max_m, float* xbox, void* stream);
 int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
                   const dinotrk_head_weights* hw, const float* query_points, int N,
                   float anchor_th, float cos_th, int frame_batch, int start_phase, int stop_after,
