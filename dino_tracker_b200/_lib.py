@@ -87,6 +87,9 @@ SIGNATURES = {
                                      _P, _P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
     "dinotrk_vit_workspace_bytes": (c_size_t, [POINTER(VitConfig), POINTER(Geom), c_int]),
     "dinotrk_vit_attention": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
+    "dinotrk_vit_attention_f16": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
+    "dinotrk_vit_stage": (c_int, [c_int, POINTER(VitConfig), POINTER(Geom), c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t,
+                                  _P]),
     "dinotrk_vit_forward": (c_int, [_P, c_int, POINTER(Geom), POINTER(VitConfig), POINTER(VitWeights), _P, _P, c_size_t, _P]),
     "dinotrk_best_buddies_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dinotrk_best_buddies_pairs": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, c_int, _P, _P, _P, c_size_t, _P]),

@@ -318,7 +318,9 @@ __device__ __forceinline__ float gelu_exact(float v) {
   p = fmaf(p, t, 0.254829592f);
   const float e = fast_exp2(-1.4426950408889634f * z * z);
   const float erf_abs = fmaf(-p * t, e, 1.f);          // erf(|v| / sqrt 2)
-  return 0.5f * v + 0.5f * fabsf(v) * erf_abs;         // 0.5 v (1 + sign(v) erf(|v| / sqrt 2))
+  // 0.5 v (1 + sign(v) erf(|v| / sqrt 2)); the explicit fmaf keeps the coalesced (vec4) and the thread-per-row
+  // (CTA-pair default) epilogues bit-identical whatever contraction the compiler would pick at each call site
+  return fmaf(v, 0.5f, __fmul_rn(0.5f * fabsf(v), erf_abs));
 }
 
 // h[r][col] = gelu(acc + bias[col])   (exact: 0.5 x (1 + erf(x / sqrt 2)))
@@ -456,17 +458,97 @@ static int launch_flash(const __half* q16, const __half* k16, const __half* v16,
   return DINOTRK_OK;
 }
 
-}  // namespace dtk
-
-using namespace dtk;
-
-extern "C" {
+// ---------------------------------------------------------------------------------------------- block stages
+// One stage of dinotrk_vit_forward each, shared with dinotrk_vit_stage.  The linear stages after the patch embedding
+// run on the tile plan of vit_row_plan (one group of all B * N1 rows); the forward makes it once per block half.
+struct VitShape {
+  int B, P, N1, D, heads, Kp;
+  size_t rows;        // B * N1
+  bool f16, pairs;    // fp16 operands (else fp32 / TF32); linear layers on CTA pairs (fp16 only)
+};
 
 // row length of the im2col matrix / patch weight: 16-byte multiple of the operand type
 static int vit_kp(const dinotrk_vit_config* c) {
   const bool f16 = c->gemm_f16 != 0 && c->attn_materialized == 0;
   return (int)align_up((size_t)3 * c->patch * c->patch, f16 ? 8 : 4);
 }
+
+static VitShape vit_shape(const dinotrk_vit_config* c, const dinotrk_geom* g, int B) {
+  VitShape s;
+  s.B = B; s.P = g->h * g->w; s.N1 = s.P + 1; s.D = c->dim; s.heads = c->heads; s.Kp = vit_kp(c);
+  s.rows = (size_t)B * s.N1;
+  s.f16 = c->gemm_f16 != 0 && c->attn_materialized == 0;
+  s.pairs = s.f16 && c->gemm_pair != 0;
+  return s;
+}
+
+static int vit_row_plan(const VitShape& s, const Plan& pl, cudaStream_t st) {
+  return plan(pl, 1, (int)s.rows, 0, 0, 0, st, s.pairs ? TC2_BM : TC_BM);
+}
+
+// y = LayerNorm(x) (eps 1e-6), x [rows][D] fp32 -> y [rows][D] (fp16 in fp16 operand mode)
+static int vit_layernorm(const VitShape& s, const float* x, const float* gw, const float* gb, void* y, cudaStream_t st) {
+  ProfRange pr(PROF_VIT_MISC, st);
+  const unsigned grid = (unsigned)((s.rows + 7) / 8);
+  if (s.f16) vit_layernorm_kernel<__half><<<grid, 256, 0, st>>>(x, gw, gb, reinterpret_cast<__half*>(y), s.rows, s.D);
+  else vit_layernorm_kernel<float><<<grid, 256, 0, st>>>(x, gw, gb, reinterpret_cast<float*>(y), s.rows, s.D);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
+// x[b][1 + p] = cols[b P + p] . patch_w + bias + pos[p]; cols [B P][Kp] (makes its own 128-row tile plan)
+static int vit_patch_embed(const VitShape& s, const Plan& pl, const void* cols, const void* w, const float* bias,
+                           const float* pos, float* x, cudaStream_t st) {
+  int rc;
+  if ((rc = plan(pl, 1, s.B * s.P, 0, 0, 0, st))) return rc;
+  EpiPatch ep{{}, x, bias, pos, s.P, s.D};
+  const int tiles = cdiv(s.B * s.P, TC_BM);
+  return s.f16 ? run_gemm<EpiPatch, 256, TcMode::F16>(cols, (uint64_t)s.B * s.P, w, 1, s.D, s.Kp, pl, 1, tiles, ep, PROF_VIT_GEMM, st)
+               : run_gemm<EpiPatch, 256>(cols, (uint64_t)s.B * s.P, w, 1, s.D, s.Kp, pl, 1, tiles, ep, PROF_VIT_GEMM, st);
+}
+
+// qkv for the fused attention: y [rows][D] . qkv_w^T + bias -> fp16 q (scaled by 64^-1/2 log2 e), k, v^T (pitch align8(N1))
+static int vit_qkv_fused(const VitShape& s, const Plan& pl, const void* y, const void* w, const float* bias, __half* q16,
+                         __half* k16, __half* v16, cudaStream_t st) {
+  const int D = s.D, N1p8 = (int)align_up((size_t)s.N1, 8);
+  EpiQKV16 eq{{}, q16, k16, v16, bias, s.N1, D, s.heads, N1p8, 0.125f * 1.4426950408889634f};  // 1/sqrt(64) * log2(e)
+  static const int epi_direct = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;   // bit 0: q / k thread-per-row too (slower)
+  eq.direct_from = (epi_direct & 1) ? 0 : 2 * D;
+  return s.pairs ? run_gemm_pair<EpiQKV16>(y, s.rows, w, 3 * D, D, pl, cdiv((int)s.rows, TC2_BM), eq, PROF_VIT_GEMM, st)
+       : s.f16 ? run_gemm<EpiQKV16, 256, TcMode::F16>(y, s.rows, w, 1, 3 * D, D, pl, 1, cdiv((int)s.rows, TC_BM), eq, PROF_VIT_GEMM, st)
+               : run_gemm<EpiQKV16, 256>(y, s.rows, w, 1, 3 * D, D, pl, 1, cdiv((int)s.rows, TC_BM), eq, PROF_VIT_GEMM, st);
+}
+
+// x[r] += ls * (a[r] . w^T + bias), a [rows][K]: proj (K = D) and fc2 (K = 4 D)
+static int vit_residual(const VitShape& s, const Plan& pl, const void* a, const void* w, int K, const float* bias,
+                        const float* ls, float* x, cudaStream_t st) {
+  EpiResidual er{{}, x, bias, ls, s.D};
+  return s.pairs ? run_gemm_pair<EpiResidual>(a, s.rows, w, s.D, K, pl, cdiv((int)s.rows, TC2_BM), er, PROF_VIT_GEMM, st)
+       : s.f16 ? run_gemm<EpiResidual, 256, TcMode::F16>(a, s.rows, w, 1, s.D, K, pl, 1, cdiv((int)s.rows, TC_BM), er, PROF_VIT_GEMM, st)
+               : run_gemm<EpiResidual, 256>(a, s.rows, w, 1, s.D, K, pl, 1, cdiv((int)s.rows, TC_BM), er, PROF_VIT_GEMM, st);
+}
+
+// h = gelu(y . fc1_w^T + bias), y [rows][D] -> h [rows][4 D] (fp16 in fp16 operand mode)
+static int vit_fc1(const VitShape& s, const Plan& pl, const void* y, const void* w, const float* bias, void* h, cudaStream_t st) {
+  const int D = s.D;
+  if (s.pairs) {
+    EpiGelu<__half> eg{{}, reinterpret_cast<__half*>(h), bias, 4 * D};
+    static const int epi_direct2 = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;  // bit 1: fp16 GELU rows written thread-per-row (64 B per thread, whole sectors)
+    eg.all_direct = (epi_direct2 & 2) ? 1 : 0;
+    return run_gemm_pair<EpiGelu<__half>>(y, s.rows, w, 4 * D, D, pl, cdiv((int)s.rows, TC2_BM), eg, PROF_VIT_GEMM, st);
+  }
+  if (s.f16)
+    return run_gemm<EpiGelu<__half>, 256, TcMode::F16>(y, s.rows, w, 1, 4 * D, D, pl, 1, cdiv((int)s.rows, TC_BM),
+                                                       EpiGelu<__half>{{}, reinterpret_cast<__half*>(h), bias, 4 * D}, PROF_VIT_GEMM, st);
+  return run_gemm<EpiGelu<float>, 256>(y, s.rows, w, 1, 4 * D, D, pl, 1, cdiv((int)s.rows, TC_BM),
+                                       EpiGelu<float>{{}, reinterpret_cast<float*>(h), bias, 4 * D}, PROF_VIT_GEMM, st);
+}
+
+}  // namespace dtk
+
+using namespace dtk;
+
+extern "C" {
 
 size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_geom* g, int B) {
   if (!c || !g) return 0;
@@ -488,6 +570,44 @@ int dinotrk_vit_attention(const void* q16, const void* k16, const void* vT16, in
   DTK_CHECK_ARG(B > 0 && heads > 0 && N1 > 0 && N1p >= N1 && N1p % 8 == 0, "vit_attention: bad sizes");
   return launch_flash(reinterpret_cast<const __half*>(q16), reinterpret_cast<const __half*>(k16),
                       reinterpret_cast<const __half*>(vT16), B, heads, N1, N1p, heads * HD, out, false, (cudaStream_t)stream);
+}
+
+int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16, int B, int heads, int N1, int N1p,
+                              void* out16, void* stream) {
+  DTK_CHECK_ARG(q16 && k16 && vT16 && out16, "vit_attention_f16: null pointer");
+  DTK_CHECK_ARG(B > 0 && heads > 0 && N1 > 0 && N1p >= N1 && N1p % 8 == 0, "vit_attention_f16: bad sizes");
+  return launch_flash(reinterpret_cast<const __half*>(q16), reinterpret_cast<const __half*>(k16),
+                      reinterpret_cast<const __half*>(vT16), B, heads, N1, N1p, heads * HD, out16, true, (cudaStream_t)stream);
+}
+
+int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom* g, int B, const void* in, const void* w,
+                      const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  DTK_CHECK_ARG(c && g && in && p0 && out0, "vit_stage: null pointer");
+  DTK_CHECK_ARG(stage >= DINOTRK_VIT_LAYERNORM && stage <= DINOTRK_VIT_FC2, "vit_stage: unknown stage %d", stage);
+  DTK_CHECK_ARG(c->gemm_f16 != 0 && c->attn_materialized == 0, "vit_stage: fp16 operand mode only");
+  DTK_CHECK_ARG(B > 0 && c->dim == c->heads * HD && c->dim <= 2048, "vit_stage: dim must be heads x 64 (<= 2048)");
+  DTK_CHECK_ARG(stage == DINOTRK_VIT_LAYERNORM || w, "vit_stage: null weight");
+  DTK_CHECK_ARG(stage == DINOTRK_VIT_QKV || stage == DINOTRK_VIT_FC1 || p1, "vit_stage: null second parameter vector");
+  DTK_CHECK_ARG(stage != DINOTRK_VIT_QKV || (out1 && out2), "vit_stage: qkv needs q, k and v^T");
+  DTK_CHECK_ARG(workspace && workspace_bytes >= DINOTRK_VIT_STAGE_WORKSPACE_BYTES, "vit_stage: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const VitShape s = vit_shape(c, g, B);
+  Arena ar(workspace, workspace_bytes);
+  Plan pl{ar.take<int>(2), ar.take<int>(2), ar.take<int>(2), ar.take<int>(2)};
+  if (!ar.ok()) return DINOTRK_EINVAL;
+  if (stage == DINOTRK_VIT_LAYERNORM) return vit_layernorm(s, reinterpret_cast<const float*>(in), p0, p1, out0, st);
+  if (stage == DINOTRK_VIT_PATCH) return vit_patch_embed(s, pl, in, w, p0, p1, reinterpret_cast<float*>(out0), st);
+  int rc;
+  if ((rc = vit_row_plan(s, pl, st))) return rc;
+  switch (stage) {
+    case DINOTRK_VIT_QKV:
+      return vit_qkv_fused(s, pl, in, w, p0, reinterpret_cast<__half*>(out0), reinterpret_cast<__half*>(out1),
+                           reinterpret_cast<__half*>(out2), st);
+    case DINOTRK_VIT_PROJ: return vit_residual(s, pl, in, w, s.D, p0, p1, reinterpret_cast<float*>(out0), st);
+    case DINOTRK_VIT_FC1: return vit_fc1(s, pl, in, w, p0, out0, st);
+    default: return vit_residual(s, pl, in, w, 4 * s.D, p0, p1, reinterpret_cast<float*>(out0), st);
+  }
 }
 
 int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const dinotrk_vit_config* c,
@@ -518,10 +638,9 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   // fp16 operand mode (default): LayerNorm / GELU / attention write fp16 activations, weights are fp16 (11-bit
   // significand like TF32, twice the tensor rate, half the operand traffic).  The validation path
   // (attn_materialized) keeps every operand fp32 / TF32.
-  const bool f16 = c->gemm_f16 != 0 && c->attn_materialized == 0;
-  const bool pairs = f16 && c->gemm_pair != 0;   // linear layers on two-CTA clusters
-  const int pair_tiles = cdiv((int)((size_t)B * (g->h * g->w + 1)), TC2_BM);
-  __half* y16 = reinterpret_cast<__half*>(y);
+  const VitShape s = vit_shape(c, g, B);
+  const bool f16 = s.f16;
+  // y and hbuf hold fp16 activations in fp16 operand mode, fp32 ones otherwise
   __half* h16 = reinterpret_cast<__half*>(hbuf);
 
   // ---- patch embedding + cls + position embedding
@@ -531,13 +650,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
     else vit_im2col_kernel<float><<<B * P, 128, 0, st>>>(frames, hbuf, B, g->H, g->W, g->h, g->w, c->patch, c->stride, Kp);
     DTK_LAUNCHED();
   }
-  if ((rc = plan(pl, 1, B * P, 0, 0, 0, st))) return rc;
-  {
-    EpiPatch ep{{}, x, wt->patch_b, wt->pos, P, D};
-    rc = f16 ? run_gemm<EpiPatch, 256, TcMode::F16>(h16, (uint64_t)B * P, wt->patch_w, 1, D, Kp, pl, 1, cdiv(B * P, TC_BM), ep, PROF_VIT_GEMM, st)
-             : run_gemm<EpiPatch, 256>(hbuf, (uint64_t)B * P, wt->patch_w, 1, D, Kp, pl, 1, cdiv(B * P, TC_BM), ep, PROF_VIT_GEMM, st);
-    if (rc) return rc;
-  }
+  if ((rc = vit_patch_embed(s, pl, hbuf, wt->patch_w, wt->patch_b, wt->pos, x, st))) return rc;
   {
     ProfRange pr(PROF_VIT_MISC, st);
     vit_cls_kernel<<<B, 256, 0, st>>>(x, wt->cls_pos, N1, D);
@@ -545,33 +658,19 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   }
 
   const int all_tiles = cdiv((int)rows, TC_BM);
-  auto layernorm = [&](const float* gw, const float* gb) -> int {
-    ProfRange pr(PROF_VIT_MISC, st);
-    if (f16) vit_layernorm_kernel<__half><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, gw, gb, y16, rows, D);
-    else vit_layernorm_kernel<float><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, gw, gb, y, rows, D);
-    DTK_LAUNCHED();
-    return DINOTRK_OK;
-  };
   for (int l = 0; l <= c->tap_layer; ++l) {
     const float* const* w = wt->blocks + (size_t)l * 14;
     // w: 0 norm1.w 1 norm1.b 2 qkv.w 3 qkv.b 4 proj.w 5 proj.b 6 ls1 7 norm2.w 8 norm2.b 9 fc1.w 10 fc1.b 11 fc2.w 12 fc2.b 13 ls2
     // (the four weight matrices are fp16 arrays in fp16 operand mode)
-    if ((rc = layernorm(w[0], w[1]))) return rc;
-    if ((rc = plan(pl, 1, (int)rows, 0, 0, 0, st, pairs ? TC2_BM : TC_BM))) return rc;
+    if ((rc = vit_layernorm(s, x, w[0], w[1], y, st))) return rc;
+    if ((rc = vit_row_plan(s, pl, st))) return rc;
     if (c->attn_materialized == 0) {
       // fused attention: fp16 q / k / v^T, scores stay in registers
       __half* q16 = reinterpret_cast<__half*>(q);
       __half* k16 = reinterpret_cast<__half*>(k);
       __half* v16 = reinterpret_cast<__half*>(vT);
-      const int N1p8 = (int)align_up((size_t)N1, 8);
-      EpiQKV16 eq{{}, q16, k16, v16, w[3], N1, D, heads, N1p8, 0.125f * 1.4426950408889634f};  // 1/sqrt(64) * log2(e)
-      static const int epi_direct = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;   // bit 0: q / k thread-per-row too (slower)
-      eq.direct_from = (epi_direct & 1) ? 0 : 2 * D;
-      rc = pairs ? run_gemm_pair<EpiQKV16>(y16, rows, w[2], 3 * D, D, pl, pair_tiles, eq, PROF_VIT_GEMM, st)
-         : f16 ? run_gemm<EpiQKV16, 256, TcMode::F16>(y16, rows, w[2], 1, 3 * D, D, pl, 1, all_tiles, eq, PROF_VIT_GEMM, st)
-               : run_gemm<EpiQKV16, 256>(y, rows, w[2], 1, 3 * D, D, pl, 1, all_tiles, eq, PROF_VIT_GEMM, st);
-      if (rc) return rc;
-      if ((rc = launch_flash(q16, k16, v16, B, heads, N1, N1p8, D, f16 ? (void*)y16 : (void*)y, f16, st))) return rc;
+      if ((rc = vit_qkv_fused(s, pl, y, w[2], w[3], q16, k16, v16, st))) return rc;
+      if ((rc = launch_flash(q16, k16, v16, B, heads, N1, (int)align_up((size_t)N1, 8), D, y, f16, st))) return rc;
     } else {
       if ((rc = run_gemm<EpiQKV, 256>(y, rows, w[2], 1, 3 * D, D, pl, 1, all_tiles, EpiQKV{{}, q, k, vT, w[3], N1, D, heads, N1p},
                                       PROF_VIT_GEMM, st))) return rc;
@@ -595,33 +694,11 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
         }
       }
     }
-    if ((rc = plan(pl, 1, (int)rows, 0, 0, 0, st, pairs ? TC2_BM : TC_BM))) return rc;
-    {
-      EpiResidual er{{}, x, w[5], w[6], D};
-      rc = pairs ? run_gemm_pair<EpiResidual>(y16, rows, w[4], D, D, pl, pair_tiles, er, PROF_VIT_GEMM, st)
-         : f16 ? run_gemm<EpiResidual, 256, TcMode::F16>(y16, rows, w[4], 1, D, D, pl, 1, all_tiles, er, PROF_VIT_GEMM, st)
-               : run_gemm<EpiResidual, 256>(y, rows, w[4], 1, D, D, pl, 1, all_tiles, er, PROF_VIT_GEMM, st);
-      if (rc) return rc;
-    }
-    if ((rc = layernorm(w[7], w[8]))) return rc;
-    if (pairs) {
-      EpiGelu<__half> eg{{}, h16, w[10], 4 * D};
-      static const int epi_direct2 = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;  // bit 1: fp16 GELU rows written thread-per-row (64 B per thread, whole sectors)
-      eg.all_direct = (epi_direct2 & 2) ? 1 : 0;
-      if ((rc = run_gemm_pair<EpiGelu<__half>>(y16, rows, w[9], 4 * D, D, pl, pair_tiles, eg, PROF_VIT_GEMM, st))) return rc;
-      if ((rc = run_gemm_pair<EpiResidual>(h16, rows, w[11], D, 4 * D, pl, pair_tiles, EpiResidual{{}, x, w[12], w[13], D},
-                                           PROF_VIT_GEMM, st))) return rc;
-    } else if (f16) {
-      if ((rc = run_gemm<EpiGelu<__half>, 256, TcMode::F16>(y16, rows, w[9], 1, 4 * D, D, pl, 1, all_tiles,
-                                                            EpiGelu<__half>{{}, h16, w[10], 4 * D}, PROF_VIT_GEMM, st))) return rc;
-      if ((rc = run_gemm<EpiResidual, 256, TcMode::F16>(h16, rows, w[11], 1, D, 4 * D, pl, 1, all_tiles,
-                                                        EpiResidual{{}, x, w[12], w[13], D}, PROF_VIT_GEMM, st))) return rc;
-    } else {
-      if ((rc = run_gemm<EpiGelu<float>, 256>(y, rows, w[9], 1, 4 * D, D, pl, 1, all_tiles,
-                                              EpiGelu<float>{{}, hbuf, w[10], 4 * D}, PROF_VIT_GEMM, st))) return rc;
-      if ((rc = run_gemm<EpiResidual, 256>(hbuf, rows, w[11], 1, D, 4 * D, pl, 1, all_tiles,
-                                           EpiResidual{{}, x, w[12], w[13], D}, PROF_VIT_GEMM, st))) return rc;
-    }
+    if ((rc = vit_row_plan(s, pl, st))) return rc;
+    if ((rc = vit_residual(s, pl, y, w[4], D, w[5], w[6], x, st))) return rc;              // proj + LayerScale + residual
+    if ((rc = vit_layernorm(s, x, w[7], w[8], y, st))) return rc;
+    if ((rc = vit_fc1(s, pl, y, w[9], w[10], hbuf, st))) return rc;
+    if ((rc = vit_residual(s, pl, hbuf, w[11], 4 * D, w[12], w[13], x, st))) return rc;   // fc2 + LayerScale + residual
   }
   {
     ProfRange pr(PROF_VIT_MISC, st);

@@ -294,6 +294,34 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
  * (the layout of the reference's attn output before `proj`, dinov2 attention.py). */
 int dinotrk_vit_attention(const void* q16, const void* k16, const void* vT16, int B, int heads, int N1, int N1p,
                           float* out, void* stream);
+/* The same with an fp16 out16 [B*N1][heads*64]: the store the forward's fp16 operand mode feeds to `proj`. */
+int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16, int B, int heads, int N1, int N1p,
+                              void* out16, void* stream);
+/* One stage of dinotrk_vit_forward on its own, with the forward's own code, for testing and timing the layers
+ * (fp16 operand mode: c->gemm_f16 = 1, c->attn_materialized = 0; c->gemm_pair picks CTA pairs or single CTAs for
+ * qkv / proj / fc1 / fc2).  N1 = g->h * g->w + 1 tokens per frame, rows = B * N1, D = c->dim, fp16 weight matrices
+ * K-major as in dinotrk_vit_weights, fp32 parameter vectors.  Per stage (in, w, p0, p1 -> out0 [, out1, out2]):
+ *   LAYERNORM  x [rows][D] fp32, -, weight [D], bias [D]  -> y [rows][D] fp16   (eps 1e-6)
+ *   PATCH      cols [B*h*w][Kp] fp16 (Kp = 3*patch*patch rounded up to 8), patch_w [D][Kp], bias [D], pos [h*w][D]
+ *              -> x [B][N1][D] fp32: x[b][1 + p] = cols[b*h*w + p] . patch_w + bias + pos[p]; x[b][0] is not written
+ *   QKV        y [rows][D] fp16, qkv_w [3D][D], bias [3D], -  -> q [B*heads][N1][64] fp16 multiplied by
+ *              64^-1/2 * log2(e), k [B*heads][N1][64] fp16, vT [B*heads][64][N1p8] fp16 (v transposed, row pitch N1p8 =
+ *              N1 rounded up to 8; columns N1..N1p8-1 are not written): dinotrk_vit_attention's inputs
+ *   PROJ       y [rows][D] fp16, proj_w [D][D], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (y . proj_w + bias)
+ *   FC1        y [rows][D] fp16, fc1_w [4D][D], bias [4D], -  -> h [rows][4D] fp16 = gelu(y . fc1_w + bias) (exact GELU
+ *              with erf to 1.5e-7)
+ *   FC2        h [rows][4D] fp16, fc2_w [D][4D], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (h . fc2_w + bias)
+ * workspace: DINOTRK_VIT_STAGE_WORKSPACE_BYTES of device memory (tile plan).  Rows past `rows` are not touched. */
+#define DINOTRK_VIT_LAYERNORM 0
+#define DINOTRK_VIT_PATCH 1
+#define DINOTRK_VIT_QKV 2
+#define DINOTRK_VIT_PROJ 3
+#define DINOTRK_VIT_FC1 4
+#define DINOTRK_VIT_FC2 5
+#define DINOTRK_VIT_STAGE_WORKSPACE_BYTES 4096
+int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom* g, int B, const void* in, const void* w,
+                      const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
+                      size_t workspace_bytes, void* stream);
 
 /* ---- best buddies (preprocessing_dino_bb/extract_dino_best_buddies.py:12-54) ------------------------ */
 /* For every ordered pair k (source frame pair_src[k], target frame pair_tgt[k]; device int32[n_pairs]):

@@ -168,6 +168,29 @@ def test_vit_full_size_against_gpu_oracle(name):
     assert cos > 0.9999
 
 
+def test_vit_full_size_frames_per_call_invariance():
+    """ViT-B/14@11 on three 854x476 frames with frames_per_call = 2 (a 2-frame call of 16216 rows, then a 1-frame call)
+    must equal each frame run alone bit for bit: a token's row lands in another tile and another CTA of the pair, with
+    the same arithmetic."""
+    from dino_tracker_b200.vit import DinoV2Features
+    sd, dim, heads, layer = _vit_sd("dinov2_vitb14", 92)
+    video = synth.random_video(3, 476, 854, seed=93).to(DEV)
+    alone = DinoV2Features(sd, heads=heads, layer=layer, device=DEV, frames_per_call=1)(video).clone()
+    batched = DinoV2Features(sd, heads=heads, layer=layer, device=DEV, frames_per_call=2)(video)
+    assert torch.equal(batched, alone), f"frames_per_call changes the features: {(batched - alone).abs().max().item()}"
+
+
+def test_vit_full_size_cta_pairs_bit_identical():
+    """ViT-L/14@15 on two 854x476 frames: the linear layers on CTA pairs and on single CTAs issue the same wgmma sequence
+    per output row and share their epilogue arithmetic, so the features are bit-identical."""
+    from dino_tracker_b200.vit import DinoV2Features
+    sd, dim, heads, layer = _vit_sd("dinov2_vitl14", 94)
+    video = synth.random_video(2, 476, 854, seed=95).to(DEV)
+    pairs = DinoV2Features(sd, heads=heads, layer=layer, device=DEV, cta_pairs=True)(video).clone()
+    single = DinoV2Features(sd, heads=heads, layer=layer, device=DEV, cta_pairs=False)(video)
+    assert torch.equal(pairs, single), f"CTA pairs change the features: {(pairs - single).abs().max().item()}"
+
+
 def _arg_max_tie(feats, query, frame, p_a, p_b, geo):
     """|difference| between the float64 correlation peaks nearest to the two candidate track points p_a, p_b (px) of
     `query` (x, y, t) in `frame`."""
