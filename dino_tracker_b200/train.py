@@ -24,6 +24,51 @@ def _head_struct(w1n, b1, w2n, b2):
     return hw
 
 
+def track_forward(tracker, emb_tpc, w1n, b1, w2n, b2, pts, tgt_slot):
+    """The tracker node's forward: the inference kernels with the maps kept.  Returns (out [B][2] in the caller's row
+    order, the head weights as passed to the kernels, saved) with saved = (emb, norms, pts_sorted, desc, dn, tgt_sorted,
+    maps, aux, order, slots): the per-map rows of pts_sorted / desc / dn / tgt_sorted / maps / aux are sorted by target
+    slot, row j being the caller's row order[j] -- the arguments ``dinotrk_track_backward`` takes."""
+    lib, dev, geom = tracker._lib, tracker._dev, tracker._geom
+    with torch.cuda.device(dev):
+        emb = emb_tpc.detach().contiguous()
+        N, P, C = emb.shape
+        B = pts.shape[0]
+        st = _lib.stream_ptr(dev)
+        norms = torch.empty(N, P, device=dev, dtype=torch.float32)
+        _lib.check(lib.dinotrk_token_norms(_lib.ptr(emb), _lib.ptr(norms), N, C, P, st), "token_norms")
+        feat = tracker.features_struct(emb, norms)
+        # maps grouped by target frame (the grouped GEMM's contract); results scattered back through `order`
+        tgt = tgt_slot.to(dev).long()
+        order = torch.argsort(tgt, stable=True)
+        tgt_sorted = tgt[order].to(torch.int32).contiguous()
+        uniq, counts = torch.unique_consecutive(tgt_sorted, return_counts=True)
+        pts_sorted = pts.to(device=dev, dtype=torch.float32)[order].contiguous()
+        slots = torch.arange(N, device=dev, dtype=torch.int32)
+        desc = torch.empty(B, C, device=dev, dtype=torch.float32)
+        dn = torch.empty(B, device=dev, dtype=torch.float32)
+        _lib.check(lib.dinotrk_sample_descriptors(_lib.ptr(emb), N, C, ctypes.byref(geom), _lib.ptr(pts_sorted), B,
+                                                  _lib.ptr(slots), N, 0, _lib.ptr(desc), _lib.ptr(dn), st), "sample_descriptors")
+        row0 = (torch.cumsum(counts, 0) - counts).to(torch.int32)
+        grp = torch.stack([uniq.to(torch.int32), row0, counts.to(torch.int32), row0]).contiguous()
+        n_groups = int(uniq.shape[0])
+        stride = lib.dinotrk_map_stride(ctypes.byref(geom))
+        maps = torch.empty(B, stride, device=dev, dtype=torch.float32)
+        ws_bytes = lib.dinotrk_corr_maps_workspace_bytes(B, n_groups, C)
+        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+        _lib.check(lib.dinotrk_corr_maps(ctypes.byref(feat), ctypes.byref(geom), _lib.ptr(desc), _lib.ptr(dn), _lib.ptr(grp[0]),
+                                         _lib.ptr(grp[1]), _lib.ptr(grp[2]), _lib.ptr(grp[3]), n_groups, B, int(counts.max()),
+                                         _lib.ptr(maps), _lib.ptr(ws), ws_bytes, st), "corr_maps")
+        hw = _head_struct(w1n, b1, w2n, b2)
+        out = torch.empty(B, 2, device=dev, dtype=torch.float32)
+        aux = torch.empty(B, 2, device=dev, dtype=torch.int32)
+        out_index = order.to(torch.int32).contiguous()
+        # full-map head kernel for every map: exact on both branches of tracker_head.py:84-98
+        _lib.check(lib.dinotrk_head(_lib.ptr(maps), B, ctypes.byref(geom), ctypes.byref(hw), _lib.ptr(out_index), _lib.ptr(out),
+                                    2, 1, _lib.ptr(aux), None, st), "head")
+    return out, hw, (emb, norms, pts_sorted, desc, dn, tgt_sorted, maps, aux, order, slots)
+
+
 class TrackFunction(torch.autograd.Function):
     """coords[B, 2] (normalised, the output of ``Tracker.forward``) = f(emb_tpc [N][P][C], w1n, b1, w2n, b2).
 
@@ -31,45 +76,9 @@ class TrackFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, emb_tpc, w1n, b1, w2n, b2, pts, tgt_slot, tracker):
-        lib, dev, geom = tracker._lib, tracker._dev, tracker._geom
-        with torch.cuda.device(dev):
-            emb = emb_tpc.detach().contiguous()
-            N, P, C = emb.shape
-            B = pts.shape[0]
-            st = _lib.stream_ptr(dev)
-            norms = torch.empty(N, P, device=dev, dtype=torch.float32)
-            _lib.check(lib.dinotrk_token_norms(_lib.ptr(emb), _lib.ptr(norms), N, C, P, st), "token_norms")
-            feat = tracker.features_struct(emb, norms)
-            # maps grouped by target frame (the grouped GEMM's contract); results scattered back through `order`
-            tgt = tgt_slot.to(dev).long()
-            order = torch.argsort(tgt, stable=True)
-            tgt_sorted = tgt[order].to(torch.int32).contiguous()
-            uniq, counts = torch.unique_consecutive(tgt_sorted, return_counts=True)
-            pts_sorted = pts.to(device=dev, dtype=torch.float32)[order].contiguous()
-            slots = torch.arange(N, device=dev, dtype=torch.int32)
-            desc = torch.empty(B, C, device=dev, dtype=torch.float32)
-            dn = torch.empty(B, device=dev, dtype=torch.float32)
-            _lib.check(lib.dinotrk_sample_descriptors(_lib.ptr(emb), N, C, ctypes.byref(geom), _lib.ptr(pts_sorted), B,
-                                                      _lib.ptr(slots), N, 0, _lib.ptr(desc), _lib.ptr(dn), st), "sample_descriptors")
-            row0 = (torch.cumsum(counts, 0) - counts).to(torch.int32)
-            grp = torch.stack([uniq.to(torch.int32), row0, counts.to(torch.int32), row0]).contiguous()
-            n_groups = int(uniq.shape[0])
-            stride = lib.dinotrk_map_stride(ctypes.byref(geom))
-            maps = torch.empty(B, stride, device=dev, dtype=torch.float32)
-            ws_bytes = lib.dinotrk_corr_maps_workspace_bytes(B, n_groups, C)
-            ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
-            _lib.check(lib.dinotrk_corr_maps(ctypes.byref(feat), ctypes.byref(geom), _lib.ptr(desc), _lib.ptr(dn), _lib.ptr(grp[0]),
-                                             _lib.ptr(grp[1]), _lib.ptr(grp[2]), _lib.ptr(grp[3]), n_groups, B, int(counts.max()),
-                                             _lib.ptr(maps), _lib.ptr(ws), ws_bytes, st), "corr_maps")
-            hw = _head_struct(w1n, b1, w2n, b2)
-            out = torch.empty(B, 2, device=dev, dtype=torch.float32)
-            aux = torch.empty(B, 2, device=dev, dtype=torch.int32)
-            out_index = order.to(torch.int32).contiguous()
-            # full-map head kernel for every map: exact on both branches of tracker_head.py:84-98
-            _lib.check(lib.dinotrk_head(_lib.ptr(maps), B, ctypes.byref(geom), ctypes.byref(hw), _lib.ptr(out_index), _lib.ptr(out),
-                                        2, 1, _lib.ptr(aux), None, st), "head")
+        out, hw, saved = track_forward(tracker, emb_tpc, w1n, b1, w2n, b2, pts, tgt_slot)
         ctx.tracker, ctx.hw = tracker, hw
-        ctx.save_for_backward(emb, norms, pts_sorted, desc, dn, tgt_sorted, maps, aux, order, slots)
+        ctx.save_for_backward(*saved)
         return out
 
     @staticmethod

@@ -80,6 +80,9 @@ def sample_descriptors(features: torch.Tensor, points: torch.Tensor, frames_set=
     ``frames_set`` (optional, N ints): ``features`` is then the WHOLE video and slot z of the
     frame set is ``features[frames_set[z]]`` -- the same values as sampling the gathered copy
     ``features[frames_set]`` (models/tracker.py:316), without materialising it.
+
+    The weights are always computed in fp32 (the leak is part of what the kernels reproduce);
+    float64 ``features`` are weighted and summed in float64.
     """
     _, C, h, w = features.shape
     N = features.shape[0] if frames_set is None else frames_set.shape[0]
@@ -103,7 +106,7 @@ def sample_descriptors(features: torch.Tensor, points: torch.Tensor, frames_set=
         (x0, y1, z1, (x1 - ix) * (iy - y0) * (iz - z0)),
         (x1, y1, z1, (ix - x0) * (iy - y0) * (iz - z0)),
     ]
-    out = torch.zeros(pts.shape[0], C, dtype=torch.float32, device=features.device)
+    out = torch.zeros(pts.shape[0], C, dtype=features.dtype, device=features.device)
     fs = None if frames_set is None else frames_set.long()
     for xi, yi, zi, wt in corners:
         ok = (xi >= 0) & (xi <= w - 1) & (yi >= 0) & (yi <= h - 1) & (zi >= 0) & (zi <= N - 1)
@@ -129,8 +132,8 @@ def corr_maps(source_desc: torch.Tensor, frames: torch.Tensor, target_idx: torch
         tf = frames_set.long()[tgt]
         B = source_desc.shape[0]
         _, C, h, w = frames.shape
-        corr = torch.empty(B, h, w, dtype=torch.float32, device=frames.device)
-        fnorm = torch.empty(B, h, w, dtype=torch.float32, device=frames.device)
+        corr = torch.empty(B, h, w, dtype=source_desc.dtype, device=frames.device)
+        fnorm = torch.empty(B, h, w, dtype=source_desc.dtype, device=frames.device)
         for f in torch.unique(tf).tolist():
             sel = tf == f
             corr[sel] = (source_desc[sel] @ frames[f].reshape(C, h * w)).reshape(-1, h, w)
@@ -160,11 +163,13 @@ def normalized_conv_weight(weight: torch.Tensor) -> torch.Tensor:
     return weight / w_sum
 
 
-def refiner(cost: torch.Tensor, head_sd: dict) -> torch.Tensor:
+def refiner(cost: torch.Tensor, head_sd: dict, normalized: bool = False) -> torch.Tensor:
     """models/networks/tracker_head.py:54-58: NormalizedConv2d(1,16,3,pad 1) -> ReLU ->
-    NormalizedConv2d(16,1,3,pad 1)."""
-    w1 = normalized_conv_weight(head_sd["cnn_refiner.0.weight"])
-    w2 = normalized_conv_weight(head_sd["cnn_refiner.2.weight"])
+    NormalizedConv2d(16,1,3,pad 1).  ``normalized=True``: the weights of ``head_sd`` are already
+    the normalised ones (what the CUDA head and its reverse pass take)."""
+    w1, w2 = head_sd["cnn_refiner.0.weight"], head_sd["cnn_refiner.2.weight"]
+    if not normalized:
+        w1, w2 = normalized_conv_weight(w1), normalized_conv_weight(w2)
     x = F.conv2d(cost, w1, bias=head_sd["cnn_refiner.0.bias"], stride=1, padding=1)
     x = torch.relu(x)
     return F.conv2d(x, w2, bias=head_sd["cnn_refiner.2.bias"], stride=1, padding=1)
@@ -181,18 +186,26 @@ def token_pixel_grid(geo: Geometry):
     return xs, ys
 
 
-def head_forward(cost_relu: torch.Tensor, head_sd: dict, geo: Geometry, return_aux: bool = False):
+def head_forward(cost_relu: torch.Tensor, head_sd: dict, geo: Geometry, return_aux: bool = False,
+                 amax=None, fb=None, normalized: bool = False):
     """models/networks/tracker_head.py:107-121 (+ soft_argmax :68-98, softmax :100-105).
 
     cost_relu: B x 1 x h x w (already ReLU'd, models/tracker.py:173).  Returns B x 2 in
     [-1, 1] (RangeNormalizer((W, H)), dst=(-1,1): x / (W-1, H-1), * 2, + (-1);
     data/dataset.py:33-35).
+
+    ``amax`` / ``fb`` (optional, B each): pin the arg-max token and the stability branch to
+    given decisions (e.g. a kernel's ``aux``) instead of taking them from this evaluation, so
+    that a higher-precision evaluation of a near-tie stays on the kernel's piecewise branch.
+    The aux dict then also holds this evaluation's own decisions ("own_argmax",
+    "own_fallback").  ``normalized``: see ``refiner``.
     """
     B, _, h, w = cost_relu.shape
     flat = cost_relu[:, 0].reshape(B, -1)
-    amax = torch.argmax(flat, dim=1)  # first maximal index
+    own_amax = torch.argmax(flat, dim=1)  # first maximal index
+    amax = own_amax if amax is None else amax.to(own_amax)
     row, col = amax // w, amax % w
-    z = refiner(cost_relu, head_sd)
+    z = refiner(cost_relu, head_sd, normalized)
     p = torch.softmax(z.reshape(B, 1, -1), dim=2).reshape(B, h, w)
     xs, ys = token_pixel_grid(geo)
     gy, gx = torch.meshgrid(ys, xs, indexing="ij")
@@ -202,7 +215,8 @@ def head_forward(cost_relu: torch.Tensor, head_sd: dict, geo: Geometry, return_a
     mask = torch.norm((grid[None] - centre[:, None, None]).to(torch.float32), dim=-1) <= geo.radius
     hm = p * mask
     s = hm.sum(dim=(1, 2))
-    fb = s < 1e-8
+    own_fb = s < 1e-8
+    fb = own_fb if fb is None else fb.to(own_fb)
     if fb.any():  # numerical-stability branch, tracker_head.py:87-94
         uniform = 1 / mask[fb].sum(dim=(1, 2))
         hm[fb] = (hm[fb] + uniform[:, None, None]) * mask[fb]
@@ -212,7 +226,8 @@ def head_forward(cost_relu: torch.Tensor, head_sd: dict, geo: Geometry, return_a
     out = point / norm
     out = (1 - (-1)) * out + (-1)
     if return_aux:
-        return out, {"argmax": amax, "fallback": fb, "logits": z[:, 0], "point_px": point}
+        return out, {"argmax": amax, "fallback": fb, "logits": z[:, 0], "point_px": point,
+                     "own_argmax": own_amax, "own_fallback": own_fb}
     return out
 
 
