@@ -2,6 +2,7 @@
 missing or fails to load, importing the product path raises."""
 import ctypes
 import os
+import struct
 import warnings
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_size_t, c_ulonglong, c_void_p
 
@@ -22,7 +23,8 @@ class HeadWeights(Structure):
 
 
 class Features(Structure):
-    _fields_ = [("tpc", c_void_p), ("norms", c_void_p), ("hi", c_void_p), ("lo", c_void_p), ("T", c_int), ("C", c_int)]
+    _fields_ = [("tpc", c_void_p), ("norms", c_void_p), ("hi", c_void_p), ("lo", c_void_p), ("T", c_int), ("C", c_int),
+                ("q8", c_void_p), ("q_fac", c_void_p), ("q_rho", c_void_p)]
 
 
 class VitConfig(Structure):
@@ -55,6 +57,7 @@ SIGNATURES = {
     "dinotrk_token_norms": (c_int, [_P, _P, c_int, c_int, c_int, _P]),
     "dinotrk_sample_descriptors": (c_int, [_P, c_int, c_int, POINTER(Geom), _P, c_int, _P, c_int, c_int, _P, _P, _P]),
     "dinotrk_split_fp16": (c_int, [_P, _P, _P, c_size_t, _P]),
+    "dinotrk_quantise_s8": (c_int, [_P, _P, c_size_t, c_int, c_int, _P, _P, _P, _P, _P]),
     "dinotrk_split_range": (c_int, [_P, c_size_t, _P, c_size_t, _P, _P]),
     "dinotrk_split_faithful": (c_int, [c_float, c_float, c_int]),
     "dinotrk_corr_track_workspace_bytes": (c_size_t, [c_int, c_int, c_int, POINTER(Geom)]),
@@ -72,11 +75,14 @@ SIGNATURES = {
     "dinotrk_infer_workspace_bytes": (c_size_t, [c_int, c_int, POINTER(Geom), c_int, c_int]),
     "dinotrk_infer_set_overlap": (c_int, [c_int]),
     "dinotrk_infer_set_path": (c_int, [c_int]),
+    "dinotrk_infer_set_coarse": (c_int, [c_int]),
     "dinotrk_infer_last_stats": (c_int, [POINTER(ctypes.c_longlong), c_int]),
     "dinotrk_infer_max_chunks": (c_size_t, [c_int, c_int, c_int]),
     "dinotrk_xw_coarse_keys_workspace_bytes": (c_size_t, [c_int, c_int, POINTER(Geom)]),
     "dinotrk_xw_coarse_keys": (c_int, [POINTER(Features), POINTER(Geom), _P, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, c_size_t,
                                        _P]),
+    "dinotrk_xw_coarse_keys_i8": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, _P, c_int, _P, _P, _P, c_int, _P, _P, _P, _P,
+                                          c_size_t, _P]),
     "dinotrk_xw_box_gemm": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P]),
     "dinotrk_infer_plan": (c_int, [c_int, c_int, c_int, _P, c_int, _P, _P, c_int, _P]),
     "dinotrk_infer": (c_int, [POINTER(Features), POINTER(Geom), POINTER(HeadWeights), _P, c_int, c_float, c_float,
@@ -183,14 +189,41 @@ def require_cuda(device):
     return dev
 
 
-def make_features(tpc, norms, hi=None, lo=None):
+def make_features(tpc, norms, hi=None, lo=None, quant=None):
+    """quant: (q8, fac, rho_f) of quantise_features, or None (the anchor phase's coarse pass then runs on fp16)."""
     f = Features()
     f.tpc, f.norms = tpc.data_ptr(), norms.data_ptr()
     f.hi = hi.data_ptr() if hi is not None else None
     f.lo = lo.data_ptr() if lo is not None else None
     f.T, f.C = tpc.shape[0], tpc.shape[2]
-    f._keep = (tpc, norms, hi, lo)  # keep the tensors alive as long as the struct
+    if quant is not None:
+        f.q8, f.q_fac, f.q_rho = (t.data_ptr() for t in quant)
+    f._keep = (tpc, norms, hi, lo, quant)  # keep the tensors alive as long as the struct
     return f
+
+
+def quantise_s8(x, norms, rows_per_group, stream):
+    """int8 rows of a [..., C] fp32 tensor for the coarse pass (include/dinotrk.h: dinotrk_quantise_s8): (q int8 [..., C],
+    fac [...], rho [...], rho_max [groups of rows_per_group rows])."""
+    C = x.shape[-1]
+    rows = x.numel() // C
+    q = torch.empty(x.shape, device=x.device, dtype=torch.int8)
+    fac = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
+    rho = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
+    rho_max = torch.empty(-(-rows // rows_per_group), device=x.device, dtype=torch.float32)
+    check(load().dinotrk_quantise_s8(ptr(x), ptr(norms), rows, C, rows_per_group, ptr(q), ptr(fac), ptr(rho), ptr(rho_max),
+                                     stream), "quantise_s8")
+    return q, fac, rho, rho_max
+
+
+def quantise_features(tpc, norms, stream):
+    """(q8 [T][P][C], fac [T][P], rho_f [T]) of a [T][P][C] feature video: the int8 operands of the anchor phase's coarse
+    pass, or None where that pass cannot run (C not a multiple of 16 or above 1040)."""
+    T, P, C = tpc.shape
+    if C % 16 or C > 1040:
+        return None
+    q, fac, _, rho_f = quantise_s8(tpc, norms, P, stream)
+    return q, fac, rho_f
 
 
 def split_range(tpc, norms, stream):
@@ -245,10 +278,12 @@ def profile_collect():
 def infer_stats():
     """{anchor-phase maps, finished by the exact-window path, re-done by the full-map path, pipeline, contraction} of the
     last infer."""
-    a = (ctypes.c_longlong * 6)()
-    check(load().dinotrk_infer_last_stats(a, 6), "infer_last_stats")
+    a = (ctypes.c_longlong * 8)()
+    check(load().dinotrk_infer_last_stats(a, 8), "infer_last_stats")
+    rho_f = struct.unpack("<f", struct.pack("<I", int(a[7])))[0]
     return {"anchor_maps": int(a[0]), "exact_window": int(a[1]), "full_map": int(a[2]), "pipeline": "exact-window" if a[3] else "full-map",
-            "full_map_by_certificate": int(a[4]), "contraction": "fp16x3" if a[5] else "fp32"}
+            "full_map_by_certificate": int(a[4]), "contraction": "fp16x3" if a[5] else "fp32",
+            "coarse": "int8" if a[6] else "fp16", "coarse_rho_f": rho_f}
 
 
 def launch_count():

@@ -9,10 +9,12 @@ constexpr int STREAM_MAX_M = 8;  // groups with at most this many descriptors us
 struct FeatView {
   const float* tpc; const float* norms; const void* hi; const void* lo;
   int T, C, P;
+  const void* q8; const float* q_fac; const float* q_rho;   // int8 coarse operands (optional, dinotrk_features)
   bool tensor() const { return hi != nullptr && lo != nullptr; }
+  bool s8() const { return q8 != nullptr && q_fac != nullptr && q_rho != nullptr; }
 };
 static inline FeatView make_view(const dinotrk_features& f, const dinotrk_geom& g) {
-  return FeatView{f.tpc, f.norms, f.hi, f.lo, f.T, f.C, g.h * g.w};
+  return FeatView{f.tpc, f.norms, f.hi, f.lo, f.T, f.C, g.h * g.w, f.q8, f.q_fac, f.q_rho};
 }
 
 constexpr int CORR_TILE = 256;   // token tile of the tensor-core correlation GEMM (= TC_BN); unit of the tile maxima

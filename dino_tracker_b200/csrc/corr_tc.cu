@@ -10,6 +10,7 @@
 #include "common.cuh"
 #include "corr.cuh"
 #include "tcgemm.cuh"
+#include "xwin.cuh"
 
 namespace dtk {
 
@@ -44,13 +45,19 @@ static CUtensorMapSwizzle swizzle_of(int bytes) {
   return bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
 }
 
+// (8-bit operands travel as UINT8: TMA copies bytes, the wgmma instruction gives them their signed type)
+static CUtensorMapDataType tmap_type(int elem) {
+  return elem == TMAP_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : elem == TMAP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+       : elem == TMAP_S8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+static int elem_bytes_of(int elem) { return elem == TMAP_F32 ? 4 : elem == TMAP_S8 ? 1 : 2; }
+
 static int encode(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
                   const cuuint32_t* box, int elem, int swizzle = 128) {
   EncodeTiledFn fn = get_encode();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return DINOTRK_ECUDA; }
   cuuint32_t estr[3] = {1, 1, 1};
-  CUtensorMapDataType dt = elem == TMAP_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                         : elem == TMAP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMapDataType dt = tmap_type(elem);
   CUresult r = fn(map, dt, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle_of(swizzle), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return DINOTRK_ECUDA; }
@@ -59,7 +66,7 @@ static int encode(CUtensorMap* map, const void* base, int rank, const cuuint64_t
 
 int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols,
                  int elem, uint64_t ld, int swizzle) {
-  const int elem_bytes = elem == TMAP_F32 ? 4 : 2;
+  const int elem_bytes = elem_bytes_of(elem);
   if (ld == 0) ld = cols;
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {ld * (uint64_t)elem_bytes};
@@ -68,7 +75,7 @@ int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t col
 }
 int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t batch, uint64_t rows, uint64_t cols, uint32_t box_rows,
                  uint32_t box_cols, int elem, uint64_t ld) {
-  const int elem_bytes = elem == TMAP_F32 ? 4 : 2;
+  const int elem_bytes = elem_bytes_of(elem);
   if (ld == 0) ld = cols;
   cuuint64_t dims[3] = {cols, rows, batch};
   cuuint64_t strides[2] = {ld * (uint64_t)elem_bytes, rows * ld * (uint64_t)elem_bytes};
@@ -84,8 +91,7 @@ int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], con
   cuuint64_t s[3] = {strides_bytes[0], strides_bytes[1], strides_bytes[2]};
   cuuint32_t b[4] = {box[0], box[1], box[2], box[3]};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUtensorMapDataType dt = elem == TMAP_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                         : elem == TMAP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMapDataType dt = tmap_type(elem);
   CUresult r = fn(map, dt, 4, const_cast<void*>(base), d, s, b, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle_of(swizzle), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (4-d) failed (%d)", (int)r); return DINOTRK_ECUDA; }
@@ -118,6 +124,23 @@ int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t 
                                          reinterpret_cast<uint2*>(lo), n4);
   DTK_LAUNCHED();
   return DINOTRK_OK;
+}
+
+// int8 operands of the coarse pass (xw_quant_row): one warp per row; rho_max[row / rows_per_group] = largest rho of the
+// group (float bits: non-negative floats order like their bits; zeroed by the caller)
+__global__ void __launch_bounds__(256)
+quant_s8_kernel(const float* __restrict__ x, const float* __restrict__ norms, size_t rows, int C, int rows_per_group,
+                int8_t* __restrict__ q, float* __restrict__ fac, float* __restrict__ rho, unsigned* __restrict__ rho_max) {
+  const size_t nw = (size_t)gridDim.x * 8;
+  for (size_t r = (size_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < rows; r += nw) {
+    const float* xr = x + r * C;
+    const float v = xw_quant_row([&](int k) { return __ldg(reinterpret_cast<const float4*>(xr + k)); }, C, norms[r],
+                                 q + r * C, fac + r);
+    if ((threadIdx.x & 31) == 0) {
+      if (rho) rho[r] = v;
+      if (rho_max) atomicMax(rho_max + r / rows_per_group, __float_as_uint(v));
+    }
+  }
 }
 
 // range[0] = max |x| (NaN counts as above every bound), range[1] = smallest non-zero norm; both as float bits, which order like
@@ -278,4 +301,20 @@ extern "C" int dinotrk_split_range(const float* x, size_t n, const float* norms,
 
 extern "C" int dinotrk_split_faithful(float max_abs, float min_norm, int C) {
   return (max_abs <= SPLIT_MAX_ABS && min_norm >= split_min_norm(C)) ? 1 : 0;
+}
+
+extern "C" int dinotrk_quantise_s8(const float* x, const float* norms, size_t rows, int C, int rows_per_group, void* q, float* fac,
+                                   float* rho, float* rho_max, void* stream) {
+  DTK_CHECK_ARG(x && norms && q && fac, "quantise_s8: null pointer");
+  DTK_CHECK_ARG(C > 0 && C % 16 == 0 && rows_per_group > 0, "quantise_s8: C must be a positive multiple of 16");
+  if (rows == 0) return DINOTRK_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rho_max) DTK_CUDA(cudaMemsetAsync(rho_max, 0, ((rows + rows_per_group - 1) / rows_per_group) * sizeof(float), st));
+  size_t grid = (rows + 7) / 8;
+  if (grid > (size_t)num_sms() * 16) grid = (size_t)num_sms() * 16;
+  ProfRange pr(PROF_MISC, st);
+  quant_s8_kernel<<<(unsigned)grid, 256, 0, st>>>(x, norms, rows, C, rows_per_group, reinterpret_cast<int8_t*>(q), fac, rho,
+                                                  reinterpret_cast<unsigned*>(rho_max));
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
 }

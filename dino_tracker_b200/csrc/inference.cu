@@ -152,9 +152,24 @@ __global__ void sample_anchor_kernel(const float* __restrict__ tpc, int T, int C
 // i - i0 + 1 -- does not depend on the anchor frame a unless the fp32 round trip of the slot index (utils.py:96-99) leaks
 // weight onto slot 0.  So every (n, i) is sampled ONCE (fp16 hi / lo halves + norm, what the tensor-path GEMMs consume) and
 // flagged if slot 0 takes part; per chunk, unflagged items are row copies, flagged ones are sampled as before.
+// int8 row of the coarse pass from a descriptor's hi / lo halves and norm, which the block has just stored (plain loads,
+// not the read-only path): warp 0 quantises d = hi + lo; returns rho on lane 0 of warp 0
+__device__ __forceinline__ float quant_desc(const __half* hi, const __half* lo, int C, const float* norm, int8_t* q, float* fac) {
+  __syncthreads();   // the block's hi / lo stores and the norm (sample_point) are visible
+  if (threadIdx.x >= 32) return 0.f;
+  const float nrm = *norm;
+  return xw_quant_row([&](int k) {
+    const uint2 a = *reinterpret_cast<const uint2*>(hi + k), b = *reinterpret_cast<const uint2*>(lo + k);
+    const float2 a0 = __half22float2(*reinterpret_cast<const __half2*>(&a.x)), a1 = __half22float2(*reinterpret_cast<const __half2*>(&a.y));
+    const float2 b0 = __half22float2(*reinterpret_cast<const __half2*>(&b.x)), b1 = __half22float2(*reinterpret_cast<const __half2*>(&b.y));
+    return make_float4(a0.x + b0.x, a0.y + b0.y, a1.x + b1.x, a1.y + b1.y);
+  }, C, nrm, q, fac);
+}
+
 __global__ void sample_unique_kernel(const float* __restrict__ tpc, int T, int C, int P, int h, int w, PointAffine pa,
                                      const float* __restrict__ traj, int frame_batch, __half* __restrict__ u_hi,
-                                     __half* __restrict__ u_lo, float* __restrict__ u_norm, int* __restrict__ u_flag) {
+                                     __half* __restrict__ u_lo, float* __restrict__ u_norm, int* __restrict__ u_flag,
+                                     int8_t* __restrict__ u_q8, float* __restrict__ u_fac, float* __restrict__ u_rho) {
   const int u = blockIdx.x;                 // n * T + i
   const int i = u % T;
   const int i0 = (i / frame_batch) * frame_batch, e = min(i0 + frame_batch, T);
@@ -170,9 +185,15 @@ __global__ void sample_unique_kernel(const float* __restrict__ tpc, int T, int C
   const int f0 = i0 + c.z0 - 1;
   const int f1 = c.z1 < 0 ? -1 : i0 + c.z1 - 1;
   sample_point(tpc, C, P, c, f0, f1, nullptr, u_norm + u, u_hi + (size_t)u * C, u_lo + (size_t)u * C);
+  if (u_q8) {   // (+ the int8 row of the coarse pass)
+    const float r = quant_desc(u_hi + (size_t)u * C, u_lo + (size_t)u * C, C, u_norm + u, u_q8 + (size_t)u * C, u_fac + u);
+    if (threadIdx.x == 0) u_rho[u] = r;
+  }
 }
 
-// descriptors (fp16 hi / lo + norm) and output slots of one chunk of anchor work items, from the unique samples
+// descriptors (fp16 hi / lo + norm; with desc_q8: + the int8 row, its factor and the map's coarse bound eps, from the
+// descriptor's residual and its anchor frame's rho_f) and output slots of one chunk of anchor work items, from the unique
+// samples
 __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C, int P, int h, int w, PointAffine pa,
                                      const float* __restrict__ traj, const int* __restrict__ qlist, int N,
                                      const int* __restrict__ grp_frame, const int* __restrict__ grp_map0,
@@ -180,7 +201,10 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
                                      const __half* __restrict__ u_hi, const __half* __restrict__ u_lo,
                                      const float* __restrict__ u_norm, const int* __restrict__ u_flag,
                                      float* __restrict__ dnorm, int* __restrict__ out_index, __half* __restrict__ desc_hi,
-                                     __half* __restrict__ desc_lo) {
+                                     __half* __restrict__ desc_lo, const int8_t* __restrict__ u_q8,
+                                     const float* __restrict__ u_fac, const float* __restrict__ u_rho,
+                                     const float* __restrict__ rho_f, int8_t* __restrict__ desc_q8, float* __restrict__ desc_fac,
+                                     float* __restrict__ desc_eps) {
   const int j = blockIdx.x;
   int lo = 0, hi = n_groups - 1;
   while (lo < hi) {
@@ -200,6 +224,12 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
     uint4* dl = reinterpret_cast<uint4*>(desc_lo + (size_t)j * C);
     for (int k = threadIdx.x; k < C / 8; k += blockDim.x) { dh[k] = __ldg(sh + k); dl[k] = __ldg(sl + k); }
     if (threadIdx.x == 0) dnorm[j] = u_norm[u];
+    if (desc_q8) {
+      const uint4* sq = reinterpret_cast<const uint4*>(u_q8 + u * C);
+      uint4* dq = reinterpret_cast<uint4*>(desc_q8 + (size_t)j * C);
+      for (int k = threadIdx.x; k < C / 16; k += blockDim.x) dq[k] = __ldg(sq + k);
+      if (threadIdx.x == 0) { desc_fac[j] = u_fac[u]; desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[a]); }
+    }
     return;
   }
   const int i0 = (i / frame_batch) * frame_batch, e = min(i0 + frame_batch, T);
@@ -210,6 +240,10 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
   int f0 = c.z0 == 0 ? a : i0 + c.z0 - 1;
   int f1 = c.z1 < 0 ? -1 : (c.z1 == 0 ? a : i0 + c.z1 - 1);
   sample_point(tpc, C, P, c, f0, f1, nullptr, dnorm + j, desc_hi + (size_t)j * C, desc_lo + (size_t)j * C);
+  if (desc_q8) {
+    const float r = quant_desc(desc_hi + (size_t)j * C, desc_lo + (size_t)j * C, C, dnorm + j, desc_q8 + (size_t)j * C, desc_fac + j);
+    if (threadIdx.x == 0) desc_eps[j] = xw_eps_s8(r, rho_f[a]);
+  }
 }
 
 // ---------------------------------------------------------------------------------- phase D
@@ -441,7 +475,14 @@ static XwAsync* xw_async() {
   return xa.state == 1 ? &xa : nullptr;
 }
 static int g_xw_path = -1;                     // -1: automatic (DTK_XW or on), 0: full-map path only, 1: exact-window path
-static long long g_infer_stats[6] = {0, 0, 0, 0, 0, 0};   // anchor-phase maps | on the exact-window path | queued | path used | queued by the certificate | tensor-core contraction
+static int g_xw_coarse = -1;                   // -1: automatic, 0: fp16 coarse pass, 1: int8 coarse pass
+// anchor-phase maps | on the exact-window path | queued | path used | queued by the certificate | tensor-core contraction |
+// int8 coarse pass | bits of the largest per-frame int8 residual
+static long long g_infer_stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+// the probe chunk queues more than this fraction of its maps on the int8 coarse pass: the rest of the phase runs the fp16
+// pass.  A queued map costs a full-map split-precision GEMM, ~3 fp16 coarse passes, while the int8 pass saves about half
+// of one per map: int8 loses above ~1/6 extra queued maps.  1/16 leaves a wide margin.
+constexpr int XW_S8_PROBE_QUEUE_DIV = 16;
 
 }  // namespace dtk
 
@@ -455,9 +496,15 @@ int dinotrk_infer_set_path(int path) {
   return DINOTRK_OK;
 }
 
+int dinotrk_infer_set_coarse(int mode) {
+  DTK_CHECK_ARG(mode >= -1 && mode <= 1, "infer_set_coarse: -1 (automatic), 0 (fp16) or 1 (int8)");
+  g_xw_coarse = mode;
+  return DINOTRK_OK;
+}
+
 int dinotrk_infer_last_stats(long long* out, int n) {
   DTK_CHECK_ARG(out && n >= 4, "infer_last_stats: need at least 4 slots");
-  for (int i = 0; i < (n < 6 ? n : 6); ++i) out[i] = g_infer_stats[i];
+  for (int i = 0; i < (n < 8 ? n : 8); ++i) out[i] = g_infer_stats[i];
   return DINOTRK_OK;
 }
 
@@ -563,6 +610,8 @@ size_t dinotrk_infer_workspace_bytes(int T, int C, const dinotrk_geom* g, int N,
   x += xw_chunk_bytes((int)chx, (int)max_cells_chunk, cdiv(g->h * g->w, XW_TILE), gcap);
   b += XW_RING * x;
   b += 2 * align_up((size_t)N * T * C * 2, 256) + 2 * align_up((size_t)N * T * 4, 256);   // unique descriptors (hi, lo, norm, flag)
+  b += align_up((size_t)N * T * C, 256) + 2 * align_up((size_t)N * T * 4, 256);           // their int8 rows, factors, residuals
+  b += XW_RING * (align_up(chx * C, 256) + 2 * align_up(chx * 4, 256));                   // chunk int8 rows, factors, eps
   b += align_up((size_t)T * g->h * g->w * 4, 256) + 256;                                  // reciprocal token norms, smallest norm
   b += align_up((size_t)N * T * nb * 16 + 64, 256);                         // cells of all chunks
   b += align_up(infer_max_chunks(T, N, ch) * (gcap + 1) * 4, 256);         // coarse tile prefixes per chunk
@@ -659,18 +708,24 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   int* d_groups = ar.take<int>(max_chunks * 5 * gcap);
   int* d_cnt = ar.take<int>(T);
   int* d_qlist = ar.take<int>((size_t)T * N);
-  struct XwSet { float* norm; float* split; int* out_index; XwChunk xc; } xr[XW_RING];
+  struct XwSet { float* norm; float* split; int* out_index; int8_t* q8; float* fac; float* eps; XwChunk xc; } xr[XW_RING];
   const int n_tiles_map = cdiv(P, XW_TILE);     // coarse keys per map
   __half* u_hi = ar.take<__half>((size_t)N * T * C);
   __half* u_lo = ar.take<__half>((size_t)N * T * C);
   float* u_norm = ar.take<float>((size_t)N * T);
   int* u_flag = ar.take<int>((size_t)N * T);
+  int8_t* u_q8 = ar.take<int8_t>((size_t)N * T * C);
+  float* u_fac = ar.take<float>((size_t)N * T);
+  float* u_rho = ar.take<float>((size_t)N * T);
   float* d_rnorms = ar.take<float>((size_t)T * P);
   unsigned* d_minnorm = ar.take<unsigned>(4);
   for (int k = 0; k < XW_RING; ++k) {
     xr[k].norm = ar.take<float>(ch);
     xr[k].split = ar.take<float>(corr_tc_workspace_bytes(ch, C) / 4);
     xr[k].out_index = ar.take<int>(ch);
+    xr[k].q8 = ar.take<int8_t>((size_t)ch * C);
+    xr[k].fac = ar.take<float>(ch);
+    xr[k].eps = ar.take<float>(ch);
     XwChunk& x = xr[k].xc;
     x.key1 = ar.take<unsigned long long>((size_t)ch * n_tiles_map);
     x.max2 = ar.take<float>((size_t)ch * n_tiles_map);
@@ -791,6 +846,8 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     if (xa && n_chunks_A > 0)
       DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING, d_cntA, (size_t)n_chunks_A * sizeof(int), cudaMemcpyDeviceToHost, st));
     DTK_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
+    std::vector<float> rho_f(fv.s8() ? T : 0);
+    if (fv.s8()) DTK_CUDA(cudaMemcpyAsync(rho_f.data(), fv.q_rho, (size_t)T * sizeof(float), cudaMemcpyDeviceToHost, st));
     DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: sizes of the anchor work lists
     if (use_xw) {   // a token below the split's faithful range (a zero one included) voids the coarse pass's error bound
       float mn;
@@ -808,6 +865,20 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     for (int a = 0; a < T; ++a) maps_C += (long long)cnt[a] * T;
     g_infer_stats[0] = maps_C; g_infer_stats[1] = 0; g_infer_stats[2] = 0; g_infer_stats[3] = use_xw ? 1 : 0; g_infer_stats[4] = 0;
     g_infer_stats[5] = tensor ? 1 : 0;
+    // coarse pass of the exact-window pipeline (decided once use_xw is final): int8 when the features carry their int8
+    // operands (forced: required), unless a frame's residual makes the bound too loose (automatic mode; below: or the probe
+    // chunk queues too many maps)
+    DTK_CHECK_ARG(g_xw_coarse != 1 || !use_xw || fv.s8(), "infer: int8 coarse pass forced without the int8 features");
+    bool s8 = use_xw && fv.s8() && g_xw_coarse != 0;
+    DTK_CHECK_ARG(!s8 || (C % 16 == 0 && C <= XW_S8_MAX_C), "infer: int8 coarse pass needs C %% 16 == 0 and C <= %d", XW_S8_MAX_C);
+    {
+      float rho_max = 0.f;
+      for (float r : rho_f) rho_max = std::max(rho_max, r);
+      if (g_xw_coarse < 0 && !(rho_max <= XW_S8_RHO_MAX)) s8 = false;
+      unsigned bits;
+      memcpy(&bits, &rho_max, sizeof(bits));
+      g_infer_stats[6] = s8 ? 1 : 0; g_infer_stats[7] = bits;
+    }
     size_t k0 = 0;            // first chunk of the full-map pipeline (> 0 after an exact-window probe)
     bool planned = false;
     if (use_xw) {
@@ -851,7 +922,8 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
           gather_anchor_kernel<<<cm.used, SAMPLE_THREADS, 0, sb>>>(tpc, T, C, P, g->h, g->w, pa, traj, d_qlist, N, gp.f, gp.map0,
                                                                   gp.item, cm.n_groups, fb, u_hi, u_lo, u_norm, u_flag, x.norm,
                                                                   x.out_index, reinterpret_cast<__half*>(hi_of(x, cm.used)),
-                                                                  reinterpret_cast<__half*>(lo_of(x, cm.used)));
+                                                                  reinterpret_cast<__half*>(lo_of(x, cm.used)), u_q8, u_fac, u_rho,
+                                                                  fv.q_rho, s8 ? x.q8 : nullptr, x.fac, x.eps);
           DTK_LAUNCHED();
         }
         if (ovl) DTK_CUDA(cudaEventRecord(xa->sample[k % XW_RING], sb));
@@ -900,7 +972,8 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       };
       {   // every (query, source frame) descriptor once; the per-chunk kernels copy rows
         ProfRange pr(PROF_SAMPLE, st);
-        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, u_hi, u_lo, u_norm, u_flag);
+        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, u_hi, u_lo, u_norm, u_flag,
+                                                               s8 ? u_q8 : nullptr, u_fac, u_rho);
         DTK_LAUNCHED();
       }
       if (ovl) {   // (the fork above was recorded before this launch: make the sampling stream wait for it)
@@ -915,11 +988,14 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         const Grp gp = grp_of(k);
         const XwCells cells = cells_of(k);
         if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, xa->sample[k % XW_RING], 0));
+        const float* eps = s8 ? x.eps : nullptr;   // (nullptr: the fp16 pass's XW_EPS)
         if ((rc = launch_xw_coarse(fv, hi_of(x, cm.used), cm.used, x.norm, gp.f, gp.r, gp.m, gp.map0, d_tiles + k * (gcap + 1),
-                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, d_rnorms))) return rc;
-        if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used, split_min_norm(C)))) return rc;
+                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, d_rnorms, s8 ? x.q8 : nullptr,
+                                   x.fac))) return rc;
+        if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used, split_min_norm(C), eps))) return rc;
         if ((rc = launch_xw_gemm(fv, *g, hi_of(x, cm.used), lo_of(x, cm.used), cm.used, cells, x.xc, st))) return rc;
-        if ((rc = launch_xw_head(fv, *g, *hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups)))
+        if ((rc = launch_xw_head(fv, *g, *hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups,
+                                 eps)))
           return rc;
         DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * (k % XW_RING), x.xc.slow_cnt + cm.n_groups, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
         DTK_CUDA(cudaEventRecord(xa->done[k % XW_RING], st));
@@ -927,6 +1003,10 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
           if ((rc = finish(0))) return rc;
           n_finished = 1;
           if (g_infer_stats[4] * 4 > (long long)cm.used) { k_end = 1; break; }
+          if (s8 && g_xw_coarse < 0 && g_infer_stats[2] * XW_S8_PROBE_QUEUE_DIV > (long long)cm.used) {
+            s8 = false;                   // the rest of the phase on the fp16 coarse pass
+            g_infer_stats[6] = 0;
+          }
         }
         if (k + 1 < metas.size() && (rc = enqueue_sample_x(k + 1))) return rc;
         while (n_finished + 2 <= k)
@@ -946,6 +1026,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       }
       k0 = k_end;                       // switched: chunks k0.. on the full-map pipeline below (same plan)
       g_infer_stats[3] = 0;
+      g_infer_stats[6] = 0;
     }
     if (!planned) {
       plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host);

@@ -19,6 +19,8 @@
 //   TF32   : single pass on fp32 data (the tensor core reads the top 19 bits)
 //   BF16   : single pass on bf16 data
 //   F16    : single pass on fp16 data (11-bit significand like TF32, twice its rate)
+//   S8     : single pass on signed 8-bit data (twice the F16 rate), exact int32 accumulators; BN = 256 and fragment
+//            epilogues only (they receive the int32 accumulators)
 // Work = grouped tiles: group g covers A rows [row0[g], row0[g] + m[g]) against B batch item batch[g];
 // m-tiles are numbered through the prefix array tile_start[] (device), n-tiles cover N.
 #pragma once
@@ -29,7 +31,7 @@
 
 namespace dtk {
 
-enum class TcMode { TF32X3 = 0, TF32 = 1, BF16 = 2, F16X3 = 3, F16 = 4 };
+enum class TcMode { TF32X3 = 0, TF32 = 1, BF16 = 2, F16X3 = 3, F16 = 4, S8 = 5 };
 
 constexpr int TC_BM = 128, TC_BN = 256;   // TC_BN: default N tile (template parameter BN overrides it)
 constexpr int TC2_BM = 256;               // M tile of a CTA pair
@@ -40,7 +42,7 @@ constexpr int TC_SMEM_MAX = 227 * 1024;
 template <TcMode MODE, int BN = TC_BN>
 struct TcCfg {
   static_assert(BN == 64 || BN == 128 || BN == 256, "N tile must be 64, 128 or 256");
-  static constexpr int kElem = (MODE == TcMode::BF16 || MODE == TcMode::F16X3 || MODE == TcMode::F16) ? 2 : 4;
+  static constexpr int kElem = MODE == TcMode::S8 ? 1 : (MODE == TcMode::BF16 || MODE == TcMode::F16X3 || MODE == TcMode::F16) ? 2 : 4;
   static constexpr int kBK = 128 / kElem;                         // elements per 128-byte swizzle row
   static constexpr int kOps = (MODE == TcMode::TF32X3 || MODE == TcMode::F16X3) ? 2 : 1;   // hi (+ lo) tiles per operand
   static constexpr int kMmaK = 32 / kElem;                        // K per wgmma
@@ -52,6 +54,9 @@ struct TcCfg {
   static_assert(kStages >= 2, "shared memory ring too shallow");
   static constexpr int kSmem = kStages * kStageBytes + kFixed;
   static constexpr bool kTF32 = (MODE == TcMode::TF32X3 || MODE == TcMode::TF32);
+  static constexpr bool kS8 = MODE == TcMode::S8;
+  using Acc = std::conditional_t<kS8, int, float>;                // accumulator element
+  static_assert(!kS8 || BN == 256, "8-bit mode: m64n256k32 only");
 };
 
 // Epilogues that declare `static constexpr bool kCoalesced = true` are called as vec4(g, row, col, float4) with lanes
@@ -68,7 +73,7 @@ template <class E> struct EpiPrefetch<E, std::enable_if_t<E::kPrefetch>> { stati
 // Fragment epilogues (`static constexpr bool kFragment = true`) skip the shared-memory round trip: right after the tile's
 // last wgmma has completed, every consumer thread calls
 //   fragment(g, r, m, n0, fc, acc)
-// with its own accumulator registers: acc[4 i + {0, 1}] are row r, acc[4 i + {2, 3}] row r + 8 (rows inside group g, which
+// with its own accumulator registers (float, or int in S8 mode): acc[4 i + {0, 1}] are row r, acc[4 i + {2, 3}] row r + 8 (rows inside group g, which
 // has m rows: rows >= m are padding), columns n0 + 8 i + fc + {0, 1}.  The 4 lanes of a quad (lane & 3) hold the same
 // two rows.  No barrier, no shared memory.
 template <class E, class = void> struct EpiFragment { static constexpr bool value = false; };
@@ -92,6 +97,7 @@ template <TcMode MODE, class Epi, int BN, bool PAIR>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi,
                                              const CUtensorMap& tmB_lo, const TcProblem& pb, const Epi& epi) {
   using Cfg = TcCfg<MODE, BN>;
+  static_assert(!Cfg::kS8 || EpiFragment<Epi>::value, "8-bit mode: fragment epilogues only");
   constexpr int TM = PAIR ? TC2_BM : TC_BM;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -172,12 +178,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
       }
     };
     int stage = 0, phase = 0;
-    float acc[BN / 2];
+    typename Cfg::Acc acc[BN / 2];
     for (int tile = unit; tile < total_tiles; tile += n_units) {
       int g, m0, n0;
       decode(tile, g, m0, n0);
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
       int prev = -1;
       for (int kb = 0; kb < KB; ++kb) {
         tc::mbar_wait(&full[stage], phase);
@@ -188,7 +194,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
         for (int ks = 0; ks < Cfg::kBK / Cfg::kMmaK; ++ks) {
           const uint32_t koff = ks * 32;  // bytes inside the 128-byte swizzle row
           const uint64_t a_hi = tc::smem_desc_sw128(sa + koff), b_hi = tc::smem_desc_sw128(sb + koff);
-          if (Cfg::kOps == 2) {
+          if constexpr (Cfg::kS8) {
+            tc::wgmma_ss_s8<BN>(acc, a_hi, b_hi, 1u);
+          } else if (Cfg::kOps == 2) {
             const uint64_t a_lo = tc::smem_desc_sw128(sa + Cfg::kABytes + koff);
             const uint64_t b_lo = tc::smem_desc_sw128(sb + Cfg::kBBytes + koff);
             // small terms first, then the dominant hi*hi
@@ -212,7 +220,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
       const int rbase = m0 + cw * 64;        // row (inside the group) of the warpgroup's first row
       if constexpr (EpiFragment<Epi>::value) {
         epi.fragment(g, rbase + fr, pb.grp_m[g], n0, fc, acc);
-      } else {
+      } else if constexpr (!Cfg::kS8) {
         // ---- epilogue: 32-column blocks through shared memory ----
         const int r = rbase + t;
         const bool row_ok = t < 64 && r < pb.grp_m[g];

@@ -9,10 +9,11 @@
 namespace dtk {
 
 // ====================================================================================================== 1. coarse GEMM
-// Epilogue of the single-pass fp16 GEMM over the `hi` halves: nothing is stored per token.  Per (map, 128-token tile), two
+// Epilogue of the single-pass GEMM (int8 operands, or fp16 over the `hi` halves): nothing is stored per token.  Per (map, 128-token tile), two
 // per 256-column GEMM tile: key1 = bits(max) << 32 | (0x7fffffff - first token holding it), max2 = second largest value
 // (>= 0).  Values are the same expression as the exact path, relu(acc / max(|d| |F|, 1e-8)), with a fast division (its
-// error is part of XW_EPS).
+// error is part of XW_EPS).  The int8 pass forms the same statistics of acc * fac_x * fac_d from its exact int32
+// accumulators (converted exactly: C <= XW_S8_MAX_C).
 //
 // A fragment epilogue (tcgemm.cuh): it works on the accumulator registers of all eight consumer warps, with no shared
 // memory and no barrier.  Per element only u = acc * (1 / |F|) is formed; the row's positive factor 1 / |d| (and the ReLU)
@@ -22,10 +23,13 @@ namespace dtk {
 // order, then the 4 lanes of the quad merge theirs by shuffles.
 constexpr int XW_GEMM_BN = 2 * XW_TILE;   // N tile of the coarse GEMM (m64n256 per consumer warpgroup)
 
+template <class Acc>   // float: fp16 pass, int: int8 pass
 struct CoarseEpi {
   static constexpr bool kFragment = true;
-  const float* rnorms;     // [T][P] 1 / |F[t][p]| (xw_rnorm_kernel; every norm is >= XW_MIN_NORM on this path)
-  const float* desc_norm;
+  static constexpr bool kS8 = std::is_same<Acc, int>::value;
+  const float* rnorms;     // [T][P] token factor: 1 / |F[t][p]| (xw_rnorm_kernel; every norm is >= XW_MIN_NORM on this
+                           // path), int8 pass: s_x / |F| (q_fac)
+  const float* desc_norm;  // row factor 1 / max(|d|, XW_MIN_NORM) (fp16 pass), desc_norm[row] itself (int8 pass: s_d / |d|)
   const int* grp_frame;
   const int* grp_row0;
   const int* grp_map0;
@@ -48,7 +52,7 @@ struct CoarseEpi {
   // folds key tile kh of the thread's two rows into s[0], s[1].  EDGE: the GEMM tile reaches past the end of the map
   template <bool EDGE>
   __device__ __forceinline__ void fold(Top2 (&s)[2], int kh, const float* rn, int n0, int fc,
-                                       const float (&acc)[XW_GEMM_BN / 2]) const {
+                                       const Acc (&acc)[XW_GEMM_BN / 2]) const {
 #pragma unroll
     for (int ii = 0; ii < XW_TILE / 8; ++ii) {   // (constant trip count: acc must stay in registers)
       const int i = kh * XW_TILE / 8 + ii;
@@ -57,12 +61,12 @@ struct CoarseEpi {
         const int col = n0 + 8 * i + fc + j;
         const bool ok = !EDGE || col < P;                // columns past the end of the map never win
         const float rnv = __ldg(rn + (ok ? col : 0));
-        push(s[0], ok ? acc[4 * i + j] * rnv : -INFINITY, col);
-        push(s[1], ok ? acc[4 * i + 2 + j] * rnv : -INFINITY, col);
+        push(s[0], ok ? (float)acc[4 * i + j] * rnv : -INFINITY, col);
+        push(s[1], ok ? (float)acc[4 * i + 2 + j] * rnv : -INFINITY, col);
       }
     }
   }
-  __device__ __forceinline__ void fragment(int g, int r, int m, int n0, int fc, const float (&acc)[XW_GEMM_BN / 2]) const {
+  __device__ __forceinline__ void fragment(int g, int r, int m, int n0, int fc, const Acc (&acc)[XW_GEMM_BN / 2]) const {
     const float* rn = rnorms + (size_t)grp_frame[g] * P;
     // after the quad's merge every lane holds all four results; lane q keeps and writes row r + 8 (q >> 1) of key tile
     // 2 (n0 / 256) + (q & 1)
@@ -84,7 +88,8 @@ struct CoarseEpi {
     }
     const int rr = r + 8 * (q >> 1), nt = n0 / XW_TILE + (q & 1);
     if (rr >= m || nt >= n_tiles) return;   // padding row, or a key tile lying completely past the end of the map
-    const float rdn = __fdividef(1.f, fmaxf(desc_norm[grp_row0[g] + rr], XW_MIN_NORM));
+    const float dv = desc_norm[grp_row0[g] + rr];
+    const float rdn = kS8 ? dv : __fdividef(1.f, fmaxf(dv, XW_MIN_NORM));
     const size_t off = (size_t)(grp_map0[g] + rr) * n_tiles + nt;
     key1[off] = ((unsigned long long)__float_as_uint(fmaxf(o.m1 * rdn, 0.f)) << 32) | (unsigned)(0x7fffffff - o.tok);
     max2[off] = fmaxf(o.m2 * rdn, 0.f);
@@ -113,24 +118,22 @@ int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cuda
   return DINOTRK_OK;
 }
 
-int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
-                     const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
-                     int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms) {
-  using Cfg = TcCfg<TcMode::F16, XW_GEMM_BN>;
-  static_assert(XW_GEMM_BN == 256 && XW_TILE == 128, "one m64n256 GEMM N tile = two 128-token key tiles (CoarseEpi::fragment)");
+template <TcMode MODE, class Acc>
+static int launch_coarse(const void* desc, int desc_rows, const void* tok, const FeatView& fv, const TcProblem& pb,
+                         const CoarseEpi<Acc>& epi, int max_tiles, cudaStream_t st) {
+  using Cfg = TcCfg<MODE, XW_GEMM_BN>;
+  constexpr int elem = MODE == TcMode::S8 ? TMAP_S8 : TMAP_F16;
   CUtensorMap tmA, tmB;
   int rc;
-  if ((rc = make_tmap_2d(&tmA, desc_hi, desc_rows, fv.C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB, fv.hi, fv.T, fv.P, fv.C, XW_GEMM_BN / 2, Cfg::kBK, TMAP_F16))) return rc;
-  auto kern = tc_gemm_pair_kernel<TcMode::F16, CoarseEpi, XW_GEMM_BN>;
+  if ((rc = make_tmap_2d(&tmA, desc, desc_rows, fv.C, TC_BM, Cfg::kBK, elem))) return rc;
+  if ((rc = make_tmap_3d(&tmB, tok, fv.T, fv.P, fv.C, XW_GEMM_BN / 2, Cfg::kBK, elem))) return rc;
+  auto kern = tc_gemm_pair_kernel<MODE, CoarseEpi<Acc>, XW_GEMM_BN>;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
     DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
     attr = true;
   }
-  TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, fv.P, fv.C};
-  CoarseEpi epi{rnorms, desc_norm, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
   const int sms = num_sms();
   const int tiles_bound = max_tiles * cdiv(fv.P, XW_GEMM_BN);
   int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
@@ -139,6 +142,22 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
   kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
   DTK_LAUNCHED();
   return DINOTRK_OK;
+}
+
+int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
+                     const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
+                     int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms, const void* desc_q8,
+                     const float* desc_fac) {
+  static_assert(XW_GEMM_BN == 256 && XW_TILE == 128, "one m64n256 GEMM N tile = two 128-token key tiles (CoarseEpi::fragment)");
+  TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, fv.P, fv.C};
+  if (desc_q8) {
+    DTK_CHECK_ARG(fv.s8() && fv.C % 16 == 0 && fv.C <= XW_S8_MAX_C, "int8 coarse pass: needs the int8 features, C %% 16 == 0 "
+                  "and C <= %d", XW_S8_MAX_C);
+    CoarseEpi<int> epi{fv.q_fac, desc_fac, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
+    return launch_coarse<TcMode::S8>(desc_q8, desc_rows, fv.q8, fv, pb, epi, max_tiles, st);
+  }
+  CoarseEpi<float> epi{rnorms, desc_norm, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
+  return launch_coarse<TcMode::F16>(desc_hi, desc_rows, fv.hi, fv, pb, epi, max_tiles, st);
 }
 
 // ====================================================================================================== 2. plan
@@ -150,7 +169,7 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
 constexpr int PLAN_WARPS = 8;
 __global__ void __launch_bounds__(PLAN_WARPS * 32)
 xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, int n_groups, int n_tiles,
-               const unsigned long long* __restrict__ key1,
+               const unsigned long long* __restrict__ key1, const float* __restrict__ eps_map,
                const float* __restrict__ max2, int* __restrict__ cand, int* __restrict__ pinfo, int* __restrict__ slow_cnt) {
   const int lane = threadIdx.x & 31;
   const int gw = blockIdx.x * PLAN_WARPS + (threadIdx.x >> 5), nw = gridDim.x * PLAN_WARPS;
@@ -171,7 +190,8 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, 
     for (int o = 16; o > 0; o >>= 1) { unsigned long long t = __shfl_xor_sync(0xffffffffu, gk, o); gk = t > gk ? t : gk; }
     const float gmax = __uint_as_float((unsigned)(gk >> 32));
     const int ptok = 0x7fffffff - (int)(gk & 0xffffffffu);
-    const float th = gmax - 2.f * XW_EPS;
+    const float eps = eps_map ? eps_map[map] : XW_EPS;
+    const float th = gmax - 2.f * eps;
     bool amb = false;
     int ncand = 0;
 #pragma unroll
@@ -186,7 +206,7 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, 
       ncand += __popc(cm);
     }
     // a (near-)zero map has no meaningful arg-max candidates; a descriptor below the split's faithful range voids the bound
-    amb = amb || ncand > XW_MAX_CAND || !(gmax > 4.f * XW_EPS) || !(desc_norm[map] >= min_norm);
+    amb = amb || ncand > XW_MAX_CAND || !(gmax > 4.f * eps) || !(desc_norm[map] >= min_norm);
     if (lane >= ncand && lane < XW_MAX_CAND) cand[(size_t)map * XW_MAX_CAND + lane] = -1;
     if (lane == 0) pinfo[map] = amb ? -1 - ptok : ptok;
   }
@@ -261,7 +281,7 @@ xw_cell_kernel(XwCells cells, int w, const int* __restrict__ cand, const int* __
 }
 
 int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, const dinotrk_geom& g, const XwChunk& xc,
-                   cudaStream_t st, int n_maps, float min_norm) {
+                   cudaStream_t st, int n_maps, float min_norm, const float* eps) {
   static_assert(XW_MAX_CAND == 4, "candidates are read as one int4");
   const int n_tiles = cdiv(g.h * g.w, XW_TILE);
   DTK_CHECK_ARG(n_tiles <= 64, "exact-window path: token grid too large (%d tiles)", n_tiles);
@@ -270,7 +290,7 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
   ProfRange pr(PROF_XW_PLAN, st);
   int grid = cdiv(n_maps, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;
-  xw_cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, min_norm, n_groups, n_tiles, xc.key1, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
+  xw_cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, min_norm, n_groups, n_tiles, xc.key1, eps, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
   DTK_LAUNCHED();
   grid = cdiv(cells.n_cells, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;
@@ -646,7 +666,8 @@ __global__ void __launch_bounds__(256)
 xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __restrict__ norms, const float* __restrict__ desc_norm,
                  const int* __restrict__ cell_frame, const int* __restrict__ cell_of, const int2* __restrict__ box_org,
                  const int* __restrict__ stat, const int* __restrict__ cand, const unsigned long long* __restrict__ key1,
-                 const float* __restrict__ max2, const float* __restrict__ xbox, float* __restrict__ win, int2* __restrict__ hin) {
+                 const float* __restrict__ max2, const float* __restrict__ xbox, float* __restrict__ win, int2* __restrict__ hin,
+                 const float* __restrict__ eps_map) {
   const int lane = threadIdx.x & 31;
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   for (int map = gw; map < n_maps; map += nw) {
@@ -673,6 +694,7 @@ xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __re
       }
     const int arow = amax / w, acol = amax - arow * w;
     // coarse bound on everything outside the window, from the tile keys
+    const float eps = eps_map ? eps_map[map] : XW_EPS;
     float mout = 0.f;
     for (int t = lane; t < n_tiles; t += 32) {
       const unsigned long long k = __ldg(key1 + (size_t)map * n_tiles + t);
@@ -680,7 +702,7 @@ xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __re
       const int tr = tk / w, tcn = tk - tr * w;
       const bool in_core = abs(tr - arow) <= 3 && abs(tcn - acol) <= 3;
       const float b = in_core ? __ldg(max2 + (size_t)map * n_tiles + t) : __uint_as_float((unsigned)(k >> 32));
-      mout = fmaxf(mout, b + XW_EPS);
+      mout = fmaxf(mout, b + eps);
     }
     // exact window + exact part of m_out
 #pragma unroll
@@ -793,7 +815,7 @@ xw_head_kernel(int n_maps, XhParams hp, dinotrk_head_weights wts, const int* __r
 
 int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head_weights& hw, const XwCells& cells,
                    const float* desc_norm, const int* grp_map0, int n_maps, const int* out_index, float* out, int out_stride,
-                   int out_mode, const XwChunk& xc, cudaStream_t st, int n_groups) {
+                   int out_mode, const XwChunk& xc, cudaStream_t st, int n_groups, const float* eps) {
   if (n_maps <= 0) return DINOTRK_OK;
   DTK_CHECK_ARG(g.radius <= 5 * g.stride, "exact-window path: disc radius %d exceeds 5 tokens", g.radius);
   XhParams hp;
@@ -820,7 +842,7 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
     int wgrid = cdiv(n_maps, 8);
     if (wgrid > sms * 8) wgrid = sms * 8;
     xw_window_kernel<<<wgrid, 256, 0, st>>>(n_maps, g.h, g.w, hp.P, hp.n_tiles, fv.norms, desc_norm, cells.frame, xc.cell_of, xc.box_org,
-                                            xc.stat, xc.cand, xc.key1, xc.max2, xc.xbox, xc.win, xc.hin);
+                                            xc.stat, xc.cand, xc.key1, xc.max2, xc.xbox, xc.win, xc.hin, eps);
     DTK_LAUNCHED();
   }
   xw_head_kernel<<<grid, XH_WARPS * 32, XH_SMEM, st>>>(n_maps, hp, hw, cells.group, grp_map0, xc.cell_of, xc.win, xc.hin, out_index,
@@ -914,6 +936,14 @@ __global__ void xw_tile_prefix_kernel(const int* __restrict__ grp_m, int n_group
   if (lane == 0) tile_start[n_groups] = base;
 }
 
+// eps[row] = xw_eps_s8(rho[row], rho_f[frame]) over the rows of group blockIdx.x
+__global__ void xw_eps_kernel(const int* __restrict__ grp_frame, const int* __restrict__ grp_row0, const int* __restrict__ grp_m,
+                              const float* __restrict__ rho, const float* __restrict__ rho_f, float* __restrict__ eps) {
+  const int g = blockIdx.x, r0 = grp_row0[g];
+  const float rf = rho_f[grp_frame[g]];
+  for (int r = threadIdx.x; r < grp_m[g]; r += blockDim.x) eps[r0 + r] = xw_eps_s8(rho[r0 + r], rf);
+}
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -953,6 +983,37 @@ int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, 
   xc.max2 = max2;
   return launch_xw_coarse(fv, desc_hi, desc_rows, desc_norm, grp_frame, grp_row0, grp_m, grp_row0, tile_start, n_groups,
                           desc_rows / TC2_BM + n_groups, xc, st, rnorms);
+}
+
+int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_q8, const float* desc_fac,
+                              const float* desc_rho, int desc_rows, const int* grp_frame, const int* grp_row0, const int* grp_m,
+                              int n_groups, unsigned long long* key1, float* max2, float* eps, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  DTK_CHECK_ARG(feat && feat->norms && feat->q8 && feat->q_fac && feat->q_rho && g && desc_q8 && desc_fac && desc_rho &&
+                grp_frame && grp_row0 && grp_m && key1 && max2, "xw_coarse_keys_i8: null pointer (the int8 features are required)");
+  DTK_CHECK_ARG(feat->T > 0 && feat->C > 0 && feat->C % 16 == 0 && feat->C <= XW_S8_MAX_C && desc_rows > 0 && n_groups >= 0,
+                "xw_coarse_keys_i8: bad sizes (C must be a multiple of 16, <= %d)", XW_S8_MAX_C);
+  DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_xw_coarse_keys_workspace_bytes(feat->T, n_groups, g),
+                "xw_coarse_keys_i8: workspace too small");
+  if (n_groups == 0) return DINOTRK_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const FeatView fv = make_view(*feat, *g);
+  Arena ar(workspace, workspace_bytes);
+  int* tile_start = ar.take<int>(n_groups + 1);
+  {
+    ProfRange pr(PROF_MISC, st);
+    xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, tile_start);
+    DTK_LAUNCHED();
+    if (eps) {
+      xw_eps_kernel<<<n_groups, 128, 0, st>>>(grp_frame, grp_row0, grp_m, desc_rho, fv.q_rho, eps);
+      DTK_LAUNCHED();
+    }
+  }
+  XwChunk xc{};
+  xc.key1 = key1;
+  xc.max2 = max2;
+  return launch_xw_coarse(fv, nullptr, desc_rows, nullptr, grp_frame, grp_row0, grp_m, grp_row0, tile_start, n_groups,
+                          desc_rows / TC2_BM + n_groups, xc, st, nullptr, desc_q8, desc_fac);
 }
 
 int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,

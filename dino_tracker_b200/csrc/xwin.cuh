@@ -6,10 +6,11 @@
 //   (ii) the map values on the 15 x 15 window around it (11 x 11 logits <- 13 x 13 hidden <- 15 x 15 inputs) and (iii) an
 //   upper bound on everything else (certificate that the stability branch, tracker_head.py:87-94, stays off).
 //
-//   1. coarse GEMM   one fp16 wgmma pass over the `hi` halves (1/3 of the split-precision work), epilogue keeps per
-//                    map and 128-token tile only (largest value, its first token, second largest value); |coarse - exact|
-//                    <= XW_EPS for every token (fp16 rounding of both operands + fp32 accumulation, see DESIGN.md).
-//   2. plan          per map: the tokens that can be the exact arg-max (coarse >= max - 2 XW_EPS); a map whose candidates
+//   1. coarse GEMM   one wgmma pass, int8 (per-token scales, the default) or fp16 over the `hi` halves; the epilogue keeps
+//                    per map and 128-token tile only (largest value, its first token, second largest value).  |coarse -
+//                    exact| <= eps for every token: XW_EPS for fp16 (rounding of both operands + fp32 accumulation), the
+//                    per-map xw_eps_s8 for int8 (relative quantisation residuals of the map's two operands, see DESIGN.md).
+//   2. plan          per map: the tokens that can be the exact arg-max (coarse >= max - 2 eps); a map whose candidates
 //                    are not all tile maxima is "ambiguous".  Maps come in CELLS = the <= 128 source frames of one (query,
 //                    anchor frame) pair: their arg-maxes cluster around the query's position in the anchor frame, so one
 //                    21 x 21 token box around the cell's median arg-max holds every map's window.
@@ -22,6 +23,8 @@
 //   Maps that are ambiguous, do not fit their cell's box or fail the certificate are queued and re-done by the full-map
 //   path (split-precision GEMM over all tokens + head kernels of head.cu) -- results never depend on the coarse values.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "corr.cuh"
 
@@ -39,6 +42,62 @@ constexpr float XW_MIN_NORM = 1e-4f;  // guard of the coarse epilogue's reciproc
                                       // >= split_min_norm(C) (corr.cuh): a smaller descriptor norm makes the map ambiguous, a
                                       // smaller token norm anywhere in the video sends the whole call to the full-map pipeline
 constexpr int XW_TILE = 128;          // tokens per coarse key (half of the coarse GEMM's N tile: two keys per tile)
+
+// ---- int8 coarse operands.  Per row x (token or descriptor): s = max|x_k| / 127, q = rint(x / s) in [-127, 127],
+// fac = s / max(|x|, XW_MIN_NORM) (the coarse epilogue's factor), rho = |x - s q| / |x| rounded up (0 for x = 0).
+// The coarse value of a map is <q_d, q_x> fac_d fac_x (int32 accumulation: exact while C 127^2 < 2^24).
+// |<d, x> - <s_d q_d, s_x q_x>| <= |<d - d^, x>| + |<d^, x - x^>| <= (rho_d + (1 + rho_d) rho_x) |d| |x|, so in cosine
+// units |coarse - exact| <= xw_eps_s8(rho_d, rho_F) with rho_F the largest rho_x of the map's frame.  XW_S8_SLACK covers
+// the exact split path's own error (2^-21 + 64 truncating adds x 2^-23, DESIGN.md 3.1) and the epilogue's fp32 roundings.
+constexpr float XW_S8_SLACK = 3.0518e-5f;   // 2^-15
+constexpr int XW_S8_MAX_C = 1040;           // C 127^2 < 2^24: the int32 -> float conversion of an accumulator is exact
+// rho_F above which the automatic mode runs the fp16 coarse pass: eps ~ 2 rho_F, and 2 eps is the candidate margin.  At
+// 0.03 (twice the largest token residual of Gaussian-like features at C = 1024, 0.0132) the margin stays below ~0.13,
+// under the typical gap between a map's maximum and the next value of another tile; features with outlier channels
+// (max |x| / rms far above Gaussian) exceed it and keep the fp16 pass.
+constexpr float XW_S8_RHO_MAX = 0.03f;
+__device__ __forceinline__ float xw_eps_s8(float rho_d, float rho_f) {
+  return __fadd_ru(__fadd_ru(rho_d, __fmul_ru(__fadd_ru(1.f, rho_d), rho_f)), XW_S8_SLACK);
+}
+
+// One warp quantises row x (element k = ld(k), C % 4 == 0) with fp32 norm `norm` (the exact path's): writes q[C], *fac
+// and returns rho (every lane).
+template <class Load>
+__device__ __forceinline__ float xw_quant_row(const Load& ld, int C, float norm, int8_t* __restrict__ q, float* __restrict__ fac) {
+  const int lane = threadIdx.x & 31;
+  float mx = 0.f;
+  for (int k = 4 * lane; k < C; k += 128) {
+    const float4 v = ld(k);
+    mx = fmaxf(mx, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  const float s = __fdiv_rn(mx, 127.f);
+  double r2 = 0.0, x2 = 0.0;
+  for (int k = 4 * lane; k < C; k += 128) {
+    const float4 v = ld(k);
+    const float vv[4] = {v.x, v.y, v.z, v.w};
+    char4 o;
+    signed char* oc = reinterpret_cast<signed char*>(&o);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float qf = s > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(vv[e], s)), -127.f), 127.f) : 0.f;
+      oc[e] = (signed char)qf;
+      const double d = (double)vv[e] - (double)s * (double)qf;   // exact: s q has <= 32 significant bits
+      r2 = fma(d, d, r2);
+      x2 = fma((double)vv[e], (double)vv[e], x2);
+    }
+    *reinterpret_cast<char4*>(q + k) = o;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    r2 += __shfl_xor_sync(0xffffffffu, r2, o);
+    x2 += __shfl_xor_sync(0xffffffffu, x2, o);
+  }
+  if (lane == 0) *fac = __fdiv_rn(s, fmaxf(norm, XW_MIN_NORM));
+  // upward at every step (the double sums' own rounding, ~C 2^-53 relative, is far below the last float ulp)
+  return x2 > 0.0 ? __double2float_ru(__ddiv_ru(__dsqrt_ru(r2), __dsqrt_rd(x2))) : 0.f;
+}
 
 // column of box token (by, bx) in a map's accumulator row
 __host__ __device__ inline int xw_col(int by, int bx) { return by * XW_BOX + bx; }
@@ -67,19 +126,22 @@ struct XwCells {          // host-planned, device-resident description of a chun
 };
 
 size_t xw_chunk_bytes(int chunk_maps, int max_cells, int n_tiles, int gcap);
-// Coarse GEMM over the chunk's groups (tile_start: prefix of ceil(m / 256) per group, all groups wide).
+// Coarse GEMM over the chunk's groups (tile_start: prefix of ceil(m / 256) per group, all groups wide): the int8 pass when
+// desc_q8 is given (desc_fac = the rows' factors, fv's int8 features), else fp16 over desc_hi and fv.hi.
 int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
                      const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
-                     int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms);
+                     int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms, const void* desc_q8 = nullptr,
+                     const float* desc_fac = nullptr);
 // rnorms = 1 / |F| for the coarse epilogue; *min_bits = bit pattern of the smallest token norm of the video
 int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cudaStream_t st);
+// eps: per-map bound on |coarse - exact| of the int8 pass (xw_eps_s8), nullptr for the fp16 pass (XW_EPS)
 int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, const dinotrk_geom& g, const XwChunk& xc,
-                   cudaStream_t st, int n_maps, float min_norm);
+                   cudaStream_t st, int n_maps, float min_norm, const float* eps);
 int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_hi, const void* desc_lo, int desc_rows,
                    const XwCells& cells, const XwChunk& xc, cudaStream_t st);
 int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head_weights& hw, const XwCells& cells,
                    const float* desc_norm, const int* grp_map0, int n_maps, const int* out_index, float* out, int out_stride,
-                   int out_mode, const XwChunk& xc, cudaStream_t st, int n_groups);
+                   int out_mode, const XwChunk& xc, cudaStream_t st, int n_groups, const float* eps);
 // Appends the queued maps' descriptor rows (fp32 optional, hi, lo, norm, out_index) to compact arrays at row_base and their
 // group arrays ([frame | row0 | m | map0] x gcap, entries grp_base ..) to cgrp.  n_slow = host copy of slow_cnt[n_groups].
 int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const float* desc_norm,

@@ -104,7 +104,7 @@ def _run_phases_on_device(model: Tracker, query_points, start, stop, batch_size,
         ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
         model.__dict__["_infer_ws"] = ws
     fb = 0 if batch_size is None else int(batch_size)
-    feat = model.features_struct(tpc, norms)
+    feat = model.features_struct(tpc, norms, quant=True)
     _lib.check(lib.dinotrk_infer(
         ctypes.byref(feat), ctypes.byref(geom), ctypes.byref(model.head_weights()), _lib.ptr(q), N,
         float(anchor_th), float(cos_th), fb, start, stop, chunk_maps, _lib.ptr(traj), _lib.ptr(cos_sims),

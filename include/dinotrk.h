@@ -54,13 +54,19 @@ typedef struct dinotrk_head_weights {
 /* A cached feature video.  tpc [T][P][C] and norms [T][P] are required.  hi / lo (optional, both or
  * neither): the fp16 split of tpc ([T][P][C] halves each, x = hi + lo) produced by dinotrk_split_fp16; when
  * present the wide correlation groups run on the wgmma tensor cores (3-pass split precision,
- * fp32-faithful), otherwise on the exact-fp32 FFMA GEMM.  C must then be a multiple of 8. */
+ * fp32-faithful), otherwise on the exact-fp32 FFMA GEMM.  C must then be a multiple of 8.
+ * q8 / q_fac / q_rho (optional, all or none; C a multiple of 16 and <= 1040): the int8 operands of the anchor phase's
+ * coarse pass, written by dinotrk_quantise_s8 with rows_per_group = h*w (q8 [T][P][C] int8, q_fac [T][P], q_rho [T] =
+ * the largest relative residual of each frame). */
 typedef struct dinotrk_features {
   const float* tpc;
   const float* norms;
   const void* hi;
   const void* lo;
   int T, C;
+  const void* q8;
+  const float* q_fac;
+  const float* q_rho;
 } dinotrk_features;
 
 int dinotrk_version(void);
@@ -75,6 +81,12 @@ int dinotrk_pack_features(const float* chw, float* tpc, float* norms, int T, int
                           void* stream);
 int dinotrk_unpack_features(const float* tpc, float* chw, int T, int C, int P, void* stream);
 int dinotrk_token_norms(const float* tpc, float* norms, int T, int C, int P, void* stream);
+/* Per row x of x [rows][C] (fp32 norms [rows], the norms the exact contractions use; C % 16 == 0): s = max|x_k| / 127
+ * (fp32), q[row][k] = rint(x_k / s) (int8, [rows][C]), fac[row] = s / max(norm, 1e-4) and the relative residual
+ * |x - s q| / |x| (float64, rounded up; 0 for a zero row) into rho[row] (optional) and, as the largest of each group of
+ * rows_per_group consecutive rows, into rho_max[ceil(rows / rows_per_group)] (optional). */
+int dinotrk_quantise_s8(const float* x, const float* norms, size_t rows, int C, int rows_per_group, void* q, float* fac,
+                        float* rho, float* rho_max, void* stream);
 /* x = hi + lo with hi = rn_fp16(x), lo = rn_fp16(x - hi) (fp16 arrays of n elements); n % 4 == 0. */
 int dinotrk_split_fp16(const float* x, void* hi, void* lo, size_t n, void* stream);
 /* The numbers the split's faithful range is stated in: range (device float[2]) = {max |x| over the n elements of x,
@@ -186,8 +198,14 @@ int dinotrk_infer_set_overlap(int mode);
  *      the DTK_XW environment variable (0 / 1) overrides.
  * dinotrk_infer_last_stats (n >= 4 slots): {anchor-phase maps, maps finished by the exact-window path, maps re-done by the
  * full-map path, pipeline used[, of the re-done maps: those queued by the head's certificate rather than by the plan[,
- * contraction: 1 = split fp16 tensor cores, 0 = exact fp32]]} of the last dinotrk_infer call that ran the anchor phase. */
+ * contraction: 1 = split fp16 tensor cores, 0 = exact fp32[, coarse pass of pipeline 1: 1 = int8, 0 = fp16 (the pass the
+ * phase finished with)[, bits of the float max over frames of feat->q_rho, 0 without int8 operands]]]]} of the last
+ * dinotrk_infer call that ran the anchor phase. */
 int dinotrk_infer_set_path(int path);
+/* Coarse pass of pipeline 1:  1 = int8 (feat->q8 required),  0 = fp16 over feat->hi,
+ * -1 (default) = int8 when feat->q8 is given and every frame's q_rho is <= 0.03, unless the probe chunk queues more than
+ *      1/16 of its maps to pipeline 0; fp16 otherwise.  No result depends on the choice. */
+int dinotrk_infer_set_coarse(int mode);
 int dinotrk_infer_last_stats(long long* out, int n);
 /* The coarse pass of pipeline 1 on its own (for testing its keys): the single-pass fp16 GEMM of desc_hi [desc_rows][C]
  * (fp16, the `hi` half of the descriptors) against feat->hi, group k correlating rows [grp_row0[k], grp_row0[k] + grp_m[k])
@@ -199,6 +217,14 @@ size_t dinotrk_xw_coarse_keys_workspace_bytes(int T, int n_groups, const dinotrk
 int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, int desc_rows,
                            const float* desc_norm, const int* grp_frame, const int* grp_row0, const int* grp_m, int n_groups,
                            unsigned long long* key1, float* max2, void* workspace, size_t workspace_bytes, void* stream);
+/* The same keys from the int8 pass: values relu(<desc_q8[j], feat->q8[frame][p]> desc_fac[j] feat->q_fac[frame][p])
+ * (desc_q8 int8 [desc_rows][C], desc_fac [desc_rows], desc_rho [desc_rows]: dinotrk_quantise_s8 of the descriptors).
+ * eps[j] (optional, float [desc_rows], rows of the groups only) receives the per-map bound on |coarse - exact cosine| the
+ * plan uses, from desc_rho[j] and feat->q_rho[frame].  feat->q8, q_fac and q_rho are required.  Workspace: as above. */
+int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_q8, const float* desc_fac,
+                              const float* desc_rho, int desc_rows, const int* grp_frame, const int* grp_row0, const int* grp_m,
+                              int n_groups, unsigned long long* key1, float* max2, float* eps, void* workspace,
+                              size_t workspace_bytes, void* stream);
 /* The exact box GEMM of pipeline 1 on its own (for testing and timing it): per cell k (device int32[n_cells] arrays), the
  * split-precision contraction (lo*hi + hi*lo + hi*hi, the full-map GEMM's sequence) of descriptor rows
  * [cell_row0[k], cell_row0[k] + cell_m[k]) (desc_hi / desc_lo: fp16 [desc_rows][C], dinotrk_split_fp16 of the fp32 rows)

@@ -21,6 +21,9 @@ Prints one JSON line:
                     tensor cores reach on this card under its power limit; it also writes the 207 MB fp16 product)
   gpu               card name, power limit and the SM clock (NVML, sampled during the timed windows)
   keys_sha256       digest of the keys, to compare builds bit for bit
+  int8              the same chunk on the int8 pass (dinotrk_xw_coarse_keys_i8 on dinotrk_quantise_s8 operands): ms, tops
+                    (2 * rows * P * C over its time), speedup over the fp16 pass, the largest per-map eps, and the SM
+                    clock sampled during its own timed windows
 """
 import argparse
 import ctypes
@@ -111,6 +114,19 @@ def main():
     def coarse():
         _lib.check(lib.dinotrk_xw_coarse_keys(*args), "xw_coarse_keys")
 
+    fq, ffac, _, frho = _lib.quantise_s8(feats, norms, P, _lib.stream_ptr())
+    fs8 = _lib.make_features(feats, norms, hi, hi, quant=(fq, ffac, frho))
+    desc8 = desc_hi.float()
+    dq, dfac, drho, _ = _lib.quantise_s8(desc8, desc8.norm(dim=1).contiguous(), rows, _lib.stream_ptr())
+    del desc8
+    eps = torch.empty(rows, dtype=torch.float32, device=dev)
+    args8 = (ctypes.byref(fs8), ctypes.byref(geom), _lib.ptr(dq), _lib.ptr(dfac), _lib.ptr(drho), rows, _lib.ptr(frame),
+             _lib.ptr(row0), _lib.ptr(m), len(GROUPS), _lib.ptr(key1), _lib.ptr(max2), _lib.ptr(eps), _lib.ptr(ws), nb,
+             _lib.stream_ptr())
+
+    def coarse8():
+        _lib.check(lib.dinotrk_xw_coarse_keys_i8(*args8), "xw_coarse_keys_i8")
+
     for _ in range(a.warmup):
         coarse()
     torch.cuda.synchronize()
@@ -124,6 +140,17 @@ def main():
     call_ms = time_windows(coarse, a.launches, a.windows)
     t1 = time.perf_counter()
     clocks = sampler.stop(t0, t1)
+    for _ in range(a.warmup):
+        coarse8()
+    torch.cuda.synchronize()
+    sampler8 = bench.ClockSampler(0)
+    sampler8.start()
+    time.sleep(0.1)
+    t0 = time.perf_counter()
+    s8_ms = time_windows(coarse8, a.launches, a.windows)
+    t1 = time.perf_counter()
+    clocks8 = sampler8.stop(t0, t1)
+    s8_med = sorted(s8_ms)[len(s8_ms) // 2]
 
     # cuBLAS yardstick on the largest group's shape, computed as the transposed product F @ D^T: both operands K-major
     # like the coarse GEMM's, and every leading dimension a multiple of 8 (an 8107-wide fp16 output row is not 16-byte
@@ -159,6 +186,9 @@ def main():
                    "ms_max": max(mm_ms), "tflops": 2.0 * mm * nn * kk / (mm_med / 1e3) / 1e12},
         "gpu": dict(gpu, sm_mhz=mhz, clock_reasons=clocks["reasons"], clock_samples=clocks["samples"]),
         "keys_sha256": digest,
+        "int8": {"ms_per_launch": s8_med, "ms_min": min(s8_ms), "ms_max": max(s8_ms), "tops": flop / (s8_med / 1e3) / 1e12,
+                 "speedup_vs_fp16": med / s8_med, "eps_max": eps.max().item(),
+                 "gpu": {"sm_mhz": clocks8["sm_mhz"], "clock_reasons": clocks8["reasons"], "clock_samples": clocks8["samples"]}},
     }))
 
 
