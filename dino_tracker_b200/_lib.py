@@ -110,6 +110,17 @@ SIGNATURES = {
     "dinotrk_delta_refine_tc": (c_int, [_P, c_int, c_int, c_int, POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p),
                                         POINTER(c_void_p), _P, _P, _P, c_int, c_int, _P, _P, _P, c_size_t, POINTER(c_void_p),
                                         c_int, c_size_t, _P]),
+    "dinotrk_delta_train_saved_bytes": (c_size_t, [c_int, c_int, c_int, POINTER(c_int)]),
+    "dinotrk_delta_train_forward_workspace_bytes": (c_size_t, [c_int, c_int, c_int, POINTER(c_int)]),
+    "dinotrk_delta_train_backward_workspace_bytes": (c_size_t, [c_int, c_int, c_int, POINTER(c_int)]),
+    "dinotrk_delta_train_forward": (c_int, [_P, c_int, c_int, c_int, POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p),
+                                            POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
+                                            POINTER(c_void_p), c_int, c_float, c_float, _P, _P, c_int, c_int, _P, _P, c_size_t,
+                                            _P, c_size_t, _P]),
+    "dinotrk_delta_train_backward": (c_int, [_P, c_int, c_int, c_int, POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p),
+                                             POINTER(c_void_p), POINTER(c_void_p), c_int, _P, _P, c_int, c_int, _P, _P, c_size_t,
+                                             POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), _P,
+                                             c_size_t, _P]),
     "dinotrk_peer_alloc": (c_int, [c_size_t, POINTER(c_void_p), ctypes.c_char_p]),
     "dinotrk_peer_open": (c_int, [ctypes.c_char_p, POINTER(c_void_p)]),
     "dinotrk_peer_close": (c_int, [_P]),

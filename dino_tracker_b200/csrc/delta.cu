@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "corr.cuh"
+#include "delta.cuh"
 #include "tcgemm.cuh"
 
 namespace dtk {
@@ -24,16 +25,6 @@ __device__ __forceinline__ void cp16(void* smem, const void* gmem, bool valid) {
   unsigned s = (unsigned)__cvta_generic_to_shared(smem);
   int sz = valid ? 16 : 0;
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(sz));
-}
-
-struct ConvShape {
-  int B, H, W, Cin, Cout, dil;  // Cin is the padded (multiple of 4) channel count of the NHWC input
-  int relu;
-};
-
-__device__ __forceinline__ int reflect(int v, int n) {
-  v = v < 0 ? -v : v;
-  return v >= n ? 2 * (n - 1) - v : v;
 }
 
 __global__ void __launch_bounds__(CONV_THREADS, 2)
@@ -283,7 +274,7 @@ __global__ void conv_plan_kernel(int* batch, int* row0, int* m, int* tile_start,
 
 template <int BN>
 static int conv_gemm(const __half* a_hi, const __half* a_lo, int rows, int Kp, const __half* w_hi, const __half* w_lo,
-                     int Cout, int* plan, const EpiConv& epi, cudaStream_t st) {
+                     int Cout, int* plan, const EpiConv& epi, cudaStream_t st, int prof) {
   using Cfg = TcCfg<TcMode::F16X3, BN>;
   CUtensorMap tA_hi, tA_lo, tB_hi, tB_lo;
   int rc;
@@ -301,31 +292,42 @@ static int conv_gemm(const __half* a_hi, const __half* a_lo, int rows, int Kp, c
   TcProblem pb{plan, plan + 4, plan + 8, plan + 12, 1, Cout, Kp};
   const int sms = num_sms();
   int tiles = cdiv(rows, TC_BM) * cdiv(Cout, BN);
-  ProfRange pr(PROF_CONV, st);
+  ProfRange pr(prof, st);
   kern<<<tiles < sms ? tiles : sms, TC_THREADS, Cfg::kSmem, st>>>(tA_hi, tA_lo, tB_hi, tB_lo, pb, epi);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
 
-constexpr size_t CONV_TC_ROWS = 32768;   // im2col rows per GEMM pass (bounds the fp16 scratch)
+size_t delta_conv_kmax(const int* channels) {
+  size_t kmax = 0;
+  for (int l = 0; l < 4; ++l) { size_t k = align_up((size_t)25 * (l == 0 ? 4 : channels[l]), 8); if (k > kmax) kmax = k; }
+  return kmax;
+}
+
+int launch_rgb_to_nhwc4(const float* frames, float* out, int B, int HW, cudaStream_t st) {
+  const size_t n = (size_t)B * HW;
+  rgb_to_nhwc4_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(frames, out, B, HW);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
 
 // one conv layer on tensor cores, row chunks of CONV_TC_ROWS output pixels
-static int launch_conv_tc(const float* in, const __half* w_hi, const __half* w_lo, const float* bias, float* out,
-                          ConvShape cs, int Kp, __half* col_hi, __half* col_lo, int* plan, cudaStream_t st) {
+int launch_conv_tc(const float* in, const __half* w_hi, const __half* w_lo, const float* bias, float* out,
+                   ConvShape cs, int Kp, __half* col_hi, __half* col_lo, int* plan, cudaStream_t st, int prof) {
   const size_t M = (size_t)cs.B * cs.H * cs.W;
   for (size_t m0 = 0; m0 < M; m0 += CONV_TC_ROWS) {
     const size_t rows = M - m0 < CONV_TC_ROWS ? M - m0 : CONV_TC_ROWS;
     {
-      ProfRange pr(PROF_CONV, st);
+      ProfRange pr(prof, st);
       im2col_split_kernel<<<(unsigned)rows, 128, 0, st>>>(in, col_hi, col_lo, cs.H, cs.W, cs.Cin, cs.dil, Kp, m0, rows);
       DTK_LAUNCHED();
       conv_plan_kernel<<<1, 32, 0, st>>>(plan, plan + 4, plan + 8, plan + 12, (int)rows);
       DTK_LAUNCHED();
     }
     EpiConv epi{out, bias, cs.Cout, cs.relu, m0};
-    int rc = cs.Cout <= 64 ? conv_gemm<64>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st)
-           : cs.Cout <= 128 ? conv_gemm<128>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st)
-                            : conv_gemm<256>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st);
+    int rc = cs.Cout <= 64 ? conv_gemm<64>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st, prof)
+           : cs.Cout <= 128 ? conv_gemm<128>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st, prof)
+                            : conv_gemm<256>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st, prof);
     if (rc) return rc;
   }
   return DINOTRK_OK;
@@ -364,8 +366,7 @@ static size_t delta_max_activation(int B, int H, int W, const int* channels) {
 }
 
 size_t dinotrk_delta_workspace_bytes(int B, int H, int W, const int* channels) {
-  size_t kmax = 0;
-  for (int l = 0; l < 4; ++l) { size_t k = align_up((size_t)25 * (l == 0 ? 4 : channels[l]), 8); if (k > kmax) kmax = k; }
+  const size_t kmax = delta_conv_kmax(channels);
   return 2 * align_up(delta_max_activation(B, H, W, channels) * sizeof(float), 256) +
          2 * align_up(CONV_TC_ROWS * kmax * 2, 256) + 8192;   // + fp16 im2col scratch of the tensor-core path
 }
@@ -391,8 +392,7 @@ static int delta_refine_impl(const float* frames, int B, int H, int W, const int
   const bool tensor = wgt_hi != nullptr && wgt_lo != nullptr;
   __half* col_hi = nullptr; __half* col_lo = nullptr; int* cplan = nullptr;
   if (tensor) {
-    size_t kmax = 0;
-    for (int l = 0; l < 4; ++l) { size_t k = align_up((size_t)25 * (l == 0 ? 4 : channels[l]), 8); if (k > kmax) kmax = k; }
+    const size_t kmax = delta_conv_kmax(channels);
     col_hi = ar.take<__half>(CONV_TC_ROWS * kmax);
     col_lo = ar.take<__half>(CONV_TC_ROWS * kmax);
     cplan = ar.take<int>(16);
@@ -400,10 +400,8 @@ static int delta_refine_impl(const float* frames, int B, int H, int W, const int
   }
 
   {
-    size_t n = (size_t)B * H * W;
     ProfRange pr(PROF_MISC, st);
-    rgb_to_nhwc4_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(frames, buf0, B, H * W);
-    DTK_LAUNCHED();
+    if (int rc = launch_rgb_to_nhwc4(frames, buf0, B, H * W, st)) return rc;
   }
   int ch = H, cw = W, cin = 4;
   float* cur = buf0;

@@ -5,8 +5,9 @@
 ``models/networks/tracker_head.py`` (keys ``cnn_refiner.{0,2}.{weight,bias}``), so the reference's
 checkpoints load bit-for-bit.  Without autograd neither module runs torch arithmetic: they fold / normalise their
 weights once per parameter version and hand them to the CUDA kernels.  With autograd (the training step,
-``dino_tracker.py:405-429``) the refiner's weight normalisation and the delta-DINO CNN (train-mode BatchNorm, cuDNN
-convolutions) are torch graphs -- library code feeding the hand-written tracker forward / backward of ``train.py``.
+``dino_tracker.py:405-429``) the refiner's weight normalisation is a torch graph; delta-DINO is one autograd node with
+CUDA forward and backward (``train.DeltaTrainFunction``) when its widths are multiples of 8, and a torch graph
+(``forward_graph``: cuDNN convolutions, BatchNorm in the module's mode) otherwise.
 """
 import ctypes
 import math
@@ -16,6 +17,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
+from . import train as _train
 
 
 class NormalizedConv2d(nn.Module):
@@ -243,6 +245,8 @@ class DeltaDINO(nn.Module):
     def forward(self, x, vit_features):
         """models/networks/delta_dino.py:53-61: returns the aligned residual B x C x h x w."""
         if self.wants_graph():
+            if self.conv_precision == "fp16x3":      # the widths the tensor-core convolutions take (as inference)
+                return _train.delta_train(self, x.float(), vit_features.shape[-2:])
             return self.forward_graph(x.float(), vit_features.shape[-2:])
         B, C, h, w = vit_features.shape
         geom = _lib.make_geom(x.shape[-2], x.shape[-1], 14, self.vit_stride, 35)

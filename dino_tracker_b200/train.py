@@ -5,12 +5,17 @@
 170-180, 303-325``).  Here the tracker part is ONE autograd node: its forward is the inference kernels with the maps kept
 (``dinotrk_sample_descriptors`` + ``dinotrk_corr_maps`` + ``dinotrk_head``), its backward is ``dinotrk_track_backward``
 (``csrc/train.cu``).  Inputs with gradient: the frame set's embeddings (token-major ``[N][P][C]``; the permutation from
-the reference's ``N x C x h x w`` and everything upstream -- delta-DINO, the residual add -- stay torch graphs) and the
-refiner's NORMALISED weights (the spatial-sum normalisation of ``conv_norm.py:34-46`` is a small torch graph on top).
+the reference's ``N x C x h x w`` and the residual add stay torch graphs) and the refiner's NORMALISED weights (the
+spatial-sum normalisation of ``conv_norm.py:34-46`` is a small torch graph on top).
+
+Delta-DINO upstream of it is a second node, ``DeltaTrainFunction`` (``csrc/delta_train.cu``): per chunk of frames the
+convolutions as split-precision wgmma GEMMs, BatchNorm on the batch statistics, BlurPool and the alignment, and the
+reverse pass of all of it down to the 16 parameter gradients.
 """
 import ctypes
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -129,6 +134,116 @@ class SampleFunction(torch.autograd.Function):
                                                             _lib.ptr(slots), T, 1, _lib.ptr(g), _lib.ptr(grad),
                                                             _lib.stream_ptr(tracker._dev)), "sample_backward")
         return grad, None, None
+
+
+_CONV, _BN = (0, 4, 8, 12), (1, 5, 9, 13)
+
+
+def _kmajor(w):
+    """Conv weights [O][I][5][5] -> K-major [O][Kp] ([O][5][5][I_pad], I padded to 4, K to a multiple of 8): the layout
+    of the forward's weight operand and of the weight gradient ``dinotrk_delta_train_backward`` writes."""
+    w = w.detach().float().permute(0, 2, 3, 1)
+    if w.shape[-1] % 4:
+        w = torch.nn.functional.pad(w, (0, 4 - w.shape[-1] % 4))
+    w = w.reshape(w.shape[0], -1)
+    if w.shape[1] % 8:
+        w = torch.nn.functional.pad(w, (0, 8 - w.shape[1] % 8))
+    return w.contiguous()
+
+
+def _from_kmajor(g, shape):
+    O, I = shape[:2]
+    ip = I + (-I) % 4
+    return g[:, :25 * ip].reshape(O, 5, 5, ip)[..., :I].permute(0, 3, 1, 2).contiguous()
+
+
+def _ptrs(ts):
+    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() if t is not None else None for t in ts])
+
+
+class DeltaTrainFunction(torch.autograd.Function):
+    """residual B x C x h x w = delta-DINO of one chunk of frames (one BatchNorm batch), aligned to the h x w token grid
+    (``DeltaDINO.forward`` with a graph, widths multiples of 8).  Forward ``dinotrk_delta_train_forward`` (BatchNorm in the
+    module's mode; train mode updates the running statistics), backward ``dinotrk_delta_train_backward``.  Inputs with
+    gradient: the 16 parameters (conv weights, conv biases, BN weights, BN biases, layer order); frames get none."""
+
+    @staticmethod
+    def forward(ctx, frames, module, vit_hw, *params):
+        lib = _lib.load()
+        dev = frames.device
+        bns = [module.layers[i] for i in _BN]
+        training = bns[0].training
+        assert all(bn.momentum is not None and bn.track_running_stats for bn in bns), "BatchNorm2d with momentum and running stats"
+        # the C entry takes one mode, momentum and eps for the four BatchNorms
+        assert all((bn.training, bn.momentum, bn.eps) == (training, bns[0].momentum, bns[0].eps) for bn in bns), \
+            "delta-DINO's four BatchNorms must share their mode, momentum and eps"
+        with torch.cuda.device(dev):
+            st = _lib.stream_ptr()
+            fr = frames.detach().float().contiguous()
+            B, _, H, W = fr.shape
+            h, w = vit_hw
+            C = module.channels[-1]
+            ch, cw = H, W
+            for _ in range(3):
+                ch, cw = (ch - 1) // 2 + 1, (cw - 1) // 2 + 1
+            ixs, iys = module.align_tables((ch, cw), (h, w), dev, vit_stride=module.vit_stride)
+            chan = (ctypes.c_int * 5)(*module.channels)
+            splits = [_lib.split_fp16(_kmajor(p), st) for p in params[0:4]]
+            vecs = [p.detach().float().contiguous() for p in params[4:16]]
+            for bn in bns:
+                assert bn.running_mean.dtype == torch.float32 and bn.running_mean.is_contiguous() and bn.running_var.is_contiguous()
+            saved_bytes = lib.dinotrk_delta_train_saved_bytes(B, H, W, chan)
+            saved = torch.empty(saved_bytes, device=dev, dtype=torch.uint8)
+            ws_bytes = lib.dinotrk_delta_train_forward_workspace_bytes(B, H, W, chan)
+            work = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+            res = torch.empty(B, h * w, C, device=dev, dtype=torch.float32)
+            _lib.check(lib.dinotrk_delta_train_forward(
+                _lib.ptr(fr), B, H, W, chan, _ptrs([s[0] for s in splits]), _ptrs([s[1] for s in splits]), _ptrs(vecs[0:4]),
+                _ptrs(vecs[4:8]), _ptrs(vecs[8:12]), _ptrs([bn.running_mean for bn in bns]), _ptrs([bn.running_var for bn in bns]),
+                int(training), float(bns[0].momentum), float(bns[0].eps), _lib.ptr(ixs), _lib.ptr(iys), h, w, _lib.ptr(res),
+                _lib.ptr(saved), saved_bytes, _lib.ptr(work), ws_bytes, st), "delta_train_forward")
+            if training:
+                for bn in bns:
+                    bn.num_batches_tracked.add_(1)
+        ctx.module, ctx.training, ctx.hw = module, training, (h, w)
+        # through save_for_backward, so that autograd frees the saved activations (~1.7 GB per 8 frames) after backward
+        ctx.save_for_backward(fr, saved, ixs, iys, *params)
+        return res.view(B, h, w, C).permute(0, 3, 1, 2)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        lib = _lib.load()
+        fr, saved, ixs, iys, *params = ctx.saved_tensors
+        dev = fr.device
+        B, _, H, W = fr.shape
+        h, w = ctx.hw
+        module = ctx.module
+        with torch.cuda.device(dev):
+            st = _lib.stream_ptr()
+            chan = (ctypes.c_int * 5)(*module.channels)
+            g = grad.to(torch.float32).permute(0, 2, 3, 1).contiguous()          # [B][h][w][C] = token-major
+            wt = [None] + [_lib.split_fp16(p.detach().float().permute(1, 2, 3, 0).reshape(p.shape[1], -1).contiguous(), st)
+                           for p in params[1:4]]
+            vecs = [p.detach().float().contiguous() for p in params[8:16]]
+            gw = [torch.empty(p.shape[0], _kmajor(p).shape[1], device=dev, dtype=torch.float32) for p in params[0:4]]
+            gv = [torch.empty(p.shape[0], device=dev, dtype=torch.float32) for p in params[4:16]]
+            ws_bytes = lib.dinotrk_delta_train_backward_workspace_bytes(B, H, W, chan)
+            work = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+            _lib.check(lib.dinotrk_delta_train_backward(
+                _lib.ptr(fr), B, H, W, chan, _ptrs([t[0] if t else None for t in wt]), _ptrs([t[1] if t else None for t in wt]),
+                _ptrs(vecs[0:4]), _ptrs(vecs[4:8]), int(ctx.training), _lib.ptr(ixs), _lib.ptr(iys), h, w, _lib.ptr(g),
+                _lib.ptr(saved), saved.numel(), _ptrs(gw), _ptrs(gv[0:4]), _ptrs(gv[4:8]), _ptrs(gv[8:12]), _lib.ptr(work),
+                ws_bytes, st), "delta_train_backward")
+        grads = [_from_kmajor(gw[i], params[i].shape) for i in range(4)] + gv
+        return (None, None, None, *[gr.to(p.dtype) for gr, p in zip(grads, params)])
+
+
+def delta_train(module, frames, vit_hw):
+    """``DeltaDINO.forward`` with a graph on the CUDA path: the aligned residual B x C x h x w of one chunk."""
+    L = module.layers
+    params = [L[i].weight for i in _CONV] + [L[i].bias for i in _CONV] + [L[i].weight for i in _BN] + [L[i].bias for i in _BN]
+    return DeltaTrainFunction.apply(frames, module, tuple(int(v) for v in vit_hw), *params)
 
 
 def sample_points(tracker, emb_chw, pts):

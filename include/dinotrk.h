@@ -286,6 +286,40 @@ int dinotrk_peer_open(const unsigned char* handle64, void** ptr);
 int dinotrk_peer_close(void* ptr);
 int dinotrk_peer_free(void* ptr);
 
+/* ---- Delta-DINO training step (delta_dino.py:22-61 with gradients, models/tracker.py:113-129) -------------------
+ * One chunk of B frames (the reference's 8-frame batches; each chunk is its own BatchNorm batch).  channels[5] =
+ * {3, c1, c2, c3, C}, c* multiples of 8; every reflect pad must be smaller than the map it pads (as torch requires).
+ * Forward: wgt_hi[l] / wgt_lo[l] = fp16 split (dinotrk_split_fp16) of the UNFOLDED conv weights, K-major
+ * [C_out][5][5][C_in_pad] with K padded to Kp = 25 * C_in_pad rounded up to 8 (C_in_pad = 4 for l = 0); conv_bias,
+ * bn_weight (gamma), bn_bias (beta), running_mean, running_var: [C_out] per layer.  training = 1: BatchNorm on the
+ * batch statistics (float64 two-pass reduction over B*H*W) and the running statistics updated in place as
+ * torch.nn.BatchNorm2d does (momentum, unbiased running_var; num_batches_tracked is the caller's); training = 0: the
+ * running statistics, left unchanged.  Writes residual_tpc [B][h*w][C] = the aligned BN output of the last layer
+ * (ixs / iys as in dinotrk_delta_refine) and fills `saved` (dinotrk_delta_train_saved_bytes: the pre-BN conv outputs and
+ * the per-channel statistics) for the backward.  B = 0 writes nothing.  Syncs: no.
+ * Backward: grad_residual_tpc [B][h*w][C]; wgtT_hi[l] / wgtT_lo[l] (l = 1..3, entry 0 unused) = fp16 split of the conv
+ * weights transposed to [C_in][5][5][C_out]; bn_weight / bn_bias / training and `saved` as given to the forward.  WRITES
+ * (does not accumulate) grad_wgt[l] [C_out][Kp] in the forward's K-major layout (columns past 25 * C_in_pad are zero),
+ * grad_bias[l], grad_bn_weight[l], grad_bn_bias[l] [C_out].  Frames get no gradient.  Every reduction runs in a fixed
+ * order: results are bit-for-bit reproducible.  The convolution GEMMs run on fp16 hi / lo splits; each gradient operand
+ * is scaled by a power of two from its max |.| first (exact), so the result does not depend on the gradient's scale.
+ * Syncs: no. */
+size_t dinotrk_delta_train_saved_bytes(int B, int H, int W, const int* channels);
+size_t dinotrk_delta_train_forward_workspace_bytes(int B, int H, int W, const int* channels);
+size_t dinotrk_delta_train_backward_workspace_bytes(int B, int H, int W, const int* channels);
+int dinotrk_delta_train_forward(const float* frames, int B, int H, int W, const int* channels, const void* const* wgt_hi,
+                                const void* const* wgt_lo, const float* const* conv_bias, const float* const* bn_weight,
+                                const float* const* bn_bias, float* const* running_mean, float* const* running_var,
+                                int training, float momentum, float eps, const float* ixs, const float* iys, int h, int w,
+                                float* residual_tpc, void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes,
+                                void* stream);
+int dinotrk_delta_train_backward(const float* frames, int B, int H, int W, const int* channels, const void* const* wgtT_hi,
+                                 const void* const* wgtT_lo, const float* const* bn_weight, const float* const* bn_bias,
+                                 int training, const float* ixs, const float* iys, int h, int w, const float* grad_residual_tpc,
+                                 const void* saved, size_t saved_bytes, float* const* grad_wgt, float* const* grad_bias,
+                                 float* const* grad_bn_weight, float* const* grad_bn_bias, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
 /* ---- DINOv2 ViT feature extractor (utils.py:32-72, models/extractor.py:41-85,137-150) -------------- */
 typedef struct dinotrk_vit_config {
   int depth, dim, heads;   /* ViT-L/14: 24, 1024, 16; ViT-B/14: 12, 768, 12 (head dim 64) */
