@@ -133,6 +133,15 @@ SIGNATURES = {
     "dinotrk_traj_nearest_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "dinotrk_traj_nearest": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, c_float, _P, _P, c_size_t, _P]),
     "dinotrk_of_filter": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, c_int, _P, _P]),
+    "dinotrk_pca_workspace_bytes": (c_size_t, [ctypes.c_longlong, c_int, c_int]),
+    "dinotrk_pca_stats": (c_int, [_P, ctypes.c_longlong, c_int, c_int, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_pca_power": (c_int, [_P, ctypes.c_longlong, c_int, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_fg_mask": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_float, c_int, c_int, _P, _P, _P, _P, c_size_t,
+                                _P]),
+    "dinotrk_mask_upsample": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, _P, _P]),
+    "dinotrk_traj_split_workspace_bytes": (c_size_t, [c_int]),
+    "dinotrk_traj_split_count": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, POINTER(c_int), _P, c_size_t, _P]),
+    "dinotrk_traj_split_emit": (c_int, [_P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
 }
 
 

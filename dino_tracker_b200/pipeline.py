@@ -65,3 +65,52 @@ def save_dino_embed_video(video01, vit: DinoV2Features, path):
     """preprocessing/save_dino_embed_video.py:9-25: writes T x C x h x w fp32 (CPU tensor) to ``path``."""
     os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
     torch.save(vit.features_chw(video01).contiguous().cpu(), path)
+
+
+PREPROCESSING_DEFAULTS = dict(threshold=1.5, min_trajectory_length=2, filter_using_direct_flow=True, direct_flow_threshold=2.5,
+                              fg_mask_threshold=0.6, dino_bb_box_size=30, dino_bb_iou_threshold=0.2)   # preprocessing.yaml
+
+
+@torch.no_grad()
+def preprocess_video(video01, vit: DinoV2Features, mask_vit: DinoV2Features, data_path, flow_fn=None, device="cuda:0",
+                     **config):
+    """preprocessing/main_preprocessing.py in one process, for a video T x 3 x H x W in [0, 1] and the paths of
+    utils.add_config_paths(data_path):
+      1. optical-flow trajectories -> of_trajectories/trajectories.pt;
+      2. the features of ``vit`` -> dino_embeddings/dino_embed_video.pt;
+      3. unless ``data_path``/masks exists: the features of ``mask_vit`` (layer 23 in the reference) go straight from the
+         ViT into the mask kernels (no feature file) -> masks/{idx:05d}.jpg;
+      4. the fg / bg split of the trajectories by the masks READ BACK from masks/ (JPEG is lossy, and ``> 0`` turns its
+         ringing near mask edges into foreground; the re-read masks are what the trainer's load_fg_masks sees), resized
+         to H x W -> of_trajectories/fg_trajectories.pt, bg_trajectories.pt;
+      5. preprocess_best_buddies -> dino_best_buddies/*, of_trajectories/trajectories_wo_direct_filter.pt.
+    ``config`` overrides PREPROCESSING_DEFAULTS.  Returns the trajectories, fg, bg and the masks [T][H][W] uint8."""
+    from . import fg_masks as fgm
+    from .trajectories import extract_trajectories
+    cfg = dict(PREPROCESSING_DEFAULTS, **config)
+    dev = torch.device(device)
+    T, _, H, W = video01.shape
+    of_dir = os.path.join(data_path, "of_trajectories")
+    os.makedirs(of_dir, exist_ok=True)
+    traj = extract_trajectories(video01, flow_fn, cfg["threshold"], cfg["min_trajectory_length"],
+                                cfg["filter_using_direct_flow"], cfg["direct_flow_threshold"], device=dev)
+    torch.save(traj.cpu(), os.path.join(of_dir, "trajectories.pt"))
+    features_chw = vit.features_chw(video01)
+    os.makedirs(os.path.join(data_path, "dino_embeddings"), exist_ok=True)
+    torch.save(features_chw.contiguous().cpu(), os.path.join(data_path, "dino_embeddings", "dino_embed_video.pt"))
+    masks_path = os.path.join(data_path, "masks")
+    if not os.path.exists(masks_path):
+        tpc = mask_vit(video01)
+        h, w = features_chw.shape[-2:]
+        masks = fgm.fg_masks(tpc.view(T, h, w, tpc.shape[-1]), (H, W), fg_mask_threshold=cfg["fg_mask_threshold"])
+        del tpc
+        fgm.save_mask_frames(masks, masks_path)
+    masks = torch.from_numpy(fgm.load_masks(masks_path, H, W)).to(dev)
+    fg, bg = fgm.split_trajectories(traj, masks)
+    torch.save(fg.cpu(), os.path.join(of_dir, "fg_trajectories.pt"))
+    torch.save(bg.cpu(), os.path.join(of_dir, "bg_trajectories.pt"))
+    preprocess_best_buddies(features_chw, video01, os.path.join(data_path, "dino_best_buddies"),
+                            os.path.join(of_dir, "trajectories_wo_direct_filter.pt"), H, W, flow_fn=flow_fn,
+                            threshold=cfg["threshold"], min_trajectory_length=cfg["min_trajectory_length"],
+                            box_size=cfg["dino_bb_box_size"], iou_thresh=cfg["dino_bb_iou_threshold"], device=dev)
+    return traj, fg, bg, masks

@@ -443,6 +443,40 @@ int dinotrk_of_filter(const float* traj, int M, int T, const int* nearest, int g
                       const float* tgt_xy, const int* pair_src, const int* pair_tgt, const int* offsets, int n_pairs, int n_pts,
                       uint8_t* keep, void* stream);
 
+/* ---- foreground masks (preprocessing/create_fg_mask.py) and the fg / bg split (split_trajectories_to_fg_bg.py) ---- */
+/* The features are token-major fp32 rows a [M][C] (M = T*h*w, the ViT's output), C % 4 == 0, C <= 1536, 16-byte
+ * aligned; q <= 4.  Offsets are 64-bit.  Every sum runs in a fixed order: two runs give the same bits.
+ * dinotrk_pca_stats: s [M] = 1 / max(|a_i|, 1e-12) (F.normalize's rule; 1 when normalize == 0) and c [C] = the column
+ * mean of diag(s) A (float64 partials over fixed row ranges).
+ * dinotrk_pca_power: one read of the rows gives X = (diag(s) A - 1cᵀ) P [M][q] and W = (diag(s) A - 1cᵀ)ᵀ X [C][q] for
+ * P [C][q]: with QR(X) = Q R, the next iterate of torch.pca_lowrank's subspace iteration is W R⁻¹.
+ * Both take a workspace of dinotrk_pca_workspace_bytes(M, C, q) bytes (q = 1 for the stats). */
+size_t dinotrk_pca_workspace_bytes(long long M, int C, int q);
+int dinotrk_pca_stats(const float* a, long long M, int C, int normalize, float* s, float* c, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int dinotrk_pca_power(const float* a, long long M, int C, int q, const float* s, const float* c, const float* P, float* X,
+                      float* W, void* workspace, size_t workspace_bytes, void* stream);
+/* create_fg_mask.py:29-42: colors [M][q] = diag(s) A V (not centred), token_mask [T][h][w] = 1 where
+ * (colors[:,0] - min) / (max - min) < threshold (fp32), and mask [T][H][W] = 255 * its nearest upsampling.  workspace:
+ * 32 bytes. */
+int dinotrk_fg_mask(const float* a, int T, int h, int w, int C, int q, const float* s, const float* V, float threshold,
+                    int H, int W, float* colors, uint8_t* token_mask, uint8_t* mask, void* workspace, size_t workspace_bytes,
+                    void* stream);
+/* F.interpolate(mode="nearest") of a 0/1 token mask [T][h][w] to [T][H][W] 0/255: source index
+ * min((int)floorf(dst * ((float)in / out)), in - 1). */
+int dinotrk_mask_upsample(const uint8_t* token_mask, int T, int h, int w, int H, int W, uint8_t* out, void* stream);
+/* mask_filter_trajectories (split_trajectories_to_fg_bg.py:55-78) of trajectories traj [N][T][2] (NaN where missing) by
+ * masks [Tm][H][W] uint8: a trajectory starts at its first step with both coordinates non-NaN, at (rint(x), rint(y))
+ * (torch.round); it is foreground when masks[start][y][x] > 0.  dinotrk_traj_split_count classifies every row, reads the
+ * foreground count back to *n_fg (host; synchronises the stream) and returns DINOTRK_EINVAL when a row has no valid step,
+ * starts outside the frame or past frame Tm - 1.  dinotrk_traj_split_emit then writes the foreground rows to
+ * fg [n_fg][T][2] and the others to bg [N - n_fg][T][2], each in row order. */
+size_t dinotrk_traj_split_workspace_bytes(int N);
+int dinotrk_traj_split_count(const float* traj, int N, int T, const uint8_t* masks, int Tm, int H, int W, int* n_fg,
+                             void* workspace, size_t workspace_bytes, void* stream);
+int dinotrk_traj_split_emit(const float* traj, int N, int T, float* fg, float* bg, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* ---- per-kernel-class device timing (CUDA events on the launching stream; bench.py roofline) ------ */
 int dinotrk_profile_classes(void);
 const char* dinotrk_profile_class_name(int cls);
