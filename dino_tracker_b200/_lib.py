@@ -142,6 +142,13 @@ SIGNATURES = {
     "dinotrk_traj_split_workspace_bytes": (c_size_t, [c_int]),
     "dinotrk_traj_split_count": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, POINTER(c_int), _P, c_size_t, _P]),
     "dinotrk_traj_split_emit": (c_int, [_P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_bb_contrastive_cos_stride": (c_int, [c_int]),
+    "dinotrk_bb_contrastive_forward_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "dinotrk_bb_contrastive_forward": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_float, _P, _P,
+                                               _P, c_size_t, _P]),
+    "dinotrk_bb_contrastive_backward_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int]),
+    "dinotrk_bb_contrastive_backward": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_float, _P, _P,
+                                                _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
 }
 
 

@@ -49,7 +49,9 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
                         const float* desc, int desc_rows, const float* desc_norm, const int* grp_frame,
                         const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                         int max_tiles, float* maps, int map_stride, float* desc_split_ws, cudaStream_t st,
-                        unsigned long long* tkeys = nullptr, bool split_ready = false, int tile_rows = 0 /* 0: default */);
+                        unsigned long long* tkeys = nullptr, bool split_ready = false, int tile_rows = 0 /* 0: default */,
+                        bool relu = true /* false: signed cosines (no tile keys) */,
+                        const float* clamp = nullptr /* [desc_rows]: per-row replacement of the norm product's 1e-8 (signed only) */);
 int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t st);
 
 // Faithful range of the fp16 hi/lo split (DESIGN.md 3.1).  Per element, x - hi - lo is at most 2^-22 |x| while lo is an fp16

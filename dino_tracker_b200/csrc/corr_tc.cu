@@ -1,6 +1,7 @@
 // Tensor-core correlation GEMM (wgmma, split-precision fp16 hi/lo) + operand splitting + TMA tensor-map helpers.
 //
 //   corr[j][p] = relu( <d_j, F[frame][p]> / max(|d_j| |F[frame][p]|, 1e-8) )     (models/tracker.py:158-173)
+// (the ReLU is a template choice: the contrastive losses keep the signed cosines, contrastive.cu)
 //
 // The contraction runs as lo*hi + hi*lo + hi*hi on the f16 tensor pipe with fp32 accumulation in registers
 // (operands pre-split into fp16 hi + fp16 lo, x = hi + lo up to 2^-22 |x|), which keeps the products
@@ -165,6 +166,7 @@ __global__ void split_range_kernel(const float* __restrict__ x, size_t n, const 
   if ((threadIdx.x & 31) == 0) { atomicMax(range, mx); atomicMin(range + 1, mn); }
 }
 
+template <bool kRelu>
 struct CorrEpi {
   const float* norms;      // [T][P]
   const float* desc_norm;  // [rows]
@@ -175,8 +177,10 @@ struct CorrEpi {
   int map_stride, P;
   unsigned long long* tkeys;   // optional [maps][n_tiles]: (tile maximum, first token holding it) keys for the head (corr.cuh)
   int n_tiles;
+  const float* clamp = nullptr;   // optional [desc rows]: per-row replacement of the norm product's 1e-8 (scaled operands)
   struct State { float mx; int tok; };
   __device__ __forceinline__ void tile_begin(State& s) const { s.mx = -1.f; s.tok = 0; }   // map values are >= 0 (ReLU)
+  __device__ __forceinline__ static float act(float v) { return kRelu ? fmaxf(v, 0.f) : v; }
   __device__ __forceinline__ void tile_end(State& s, int g, int r, int nt) const {
     if (tkeys)   // + 0.f: never the bit pattern of -0
       tkeys[(size_t)(grp_map0[g] + r) * n_tiles + nt] =
@@ -184,6 +188,7 @@ struct CorrEpi {
   }
   __device__ __forceinline__ void operator()(State& s, int g, int r, int col0, const float (&f)[32], int ncols) const {
     const float dn = desc_norm[grp_row0[g] + r];
+    const float eps = clamp ? clamp[grp_row0[g] + r] : 1e-8f;
     const float* fn = norms + (size_t)grp_frame[g] * P + col0;
     float* out = maps + (size_t)(grp_map0[g] + r) * map_stride + col0;
     if (ncols == 32) {
@@ -192,10 +197,10 @@ struct CorrEpi {
         // norms rows are only 4-byte aligned (P is odd): scalar broadcast loads
         float4 n4 = make_float4(__ldg(fn + i), __ldg(fn + i + 1), __ldg(fn + i + 2), __ldg(fn + i + 3));
         float4 o;
-        o.x = fmaxf(__fdiv_rn(f[i + 0], fmaxf(__fmul_rn(dn, n4.x), 1e-8f)), 0.f);
-        o.y = fmaxf(__fdiv_rn(f[i + 1], fmaxf(__fmul_rn(dn, n4.y), 1e-8f)), 0.f);
-        o.z = fmaxf(__fdiv_rn(f[i + 2], fmaxf(__fmul_rn(dn, n4.z), 1e-8f)), 0.f);
-        o.w = fmaxf(__fdiv_rn(f[i + 3], fmaxf(__fmul_rn(dn, n4.w), 1e-8f)), 0.f);
+        o.x = act(__fdiv_rn(f[i + 0], fmaxf(__fmul_rn(dn, n4.x), eps)));
+        o.y = act(__fdiv_rn(f[i + 1], fmaxf(__fmul_rn(dn, n4.y), eps)));
+        o.z = act(__fdiv_rn(f[i + 2], fmaxf(__fmul_rn(dn, n4.z), eps)));
+        o.w = act(__fdiv_rn(f[i + 3], fmaxf(__fmul_rn(dn, n4.w), eps)));
         *reinterpret_cast<float4*>(out + i) = o;
         // strict >: the first token of the tile holding the maximum (columns are visited in increasing order)
         if (o.x > s.mx) { s.mx = o.x; s.tok = col0 + i; }
@@ -207,7 +212,7 @@ struct CorrEpi {
 #pragma unroll
       for (int i = 0; i < 32; ++i)
         if (i < ncols) {
-          const float o = fmaxf(__fdiv_rn(f[i], fmaxf(__fmul_rn(dn, fn[i]), 1e-8f)), 0.f);
+          const float o = act(__fdiv_rn(f[i], fmaxf(__fmul_rn(dn, fn[i]), eps)));
           out[i] = o;
           if (o > s.mx) { s.mx = o; s.tok = col0 + i; }
         }
@@ -226,15 +231,47 @@ int corr_tc_tile_rows() {
 
 size_t corr_tc_workspace_bytes(int total_rows, int C) { return 2 * align_up((size_t)total_rows * C * 2, 256); }
 
+template <bool kRelu>
+static int corr_gemm_tc_launch(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi,
+                               const CUtensorMap& tmB_lo, const TcProblem& pb, const CorrEpi<kRelu>& epi, bool pairs,
+                               int tiles_bound, cudaStream_t st) {
+  using Cfg = TcCfg<TcMode::F16X3>;
+  static PerDev<bool> attr_dev;
+  bool& attr = attr_dev.get();
+  if (!attr) {
+    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TcMode::F16X3, CorrEpi<kRelu>>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  Cfg::kSmem));
+    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi<kRelu>>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+    attr = true;
+  }
+  const int sms = num_sms();
+  ProfRange pr(PROF_CORR_GEMM, st);
+  if (pairs) {
+    int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
+    if (grid < 2) grid = 2;
+    tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi<kRelu>><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo,
+                                                                                            pb, epi);
+    DTK_LAUNCHED();
+    return DINOTRK_OK;
+  }
+  int grid = tiles_bound < sms ? tiles_bound : sms;
+  if (grid < 1) grid = 1;
+  tc_gemm_kernel<TcMode::F16X3, CorrEpi<kRelu>><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
 // wide groups on tensor cores; tile_start must already hold the plan (corr_plan_kernel).
 int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* norms, int T, int C, int P,
                         const float* desc, int desc_rows, const float* desc_norm, const int* grp_frame,
                         const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                         int max_tiles, float* maps, int map_stride, float* desc_split_ws, cudaStream_t st,
-                        unsigned long long* tkeys, bool split_ready, int tile_rows) {
+                        unsigned long long* tkeys, bool split_ready, int tile_rows, bool relu, const float* clamp) {
   using Cfg = TcCfg<TcMode::F16X3>;
   static_assert(TC_BN == CORR_TILE, "the tile maxima are per GEMM N tile");
   DTK_CHECK_ARG(C % 8 == 0, "corr (tensor path): C must be a multiple of 8");
+  DTK_CHECK_ARG(relu || tkeys == nullptr, "corr (tensor path): tile keys need the ReLU maps");
   char* d_hi = reinterpret_cast<char*>(desc_split_ws);
   char* d_lo = d_hi + align_up((size_t)desc_rows * C * 2, 256);
   int rc = split_ready ? DINOTRK_OK : launch_split_f16(desc, d_hi, d_lo, (size_t)desc_rows * C, st);
@@ -246,32 +283,17 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
   if ((rc = make_tmap_2d(&tmA_lo, d_lo, desc_rows, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
   if ((rc = make_tmap_3d(&tmB_hi, tpc_hi, T, P, C, b_box, Cfg::kBK, TMAP_F16))) return rc;
   if ((rc = make_tmap_3d(&tmB_lo, tpc_lo, T, P, C, b_box, Cfg::kBK, TMAP_F16))) return rc;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TcMode::F16X3, CorrEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  Cfg::kSmem));
-    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  Cfg::kSmem));
-    attr = true;
-  }
   TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
-  CorrEpi epi{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, tkeys, cdiv(P, CORR_TILE)};
-  const int sms = num_sms();
-  int tiles_bound = max_tiles * cdiv(P, TC_BN);
-  ProfRange pr(PROF_CORR_GEMM, st);
-  if (pairs) {
-    int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
-    if (grid < 2) grid = 2;
-    tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
-    DTK_LAUNCHED();
-    return DINOTRK_OK;
-  }
-  int grid = tiles_bound < sms ? tiles_bound : sms;
-  if (grid < 1) grid = 1;
-  tc_gemm_kernel<TcMode::F16X3, CorrEpi><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
+  const int tiles_bound = max_tiles * cdiv(P, TC_BN);
+  if (relu)
+    return corr_gemm_tc_launch<true>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb,
+                                     CorrEpi<true>{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, tkeys,
+                                                   cdiv(P, CORR_TILE)},
+                                     pairs, tiles_bound, st);
+  return corr_gemm_tc_launch<false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb,
+                                    CorrEpi<false>{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, nullptr,
+                                                   cdiv(P, CORR_TILE), clamp},
+                                    pairs, tiles_bound, st);
 }
 
 }  // namespace dtk

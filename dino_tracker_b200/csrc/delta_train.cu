@@ -290,21 +290,6 @@ __global__ void amax_kernel(const float* __restrict__ g, size_t n, unsigned* __r
   if ((threadIdx.x & 31) == 0) atomicMax(amax, m);
 }
 
-// power of two that puts max |g| in [2^13, 2^14) (1 for an all-zero tensor); exponents clamped to keep 2^e finite
-__device__ __forceinline__ int grad_exp(unsigned amax_bits) {
-  const float m = __uint_as_float(amax_bits);
-  if (!(m > 0.f)) return 0;
-  int e;
-  frexpf(m, &e);
-  e = 14 - e;
-  return e > 126 ? 126 : (e < -126 ? -126 : e);
-}
-
-__device__ __forceinline__ void split16(float v, __half& h, __half& l) {
-  h = __float2half_rn(v);
-  l = __float2half_rn(v - __half2float(h));
-}
-
 // dgrad operand: zero-padded im2col of dY on the padded input domain (Hp = H + 4d, Wp = W + 4d), scaled and split.
 // A[m = (b, py, px)][k = (ky*5 + kx)*C + co] = dY[b][py - ky d][px - kx d][co]  (0 outside the H x W output)
 __global__ void col_dgrad_split_kernel(const float* __restrict__ dy, const unsigned* __restrict__ amax, __half* __restrict__ hi,

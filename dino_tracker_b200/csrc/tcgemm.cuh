@@ -24,6 +24,8 @@
 // Work = grouped tiles: group g covers A rows [row0[g], row0[g] + m[g]) against B batch item batch[g];
 // m-tiles are numbered through the prefix array tile_start[] (device), n-tiles cover N.
 #pragma once
+#include <cuda_fp16.h>
+
 #include <type_traits>
 
 #include "common.cuh"
@@ -58,6 +60,22 @@ struct TcCfg {
   using Acc = std::conditional_t<kS8, int, float>;                // accumulator element
   static_assert(!kS8 || BN == 256, "8-bit mode: m64n256k32 only");
 };
+
+// ---- scaled hi / lo split of gradient operands (delta_train.cu, contrastive.cu) ----
+// power of two that puts max |g| in [2^13, 2^14) (1 for an all-zero tensor); exponents clamped to keep 2^e finite
+__device__ __forceinline__ int grad_exp(unsigned amax_bits) {
+  const float m = __uint_as_float(amax_bits);
+  if (!(m > 0.f)) return 0;
+  int e;
+  frexpf(m, &e);
+  e = 14 - e;
+  return e > 126 ? 126 : (e < -126 ? -126 : e);
+}
+
+__device__ __forceinline__ void split16(float v, __half& h, __half& l) {
+  h = __float2half_rn(v);
+  l = __float2half_rn(v - __half2float(h));
+}
 
 // Epilogues that declare `static constexpr bool kCoalesced = true` are called as vec4(g, row, col, float4) with lanes
 // running along a row; they also provide `bool direct(int col0)` to keep the thread-per-row call for selected column ranges.

@@ -477,6 +477,36 @@ int dinotrk_traj_split_count(const float* traj, int N, int T, const uint8_t* mas
 int dinotrk_traj_split_emit(const float* traj, int N, int T, float* fg, float* bg, void* workspace, size_t workspace_bytes,
                             void* stream);
 
+/* ---- best-buddy contrastive losses of the training step (dino_tracker.py:332-344) -------------------------------- */
+/* get_bb_pairs_contrastive_loss for all pairs of one loss in one call.  E [N][P][C] is the frame set's token-major
+ * embeddings, S / U [B][C] the source / target descriptors of the sampled best buddies; C % 8 == 0.  Group g (host
+ * int32 tables) owns rows [grp_row0[g], grp_row0[g] + grp_rows[g]) and the frame slots grp_src[g] / grp_tgt[g]; groups
+ * do not overlap, empty groups are skipped, rows of no group are ignored (zero gradient).  cos(a, b) = <a, b> /
+ * max(|a| |b|, 1e-8).  Per row r of group g:
+ *   out[0][r] = bb = cos(S_r, U_r)
+ *   out[1][r] = lse_st = log sum_n exp(cos(S_r, E[t_g][n]) / tau),  out[2][r] = lse_ts (U_r against E[s_g])
+ *   out[3][r] = loss_st = lse_st - bb / tau,  out[4][r] = loss_ts = lse_ts - bb / tau
+ *   out[5][r] / out[6][r] = the row sums of both cosine rows
+ * (out = [7][B] fp32).  The forward keeps the cosines in cos [2B][dinotrk_bb_contrastive_cos_stride(P)] (S rows, then U
+ * rows) for the backward.  Cosines run on the split-fp16 wgmma GEMM over copies of E and [S; U] scaled by powers of two
+ * (DESIGN.md 3.3): the results do not depend on the inputs' scale.  The backward takes the forward's cos / out and the upstream gradients of loss_st [B], loss_ts [B] and
+ * of the per-group means mean_r(bb) and (mean(cos_st) + mean(cos_ts)) / 2 ([n_groups] each); it OVERWRITES dS, dU [B][C]
+ * and ADDS the full-frame terms into dE [N][P][C].  Every sum runs in a fixed order: two runs give the same bits.
+ * Argument errors (C, frame slots, rows, a short workspace) return DINOTRK_EINVAL before any launch. */
+int dinotrk_bb_contrastive_cos_stride(int P);
+size_t dinotrk_bb_contrastive_forward_workspace_bytes(int N, int P, int C, int B, int n_groups);
+int dinotrk_bb_contrastive_forward(const float* E, int N, int P, int C, const float* S, const float* U, int B,
+                                   const int* grp_src, const int* grp_tgt, const int* grp_row0, const int* grp_rows, int n_groups,
+                                   float tau, float* cos, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* 0 on invalid arguments */
+size_t dinotrk_bb_contrastive_backward_workspace_bytes(int N, int P, int C, int B, const int* grp_src, const int* grp_tgt,
+                                                       const int* grp_row0, const int* grp_rows, int n_groups);
+int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const float* S, const float* U, int B,
+                                    const int* grp_src, const int* grp_tgt, const int* grp_row0, const int* grp_rows,
+                                    int n_groups, float tau, const float* cos, const float* out, const float* g_st,
+                                    const float* g_ts, const float* g_bbmean, const float* g_cmean, float* dS, float* dU,
+                                    float* dE, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- per-kernel-class device timing (CUDA events on the launching stream; bench.py roofline) ------ */
 int dinotrk_profile_classes(void);
 const char* dinotrk_profile_class_name(int cls);
