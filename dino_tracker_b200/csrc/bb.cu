@@ -219,7 +219,6 @@ int dinotrk_best_buddies_pairs(const dinotrk_features* feat, const dinotrk_geom*
   DTK_CHECK_ARG(C % 8 == 0 && n_pairs >= 0, "best_buddies: C must be a multiple of 8");
   DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_best_buddies_workspace_bytes(n_pairs, P), "best_buddies: workspace too small");
   if (n_pairs == 0) return DINOTRK_OK;
-  using Cfg = TcCfg<TcMode::F16X3>;
   cudaStream_t st = (cudaStream_t)stream;
   const int n_tiles = cdiv(P, TC_BN);
   Arena ar(workspace, workspace_bytes);
@@ -232,26 +231,11 @@ int dinotrk_best_buddies_pairs(const dinotrk_features* feat, const dinotrk_geom*
     bb_plan_kernel<<<cdiv(n_pairs, 128), 128, 0, st>>>(n_pairs, P, pair_src, row0, m, tile_start);
     DTK_LAUNCHED();
   }
-  CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
-  int rc;
-  if ((rc = make_tmap_2d(&tmA_hi, feat->hi, (uint64_t)T * P, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_2d(&tmA_lo, feat->lo, (uint64_t)T * P, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB_hi, feat->hi, T, P, C, TC_BN, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB_lo, feat->lo, T, P, C, TC_BN, Cfg::kBK, TMAP_F16))) return rc;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TcMode::F16X3, BBEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  TcProblem pb{pair_tgt, row0, m, tile_start, n_pairs, P, C};
+  // A: the source frames' tokens, B: the target frames (one batch item per frame)
+  const TcOperands op{feat->hi, feat->lo, (uint64_t)T * P, 0, feat->hi, feat->lo, (uint64_t)T, 0};
+  const TcProblem pb{pair_tgt, row0, m, tile_start, n_pairs, P, C};
   BBEpi epi{feat->norms, pair_src, pair_tgt, part, P, n_tiles};
-  const int sms = num_sms();
-  {
-    ProfRange pr(PROF_BB, st);
-    tc_gemm_kernel<TcMode::F16X3, BBEpi><<<sms, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
-    DTK_LAUNCHED();
-  }
+  if (int rc = tc_launch<TcMode::F16X3, BBEpi>(op, pb, n_pairs * cdiv(P, TC_BM), epi, st, PROF_BB)) return rc;
   {
     ProfRange pr(PROF_BB, st);
     size_t warps = (size_t)n_pairs * P;

@@ -49,10 +49,11 @@ enum ProfClass {
 extern bool g_prof_on;
 void prof_begin(int cls, cudaStream_t st);
 void prof_end(cudaStream_t st);
+// ranges do not nest; a negative class records nothing (for code that runs inside the caller's range)
 struct ProfRange {
   cudaStream_t st;
   bool on;
-  ProfRange(int cls, cudaStream_t s) : st(s), on(g_prof_on) { if (on) prof_begin(cls, st); }
+  ProfRange(int cls, cudaStream_t s) : st(s), on(g_prof_on && cls >= 0) { if (on) prof_begin(cls, st); }
   ~ProfRange() { if (on) prof_end(st); }
 };
 

@@ -164,16 +164,6 @@ cl_drow_kernel(ClGrad gr, int Pp, float* __restrict__ dbuf, float* __restrict__ 
   if (threadIdx.x == 0) rcorr[R] = s;
 }
 
-// max |x| as float bits (a max: the same bits in any order)
-__global__ void cl_amax_kernel(const float* __restrict__ x, size_t n, unsigned* __restrict__ amax) {
-  unsigned m = 0u;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    m = max(m, __float_as_uint(fabsf(x[i])));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) atomicMax(amax, m);
-}
-
 // Descriptor rows of the forward GEMM, warp per row: each row split after its own power of two (max |.| in [2^13, 2^14)),
 // its norm scaled alike, and the reference's 1e-8 clamp carried to the scaled product of the row's and the frame set's
 // norms (same decisions, same quotients as the unscaled product).
@@ -367,41 +357,6 @@ __global__ void cl_tok_corr_kernel(ClGrad gr, const float* __restrict__ E, const
   for (int c = lane; c < C; c += 32) o[c] -= coef * e[c];
 }
 
-// grouped F16X3 GEMM over one K chunk [k0, k0 + kc): A [a_rows][lda] fp16 hi / lo, B [nb][C][ldb]
-template <int BN, class Epi>
-static int cl_gemm(const __half* a_hi, const __half* a_lo, uint64_t a_rows, int lda, const __half* b_hi, const __half* b_lo,
-                   int nb, int C, int ldb, int k0, int kc, const TcProblem& pb0, int tiles, const Epi& epi, cudaStream_t st) {
-  using Cfg = TcCfg<TcMode::F16X3, BN>;
-  CUtensorMap tA_hi, tA_lo, tB_hi, tB_lo;
-  int rc;
-  if ((rc = make_tmap_2d(&tA_hi, a_hi + k0, a_rows, kc, TC_BM, Cfg::kBK, TMAP_F16, lda))) return rc;
-  if ((rc = make_tmap_2d(&tA_lo, a_lo + k0, a_rows, kc, TC_BM, Cfg::kBK, TMAP_F16, lda))) return rc;
-  if ((rc = make_tmap_3d(&tB_hi, b_hi + k0, nb, C, kc, BN, Cfg::kBK, TMAP_F16, ldb))) return rc;
-  if ((rc = make_tmap_3d(&tB_lo, b_lo + k0, nb, C, kc, BN, Cfg::kBK, TMAP_F16, ldb))) return rc;
-  auto kern = tc_gemm_kernel<TcMode::F16X3, Epi, BN>;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  TcProblem pb = pb0;
-  pb.N = C;
-  pb.K = kc;
-  const int all = tiles * cdiv(C, BN), sms = num_sms();
-  kern<<<all < sms ? all : sms, TC_THREADS, Cfg::kSmem, st>>>(tA_hi, tA_lo, tB_hi, tB_lo, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
-
-template <class Epi>
-static int cl_gemm_any(const __half* a_hi, const __half* a_lo, uint64_t a_rows, int lda, const __half* b_hi, const __half* b_lo,
-                       int nb, int C, int ldb, int k0, int kc, const TcProblem& pb, int tiles, const Epi& epi, cudaStream_t st) {
-  if (C <= 64) return cl_gemm<64>(a_hi, a_lo, a_rows, lda, b_hi, b_lo, nb, C, ldb, k0, kc, pb, tiles, epi, st);
-  if (C <= 128) return cl_gemm<128>(a_hi, a_lo, a_rows, lda, b_hi, b_lo, nb, C, ldb, k0, kc, pb, tiles, epi, st);
-  return cl_gemm<256>(a_hi, a_lo, a_rows, lda, b_hi, b_lo, nb, C, ldb, k0, kc, pb, tiles, epi, st);
-}
-
 // ---- host-side plan --------------------------------------------------------------------------------------------------
 // Directional groups: k = g (S rows against frame t_g) and k = G + g (U rows, stored at B + row, against frame s_g).
 struct ClPlan {
@@ -568,8 +523,7 @@ int dinotrk_bb_contrastive_forward(const float* E, int N, int P, int C, const fl
   DTK_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), st));
   const size_t nd = (size_t)2 * B * C;
   const unsigned ge = (unsigned)std::min<size_t>((toks * C + 255) / 256, (size_t)num_sms() * 16);
-  cl_amax_kernel<<<ge, 256, 0, st>>>(E, toks * C, amax);
-  DTK_LAUNCHED();
+  if ((rc = launch_amax(E, toks * C, amax, ge, st))) return rc;
   cl_split_rows_kernel<<<ge, 256, 0, st>>>(E, amax, e_hi, e_lo, toks * C);
   DTK_LAUNCHED();
   __half* d_hi = reinterpret_cast<__half*>(split_ws);   // launch_corr_gemm_tc's layout of a ready split
@@ -697,12 +651,12 @@ int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const f
   cl_transpose_split_kernel<<<dim3(cdiv(Kx, 32), cdiv(C, 32), N), tb, 0, st>>>(SrcDescT{desc, dn, d_frame_rows, C, Kx}, Kx, C,
                                                                                  Kx, b2_hi, b2_lo);
   DTK_LAUNCHED();
-  // GEMM 1: dS / dU over K = P in chains of CL_K_CHUNK, the first chain overwrites
-  TcProblem pb1{d_frame, d_row0, d_m, d_tiles, pl.G2, C, 0};
+  // GEMM 1: dS / dU over K = P in chains of CL_K_CHUNK, the first chain overwrites; one launch per chain [k0, k0 + kc)
   for (int k0 = 0; k0 < P; k0 += CL_K_CHUNK) {
     EpiDesc epi{dS, dU, dn, d_row0, amax, B, C, k0 > 0};
-    if ((rc = cl_gemm_any(a1_hi, a1_lo, (uint64_t)2 * B, Pp, b1_hi, b1_lo, N, C, Pp, k0, std::min(CL_K_CHUNK, P - k0), pb1,
-                          pl.tiles1, epi, st)))
+    const TcProblem pb{d_frame, d_row0, d_m, d_tiles, pl.G2, C, std::min(CL_K_CHUNK, P - k0)};
+    if ((rc = tc_launch_bn<TcMode::F16X3>({a1_hi + k0, a1_lo + k0, (uint64_t)2 * B, (uint64_t)Pp, b1_hi + k0, b1_lo + k0,
+                                           (uint64_t)N, (uint64_t)Pp}, pb, pl.tiles1, epi, st)))
       return rc;
   }
   cl_row_finish_kernel<<<(unsigned)((2 * (size_t)B * 32 + 255) / 256), 256, 0, st>>>(
@@ -712,12 +666,13 @@ int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const f
   cl_tok_corr_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(gr, E, desc, d_frame_rows, d_frame_k, N, Kx, C, dE);
   DTK_LAUNCHED();
   if (pl.tiles2 > 0) {
-    TcProblem pb2{d_fb, d_fr0, d_fm, d_ft, N, C, 0};
     EpiTok epi{dE, en, d_fb, amax, P, C};
-    for (int k0 = 0; k0 < Kx; k0 += CL_K_CHUNK)
-      if ((rc = cl_gemm_any(a2_hi, a2_lo, (uint64_t)N * Pp, Kx, b2_hi, b2_lo, N, C, Kx, k0, std::min(CL_K_CHUNK, Kx - k0), pb2,
-                            pl.tiles2, epi, st)))
+    for (int k0 = 0; k0 < Kx; k0 += CL_K_CHUNK) {
+      const TcProblem pb{d_fb, d_fr0, d_fm, d_ft, N, C, std::min(CL_K_CHUNK, Kx - k0)};
+      if ((rc = tc_launch_bn<TcMode::F16X3>({a2_hi + k0, a2_lo + k0, (uint64_t)N * Pp, (uint64_t)Kx, b2_hi + k0, b2_lo + k0,
+                                             (uint64_t)N, (uint64_t)Kx}, pb, pl.tiles2, epi, st)))
         return rc;
+    }
   }
   return DINOTRK_OK;
 }

@@ -1,4 +1,5 @@
-// Tensor-core correlation GEMM (wgmma, split-precision fp16 hi/lo) + operand splitting + TMA tensor-map helpers.
+// Tensor-core correlation GEMM (wgmma, split-precision fp16 hi/lo) + operand splitting + TMA tensor-map helpers + the
+// uniform group plan and max |x| kernels that tcgemm.cuh declares.
 //
 //   corr[j][p] = relu( <d_j, F[frame][p]> / max(|d_j| |F[frame][p]|, 1e-8) )     (models/tracker.py:158-173)
 // (the ReLU is a template choice: the contrastive losses keep the signed cosines, contrastive.cu)
@@ -127,6 +128,43 @@ int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t 
   return DINOTRK_OK;
 }
 
+// uniform group tables of the wgmma GEMM (tcgemm.cuh, launch_tc_plan)
+__global__ void tc_plan_kernel(int* batch, int* row0, int* m, int* tile_start, int n_groups, int rows, int row_stride,
+                               int row_base, int batch_base, int tile_rows) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    int acc = 0;
+    for (int g = 0; g < n_groups; ++g) {
+      batch[g] = batch_base + g; row0[g] = row_base + g * row_stride; m[g] = rows; tile_start[g] = acc;
+      acc += (rows + tile_rows - 1) / tile_rows;
+    }
+    tile_start[n_groups] = acc;
+  }
+}
+
+int launch_tc_plan(const TcPlan& pl, int n_groups, int rows, int row_stride, int row_base, int batch_base, int tile_rows,
+                   cudaStream_t st) {
+  tc_plan_kernel<<<1, 32, 0, st>>>(pl.batch, pl.row0, pl.m, pl.tile_start, n_groups, rows, row_stride, row_base, batch_base,
+                                   tile_rows);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
+// max |g| as the bits of a non-negative float (integer order = float order; the max does not depend on the order)
+__global__ void amax_kernel(const float* __restrict__ g, size_t n, unsigned* __restrict__ amax) {
+  unsigned m = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    m = max(m, __float_as_uint(fabsf(g[i])));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(amax, m);
+}
+
+int launch_amax(const float* x, size_t n, unsigned* amax, unsigned grid, cudaStream_t st) {
+  amax_kernel<<<grid, 256, 0, st>>>(x, n, amax);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
 // int8 operands of the coarse pass (xw_quant_row): one warp per row; rho_max[row / rows_per_group] = largest rho of the
 // group (float bits: non-negative floats order like their bits; zeroed by the caller)
 __global__ void __launch_bounds__(256)
@@ -231,44 +269,12 @@ int corr_tc_tile_rows() {
 
 size_t corr_tc_workspace_bytes(int total_rows, int C) { return 2 * align_up((size_t)total_rows * C * 2, 256); }
 
-template <bool kRelu>
-static int corr_gemm_tc_launch(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi,
-                               const CUtensorMap& tmB_lo, const TcProblem& pb, const CorrEpi<kRelu>& epi, bool pairs,
-                               int tiles_bound, cudaStream_t st) {
-  using Cfg = TcCfg<TcMode::F16X3>;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TcMode::F16X3, CorrEpi<kRelu>>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  Cfg::kSmem));
-    DTK_CUDA(cudaFuncSetAttribute(tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi<kRelu>>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  const int sms = num_sms();
-  ProfRange pr(PROF_CORR_GEMM, st);
-  if (pairs) {
-    int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
-    if (grid < 2) grid = 2;
-    tc_gemm_pair_kernel<TcMode::F16X3, CorrEpi<kRelu>><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo,
-                                                                                            pb, epi);
-    DTK_LAUNCHED();
-    return DINOTRK_OK;
-  }
-  int grid = tiles_bound < sms ? tiles_bound : sms;
-  if (grid < 1) grid = 1;
-  tc_gemm_kernel<TcMode::F16X3, CorrEpi<kRelu>><<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
-
 // wide groups on tensor cores; tile_start must already hold the plan (corr_plan_kernel).
 int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* norms, int T, int C, int P,
                         const float* desc, int desc_rows, const float* desc_norm, const int* grp_frame,
                         const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                         int max_tiles, float* maps, int map_stride, float* desc_split_ws, cudaStream_t st,
                         unsigned long long* tkeys, bool split_ready, int tile_rows, bool relu, const float* clamp) {
-  using Cfg = TcCfg<TcMode::F16X3>;
   static_assert(TC_BN == CORR_TILE, "the tile maxima are per GEMM N tile");
   DTK_CHECK_ARG(C % 8 == 0, "corr (tensor path): C must be a multiple of 8");
   DTK_CHECK_ARG(relu || tkeys == nullptr, "corr (tensor path): tile keys need the ReLU maps");
@@ -277,23 +283,17 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
   int rc = split_ready ? DINOTRK_OK : launch_split_f16(desc, d_hi, d_lo, (size_t)desc_rows * C, st);
   if (rc) return rc;
   const bool pairs = (tile_rows > 0 ? tile_rows : corr_tc_tile_rows()) == TC2_BM;   // tile_start was planned with this M tile
-  CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
-  const uint32_t b_box = pairs ? TC_BN / 2 : TC_BN;    // a CTA of a pair loads half of the B tile (multicast to both)
-  if ((rc = make_tmap_2d(&tmA_hi, d_hi, desc_rows, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_2d(&tmA_lo, d_lo, desc_rows, C, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB_hi, tpc_hi, T, P, C, b_box, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB_lo, tpc_lo, T, P, C, b_box, Cfg::kBK, TMAP_F16))) return rc;
-  TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
-  const int tiles_bound = max_tiles * cdiv(P, TC_BN);
+  const TcOperands op{d_hi, d_lo, (uint64_t)desc_rows, 0, tpc_hi, tpc_lo, (uint64_t)T, 0};
+  const TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
+  auto run = [&](const auto& epi) {
+    using Epi = std::decay_t<decltype(epi)>;
+    return pairs ? tc_launch<TcMode::F16X3, Epi, TC_BN, true>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM)
+                 : tc_launch<TcMode::F16X3, Epi>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM);
+  };
   if (relu)
-    return corr_gemm_tc_launch<true>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb,
-                                     CorrEpi<true>{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, tkeys,
-                                                   cdiv(P, CORR_TILE)},
-                                     pairs, tiles_bound, st);
-  return corr_gemm_tc_launch<false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb,
-                                    CorrEpi<false>{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, nullptr,
-                                                   cdiv(P, CORR_TILE), clamp},
-                                    pairs, tiles_bound, st);
+    return run(CorrEpi<true>{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, tkeys, cdiv(P, CORR_TILE)});
+  return run(CorrEpi<false>{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, nullptr, cdiv(P, CORR_TILE),
+                            clamp});
 }
 
 }  // namespace dtk

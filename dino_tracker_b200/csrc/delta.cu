@@ -268,36 +268,6 @@ struct EpiConv {
   }
 };
 
-__global__ void conv_plan_kernel(int* batch, int* row0, int* m, int* tile_start, int rows) {
-  if (threadIdx.x == 0) { batch[0] = 0; row0[0] = 0; m[0] = rows; tile_start[0] = 0; tile_start[1] = (rows + TC_BM - 1) / TC_BM; }
-}
-
-template <int BN>
-static int conv_gemm(const __half* a_hi, const __half* a_lo, int rows, int Kp, const __half* w_hi, const __half* w_lo,
-                     int Cout, int* plan, const EpiConv& epi, cudaStream_t st, int prof) {
-  using Cfg = TcCfg<TcMode::F16X3, BN>;
-  CUtensorMap tA_hi, tA_lo, tB_hi, tB_lo;
-  int rc;
-  if ((rc = make_tmap_2d(&tA_hi, a_hi, rows, Kp, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_2d(&tA_lo, a_lo, rows, Kp, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tB_hi, w_hi, 1, Cout, Kp, BN, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tB_lo, w_lo, 1, Cout, Kp, BN, Cfg::kBK, TMAP_F16))) return rc;
-  auto kern = tc_gemm_kernel<TcMode::F16X3, EpiConv, BN>;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  TcProblem pb{plan, plan + 4, plan + 8, plan + 12, 1, Cout, Kp};
-  const int sms = num_sms();
-  int tiles = cdiv(rows, TC_BM) * cdiv(Cout, BN);
-  ProfRange pr(prof, st);
-  kern<<<tiles < sms ? tiles : sms, TC_THREADS, Cfg::kSmem, st>>>(tA_hi, tA_lo, tB_hi, tB_lo, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
-
 size_t delta_conv_kmax(const int* channels) {
   size_t kmax = 0;
   for (int l = 0; l < 4; ++l) { size_t k = align_up((size_t)25 * (l == 0 ? 4 : channels[l]), 8); if (k > kmax) kmax = k; }
@@ -315,20 +285,20 @@ int launch_rgb_to_nhwc4(const float* frames, float* out, int B, int HW, cudaStre
 int launch_conv_tc(const float* in, const __half* w_hi, const __half* w_lo, const float* bias, float* out,
                    ConvShape cs, int Kp, __half* col_hi, __half* col_lo, int* plan, cudaStream_t st, int prof) {
   const size_t M = (size_t)cs.B * cs.H * cs.W;
+  const TcPlan pl{plan, plan + 4, plan + 8, plan + 12};
   for (size_t m0 = 0; m0 < M; m0 += CONV_TC_ROWS) {
     const size_t rows = M - m0 < CONV_TC_ROWS ? M - m0 : CONV_TC_ROWS;
+    int rc;
     {
       ProfRange pr(prof, st);
       im2col_split_kernel<<<(unsigned)rows, 128, 0, st>>>(in, col_hi, col_lo, cs.H, cs.W, cs.Cin, cs.dil, Kp, m0, rows);
       DTK_LAUNCHED();
-      conv_plan_kernel<<<1, 32, 0, st>>>(plan, plan + 4, plan + 8, plan + 12, (int)rows);
-      DTK_LAUNCHED();
+      if ((rc = launch_tc_plan(pl, 1, (int)rows, 0, 0, 0, TC_BM, st))) return rc;
     }
     EpiConv epi{out, bias, cs.Cout, cs.relu, m0};
-    int rc = cs.Cout <= 64 ? conv_gemm<64>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st, prof)
-           : cs.Cout <= 128 ? conv_gemm<128>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st, prof)
-                            : conv_gemm<256>(col_hi, col_lo, (int)rows, Kp, w_hi, w_lo, cs.Cout, plan, epi, st, prof);
-    if (rc) return rc;
+    if ((rc = tc_launch_bn<TcMode::F16X3>({col_hi, col_lo, rows, 0, w_hi, w_lo, 1, 0}, pl.problem(1, cs.Cout, Kp),
+                                          cdiv((int)rows, TC_BM), epi, st, prof)))
+      return rc;
   }
   return DINOTRK_OK;
 }

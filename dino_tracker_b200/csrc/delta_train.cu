@@ -280,16 +280,6 @@ __global__ void bn_backward_kernel(const float* __restrict__ y, float* __restric
   g[i] = (float)(k * d);
 }
 
-// max |g| as the bits of a non-negative float (integer order = float order; the max does not depend on the order)
-__global__ void amax_kernel(const float* __restrict__ g, size_t n, unsigned* __restrict__ amax) {
-  unsigned m = 0;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    m = max(m, __float_as_uint(fabsf(g[i])));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) atomicMax(amax, m);
-}
-
 // dgrad operand: zero-padded im2col of dY on the padded input domain (Hp = H + 4d, Wp = W + 4d), scaled and split.
 // A[m = (b, py, px)][k = (ky*5 + kx)*C + co] = dY[b][py - ky d][px - kx d][co]  (0 outside the H x W output)
 __global__ void col_dgrad_split_kernel(const float* __restrict__ dy, const unsigned* __restrict__ amax, __half* __restrict__ hi,
@@ -475,57 +465,9 @@ struct EpiScaled {
   }
 };
 
-// G groups: group g = A rows [g * rows_per_group, + m) against B batch item g; tile_start = g * ceil(m / TC_BM)
-__global__ void group_plan_kernel(int* plan, int G, int rows_per_group, int m) {
-  for (int g = threadIdx.x; g <= G; g += blockDim.x) {
-    if (g < G) { plan[g] = g; plan[G + g] = g * rows_per_group; plan[2 * G + g] = m; }
-    plan[3 * G + g] = g * ((m + TC_BM - 1) / TC_BM);
-  }
-}
-
-template <int BN>
-static int scaled_gemm(const __half* a_hi, const __half* a_lo, uint64_t a_rows, int K, int ld, const __half* b_hi,
-                       const __half* b_lo, int G, int N, int rows_per_group, int m, int* plan, const EpiScaled& epi, int prof,
-                       cudaStream_t st) {
-  using Cfg = TcCfg<TcMode::F16X3, BN>;
-  CUtensorMap tA_hi, tA_lo, tB_hi, tB_lo;
-  int rc;
-  if ((rc = make_tmap_2d(&tA_hi, a_hi, a_rows, K, TC_BM, Cfg::kBK, TMAP_F16, ld))) return rc;
-  if ((rc = make_tmap_2d(&tA_lo, a_lo, a_rows, K, TC_BM, Cfg::kBK, TMAP_F16, ld))) return rc;
-  if ((rc = make_tmap_3d(&tB_hi, b_hi, G, N, K, BN, Cfg::kBK, TMAP_F16, ld))) return rc;
-  if ((rc = make_tmap_3d(&tB_lo, b_lo, G, N, K, BN, Cfg::kBK, TMAP_F16, ld))) return rc;
-  auto kern = tc_gemm_kernel<TcMode::F16X3, EpiScaled, BN>;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  ProfRange pr(prof, st);
-  group_plan_kernel<<<1, 128, 0, st>>>(plan, G, rows_per_group, m);
-  DTK_LAUNCHED();
-  TcProblem pb{plan, plan + G, plan + 2 * G, plan + 3 * G, G, N, K};
-  const int tiles = G * cdiv(m, TC_BM) * cdiv(N, BN), sms = num_sms();
-  kern<<<tiles < sms ? tiles : sms, TC_THREADS, Cfg::kSmem, st>>>(tA_hi, tA_lo, tB_hi, tB_lo, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
-
-static int gemm_bn(int N) { return N <= 64 ? 64 : N <= 128 ? 128 : 256; }
-
-static int scaled_gemm_any(const __half* a_hi, const __half* a_lo, uint64_t a_rows, int K, int ld, const __half* b_hi,
-                           const __half* b_lo, int G, int N, int rows_per_group, int m, int* plan, const EpiScaled& epi, int prof,
-                           cudaStream_t st) {
-  switch (gemm_bn(N)) {
-    case 64: return scaled_gemm<64>(a_hi, a_lo, a_rows, K, ld, b_hi, b_lo, G, N, rows_per_group, m, plan, epi, prof, st);
-    case 128: return scaled_gemm<128>(a_hi, a_lo, a_rows, K, ld, b_hi, b_lo, G, N, rows_per_group, m, plan, epi, prof, st);
-    default: return scaled_gemm<256>(a_hi, a_lo, a_rows, K, ld, b_hi, b_lo, G, N, rows_per_group, m, plan, epi, prof, st);
-  }
-}
-
 // pixel splits of a layer's weight-gradient GEMM: S groups (a fixed function of the shape) of Kc pixels per launch
 static void wgrad_split(const TrainGeom& g, int l, size_t col_elems, int* S_out, int* Kc_out) {
-  const int tiles = cdiv(g.cout[l], TC_BM) * cdiv(g.Kp[l], gemm_bn(g.Kp[l]));
+  const int tiles = cdiv(g.cout[l], TC_BM) * cdiv(g.Kp[l], tc_bn(g.Kp[l]));
   int S = cdiv(WG_TARGET_TILES, tiles);
   S = S < 1 ? 1 : (S > WG_MAX_SPLITS ? WG_MAX_SPLITS : S);
   const size_t per = (size_t)S * (g.cout[l] + g.Kp[l]);
@@ -800,8 +742,7 @@ int dinotrk_delta_train_backward(const float* frames, int B, int H, int W, const
       chan_sum_kernel<<<cb, 128, 0, st>>>(ws.part, nblk, C, grad_bias[l]);
       DTK_LAUNCHED();
       DTK_CUDA(cudaMemsetAsync(ws.amax, 0, sizeof(unsigned), st));
-      amax_kernel<<<1024, 256, 0, st>>>(ws.g, M * C, ws.amax);
-      DTK_LAUNCHED();
+      if (int rc = launch_amax(ws.g, M * C, ws.amax, 1024, st)) return rc;
       if (int rc = layer_input(frames, g, l, sv, bn_weight, bn_bias, ws.x, st)) return rc;
     }
     {   // weight gradient: pixel chunks of S x Kc, S groups per launch, partials summed in order
@@ -821,10 +762,15 @@ int dinotrk_delta_train_backward(const float* frames, int B, int H, int W, const
                                                                                       g.dil[l], Kp, M, p0, Kc);
           DTK_LAUNCHED();
         }
-        EpiScaled epi{ws.wpart, ws.amax, (size_t)Kp, 0, C, 0};
-        if (int rc = scaled_gemm_any(a_hi, a_lo, (uint64_t)S * C, Kc, Kc, b_hi, b_lo, S, Kp, C, C, ws.plan, epi, PROF_DELTA_WGRAD,
-                                     st))
-          return rc;
+        {   // S groups: group s = the C rows of dY^T chunk s against the im2col^T chunk s
+          ProfRange pr(PROF_DELTA_WGRAD, st);
+          const TcPlan pl{ws.plan, ws.plan + S, ws.plan + 2 * S, ws.plan + 3 * S};
+          if (int rc = launch_tc_plan(pl, S, C, C, 0, 0, TC_BM, st)) return rc;
+          EpiScaled epi{ws.wpart, ws.amax, (size_t)Kp, 0, C, 0};
+          if (int rc = tc_launch_bn<TcMode::F16X3>({a_hi, a_lo, (uint64_t)S * C, (uint64_t)Kc, b_hi, b_lo, (uint64_t)S, (uint64_t)Kc},
+                                                   pl.problem(S, Kp, Kc), S * cdiv(C, TC_BM), epi, st))
+            return rc;
+        }
         ProfRange pr(PROF_DELTA_WGRAD, st);
         const size_t n = (size_t)C * Kp;
         wgrad_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws.wpart, S, n, ws.wacc, p0 == 0,
@@ -847,9 +793,13 @@ int dinotrk_delta_train_backward(const float* frames, int B, int H, int W, const
         }
         for (int k0 = 0; k0 < Kd; k0 += GEMM_K_CHUNK) {   // K slices summed into the output in order
           const int kc = Kd - k0 < GEMM_K_CHUNK ? Kd - k0 : GEMM_K_CHUNK;
+          ProfRange pr(PROF_DELTA_DGRAD, st);
+          const TcPlan pl{ws.plan, ws.plan + 1, ws.plan + 2, ws.plan + 3};
+          if (int rc = launch_tc_plan(pl, 1, (int)rows, 0, 0, 0, TC_BM, st)) return rc;
           EpiScaled epi{ws.xp, ws.amax, (size_t)N, m0, 0, k0 > 0};
-          if (int rc = scaled_gemm_any(ws.col_hi + k0, ws.col_lo + k0, rows, kc, Kd, (const __half*)wgtT_hi[l] + k0,
-                                       (const __half*)wgtT_lo[l] + k0, 1, N, 0, (int)rows, ws.plan, epi, PROF_DELTA_DGRAD, st))
+          if (int rc = tc_launch_bn<TcMode::F16X3>({ws.col_hi + k0, ws.col_lo + k0, rows, (uint64_t)Kd, (const __half*)wgtT_hi[l] + k0,
+                                                    (const __half*)wgtT_lo[l] + k0, 1, (uint64_t)Kd},
+                                                   pl.problem(1, N, kc), cdiv((int)rows, TC_BM), epi, st))
             return rc;
         }
       }

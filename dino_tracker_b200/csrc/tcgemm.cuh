@@ -320,4 +320,71 @@ tc_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   tc_gemm_body<MODE, Epi, BN, true>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, pb, epi);
 }
 
+// ---- host side ----
+// Device group tables of a TcProblem
+struct TcPlan {
+  int* batch; int* row0; int* m; int* tile_start;
+  TcProblem problem(int n_groups, int N, int K) const { return {batch, row0, m, tile_start, n_groups, N, K}; }
+};
+
+// Uniform tables: group g = `rows` A rows from row_base + g * row_stride against B batch item batch_base + g, in M tiles of
+// tile_rows (TC_BM, or TC2_BM for the pair kernel).  One single-thread launch (corr_tc.cu).
+int launch_tc_plan(const TcPlan& pl, int n_groups, int rows, int row_stride, int row_base, int batch_base, int tile_rows,
+                   cudaStream_t st);
+
+// *amax = max(*amax, max |x|) as the bits of a non-negative float, for grad_exp (corr_tc.cu; 256 threads per block)
+int launch_amax(const float* x, size_t n, unsigned* amax, unsigned grid, cudaStream_t st);
+
+// Operands: A [a_rows][K], B [b_batch][N][K], row pitches lda / ldb in elements (0: dense).  The lo parts are read in the
+// split modes only (TcCfg::kOps == 2).
+struct TcOperands {
+  const void* a_hi; const void* a_lo; uint64_t a_rows, lda;
+  const void* b_hi; const void* b_lo; uint64_t b_batch, ldb;
+};
+
+// One launch of tc_gemm_kernel (or tc_gemm_pair_kernel when PAIR) on pb.  m_tiles bounds the M tiles of the plan (TC_BM
+// rows, TC2_BM for pairs); the grid is one CTA (pair) per output tile up to one per SM, at least one.  prof >= 0 times the
+// launch under that profile class.
+template <TcMode MODE, class Epi, int BN = TC_BN, bool PAIR = false>
+int tc_launch(const TcOperands& op, const TcProblem& pb, int m_tiles, const Epi& epi, cudaStream_t st, int prof = -1) {
+  using Cfg = TcCfg<MODE, BN>;
+  constexpr int elem = MODE == TcMode::S8 ? TMAP_S8 : MODE == TcMode::BF16 ? TMAP_BF16 : Cfg::kElem == 2 ? TMAP_F16 : TMAP_F32;
+  CUtensorMap ta[2], tb[2];
+  for (int i = 0; i < Cfg::kOps; ++i) {   // single-pass modes pass the hi maps twice
+    if (int rc = make_tmap_2d(&ta[i], i ? op.a_lo : op.a_hi, op.a_rows, pb.K, TC_BM, Cfg::kBK, elem, op.lda)) return rc;
+    if (int rc = make_tmap_3d(&tb[i], i ? op.b_lo : op.b_hi, op.b_batch, pb.N, pb.K, PAIR ? BN / 2 : BN, Cfg::kBK, elem, op.ldb))
+      return rc;
+  }
+  const auto kern = [] {   // if constexpr: only the kernel launched here is instantiated
+    if constexpr (PAIR) return tc_gemm_pair_kernel<MODE, Epi, BN>;
+    else return tc_gemm_kernel<MODE, Epi, BN>;
+  }();
+  static PerDev<bool> attr_dev;   // one per instantiation
+  bool& attr = attr_dev.get();
+  if (!attr) {
+    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+    attr = true;
+  }
+  const int units = PAIR ? num_sms() / 2 : num_sms();
+  long long n = (long long)m_tiles * cdiv(pb.N, BN);
+  if (n > units) n = units;
+  const int grid = (PAIR ? 2 : 1) * (n < 1 ? 1 : (int)n);
+  ProfRange pr(prof, st);
+  kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(ta[0], ta[Cfg::kOps - 1], tb[0], tb[Cfg::kOps - 1], pb, epi);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
+// N tile by N: 64, 128 or 256
+inline int tc_bn(int N) { return N <= 64 ? 64 : N <= 128 ? 128 : 256; }
+
+template <TcMode MODE, class Epi>
+int tc_launch_bn(const TcOperands& op, const TcProblem& pb, int m_tiles, const Epi& epi, cudaStream_t st, int prof = -1) {
+  switch (tc_bn(pb.N)) {
+    case 64: return tc_launch<MODE, Epi, 64>(op, pb, m_tiles, epi, st, prof);
+    case 128: return tc_launch<MODE, Epi, 128>(op, pb, m_tiles, epi, st, prof);
+    default: return tc_launch<MODE, Epi, 256>(op, pb, m_tiles, epi, st, prof);
+  }
+}
+
 }  // namespace dtk

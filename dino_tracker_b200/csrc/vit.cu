@@ -134,19 +134,6 @@ __global__ void vit_tap_kernel(const float* __restrict__ x, float* __restrict__ 
   reinterpret_cast<float4*>(tpc)[i] = reinterpret_cast<const float4*>(x)[((b * (P + 1) + 1 + p)) * n4 + c];
 }
 
-// group tables for the GEMMs: kind 0: one group of m rows; kind 1: `heads` groups (attention)
-__global__ void vit_plan_kernel(int* batch, int* row0, int* m, int* tile_start, int n_groups, int rows, int row_stride,
-                                int row_base, int batch_base, int tile_rows) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    int acc = 0;
-    for (int g = 0; g < n_groups; ++g) {
-      batch[g] = batch_base + g; row0[g] = row_base + g * row_stride; m[g] = rows; tile_start[g] = acc;
-      acc += (rows + tile_rows - 1) / tile_rows;
-    }
-    tile_start[n_groups] = acc;
-  }
-}
-
 // ---------------------------------------------------------------------------------------------- epilogues
 struct EpiBase {
   struct State {};
@@ -368,70 +355,16 @@ struct EpiGelu : EpiBase {
   }
 };
 
-struct Plan { int* batch; int* row0; int* m; int* tile_start; };
-
-template <class Epi, int BN, TcMode MODE = TcMode::TF32>
-static int run_gemm(const void* A, uint64_t a_rows, const void* Bm, uint64_t b_batch, uint64_t b_rows, int K,
-                    const Plan& pl, int n_groups, int max_tiles, const Epi& epi, int prof_cls, cudaStream_t st,
-                    uint64_t ld = 0) {
-  using Cfg = TcCfg<MODE, BN>;
-  constexpr int kT = MODE == TcMode::F16 ? TMAP_F16 : TMAP_F32;
-  CUtensorMap tmA, tmB;
-  int rc;
-  if ((rc = make_tmap_2d(&tmA, A, a_rows, K, TC_BM, Cfg::kBK, kT, ld))) return rc;
-  if ((rc = make_tmap_3d(&tmB, Bm, b_batch, b_rows, K, BN, Cfg::kBK, kT, ld))) return rc;
-  auto kern = tc_gemm_kernel<MODE, Epi, BN>;
-  static PerDev<bool> attr_dev;  // one static per template instantiation
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  TcProblem pb{pl.batch, pl.row0, pl.m, pl.tile_start, n_groups, (int)b_rows, K};
-  const int sms = num_sms();
-  int tiles = max_tiles * cdiv((int)b_rows, BN);
-  int grid = tiles < sms ? tiles : sms;
-  ProfRange pr(prof_cls, st);
-  kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
-
-static int plan(const Plan& pl, int n_groups, int rows, int row_stride, int row_base, int batch_base, cudaStream_t st,
+// group tables for the GEMMs: one group of `rows` rows, or `heads` groups (attention)
+static int plan(const TcPlan& pl, int n_groups, int rows, int row_stride, int row_base, int batch_base, cudaStream_t st,
                 int tile_rows = TC_BM) {
   ProfRange pr(PROF_VIT_MISC, st);
-  vit_plan_kernel<<<1, 32, 0, st>>>(pl.batch, pl.row0, pl.m, pl.tile_start, n_groups, rows, row_stride, row_base, batch_base,
-                                    tile_rows);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
+  return launch_tc_plan(pl, n_groups, rows, row_stride, row_base, batch_base, tile_rows, st);
 }
 
-// CTA-pair variant (a cluster of two CTAs sharing the B tile by multicast, 256 x 256 tiles) for the single-pass fp16
-// linear layers; the plan must be in 256-row tiles.
-template <class Epi>
-static int run_gemm_pair(const void* A, uint64_t a_rows, const void* Bm, uint64_t b_rows, int K, const Plan& pl,
-                         int max_tiles, const Epi& epi, int prof_cls, cudaStream_t st) {
-  using Cfg = TcCfg<TcMode::F16, TC_BN>;
-  CUtensorMap tmA, tmB;
-  int rc;
-  if ((rc = make_tmap_2d(&tmA, A, a_rows, K, TC_BM, Cfg::kBK, TMAP_F16))) return rc;
-  if ((rc = make_tmap_3d(&tmB, Bm, 1, b_rows, K, TC_BN / 2, Cfg::kBK, TMAP_F16))) return rc;
-  auto kern = tc_gemm_pair_kernel<TcMode::F16, Epi, TC_BN>;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  TcProblem pb{pl.batch, pl.row0, pl.m, pl.tile_start, 1, (int)b_rows, K};
-  const int sms = num_sms();
-  int pairs = max_tiles * cdiv((int)b_rows, TC_BN);
-  int grid = 2 * (pairs < sms / 2 ? pairs : sms / 2);
-  ProfRange pr(prof_cls, st);
-  kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
+// The linear layers run on the CTA-pair kernel (a cluster of two CTAs sharing the B tile by multicast, 256 x 256 tiles,
+// single-pass fp16; the plan must be in 256-row tiles), or on the one-CTA kernel in fp16 or TF32.  a [rows][K] . w^T
+static TcOperands linear_operands(const void* a, uint64_t rows, const void* w) { return {a, nullptr, rows, 0, w, nullptr, 1, 0}; }
 
 constexpr int VIT_ROW_CHUNK = 1024;  // query rows per attention-score chunk
 
@@ -482,7 +415,7 @@ static VitShape vit_shape(const dinotrk_vit_config* c, const dinotrk_geom* g, in
   return s;
 }
 
-static int vit_row_plan(const VitShape& s, const Plan& pl, cudaStream_t st) {
+static int vit_row_plan(const VitShape& s, const TcPlan& pl, cudaStream_t st) {
   return plan(pl, 1, (int)s.rows, 0, 0, 0, st, s.pairs ? TC2_BM : TC_BM);
 }
 
@@ -497,51 +430,61 @@ static int vit_layernorm(const VitShape& s, const float* x, const float* gw, con
 }
 
 // x[b][1 + p] = cols[b P + p] . patch_w + bias + pos[p]; cols [B P][Kp] (makes its own 128-row tile plan)
-static int vit_patch_embed(const VitShape& s, const Plan& pl, const void* cols, const void* w, const float* bias,
+static int vit_patch_embed(const VitShape& s, const TcPlan& pl, const void* cols, const void* w, const float* bias,
                            const float* pos, float* x, cudaStream_t st) {
   int rc;
   if ((rc = plan(pl, 1, s.B * s.P, 0, 0, 0, st))) return rc;
   EpiPatch ep{{}, x, bias, pos, s.P, s.D};
+  const TcOperands op = linear_operands(cols, (uint64_t)s.B * s.P, w);
   const int tiles = cdiv(s.B * s.P, TC_BM);
-  return s.f16 ? run_gemm<EpiPatch, 256, TcMode::F16>(cols, (uint64_t)s.B * s.P, w, 1, s.D, s.Kp, pl, 1, tiles, ep, PROF_VIT_GEMM, st)
-               : run_gemm<EpiPatch, 256>(cols, (uint64_t)s.B * s.P, w, 1, s.D, s.Kp, pl, 1, tiles, ep, PROF_VIT_GEMM, st);
+  return s.f16 ? tc_launch<TcMode::F16, EpiPatch>(op, pl.problem(1, s.D, s.Kp), tiles, ep, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, EpiPatch>(op, pl.problem(1, s.D, s.Kp), tiles, ep, st, PROF_VIT_GEMM);
 }
 
 // qkv for the fused attention: y [rows][D] . qkv_w^T + bias -> fp16 q (scaled by 64^-1/2 log2 e), k, v^T (pitch align8(N1))
-static int vit_qkv_fused(const VitShape& s, const Plan& pl, const void* y, const void* w, const float* bias, __half* q16,
+static int vit_qkv_fused(const VitShape& s, const TcPlan& pl, const void* y, const void* w, const float* bias, __half* q16,
                          __half* k16, __half* v16, cudaStream_t st) {
   const int D = s.D, N1p8 = (int)align_up((size_t)s.N1, 8);
   EpiQKV16 eq{{}, q16, k16, v16, bias, s.N1, D, s.heads, N1p8, 0.125f * 1.4426950408889634f};  // 1/sqrt(64) * log2(e)
   static const int epi_direct = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;   // bit 0: q / k thread-per-row too (slower)
   eq.direct_from = (epi_direct & 1) ? 0 : 2 * D;
-  return s.pairs ? run_gemm_pair<EpiQKV16>(y, s.rows, w, 3 * D, D, pl, cdiv((int)s.rows, TC2_BM), eq, PROF_VIT_GEMM, st)
-       : s.f16 ? run_gemm<EpiQKV16, 256, TcMode::F16>(y, s.rows, w, 1, 3 * D, D, pl, 1, cdiv((int)s.rows, TC_BM), eq, PROF_VIT_GEMM, st)
-               : run_gemm<EpiQKV16, 256>(y, s.rows, w, 1, 3 * D, D, pl, 1, cdiv((int)s.rows, TC_BM), eq, PROF_VIT_GEMM, st);
+  const TcOperands op = linear_operands(y, s.rows, w);
+  const TcProblem pb = pl.problem(1, 3 * D, D);
+  const int tiles = cdiv((int)s.rows, TC_BM);
+  return s.pairs ? tc_launch<TcMode::F16, EpiQKV16, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), eq, st, PROF_VIT_GEMM)
+       : s.f16 ? tc_launch<TcMode::F16, EpiQKV16>(op, pb, tiles, eq, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, EpiQKV16>(op, pb, tiles, eq, st, PROF_VIT_GEMM);
 }
 
 // x[r] += ls * (a[r] . w^T + bias), a [rows][K]: proj (K = D) and fc2 (K = 4 D)
-static int vit_residual(const VitShape& s, const Plan& pl, const void* a, const void* w, int K, const float* bias,
+static int vit_residual(const VitShape& s, const TcPlan& pl, const void* a, const void* w, int K, const float* bias,
                         const float* ls, float* x, cudaStream_t st) {
   EpiResidual er{{}, x, bias, ls, s.D};
-  return s.pairs ? run_gemm_pair<EpiResidual>(a, s.rows, w, s.D, K, pl, cdiv((int)s.rows, TC2_BM), er, PROF_VIT_GEMM, st)
-       : s.f16 ? run_gemm<EpiResidual, 256, TcMode::F16>(a, s.rows, w, 1, s.D, K, pl, 1, cdiv((int)s.rows, TC_BM), er, PROF_VIT_GEMM, st)
-               : run_gemm<EpiResidual, 256>(a, s.rows, w, 1, s.D, K, pl, 1, cdiv((int)s.rows, TC_BM), er, PROF_VIT_GEMM, st);
+  const TcOperands op = linear_operands(a, s.rows, w);
+  const TcProblem pb = pl.problem(1, s.D, K);
+  const int tiles = cdiv((int)s.rows, TC_BM);
+  return s.pairs ? tc_launch<TcMode::F16, EpiResidual, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), er, st, PROF_VIT_GEMM)
+       : s.f16 ? tc_launch<TcMode::F16, EpiResidual>(op, pb, tiles, er, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, EpiResidual>(op, pb, tiles, er, st, PROF_VIT_GEMM);
 }
 
 // h = gelu(y . fc1_w^T + bias), y [rows][D] -> h [rows][4 D] (fp16 in fp16 operand mode)
-static int vit_fc1(const VitShape& s, const Plan& pl, const void* y, const void* w, const float* bias, void* h, cudaStream_t st) {
+static int vit_fc1(const VitShape& s, const TcPlan& pl, const void* y, const void* w, const float* bias, void* h, cudaStream_t st) {
   const int D = s.D;
+  const TcOperands op = linear_operands(y, s.rows, w);
+  const TcProblem pb = pl.problem(1, 4 * D, D);
+  const int tiles = cdiv((int)s.rows, TC_BM);
   if (s.pairs) {
     EpiGelu<__half> eg{{}, reinterpret_cast<__half*>(h), bias, 4 * D};
     static const int epi_direct2 = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;  // bit 1: fp16 GELU rows written thread-per-row (64 B per thread, whole sectors)
     eg.all_direct = (epi_direct2 & 2) ? 1 : 0;
-    return run_gemm_pair<EpiGelu<__half>>(y, s.rows, w, 4 * D, D, pl, cdiv((int)s.rows, TC2_BM), eg, PROF_VIT_GEMM, st);
+    return tc_launch<TcMode::F16, EpiGelu<__half>, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), eg, st, PROF_VIT_GEMM);
   }
   if (s.f16)
-    return run_gemm<EpiGelu<__half>, 256, TcMode::F16>(y, s.rows, w, 1, 4 * D, D, pl, 1, cdiv((int)s.rows, TC_BM),
-                                                       EpiGelu<__half>{{}, reinterpret_cast<__half*>(h), bias, 4 * D}, PROF_VIT_GEMM, st);
-  return run_gemm<EpiGelu<float>, 256>(y, s.rows, w, 1, 4 * D, D, pl, 1, cdiv((int)s.rows, TC_BM),
-                                       EpiGelu<float>{{}, reinterpret_cast<float*>(h), bias, 4 * D}, PROF_VIT_GEMM, st);
+    return tc_launch<TcMode::F16, EpiGelu<__half>>(op, pb, tiles, EpiGelu<__half>{{}, reinterpret_cast<__half*>(h), bias, 4 * D}, st,
+                                                   PROF_VIT_GEMM);
+  return tc_launch<TcMode::TF32, EpiGelu<float>>(op, pb, tiles, EpiGelu<float>{{}, reinterpret_cast<float*>(h), bias, 4 * D}, st,
+                                                 PROF_VIT_GEMM);
 }
 
 }  // namespace dtk
@@ -594,7 +537,7 @@ int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom
   cudaStream_t st = (cudaStream_t)stream;
   const VitShape s = vit_shape(c, g, B);
   Arena ar(workspace, workspace_bytes);
-  Plan pl{ar.take<int>(2), ar.take<int>(2), ar.take<int>(2), ar.take<int>(2)};
+  TcPlan pl{ar.take<int>(2), ar.take<int>(2), ar.take<int>(2), ar.take<int>(2)};
   if (!ar.ok()) return DINOTRK_EINVAL;
   if (stage == DINOTRK_VIT_LAYERNORM) return vit_layernorm(s, reinterpret_cast<const float*>(in), p0, p1, out0, st);
   if (stage == DINOTRK_VIT_PATCH) return vit_patch_embed(s, pl, in, w, p0, p1, reinterpret_cast<float*>(out0), st);
@@ -631,7 +574,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   size_t hid = rows * 4 * D, col = (size_t)B * P * Kp;
   float* hbuf = ar.take<float>(hid > col ? hid : col);
   float* S = ar.take<float>((size_t)heads * VIT_ROW_CHUNK * N1p);
-  Plan pl{ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2)};
+  TcPlan pl{ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2)};
   DTK_CHECK_ARG(ar.ok(), "vit_forward: workspace arena overflow");
   int rc;
 
@@ -672,25 +615,26 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
       if ((rc = vit_qkv_fused(s, pl, y, w[2], w[3], q16, k16, v16, st))) return rc;
       if ((rc = launch_flash(q16, k16, v16, B, heads, N1, (int)align_up((size_t)N1, 8), D, y, f16, st))) return rc;
     } else {
-      if ((rc = run_gemm<EpiQKV, 256>(y, rows, w[2], 1, 3 * D, D, pl, 1, all_tiles, EpiQKV{{}, q, k, vT, w[3], N1, D, heads, N1p},
-                                      PROF_VIT_GEMM, st))) return rc;
+      if ((rc = tc_launch<TcMode::TF32, EpiQKV>(linear_operands(y, rows, w[2]), pl.problem(1, 3 * D, D), all_tiles,
+                                                EpiQKV{{}, q, k, vT, w[3], N1, D, heads, N1p}, st, PROF_VIT_GEMM))) return rc;
       // attention, per frame and chunk of query rows: S = q k^T (all heads) -> softmax -> y = S v
       for (int b = 0; b < B; ++b) {
         for (int c0 = 0; c0 < N1; c0 += VIT_ROW_CHUNK) {
           const int rc_rows = N1 - c0 < VIT_ROW_CHUNK ? N1 - c0 : VIT_ROW_CHUNK;
           if ((rc = plan(pl, heads, rc_rows, N1, (b * heads) * N1 + c0, b * heads, st))) return rc;
-          if ((rc = run_gemm<EpiStore, 256>(q, rows * heads, k, (uint64_t)B * heads, N1, HD, pl, heads,
-                                            heads * cdiv(rc_rows, TC_BM), EpiStore{{}, S, N1p, VIT_ROW_CHUNK},
-                                            PROF_VIT_ATTN, st))) return rc;
+          if ((rc = tc_launch<TcMode::TF32, EpiStore>({q, nullptr, rows * heads, 0, k, nullptr, (uint64_t)B * heads, 0},
+                                                      pl.problem(heads, N1, HD), heads * cdiv(rc_rows, TC_BM),
+                                                      EpiStore{{}, S, N1p, VIT_ROW_CHUNK}, st, PROF_VIT_ATTN))) return rc;
           {
             ProfRange pr(PROF_VIT_ATTN, st);  // rows of S live at (head * VIT_ROW_CHUNK + r)
             vit_softmax_kernel<<<dim3(rc_rows, heads), 256, (size_t)N1 * 4, st>>>(S, N1, N1p, (size_t)VIT_ROW_CHUNK * N1p);
             DTK_LAUNCHED();
           }
           if ((rc = plan(pl, heads, rc_rows, VIT_ROW_CHUNK, 0, b * heads, st))) return rc;
-          if ((rc = run_gemm<EpiPV, 64>(S, (uint64_t)heads * VIT_ROW_CHUNK, vT, (uint64_t)B * heads, HD, N1, pl, heads,
-                                        heads * cdiv(rc_rows, TC_BM), EpiPV{{}, y, (size_t)b * N1 + c0, D},
-                                        PROF_VIT_ATTN, st, (uint64_t)N1p))) return rc;
+          if ((rc = tc_launch<TcMode::TF32, EpiPV, 64>({S, nullptr, (uint64_t)heads * VIT_ROW_CHUNK, (uint64_t)N1p, vT, nullptr,
+                                                        (uint64_t)B * heads, (uint64_t)N1p},
+                                                       pl.problem(heads, HD, N1), heads * cdiv(rc_rows, TC_BM),
+                                                       EpiPV{{}, y, (size_t)b * N1 + c0, D}, st, PROF_VIT_ATTN))) return rc;
         }
       }
     }

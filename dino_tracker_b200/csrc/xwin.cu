@@ -118,32 +118,6 @@ int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cuda
   return DINOTRK_OK;
 }
 
-template <TcMode MODE, class Acc>
-static int launch_coarse(const void* desc, int desc_rows, const void* tok, const FeatView& fv, const TcProblem& pb,
-                         const CoarseEpi<Acc>& epi, int max_tiles, cudaStream_t st) {
-  using Cfg = TcCfg<MODE, XW_GEMM_BN>;
-  constexpr int elem = MODE == TcMode::S8 ? TMAP_S8 : TMAP_F16;
-  CUtensorMap tmA, tmB;
-  int rc;
-  if ((rc = make_tmap_2d(&tmA, desc, desc_rows, fv.C, TC_BM, Cfg::kBK, elem))) return rc;
-  if ((rc = make_tmap_3d(&tmB, tok, fv.T, fv.P, fv.C, XW_GEMM_BN / 2, Cfg::kBK, elem))) return rc;
-  auto kern = tc_gemm_pair_kernel<MODE, CoarseEpi<Acc>, XW_GEMM_BN>;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr = true;
-  }
-  const int sms = num_sms();
-  const int tiles_bound = max_tiles * cdiv(fv.P, XW_GEMM_BN);
-  int grid = 2 * (tiles_bound < sms / 2 ? tiles_bound : sms / 2);
-  if (grid < 2) grid = 2;
-  ProfRange pr(PROF_XW_COARSE, st);
-  kern<<<grid, TC_THREADS, Cfg::kSmem, st>>>(tmA, tmA, tmB, tmB, pb, epi);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
-}
-
 int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
                      const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                      int max_tiles, const XwChunk& xc, cudaStream_t st, const float* rnorms, const void* desc_q8,
@@ -154,10 +128,12 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
     DTK_CHECK_ARG(fv.s8() && fv.C % 16 == 0 && fv.C <= XW_S8_MAX_C, "int8 coarse pass: needs the int8 features, C %% 16 == 0 "
                   "and C <= %d", XW_S8_MAX_C);
     CoarseEpi<int> epi{fv.q_fac, desc_fac, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
-    return launch_coarse<TcMode::S8>(desc_q8, desc_rows, fv.q8, fv, pb, epi, max_tiles, st);
+    return tc_launch<TcMode::S8, CoarseEpi<int>, XW_GEMM_BN, true>({desc_q8, nullptr, (uint64_t)desc_rows, 0, fv.q8, nullptr,
+                                                                    (uint64_t)fv.T, 0}, pb, max_tiles, epi, st, PROF_XW_COARSE);
   }
   CoarseEpi<float> epi{rnorms, desc_norm, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
-  return launch_coarse<TcMode::F16>(desc_hi, desc_rows, fv.hi, fv, pb, epi, max_tiles, st);
+  return tc_launch<TcMode::F16, CoarseEpi<float>, XW_GEMM_BN, true>({desc_hi, nullptr, (uint64_t)desc_rows, 0, fv.hi, nullptr,
+                                                                     (uint64_t)fv.T, 0}, pb, max_tiles, epi, st, PROF_XW_COARSE);
 }
 
 // ====================================================================================================== 2. plan

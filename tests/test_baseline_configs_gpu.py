@@ -107,7 +107,7 @@ def test_config1_against_gpu_oracle(C):
 
 def test_delta_dino_shipped_widths_against_gpu_oracle():
     """a2 at the widths the reference ships ([3, 64, 128, 256, 1024], models/networks/delta_dino.py:10) on full frames:
-    the conv_gemm<256> instantiation with K = 6400 and dilation 2 that bench.py times."""
+    the convolution GEMM with 256-column tiles, K = 6400 and dilation 2 that bench.py times."""
     from dino_tracker_b200 import Tracker
     oracle.use_exact_fp32()
     channels = [3, 64, 128, 256, 1024]
