@@ -149,6 +149,12 @@ SIGNATURES = {
     "dinotrk_bb_contrastive_backward_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int]),
     "dinotrk_bb_contrastive_backward": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_float, _P, _P,
                                                 _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_sampler_workspace_bytes": (c_size_t, [c_int]),
+    "dinotrk_sampler_prepare_count": (c_int, [_P, c_int, c_int, POINTER(c_int), _P, c_size_t, _P]),
+    "dinotrk_sampler_prepare_emit": (c_int, [_P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_sampler_count": (c_int, [_P, c_int, c_int, _P, c_int, POINTER(c_int), _P, c_size_t, _P]),
+    "dinotrk_sampler_select": (c_int, [_P, c_int, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_sampler_gather": (c_int, [_P, c_int, _P, _P, c_int, _P, _P, _P]),
 }
 
 

@@ -507,6 +507,34 @@ int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const f
                                     const float* g_ts, const float* g_bbmean, const float* g_cmean, float* dS, float* dU,
                                     float* dE, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- training-batch sampler (data/dataset.py:56-258 LongRangeSampler / DinoTrackerSampler) ------------------------ */
+/* Trajectories traj [N][T][2] fp32 (NaN where missing).  The sampler stores the valid rows (more than one step with both
+ * coordinates non-NaN, dataset.py:100-106) in their order, rows [N'][T][2], and per stored row the bitmask of its valid
+ * steps, bits [N'][ceil(T / 32)] uint32 (bit t % 32 of word t / 32).  traj, rows (and gather's rows) may be device or
+ * pinned host memory: pinned rows are read and written through the device's mapping, only where needed; pageable host
+ * memory is an argument error.  Every element offset is 64-bit; N < 2^31 rows, T <= 65536.  All calls take a workspace
+ * of dinotrk_sampler_workspace_bytes(N) bytes; count and select must share it (select reads count's block scan).
+ * Argument errors return DINOTRK_EINVAL before any launch.  Profile class "sampler".
+ *   prepare_count: *n_valid = N' (host; syncs the stream).  prepare_emit: writes rows [N'] and bits [N'] (no sync).
+ *   count: frames [n_frames] int64 are the drawn frame indices (distinct, in [0, T)); a stored row is a candidate when
+ *     popcount(bits & frame mask) >= 2 (dataset.py:171).  Writes per-block counts and their scan into the workspace and
+ *     reads the total back to *n_cand (host; syncs the stream).
+ *   select: for positions perm [m] (< *n_cand, m <= N) among the candidates in row order, row_ids [m] int64 = the stored
+ *     row and mat [m][T] fp32 = 1 at the frames that are drawn and valid on that row, else 0 (dataset.py:180-183).  No sync.
+ *   gather: t1 / t2 [m][3] = (x, y, t) of rows[row_ids[i]] at steps draws[i][0] / draws[i][1] (draws [m][2] int64, the
+ *     multinomial's output; dataset.py:184-188).  No sync. */
+size_t dinotrk_sampler_workspace_bytes(int N);
+int dinotrk_sampler_prepare_count(const float* traj, int N, int T, int* n_valid, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+int dinotrk_sampler_prepare_emit(const float* traj, int N, int T, float* rows, uint32_t* bits, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+int dinotrk_sampler_count(const uint32_t* bits, int N, int T, const int64_t* frames, int n_frames, int* n_cand,
+                          void* workspace, size_t workspace_bytes, void* stream);
+int dinotrk_sampler_select(const uint32_t* bits, int N, int T, const int64_t* frames, int n_frames, const int64_t* perm,
+                           int m, int64_t* row_ids, float* mat, void* workspace, size_t workspace_bytes, void* stream);
+int dinotrk_sampler_gather(const float* rows, int T, const int64_t* row_ids, const int64_t* draws, int m, float* t1,
+                           float* t2, void* stream);
+
 /* ---- per-kernel-class device timing (CUDA events on the launching stream; bench.py roofline) ------ */
 int dinotrk_profile_classes(void);
 const char* dinotrk_profile_class_name(int cls);
