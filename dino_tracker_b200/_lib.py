@@ -41,6 +41,14 @@ class FlowVideo(Structure):
     _fields_ = [("fwd", c_void_p), ("bwd", c_void_p), ("T", c_int), ("H", c_int), ("W", c_int)]
 
 
+RAFT_NCONV = 45   # include/dinotrk.h DINOTRK_RAFT_NCONV
+
+
+class RaftWeights(Structure):
+    _fields_ = [("w_hi", c_void_p * RAFT_NCONV), ("w_lo", c_void_p * RAFT_NCONV), ("bias", c_void_p * RAFT_NCONV),
+                ("scale", c_float * RAFT_NCONV)]
+
+
 class DinotrkError(RuntimeError):
     pass
 
@@ -155,6 +163,11 @@ SIGNATURES = {
     "dinotrk_sampler_count": (c_int, [_P, c_int, c_int, _P, c_int, POINTER(c_int), _P, c_size_t, _P]),
     "dinotrk_sampler_select": (c_int, [_P, c_int, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_size_t, _P]),
     "dinotrk_sampler_gather": (c_int, [_P, c_int, _P, _P, c_int, _P, _P, _P]),
+    "dinotrk_raft_encode_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dinotrk_raft_encode": (c_int, [_P, c_int, c_int, c_int, c_int, POINTER(RaftWeights), _P, _P, _P, c_size_t, _P]),
+    "dinotrk_raft_flow_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "dinotrk_raft_flow": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, POINTER(c_int), c_int, c_int, POINTER(RaftWeights), _P,
+                                  _P, c_size_t, _P]),
 }
 
 

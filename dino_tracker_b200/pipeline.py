@@ -39,10 +39,11 @@ def track_video(video01, vit: DinoV2Features, query_points, head_state_dict=None
 
 @torch.no_grad()
 def preprocess_best_buddies(features_chw, video01, dino_bb_dir, traj_path, h, w, stride=7, flow_fn=None, threshold=1.0,
-                            min_trajectory_length=2, box_size=50, iou_thresh=0.2, device="cuda:0"):
+                            min_trajectory_length=2, box_size=50, iou_thresh=0.2, device="cuda:0", flows=None):
     """preprocessing_dino_bb/main_dino_bb_preprocessing.py in one process: best buddies of the features (T x C x h' x w'),
     optical-flow trajectories of the video (T x 3 x h x w in [0, 1], no direct-flow filtering), the flow filter of the
-    best buddies, then their NMS.  Features and trajectories stay on the GPU.  Writes the reference's three files:
+    best buddies, then their NMS.  Features and trajectories stay on the GPU.  ``flows``: the consecutive flows
+    (fwd, bwd, None) of ``trajectories.video_flows`` when already computed.  Writes the reference's three files:
     ``dino_bb_dir``/dino_best_buddies.pt, ``traj_path`` and ``dino_bb_dir``/dino_best_buddies_filtered.pt.  Returns
     (best buddies, trajectories, filtered best buddies)."""
     from . import best_buddies as bbm
@@ -52,7 +53,7 @@ def preprocess_best_buddies(features_chw, video01, dino_bb_dir, traj_path, h, w,
     bb = bbm.best_buddies(features_chw, h, w, stride=stride, device=dev)
     os.makedirs(dino_bb_dir, exist_ok=True)
     torch.save(bb, os.path.join(dino_bb_dir, "dino_best_buddies.pt"))
-    traj = extract_trajectories(video01, flow_fn, threshold, min_trajectory_length, device=dev)
+    traj = extract_trajectories(video01, flow_fn, threshold, min_trajectory_length, device=dev, flows=flows)
     os.makedirs(os.path.dirname(traj_path) or ".", exist_ok=True)
     torch.save(traj.cpu(), traj_path)
     filtered = bbm.nms_dict(bbm.of_filter(bb, traj, h, w, stride), pk, stride, box_size, iou_thresh)
@@ -84,16 +85,21 @@ def preprocess_video(video01, vit: DinoV2Features, mask_vit: DinoV2Features, dat
          ringing near mask edges into foreground; the re-read masks are what the trainer's load_fg_masks sees), resized
          to H x W -> of_trajectories/fg_trajectories.pt, bg_trajectories.pt;
       5. preprocess_best_buddies -> dino_best_buddies/*, of_trajectories/trajectories_wo_direct_filter.pt.
-    ``config`` overrides PREPROCESSING_DEFAULTS.  Returns the trajectories, fg, bg and the masks [T][H][W] uint8."""
+    A ``flow_fn`` with a ``video_flows`` method (``raft.RaftLarge``) encodes the frames once, and the consecutive flows
+    of steps 1 and 5 are computed once.  ``config`` overrides PREPROCESSING_DEFAULTS.  Returns the trajectories, fg, bg and the masks [T][H][W] uint8."""
     from . import fg_masks as fgm
-    from .trajectories import extract_trajectories
+    from .trajectories import extract_trajectories, video_flows
     cfg = dict(PREPROCESSING_DEFAULTS, **config)
     dev = torch.device(device)
     T, _, H, W = video01.shape
     of_dir = os.path.join(data_path, "of_trajectories")
     os.makedirs(of_dir, exist_ok=True)
+    flows = bb_flows = None
+    if hasattr(flow_fn, "video_flows"):
+        flows = video_flows(video01, flow_fn, cfg["filter_using_direct_flow"], device=dev)
+        bb_flows = (flows[0], flows[1], None)
     traj = extract_trajectories(video01, flow_fn, cfg["threshold"], cfg["min_trajectory_length"],
-                                cfg["filter_using_direct_flow"], cfg["direct_flow_threshold"], device=dev)
+                                cfg["filter_using_direct_flow"], cfg["direct_flow_threshold"], device=dev, flows=flows)
     torch.save(traj.cpu(), os.path.join(of_dir, "trajectories.pt"))
     features_chw = vit.features_chw(video01)
     os.makedirs(os.path.join(data_path, "dino_embeddings"), exist_ok=True)
@@ -112,5 +118,6 @@ def preprocess_video(video01, vit: DinoV2Features, mask_vit: DinoV2Features, dat
     preprocess_best_buddies(features_chw, video01, os.path.join(data_path, "dino_best_buddies"),
                             os.path.join(of_dir, "trajectories_wo_direct_filter.pt"), H, W, flow_fn=flow_fn,
                             threshold=cfg["threshold"], min_trajectory_length=cfg["min_trajectory_length"],
-                            box_size=cfg["dino_bb_box_size"], iou_thresh=cfg["dino_bb_iou_threshold"], device=dev)
+                            box_size=cfg["dino_bb_box_size"], iou_thresh=cfg["dino_bb_iou_threshold"], device=dev,
+                            flows=bb_flows)
     return traj, fg, bg, masks

@@ -1,7 +1,9 @@
 """Optical-flow trajectories (``preprocessing/extract_trajectories.py``) over libdinotrk.
 
-The flow network stays torchvision's RAFT (``raft_large``, as in the reference) and comes in through ``flow_fn(a, b)``:
-frames a, b [B][3][H][W] in [0, 1] -> flows a -> b [B][2][H][W].  Everything done with the flows runs in the library
+The flow network comes in through ``flow_fn(a, b)``: frames a, b [B][3][H][W] in [0, 1] -> flows a -> b [B][2][H][W].
+The default is torchvision's RAFT (``raft_large``, as in the reference); ``raft.RaftLarge`` runs the same network on the
+library, and as a provider with a ``video_flows`` method it encodes every frame once and batches the consecutive and
+the direct pairs (``video_flows`` below).  Everything done with the flows runs in the library
 (include/dinotrk.h: dinotrk_flow_masks, dinotrk_traj_chain / _emit): one thread walks one pixel through the frames,
 and only the number of kept trajectories of each start frame is read back, to size its output.
 """
@@ -92,15 +94,31 @@ def chain_trajectories(fwd, bwd, direct=None, threshold=1.0, min_trajectory_leng
 
 
 @torch.no_grad()
-def extract_trajectories(video01, flow_fn=None, threshold=1.0, min_trajectory_length=2, filter_using_direct_flow=False,
-                         direct_flow_threshold=None, device="cuda:0", direct_batch=16):
-    """``save_trajectories`` of extract_trajectories.py:163-268 on a video [T][3][H][W] in [0, 1]: flows of consecutive
-    frames (both directions), with ``filter_using_direct_flow`` the direct flows of every start frame to the later frames
-    (batches of 16), then the chaining.  Returns [M][T][2] fp32 on ``device``."""
+def video_flows(video01, flow_fn=None, filter_using_direct_flow=False, device="cuda:0", direct_batch=16):
+    """The flows ``extract_trajectories`` chains: (fwd, bwd, direct) with fwd / bwd [T-1][2][H][W] the consecutive flows
+    and ``direct`` None or the callable s -> (flows s -> s+1+k, flows s+1+k -> s) of ``chain_trajectories``.  A provider
+    with a ``video_flows(video01, groups)`` method (``raft.RaftLarge``) gets the consecutive pairs as one group and each
+    start frame's direct pairs as one more, in chaining order; a plain ``flow_fn`` is called pair by pair as
+    extract_trajectories.py does (the direct flows in batches of ``direct_batch``)."""
     dev = _lib.require_cuda(device)
     flow_fn = flow_fn or raft_flow_fn(dev)
     video01 = video01.to(dev, torch.float32)
     T = video01.shape[0]
+    if hasattr(flow_fn, "video_flows"):
+        groups = [[(i, i + 1) for i in range(T - 1)] + [(i + 1, i) for i in range(T - 1)]]
+        if filter_using_direct_flow:
+            groups += [[(s, t) for t in range(s + 1, T)] + [(t, s) for t in range(s + 1, T)] for s in range(T - 1)]
+        it = flow_fn.video_flows(video01, groups)
+        f = next(it)
+        pending = iter(range(T - 1))
+
+        def direct_provider(s):
+            if next(pending) != s:
+                raise RuntimeError("direct flows are produced in start-frame order")
+            g = next(it)
+            return g[:T - 1 - s], g[T - 1 - s:]
+        return f[:T - 1], f[T - 1:], direct_provider if filter_using_direct_flow else None
+
     fwd, bwd = [], []
     for i in range(T - 1):
         pair = video01[i:i + 2]
@@ -118,6 +136,19 @@ def extract_trajectories(video01, flow_fn=None, threshold=1.0, min_trajectory_le
             bf.append(flow_fn(dst[i:i + direct_batch], src[i:i + direct_batch]))
         return torch.cat(ff), torch.cat(bf)
 
+    return fwd, bwd, direct if filter_using_direct_flow else None
+
+
+@torch.no_grad()
+def extract_trajectories(video01, flow_fn=None, threshold=1.0, min_trajectory_length=2, filter_using_direct_flow=False,
+                         direct_flow_threshold=None, device="cuda:0", direct_batch=16, flows=None):
+    """``save_trajectories`` of extract_trajectories.py:163-268 on a video [T][3][H][W] in [0, 1]: flows of consecutive
+    frames (both directions), with ``filter_using_direct_flow`` the direct flows of every start frame to the later frames
+    (``video_flows``), then the chaining.  ``flows``: the (fwd, bwd, direct) of ``video_flows`` when already computed.
+    Returns [M][T][2] fp32 on ``device``."""
+    if flows is None:
+        flows = video_flows(video01, flow_fn, filter_using_direct_flow, device, direct_batch)
+    fwd, bwd, direct = flows
     return chain_trajectories(fwd, bwd, direct if filter_using_direct_flow else None, threshold, min_trajectory_length,
                               direct_flow_threshold)
 

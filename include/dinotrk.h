@@ -535,6 +535,48 @@ int dinotrk_sampler_select(const uint32_t* bits, int N, int T, const int64_t* fr
 int dinotrk_sampler_gather(const float* rows, int T, const int64_t* row_ids, const int64_t* draws, int m, float* t1,
                            float* t2, void* stream);
 
+/* ---- RAFT-large optical flow (torchvision models/optical_flow/raft.py raft_large, eval mode) ---------------------- */
+/* Weights: one entry per convolution in torchvision's parameter order.  w_hi / w_lo are the fp16 split
+ * (dinotrk_split_fp16) of the K-major matrix [Np][Kp]: row n = output channel, k = (ky * kw + kx) * C_in + ci with the
+ * input channels in torchvision's concatenation order, Kp = kh * kw * C_in rounded up to 8, Np = C_out rounded up to
+ * 64 (C_out <= 64), 128 (C_out <= 128) or a multiple of 256, padding rows zero; bias [Np] fp32.  Entries 0-15 are the
+ * feature encoder (stem, layer1-3 blocks as conv1, conv2 and, for the strided first blocks, the 1 x 1 projection, then
+ * the final 1 x 1), 16-31 the context encoder in the same order with its eval-mode BatchNorm folded into weight and
+ * bias.  A GRU's convz and convr are ONE entry: the [z; r] matrix with C_out = 256.  scale[i]: a power of two the
+ * matrix was divided by before the split (its largest entry in [2^13, 2^14): the fp16 lo halves of small weights would
+ * otherwise be subnormal); the GEMM's result is multiplied by it (exact) before the bias is added. */
+enum {
+  DINOTRK_RAFT_FNET = 0, DINOTRK_RAFT_CNET = 16, DINOTRK_RAFT_CONVCORR1 = 32, DINOTRK_RAFT_CONVCORR2, DINOTRK_RAFT_CONVFLOW1,
+  DINOTRK_RAFT_CONVFLOW2, DINOTRK_RAFT_MOTION_CONV, DINOTRK_RAFT_GRU1_ZR, DINOTRK_RAFT_GRU1_Q, DINOTRK_RAFT_GRU2_ZR,
+  DINOTRK_RAFT_GRU2_Q, DINOTRK_RAFT_FLOW_HEAD1, DINOTRK_RAFT_FLOW_HEAD2, DINOTRK_RAFT_MASK1, DINOTRK_RAFT_MASK2,
+  DINOTRK_RAFT_NCONV
+};
+typedef struct {
+  const void* w_hi[DINOTRK_RAFT_NCONV];
+  const void* w_lo[DINOTRK_RAFT_NCONV];
+  const float* bias[DINOTRK_RAFT_NCONV];
+  float scale[DINOTRK_RAFT_NCONV];
+} dinotrk_raft_weights;
+/* Frames are [T][3][H][W] fp32 in [0, 1], H, W >= 121 so that the frame replicate-padded to a multiple of 8 (the extra
+ * row / column split as torchvision's "sintel" InputPadder) has a 1/8 grid of at least 16 x 16.  Each frame is mapped
+ * by 2x - 1 and encoded once: fmap [T][h8 * w8][256] (feature encoder, InstanceNorm statistics in float64 in a fixed
+ * order) and, for the first T_ctx frames (the ones flows start from), ctx [T_ctx][h8 * w8][256] = tanh(hidden 128) |
+ * relu(context 128) (context encoder; ctx may be NULL when T_ctx = 0).  Workspaces are for one frame size; 0 on invalid
+ * arguments. */
+size_t dinotrk_raft_encode_workspace_bytes(int H, int W);
+int dinotrk_raft_encode(const float* frames, int T, int T_ctx, int H, int W, const dinotrk_raft_weights* w, float* fmap,
+                        float* ctx, void* workspace, size_t workspace_bytes, void* stream);
+/* Flows [n_pairs][2][H][W] of the pairs (host int32 [n_pairs][2], frames (i, j), the flow i -> j) after
+ * num_flow_updates updates: raft_large(frame_i, frame_j, num_flow_updates)[-1], cropped to H x W; every i < T_ctx.  fmap_hi / fmap_lo:
+ * the fp16 split of fmap for the correlation volume on the F16X3 GEMM (fp32-faithful inside the split's range, see
+ * dinotrk_split_faithful), or both NULL for the exact-fp32 GEMM.  A pair's flow does not depend on the other pairs of
+ * the call: the same bits in any batch.  The workspace holds each pair's correlation pyramid (4 * h8 w8 * (h8 w8 + the
+ * three pooled levels) bytes) and its update-block activations. */
+size_t dinotrk_raft_flow_workspace_bytes(int H, int W, int n_pairs);
+int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_lo, const float* ctx, int T, int H, int W,
+                      const int* pairs, int n_pairs, int num_flow_updates, const dinotrk_raft_weights* w, float* flows,
+                      void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- per-kernel-class device timing (CUDA events on the launching stream; bench.py roofline) ------ */
 int dinotrk_profile_classes(void);
 const char* dinotrk_profile_class_name(int cls);
