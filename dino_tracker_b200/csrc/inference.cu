@@ -191,21 +191,20 @@ __global__ void sample_unique_kernel(const float* __restrict__ tpc, int T, int C
   }
 }
 
-// descriptors (fp16 hi / lo + norm; with desc_q8: + the int8 row, its factor and the map's coarse bound eps, from the
-// descriptor's residual and its anchor frame's rho_f) and output slots of one chunk of anchor work items, from the unique
-// samples
-__global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C, int P, int h, int w, PointAffine pa,
-                                     const float* __restrict__ traj, const int* __restrict__ qlist, int N,
-                                     const int* __restrict__ grp_frame, const int* __restrict__ grp_map0,
-                                     const int* __restrict__ grp_item0, int n_groups, int frame_batch,
-                                     const __half* __restrict__ u_hi, const __half* __restrict__ u_lo,
-                                     const float* __restrict__ u_norm, const int* __restrict__ u_flag,
-                                     float* __restrict__ dnorm, int* __restrict__ out_index, __half* __restrict__ desc_hi,
-                                     __half* __restrict__ desc_lo, const int8_t* __restrict__ u_q8,
-                                     const float* __restrict__ u_fac, const float* __restrict__ u_rho,
-                                     const float* __restrict__ rho_f, int8_t* __restrict__ desc_q8, float* __restrict__ desc_fac,
-                                     float* __restrict__ desc_eps) {
-  const int j = blockIdx.x;
+// Per-map scalars of one chunk of anchor work items, one thread per map: the output slot, the map's row in the GEMMs' A
+// arrays (arow) and, for an unflagged source point, the norm and the coarse bound eps (from the descriptor's residual and
+// its anchor frame's rho_f; with_eps: the int8 coarse pass runs) of its unique sample.  A group whose first row lies below
+// n_unique is read IN PLACE from the unique table (its rows there are consecutive, the planner saw to that); the maps of
+// the other groups get row chunk_row0 + map of the chunk's own descriptor arrays, which gather_anchor_kernel fills.
+__global__ void anchor_scalars_kernel(int T, const int* __restrict__ qlist, int N, const int* __restrict__ grp_frame,
+                                      const int* __restrict__ grp_row0, const int* __restrict__ grp_map0,
+                                      const int* __restrict__ grp_item0, int n_groups, int n_maps, int n_unique, int chunk_row0,
+                                      const float* __restrict__ u_norm, const int* __restrict__ u_flag,
+                                      const float* __restrict__ u_rho, const float* __restrict__ rho_f, bool with_eps,
+                                      int* __restrict__ out_index, int* __restrict__ arow, float* __restrict__ dnorm,
+                                      float* __restrict__ desc_eps) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_maps) return;
   int lo = 0, hi = n_groups - 1;
   while (lo < hi) {
     int mid = (lo + hi + 1) >> 1;
@@ -216,19 +215,52 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
   const int slot = uu / T, i = uu - slot * T;
   const int n = qlist[(size_t)a * N + slot];
   const size_t u = (size_t)n * T + i;
-  if (threadIdx.x == 0) out_index[j] = (n * T + a) * T + i;
+  out_index[j] = (n * T + a) * T + i;
+  const int r0 = grp_row0[lo];
+  arow[j] = r0 < n_unique ? r0 + (j - grp_map0[lo]) : chunk_row0 + j;
+  if (u_flag[u]) return;   // sampled per work item: gather_anchor_kernel writes the norm and eps
+  dnorm[j] = u_norm[u];
+  if (with_eps) desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[a]);
+}
+
+// descriptors (fp16 hi / lo; with desc_q8: + the int8 row and its factor) of the GATHERED maps of one chunk of anchor work
+// items: row copies from the unique samples, or, for a flagged source point, the sample itself with its norm and eps.
+// One block per map of [map_lo, map_lo + gridDim.x); maps of in-place groups are left alone.  desc_* / dnorm / desc_fac /
+// desc_eps are the chunk's arrays (row = map).
+__global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C, int P, int h, int w, PointAffine pa,
+                                     const float* __restrict__ traj, const int* __restrict__ qlist, int N,
+                                     const int* __restrict__ grp_frame, const int* __restrict__ grp_row0,
+                                     const int* __restrict__ grp_map0, const int* __restrict__ grp_item0, int n_groups,
+                                     int n_unique, int map_lo, int frame_batch, const __half* __restrict__ u_hi,
+                                     const __half* __restrict__ u_lo, const int* __restrict__ u_flag,
+                                     float* __restrict__ dnorm, __half* __restrict__ desc_hi,
+                                     __half* __restrict__ desc_lo, const int8_t* __restrict__ u_q8,
+                                     const float* __restrict__ u_fac, const float* __restrict__ rho_f,
+                                     int8_t* __restrict__ desc_q8, float* __restrict__ desc_fac,
+                                     float* __restrict__ desc_eps) {
+  const int j = map_lo + blockIdx.x;
+  int lo = 0, hi = n_groups - 1;
+  while (lo < hi) {
+    int mid = (lo + hi + 1) >> 1;
+    if (grp_map0[mid] <= j) lo = mid; else hi = mid - 1;
+  }
+  if (grp_row0[lo] < n_unique) return;   // read in place
+  const int a = grp_frame[lo];
+  const int uu = grp_item0[lo] + (j - grp_map0[lo]);
+  const int slot = uu / T, i = uu - slot * T;
+  const int n = qlist[(size_t)a * N + slot];
+  const size_t u = (size_t)n * T + i;
   if (!u_flag[u]) {
     const uint4* sh = reinterpret_cast<const uint4*>(u_hi + u * C);
     const uint4* sl = reinterpret_cast<const uint4*>(u_lo + u * C);
     uint4* dh = reinterpret_cast<uint4*>(desc_hi + (size_t)j * C);
     uint4* dl = reinterpret_cast<uint4*>(desc_lo + (size_t)j * C);
     for (int k = threadIdx.x; k < C / 8; k += blockDim.x) { dh[k] = __ldg(sh + k); dl[k] = __ldg(sl + k); }
-    if (threadIdx.x == 0) dnorm[j] = u_norm[u];
     if (desc_q8) {
       const uint4* sq = reinterpret_cast<const uint4*>(u_q8 + u * C);
       uint4* dq = reinterpret_cast<uint4*>(desc_q8 + (size_t)j * C);
       for (int k = threadIdx.x; k < C / 16; k += blockDim.x) dq[k] = __ldg(sq + k);
-      if (threadIdx.x == 0) { desc_fac[j] = u_fac[u]; desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[a]); }
+      if (threadIdx.x == 0) desc_fac[j] = u_fac[u];
     }
     return;
   }
@@ -310,9 +342,11 @@ __global__ void occlusion_kernel(const float* __restrict__ traj, const float* __
 struct GroupBuf {  // host mirror of the per-chunk group arrays: [frame | row0 | m | map0 | item0] x cap
   std::vector<int> v;
   int cap, n;
+  bool overflow = false;   // a push beyond cap (dropped): the caller's bound on the groups of a chunk was wrong
   explicit GroupBuf(int c) : v((size_t)5 * c), cap(c), n(0) {}
   void clear() { n = 0; }
   void push(int frame, int row0, int m, int map0, int item0) {
+    if (n >= cap) { overflow = true; return; }
     v[n] = frame; v[cap + n] = row0; v[2 * cap + n] = m; v[3 * cap + n] = map0; v[4 * cap + n] = item0; ++n;
   }
 };
@@ -321,42 +355,89 @@ struct GroupBuf {  // host mirror of the per-chunk group arrays: [frame | row0 |
 // A phase's work items are cut into chunks of <= ch correlation maps; inside a chunk, items of the same target
 // frame form one group = [frame | first descriptor row | number of rows m | first map | first item] (GroupBuf order).
 //   kind 0 (trajectories): items = (frame t, query row n), t-major; descriptor rows are the N query rows.
-//   kind 1 (anchors): items of anchor frame a = cnt[a] * T pairs (slot, i), a-major; descriptor rows are per chunk.
-struct ChunkMeta { int used, maxm, n_groups; bool no_thin; };
+//   kind 1 (anchors): items of anchor frame a = cnt[a] * T pairs (slot, i), a-major; descriptor rows are per chunk
+//   (row = map), or, with AnchorRows, rows of one array that holds the unique table and the chunks' own rows behind it.
+struct ChunkMeta { int used, maxm, n_groups; bool no_thin; int n_gathered, gather_lo, gather_hi; };   // gathered maps lie in [lo, hi)
+// Descriptor rows of the exact-window pipeline.  The descriptor of item (slot, i) of anchor frame a is row n T + i of the
+// unique table, n = qlist[a][slot], unless query n is flagged (qflag: some source frame's sample depends on the anchor
+// frame).  So the T-item cells of consecutive unflagged queries are consecutive rows there and a GEMM can read them in
+// place.  A frame's span of a chunk is cut into groups at the runs of consecutive unflagged queries; a run is read in place
+// when padding it to whole 256-row tiles of the coarse GEMM costs at most 1 / XW_INPLACE_PAD_DIV of its rows.  Shorter runs
+// and flagged queries are gathered into the chunk's own rows (row gather_row0 + ring slot * ring_stride + map), adjacent
+// ones as one group.
+constexpr int XW_INPLACE_PAD_DIV = 16;
+constexpr int XW_INPLACE_MIN_ROWS = TC2_BM_ROWS - TC2_BM_ROWS / (XW_INPLACE_PAD_DIV + 1);   // 241: the shortest such run
+struct AnchorRows { const int* qlist; const unsigned char* qflag; int gather_row0, ring, ring_stride; };
 // align: anchor-phase chunks are cut at multiples of `align` items per frame (T for the exact-window path: whole cells).
 // first_cap > 0: capacity of the first anchor-phase chunk only (the probe chunk of the exact-window pipeline).
-static void plan_chunks(int kind, int T, int N, const int* cnt, int ch_all, int gcap, std::vector<ChunkMeta>& metas,
-                        std::vector<int>& plan_host, int align = 1, int first_cap = 0) {
+// rows (with align = T): see AnchorRows; the chunks hold the same items with or without it.  False: gcap was too small.
+static bool plan_chunks(int kind, int T, int N, const int* cnt, int ch_all, int gcap, std::vector<ChunkMeta>& metas,
+                        std::vector<int>& plan_host, int align = 1, int first_cap = 0, const AnchorRows* rows = nullptr) {
   int ch = ch_all;
   metas.clear(); plan_host.clear();
   GroupBuf gb(gcap);
-  auto commit_chunk = [&](int used, int maxm) {
+  int n_gathered = 0, gather_lo = 0, gather_hi = 0;
+  auto commit_chunk = [&](int used) {
     bool no_thin = true;
-    for (int k = 0; k < gb.n; ++k) no_thin = no_thin && gb.v[2 * gb.cap + k] > STREAM_MAX_M;
-    metas.push_back(ChunkMeta{used, maxm, gb.n, no_thin});
+    int maxm = 0;
+    for (int k = 0; k < gb.n; ++k) {
+      no_thin = no_thin && gb.v[2 * gb.cap + k] > STREAM_MAX_M;
+      maxm = std::max(maxm, gb.v[2 * gb.cap + k]);
+    }
+    metas.push_back(ChunkMeta{used, maxm, gb.n, no_thin, n_gathered, gather_lo, gather_hi});
     plan_host.insert(plan_host.end(), gb.v.begin(), gb.v.end());
+    n_gathered = gather_lo = gather_hi = 0;
+  };
+  // groups of the span [item0, item0 + m) of anchor frame a, maps map0 .. of the chunk being filled
+  auto push_span = [&](int a, int map0, int m, int item0) {
+    if (!rows) { gb.push(a, map0, m, map0, item0); return; }
+    const int* ql = rows->qlist + (size_t)a * N;
+    const int chunk_row0 = rows->gather_row0 + (int)(metas.size() % rows->ring) * rows->ring_stride;
+    const int s0 = item0 / T, s1 = (item0 + m) / T;
+    int gs = -1;   // first slot of the gathered group being collected
+    auto close_gathered = [&](int s_end) {
+      if (gs < 0) return;
+      const int gm = (s_end - gs) * T, gmap = map0 + (gs - s0) * T;
+      gb.push(a, chunk_row0 + gmap, gm, gmap, gs * T);
+      if (n_gathered == 0) gather_lo = gmap;
+      n_gathered += gm; gather_hi = gmap + gm;
+      gs = -1;
+    };
+    for (int s = s0; s < s1;) {
+      const bool flagged = rows->qflag[ql[s]] != 0;
+      int e = s + 1;
+      while (!flagged && e < s1 && ql[e] == ql[e - 1] + 1 && !rows->qflag[ql[e]]) ++e;
+      const int r = (e - s) * T, pad = (r + TC2_BM_ROWS - 1) / TC2_BM_ROWS * TC2_BM_ROWS - r;
+      if (!flagged && (long long)pad * XW_INPLACE_PAD_DIV <= r) {
+        close_gathered(s);
+        gb.push(a, ql[s] * T, r, map0 + (s - s0) * T, s * T);
+      } else if (gs < 0) {
+        gs = s;
+      }
+      s = e;
+    }
+    close_gathered(s1);
   };
   if (kind == 0) {
     int t = 0, row = 0;  // next work item: (frame t, query row)
     while (t < T) {
       gb.clear();
-      int used = 0, maxm = 0;
+      int used = 0;
       while (t < T && used < ch && gb.n < gcap) {
         int m = N - row;
         if (m > ch - used) m = ch - used;
         gb.push(t, row, m, used, 0);
         used += m; row += m;
-        if (m > maxm) maxm = m;
         if (row == N) { row = 0; ++t; }
       }
-      commit_chunk(used, maxm);
+      commit_chunk(used);
     }
   } else {
     int a = 0;
     long long item = 0;  // next work item: anchor frame a, item index within a (slot * T + i)
     while (a < T) {
       gb.clear();
-      int used = 0, maxm = 0;
+      int used = 0;
       ch = (metas.empty() && first_cap > 0 && first_cap < ch_all) ? first_cap : ch_all;
       while (a < T && used < ch && gb.n < gcap) {
         long long tot = (long long)cnt[a] * T;
@@ -367,21 +448,21 @@ static void plan_chunks(int kind, int T, int N, const int* cnt, int ch_all, int 
           if (m == 0) m = align;                    // (ch >= align is guaranteed by the caller)
         }
         if (m > 0) {
-          gb.push(a, used, (int)m, used, (int)item);
+          push_span(a, used, (int)m, (int)item);
           used += (int)m; item += m;
-          if ((int)m > maxm) maxm = (int)m;
         }
         if (item >= tot) { item = 0; ++a; }
       }
       if (used == 0) break;
-      commit_chunk(used, maxm);
+      commit_chunk(used);
     }
   }
+  return !gb.overflow;
 }
 
 // ---- cells of the exact-window path (xwin.cuh): the <= 128 source frames of one (query slot, anchor frame) ----
 struct CellPlan {
-  std::vector<int> v;               // per chunk: [row0 | m | frame | group] x (cells of the chunk), chunks back to back
+  std::vector<int> v;               // per chunk: [first map | m | frame | group | first A row] x (cells of the chunk), chunks back to back
   std::vector<size_t> first;        // first cell of chunk k in v's cell numbering (size chunks + 1)
   std::vector<int> tiles;           // per chunk: (gcap + 1) prefix of ceil(m / 256) per group (coarse GEMM)
   int max_m = 0;
@@ -389,19 +470,19 @@ struct CellPlan {
 static void plan_cells(int T, int gcap, const std::vector<ChunkMeta>& metas, const std::vector<int>& plan_host, CellPlan& cp) {
   const int nb = (T + XW_MAX_CELL - 1) / XW_MAX_CELL, rb = (T + nb - 1) / nb;
   cp.v.clear(); cp.first.assign(1, 0); cp.tiles.clear(); cp.max_m = 0;
-  std::vector<int> r0, mm, fr, gr;
+  std::vector<int> r0, mm, fr, gr, ar;
   for (size_t k = 0; k < metas.size(); ++k) {
     const int* gb = plan_host.data() + k * 5 * gcap;
-    r0.clear(); mm.clear(); fr.clear(); gr.clear();
+    r0.clear(); mm.clear(); fr.clear(); gr.clear(); ar.clear();
     int pre = 0;
     for (int g = 0; g < metas[k].n_groups; ++g) {
-      const int frame = gb[g], row0 = gb[gcap + g], m = gb[2 * gcap + g];
+      const int frame = gb[g], row0 = gb[gcap + g], m = gb[2 * gcap + g], map0 = gb[3 * gcap + g];
       cp.tiles.push_back(pre);
       pre += (m + TC2_BM_ROWS - 1) / TC2_BM_ROWS;
       for (int s0 = 0; s0 < m; s0 += T)
         for (int b = 0; b < T; b += rb) {
           const int cm = std::min(rb, T - b);
-          r0.push_back(row0 + s0 + b); mm.push_back(cm); fr.push_back(frame); gr.push_back(g);
+          r0.push_back(map0 + s0 + b); mm.push_back(cm); fr.push_back(frame); gr.push_back(g); ar.push_back(row0 + s0 + b);
           cp.max_m = std::max(cp.max_m, cm);
         }
     }
@@ -411,6 +492,7 @@ static void plan_cells(int T, int gcap, const std::vector<ChunkMeta>& metas, con
     cp.v.insert(cp.v.end(), mm.begin(), mm.end());
     cp.v.insert(cp.v.end(), fr.begin(), fr.end());
     cp.v.insert(cp.v.end(), gr.begin(), gr.end());
+    cp.v.insert(cp.v.end(), ar.begin(), ar.end());
     cp.first.push_back(cp.first.back() + n);
   }
 }
@@ -477,8 +559,10 @@ static XwAsync* xw_async() {
 static int g_xw_path = -1;                     // -1: automatic (DTK_XW or on), 0: full-map path only, 1: exact-window path
 static int g_xw_coarse = -1;                   // -1: automatic, 0: fp16 coarse pass, 1: int8 coarse pass
 // anchor-phase maps | on the exact-window path | queued | path used | queued by the certificate | tensor-core contraction |
-// int8 coarse pass | bits of the largest per-frame int8 residual
-static long long g_infer_stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+// int8 coarse pass | bits of the largest per-frame int8 residual | exact-window maps whose descriptor was read in place from
+// the unique table | those gathered into the chunk's rows
+constexpr int INFER_STATS = 10;
+static long long g_infer_stats[INFER_STATS] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 // the probe chunk queues more than this fraction of its maps on the int8 coarse pass: the rest of the phase runs the fp16
 // pass.  A queued map costs a full-map split-precision GEMM, ~3 fp16 coarse passes, while the int8 pass saves about half
 // of one per map: int8 loses above ~1/6 extra queued maps.  1/16 leaves a wide margin.
@@ -504,13 +588,17 @@ int dinotrk_infer_set_coarse(int mode) {
 
 int dinotrk_infer_last_stats(long long* out, int n) {
   DTK_CHECK_ARG(out && n >= 4, "infer_last_stats: need at least 4 slots");
-  for (int i = 0; i < (n < 8 ? n : 8); ++i) out[i] = g_infer_stats[i];
+  for (int i = 0; i < (n < INFER_STATS ? n : INFER_STATS); ++i) out[i] = g_infer_stats[i];
   return DINOTRK_OK;
 }
 
 static int infer_chunk_maps(int chunk_maps) { return chunk_maps > 0 ? chunk_maps : 4096; }
 // chunks of the anchor phase hold whole (query, anchor frame) cells of T maps: never smaller than T
 static int infer_chunk_eff(int chunk_maps, int T) { const int c = infer_chunk_maps(chunk_maps); return c > T ? c : T; }
+// capacity of a chunk's group arrays.  Trajectory phase and full-map anchor phase: one group per frame.  Exact-window anchor
+// phase: a frame's span is cut at its in-place runs, each of >= XW_INPLACE_MIN_ROWS rows, with at most one gathered group
+// before each and one behind the last: <= T + 2 (ch / XW_INPLACE_MIN_ROWS) groups.
+static int infer_gcap(int T, int ch) { return T + 2 + 2 * (ch / XW_INPLACE_MIN_ROWS + 1); }
 // upper bound on the number of chunks of one phase (phase C has the most work items: N * T * T)
 // (anchor-phase chunks are cut at whole cells of T maps: a full chunk holds at least the largest multiple of T <= ch)
 static size_t infer_max_chunks(int T, int N, size_t ch) {
@@ -540,6 +628,34 @@ int dinotrk_infer_plan(int kind, int T, int N, const int* anchor_counts, int chu
     for (size_t k = 0; k < metas.size(); ++k) {
       meta[4 * k] = metas[k].used; meta[4 * k + 1] = metas[k].maxm; meta[4 * k + 2] = metas[k].n_groups;
       meta[4 * k + 3] = metas[k].no_thin ? 1 : 0;
+    }
+  return DINOTRK_OK;
+}
+
+int dinotrk_infer_anchor_gcap(int T, int chunk_maps) { return T > 0 ? infer_gcap(T, infer_chunk_eff(chunk_maps, T)) : 0; }
+
+int dinotrk_infer_plan_anchors(int T, int N, const int* anchor_counts, const int* qlist, const unsigned char* query_flag,
+                               int chunk_maps, int probe, int* groups, int* meta, int max_chunks, int* n_chunks) {
+  DTK_CHECK_ARG(T > 0 && N >= 0 && anchor_counts && qlist && query_flag && n_chunks, "infer_plan_anchors: bad arguments");
+  for (int a = 0; a < T; ++a) {
+    DTK_CHECK_ARG(anchor_counts[a] >= 0 && anchor_counts[a] <= N, "infer_plan_anchors: count of frame %d out of range", a);
+    for (int k = 0; k < anchor_counts[a]; ++k)
+      DTK_CHECK_ARG(qlist[(size_t)a * N + k] >= 0 && qlist[(size_t)a * N + k] < N, "infer_plan_anchors: query out of range");
+  }
+  const int ch = infer_chunk_eff(chunk_maps, T), gcap = infer_gcap(T, ch);
+  const AnchorRows rows{qlist, query_flag, N * T, XW_RING, ch};
+  std::vector<ChunkMeta> metas;
+  std::vector<int> plan_host;
+  const bool fits = plan_chunks(1, T, N, anchor_counts, ch, gcap, metas, plan_host, T,
+                                probe ? std::max(T, (XW_PROBE_MAPS / T) * T) : 0, &rows);
+  DTK_CHECK_ARG(fits, "infer_plan_anchors: a chunk has more than %d groups", gcap);
+  *n_chunks = (int)metas.size();
+  DTK_CHECK_ARG((int)metas.size() <= max_chunks || (!groups && !meta), "infer_plan_anchors: %zu chunks, room for %d", metas.size(), max_chunks);
+  if (groups) std::copy(plan_host.begin(), plan_host.end(), groups);
+  if (meta)
+    for (size_t k = 0; k < metas.size(); ++k) {
+      meta[5 * k] = metas[k].used; meta[5 * k + 1] = metas[k].maxm; meta[5 * k + 2] = metas[k].n_groups;
+      meta[5 * k + 3] = metas[k].no_thin ? 1 : 0; meta[5 * k + 4] = metas[k].n_gathered;
     }
   return DINOTRK_OK;
 }
@@ -586,7 +702,7 @@ int dinotrk_corr_track(const dinotrk_features* feat, const dinotrk_geom* g,
 size_t dinotrk_infer_workspace_bytes(int T, int C, const dinotrk_geom* g, int N, int chunk_maps) {
   if (!g) return 0;
   const size_t ch = infer_chunk_eff(chunk_maps, T), ms = dinotrk_map_stride(g);
-  const int gcap = T + 2;
+  const int gcap = infer_gcap(T, (int)ch);
   size_t b = 0;
   b += align_up((size_t)N * C * 4, 256) + align_up((size_t)N * 4, 256);   // descA, normA
   size_t c = 0;                                                            // per chunk buffer set (two: pipelining)
@@ -600,20 +716,21 @@ size_t dinotrk_infer_workspace_bytes(int T, int C, const dinotrk_geom* g, int N,
   b += 4 * align_up(ch * 4, 256);                                          // out_index ring
   b += align_up(infer_max_chunks(T, N, ch) * 5 * gcap * 4, 256);           // group arrays of every chunk of a phase
   b += align_up((size_t)T * 4, 256) + align_up((size_t)T * N * 4, 256);    // cnt, qlist
-  // exact-window pipeline: ring of XW_RING chunk sets (descriptors fp32 + fp16 hi/lo, norms, out_index, keys, boxes),
-  // the cells of every chunk of the phase, coarse-GEMM tile prefixes, compact group arrays of the full-map queue
+  // exact-window pipeline: the unique descriptors with the rows of a ring of XW_RING chunks behind them, the ring's per-map
+  // arrays (out_index, eps, A row, keys, boxes), the cells of every chunk of the phase, coarse-GEMM tile prefixes, compact
+  // group arrays of the full-map queue
   const size_t chx = ch;
   const int nb = (T + XW_MAX_CELL - 1) / XW_MAX_CELL;
   const size_t max_cells_chunk = chx + 2;                                  // cells have >= 1 row
   size_t x = 0;
-  x += align_up(chx * 4, 256) + corr_tc_workspace_bytes((int)chx, C) + 256 + align_up(chx * 4, 256);   // norms, hi / lo, out_index
+  x += 3 * align_up(chx * 4, 256);                                         // out_index, eps, A row
   x += xw_chunk_bytes((int)chx, (int)max_cells_chunk, cdiv(g->h * g->w, XW_TILE), gcap);
   b += XW_RING * x;
-  b += 2 * align_up((size_t)N * T * C * 2, 256) + 2 * align_up((size_t)N * T * 4, 256);   // unique descriptors (hi, lo, norm, flag)
-  b += align_up((size_t)N * T * C, 256) + 2 * align_up((size_t)N * T * 4, 256);           // their int8 rows, factors, residuals
-  b += XW_RING * (align_up(chx * C, 256) + 2 * align_up(chx * 4, 256));                   // chunk int8 rows, factors, eps
+  const size_t rows = (size_t)N * T + XW_RING * chx;                                      // unique table + the ring's rows
+  b += 2 * align_up(rows * C * 2, 256) + align_up(rows * C, 256) + 2 * align_up(rows * 4, 256);   // hi, lo, int8, norm, factor
+  b += 2 * align_up((size_t)N * T * 4, 256);                                              // flags, residuals of the unique rows
   b += align_up((size_t)T * g->h * g->w * 4, 256) + 256;                                  // reciprocal token norms, smallest norm
-  b += align_up((size_t)N * T * nb * 16 + 64, 256);                         // cells of all chunks
+  b += align_up((size_t)N * T * nb * 20 + 64, 256);                         // cells of all chunks
   b += align_up(infer_max_chunks(T, N, ch) * (gcap + 1) * 4, 256);         // coarse tile prefixes per chunk
   {
     const size_t sg = std::min<size_t>(infer_max_chunks(T, N, ch) * (size_t)gcap, 16384);
@@ -684,7 +801,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   const int P = g->h * g->w, ms = dinotrk_map_stride(g);
   const int ch = infer_chunk_eff(chunk_maps, T);
   const int fb = frame_batch > 0 ? (frame_batch < T ? frame_batch : T) : T;
-  const int gcap = T + 2;
+  const int gcap = infer_gcap(T, ch);
   const PointAffine pa = make_point_affine(*g);
 
   Arena ar(workspace, workspace_bytes);
@@ -708,23 +825,27 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   int* d_groups = ar.take<int>(max_chunks * 5 * gcap);
   int* d_cnt = ar.take<int>(T);
   int* d_qlist = ar.take<int>((size_t)T * N);
-  struct XwSet { float* norm; float* split; int* out_index; int8_t* q8; float* fac; float* eps; XwChunk xc; } xr[XW_RING];
+  // Descriptor rows of the exact-window GEMMs, one row numbering for every per-row array: rows [0, N T) are the unique
+  // table (row n T + i: trajectory point i of query n), rows N T + k ch + j the gathered map j of ring slot k.  One A
+  // tensor map per operand covers both, so a group reads its rows wherever they are.
+  struct XwSet { int row0; float* norm; int* out_index; int* arow; float* eps; XwChunk xc; } xr[XW_RING];
   const int n_tiles_map = cdiv(P, XW_TILE);     // coarse keys per map
-  __half* u_hi = ar.take<__half>((size_t)N * T * C);
-  __half* u_lo = ar.take<__half>((size_t)N * T * C);
-  float* u_norm = ar.take<float>((size_t)N * T);
+  const int n_unique = N * T;
+  const size_t xw_rows = (size_t)n_unique + (size_t)XW_RING * ch;
+  __half* u_hi = ar.take<__half>(xw_rows * C);
+  __half* u_lo = ar.take<__half>(xw_rows * C);
+  int8_t* u_q8 = ar.take<int8_t>(xw_rows * C);
+  float* u_norm = ar.take<float>(xw_rows);
+  float* u_fac = ar.take<float>(xw_rows);
   int* u_flag = ar.take<int>((size_t)N * T);
-  int8_t* u_q8 = ar.take<int8_t>((size_t)N * T * C);
-  float* u_fac = ar.take<float>((size_t)N * T);
   float* u_rho = ar.take<float>((size_t)N * T);
   float* d_rnorms = ar.take<float>((size_t)T * P);
   unsigned* d_minnorm = ar.take<unsigned>(4);
   for (int k = 0; k < XW_RING; ++k) {
-    xr[k].norm = ar.take<float>(ch);
-    xr[k].split = ar.take<float>(corr_tc_workspace_bytes(ch, C) / 4);
+    xr[k].row0 = n_unique + k * ch;
+    xr[k].norm = u_norm + xr[k].row0;   // per map; for a gathered map also its row's
     xr[k].out_index = ar.take<int>(ch);
-    xr[k].q8 = ar.take<int8_t>((size_t)ch * C);
-    xr[k].fac = ar.take<float>(ch);
+    xr[k].arow = ar.take<int>(ch);
     xr[k].eps = ar.take<float>(ch);
     XwChunk& x = xr[k].xc;
     x.key1 = ar.take<unsigned long long>((size_t)ch * n_tiles_map);
@@ -741,13 +862,14 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     x.slow_cnt = ar.take<int>(gcap + 2);
   }
   const int cell_nb = (T + XW_MAX_CELL - 1) / XW_MAX_CELL;
-  int* d_cells = ar.take<int>((size_t)N * T * cell_nb * 4 + 16);
+  int* d_cells = ar.take<int>((size_t)N * T * cell_nb * 5 + 16);
   int* d_tiles = ar.take<int>(max_chunks * (gcap + 1));
   const int sg_cap = (int)std::min<size_t>(max_chunks * (size_t)gcap, 16384);   // groups of the accumulated full-map queue
   int* d_cgrp = ar.take<int>((size_t)4 * sg_cap);
   int* d_splan = ar.take<int>((size_t)sg_cap + 1);
   int* d_cntA = ar.take<int>(64);
   DTK_CHECK_ARG(ar.ok(), "infer: workspace arena overflow");
+  DTK_CHECK_ARG(xw_rows <= 0x7fffffffu, "infer: %zu descriptor rows exceed the row index", xw_rows);
   const bool tensor = fv.tensor();   // tensor-core GEMM: tile keys for the head, fp16 split fused into the samplers
 
   // The chunks of a phase are planned on the host in one go and their group arrays uploaded with ONE copy, so the
@@ -848,7 +970,22 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     DTK_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
     std::vector<float> rho_f(fv.s8() ? T : 0);
     if (fv.s8()) DTK_CUDA(cudaMemcpyAsync(rho_f.data(), fv.q_rho, (size_t)T * sizeof(float), cudaMemcpyDeviceToHost, st));
-    DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: sizes of the anchor work lists
+    std::vector<int> qlist_h, uflag_h;
+    if (use_xw) {
+      // every (query, source frame) descriptor once, before the host waits (it depends on the trajectories only); with the
+      // int8 rows whenever the int8 coarse pass can still be chosen.  The planner needs the anchor lists and the flags.
+      const bool q8 = fv.s8() && g_xw_coarse != 0 && C % 16 == 0 && C <= XW_S8_MAX_C;
+      {
+        ProfRange pr(PROF_SAMPLE, st);
+        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, u_hi, u_lo, u_norm, u_flag,
+                                                               q8 ? u_q8 : nullptr, u_fac, u_rho);
+        DTK_LAUNCHED();
+      }
+      qlist_h.resize((size_t)T * N); uflag_h.resize((size_t)N * T);
+      DTK_CUDA(cudaMemcpyAsync(qlist_h.data(), d_qlist, qlist_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+      DTK_CUDA(cudaMemcpyAsync(uflag_h.data(), u_flag, uflag_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+    }
+    DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: the anchor work lists
     if (use_xw) {   // a token below the split's faithful range (a zero one included) voids the coarse pass's error bound
       float mn;
       memcpy(&mn, xa->host_cnt + 2 * XW_RING + 16, sizeof(float));
@@ -864,7 +1001,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     long long maps_C = 0;
     for (int a = 0; a < T; ++a) maps_C += (long long)cnt[a] * T;
     g_infer_stats[0] = maps_C; g_infer_stats[1] = 0; g_infer_stats[2] = 0; g_infer_stats[3] = use_xw ? 1 : 0; g_infer_stats[4] = 0;
-    g_infer_stats[5] = tensor ? 1 : 0;
+    g_infer_stats[5] = tensor ? 1 : 0; g_infer_stats[8] = 0; g_infer_stats[9] = 0;
     // coarse pass of the exact-window pipeline (decided once use_xw is final): int8 when the features carry their int8
     // operands (forced: required), unless a frame's residual makes the bound too loose (automatic mode; below: or the probe
     // chunk queues too many maps)
@@ -887,13 +1024,18 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       // the full-map pipeline directly.  The probe is the same set of work items for every chunk size >= XW_PROBE_MAPS.
       const bool probing = pathsel < 0;
       const int probe_cap = std::max(T, (XW_PROBE_MAPS / T) * T);
-      plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host, T, probing ? probe_cap : 0);
+      std::vector<unsigned char> qflag(N, 0);   // a query with a flagged source frame is never read in place
+      for (size_t u = 0; u < uflag_h.size(); ++u)
+        if (uflag_h[u]) qflag[u / T] = 1;
+      const AnchorRows rows{qlist_h.data(), qflag.data(), n_unique, XW_RING, ch};
+      DTK_CHECK_ARG(plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host, T, probing ? probe_cap : 0, &rows),
+                    "infer: a chunk of the anchor phase has more than %d groups", gcap);
       int rc = upload_plan();
       if (rc) return rc;
       planned = true;
       CellPlan cp;
       plan_cells(T, gcap, metas, plan_host, cp);
-      DTK_CHECK_ARG(cp.first.back() * 4 <= (size_t)N * T * cell_nb * 4 + 16, "infer: cell plan exceeds its bound");
+      DTK_CHECK_ARG(cp.first.back() * 5 <= (size_t)N * T * cell_nb * 5 + 16, "infer: cell plan exceeds its bound");
       if (!cp.v.empty()) DTK_CUDA(cudaMemcpyAsync(d_cells, cp.v.data(), cp.v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
       if (!cp.tiles.empty()) DTK_CUDA(cudaMemcpyAsync(d_tiles, cp.tiles.data(), cp.tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
       InferAsync* ia = infer_async();
@@ -903,13 +1045,12 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         DTK_CUDA(cudaEventRecord(ia->fork, st));
         DTK_CUDA(cudaStreamWaitEvent(sb, ia->fork, 0));
       }
-      auto hi_of = [&](const XwSet& x, int rows) { (void)rows; return reinterpret_cast<char*>(x.split); };
-      auto lo_of = [&](const XwSet& x, int rows) { return reinterpret_cast<char*>(x.split) + align_up((size_t)rows * C * 2, 256); };
       auto cells_of = [&](size_t k) {
         XwCells c;
         const int n = (int)(cp.first[k + 1] - cp.first[k]);
-        const int* base = d_cells + 4 * cp.first[k];
-        c.row0 = base; c.m = base + n; c.frame = base + 2 * n; c.group = base + 3 * n; c.n_cells = n; c.max_m = cp.max_m;
+        const int* base = d_cells + 5 * cp.first[k];
+        c.row0 = base; c.m = base + n; c.frame = base + 2 * n; c.group = base + 3 * n; c.arow = base + 4 * n;
+        c.n_cells = n; c.max_m = cp.max_m;
         return c;
       };
       auto enqueue_sample_x = [&](size_t k) -> int {
@@ -919,12 +1060,18 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         if (ovl && k >= XW_RING) DTK_CUDA(cudaStreamWaitEvent(sb, xa->freed[k % XW_RING], 0));   // chunk k - 4 is through
         {
           ProfRange pr(PROF_SAMPLE, sb);
-          gather_anchor_kernel<<<cm.used, SAMPLE_THREADS, 0, sb>>>(tpc, T, C, P, g->h, g->w, pa, traj, d_qlist, N, gp.f, gp.map0,
-                                                                  gp.item, cm.n_groups, fb, u_hi, u_lo, u_norm, u_flag, x.norm,
-                                                                  x.out_index, reinterpret_cast<__half*>(hi_of(x, cm.used)),
-                                                                  reinterpret_cast<__half*>(lo_of(x, cm.used)), u_q8, u_fac, u_rho,
-                                                                  fv.q_rho, s8 ? x.q8 : nullptr, x.fac, x.eps);
+          anchor_scalars_kernel<<<cdiv(cm.used, 256), 256, 0, sb>>>(T, d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, cm.used,
+                                                                   n_unique, x.row0, u_norm, u_flag, u_rho, fv.q_rho, s8, x.out_index,
+                                                                   x.arow, x.norm, x.eps);
           DTK_LAUNCHED();
+          if (cm.n_gathered > 0) {
+            const size_t r0 = (size_t)x.row0;
+            gather_anchor_kernel<<<cm.gather_hi - cm.gather_lo, SAMPLE_THREADS, 0, sb>>>(
+                tpc, T, C, P, g->h, g->w, pa, traj, d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, n_unique, cm.gather_lo, fb, u_hi, u_lo, u_flag,
+                                                                    x.norm, u_hi + r0 * C, u_lo + r0 * C, u_q8, u_fac, fv.q_rho,
+                                                                    s8 ? u_q8 + r0 * C : nullptr, u_fac + r0, x.eps);
+            DTK_LAUNCHED();
+          }
         }
         if (ovl) DTK_CUDA(cudaEventRecord(xa->sample[k % XW_RING], sb));
         return DINOTRK_OK;
@@ -962,7 +1109,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
           const ChunkBufs& b = cb[0];
           char* c_hi = reinterpret_cast<char*>(b.split);
           char* c_lo = c_hi + align_up((size_t)ch * C * 2, 256);          // layout of a descriptor array of `ch` rows
-          int rc2 = launch_xw_compact(nullptr, hi_of(x, cm.used), lo_of(x, cm.used), x.norm, x.out_index, C, gp.f, gp.map0, cm.n_groups,
+          int rc2 = launch_xw_compact(nullptr, u_hi, u_lo, x.arow, x.norm, x.out_index, C, gp.f, gp.map0, cm.n_groups,
                                       n_slow, x.xc, nullptr, c_hi, c_lo, b.norm, out_index_ring[0], d_cgrp, sg_cap, st, q_rows, q_groups);
           if (rc2) return rc2;
           q_rows += n_slow; q_groups += cm.n_groups;
@@ -970,16 +1117,6 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         DTK_CUDA(cudaEventRecord(xa->freed[j % XW_RING], st));
         return DINOTRK_OK;
       };
-      {   // every (query, source frame) descriptor once; the per-chunk kernels copy rows
-        ProfRange pr(PROF_SAMPLE, st);
-        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, u_hi, u_lo, u_norm, u_flag,
-                                                               s8 ? u_q8 : nullptr, u_fac, u_rho);
-        DTK_LAUNCHED();
-      }
-      if (ovl) {   // (the fork above was recorded before this launch: make the sampling stream wait for it)
-        DTK_CUDA(cudaEventRecord(ia->fork, st));
-        DTK_CUDA(cudaStreamWaitEvent(sb, ia->fork, 0));
-      }
       if (!metas.empty() && (rc = enqueue_sample_x(0))) return rc;
       size_t n_finished = 0, k_end = metas.size();
       for (size_t k = 0; k < metas.size(); ++k) {
@@ -989,11 +1126,12 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         const XwCells cells = cells_of(k);
         if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, xa->sample[k % XW_RING], 0));
         const float* eps = s8 ? x.eps : nullptr;   // (nullptr: the fp16 pass's XW_EPS)
-        if ((rc = launch_xw_coarse(fv, hi_of(x, cm.used), cm.used, x.norm, gp.f, gp.r, gp.m, gp.map0, d_tiles + k * (gcap + 1),
-                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, d_rnorms, s8 ? x.q8 : nullptr,
-                                   x.fac))) return rc;
+        g_infer_stats[8] += cm.used - cm.n_gathered; g_infer_stats[9] += cm.n_gathered;
+        if ((rc = launch_xw_coarse(fv, u_hi, (int)xw_rows, u_norm, gp.f, gp.r, gp.m, gp.map0, d_tiles + k * (gcap + 1),
+                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, d_rnorms, s8 ? u_q8 : nullptr,
+                                   u_fac))) return rc;
         if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used, split_min_norm(C), eps))) return rc;
-        if ((rc = launch_xw_gemm(fv, *g, hi_of(x, cm.used), lo_of(x, cm.used), cm.used, cells, x.xc, st))) return rc;
+        if ((rc = launch_xw_gemm(fv, *g, u_hi, u_lo, (int)xw_rows, cells, x.xc, st))) return rc;
         if ((rc = launch_xw_head(fv, *g, *hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups,
                                  eps)))
           return rc;
@@ -1024,9 +1162,13 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         NvtxRange nvd("dinotrk.infer.D.occlusion");
         return dinotrk_occlusion(traj, cos_sims, anchors, N, T, anchor_th, cos_th, occ, stream);
       }
-      k0 = k_end;                       // switched: chunks k0.. on the full-map pipeline below (same plan)
+      // switched: chunks k0.. on the full-map pipeline below.  The same chunks, their rows per chunk again.  (Everything
+      // that read the plan is in the caller's stream by now, so the upload is ordered behind it.)
+      k0 = k_end;
       g_infer_stats[3] = 0;
       g_infer_stats[6] = 0;
+      plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host, T, probing ? probe_cap : 0);
+      if ((rc = upload_plan())) return rc;
     }
     if (!planned) {
       plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host);

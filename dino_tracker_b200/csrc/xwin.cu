@@ -390,7 +390,7 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
       for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
         const int2 org = box_org[cell];
         if (org.y == INT_MIN) continue;            // every map of the cell takes the full-map path
-        const int drow = cells.row0[cell], frame = cells.frame[cell];
+        const int drow = cells.arow[cell], frame = cells.frame[cell];
         for (int part = 0; part < (MB == 64 ? 1 : 2); ++part) {
           for (int kb = 0; kb < KB; ++kb) {
             const int k0 = kb * Cfg::kBK;
@@ -832,7 +832,7 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
 // also writes the compact group arrays.  Rows of a group keep their queue order (arbitrary, results do not depend on it).
 __global__ void __launch_bounds__(128)
 xw_compact_kernel(const float4* __restrict__ desc, const uint4* __restrict__ dhi, const uint4* __restrict__ dlo,
-                  const float* __restrict__ desc_norm, const int* __restrict__ out_index, int C, const int* __restrict__ grp_frame,
+                  const int* __restrict__ arow, const float* __restrict__ desc_norm, const int* __restrict__ out_index, int C, const int* __restrict__ grp_frame,
                   const int* __restrict__ grp_map0, int n_groups, const int* __restrict__ slow_cnt,
                   const int* __restrict__ slow_list, float4* __restrict__ c_desc, uint4* __restrict__ c_hi, uint4* __restrict__ c_lo,
                   float* __restrict__ c_norm, int* __restrict__ c_out_index, int* __restrict__ cgrp, int gcap, int row_base,
@@ -856,24 +856,25 @@ xw_compact_kernel(const float4* __restrict__ desc, const uint4* __restrict__ dhi
   if (s_g < 0) return;
   const int b = row_base + bb;
   const int src = slow_list[grp_map0[s_g] + s_pos];
+  const size_t srow = arow ? arow[src] : src;
   if (desc != nullptr)   // (the fp32 copy only feeds the non-tensor GEMMs)
-    for (int i = threadIdx.x; i < C / 4; i += blockDim.x) c_desc[(size_t)b * (C / 4) + i] = desc[(size_t)src * (C / 4) + i];
+    for (int i = threadIdx.x; i < C / 4; i += blockDim.x) c_desc[(size_t)b * (C / 4) + i] = desc[srow * (C / 4) + i];
   if (dhi != nullptr)
     for (int i = threadIdx.x; i < C / 8; i += blockDim.x) {
-      c_hi[(size_t)b * (C / 8) + i] = dhi[(size_t)src * (C / 8) + i];
-      c_lo[(size_t)b * (C / 8) + i] = dlo[(size_t)src * (C / 8) + i];
+      c_hi[(size_t)b * (C / 8) + i] = dhi[srow * (C / 8) + i];
+      c_lo[(size_t)b * (C / 8) + i] = dlo[srow * (C / 8) + i];
     }
   if (threadIdx.x == 0) { c_norm[b] = desc_norm[src]; c_out_index[b] = out_index[src]; }
 }
 
-int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const float* desc_norm,
+int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const int* arow, const float* desc_norm,
                       const int* out_index, int C, const int* grp_frame, const int* grp_map0, int n_groups, int n_slow,
                       const XwChunk& xc, float* c_desc, void* c_hi, void* c_lo, float* c_norm, int* c_out_index, int* cgrp,
                       int gcap, cudaStream_t st, int row_base, int grp_base) {
   if (n_slow <= 0) return DINOTRK_OK;
   ProfRange pr(PROF_MISC, st);
   xw_compact_kernel<<<n_slow, 128, 0, st>>>(reinterpret_cast<const float4*>(desc), reinterpret_cast<const uint4*>(desc_hi),
-                                            reinterpret_cast<const uint4*>(desc_lo), desc_norm, out_index, C, grp_frame, grp_map0,
+                                            reinterpret_cast<const uint4*>(desc_lo), arow, desc_norm, out_index, C, grp_frame, grp_map0,
                                             n_groups, xc.slow_cnt, xc.slow_list, reinterpret_cast<float4*>(c_desc),
                                             reinterpret_cast<uint4*>(c_hi), reinterpret_cast<uint4*>(c_lo), c_norm, c_out_index, cgrp,
                                             gcap, row_base, grp_base);
@@ -1001,7 +1002,7 @@ int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, con
                 max_m <= XW_MAX_CELL, "xw_box_gemm: bad sizes (C must be a multiple of 8, cells of 1..%d rows)", XW_MAX_CELL);
   DTK_CHECK_ARG(reinterpret_cast<uintptr_t>(box_org) % 8 == 0, "xw_box_gemm: box_org must be 8-byte aligned");
   const FeatView fv = make_view(*feat, *g);
-  const XwCells cells{cell_row0, cell_m, cell_frame, nullptr, n_cells, max_m};
+  const XwCells cells{cell_row0, cell_row0, cell_m, cell_frame, nullptr, n_cells, max_m};
   XwChunk xc{};
   xc.box_org = reinterpret_cast<int2*>(const_cast<int*>(box_org));
   xc.xbox = xbox;

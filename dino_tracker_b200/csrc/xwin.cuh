@@ -118,7 +118,8 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
 };
 
 struct XwCells {          // host-planned, device-resident description of a chunk's cells
-  const int* row0;     // [cells] first descriptor row (= first map) of the cell
+  const int* row0;     // [cells] first map of the cell (chunk-local: indexes the per-map arrays)
+  const int* arow;     // [cells] first descriptor row of the cell in the GEMM's A arrays (consecutive rows, like its maps)
   const int* m;        // [cells] rows
   const int* frame;    // [cells] anchor frame
   const int* group;    // [cells] group index (for the slow queues)
@@ -144,7 +145,8 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
                    int out_mode, const XwChunk& xc, cudaStream_t st, int n_groups, const float* eps);
 // Appends the queued maps' descriptor rows (fp32 optional, hi, lo, norm, out_index) to compact arrays at row_base and their
 // group arrays ([frame | row0 | m | map0] x gcap, entries grp_base ..) to cgrp.  n_slow = host copy of slow_cnt[n_groups].
-int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const float* desc_norm,
+// arow[map] = the map's row in desc / desc_hi / desc_lo (nullptr: the map index); norm and out_index are per map.
+int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const int* arow, const float* desc_norm,
                       const int* out_index, int C, const int* grp_frame, const int* grp_map0, int n_groups, int n_slow,
                       const XwChunk& xc, float* c_desc, void* c_hi, void* c_lo, float* c_norm, int* c_out_index, int* cgrp,
                       int gcap, cudaStream_t st, int row_base = 0, int grp_base = 0);

@@ -179,6 +179,20 @@ size_t dinotrk_infer_workspace_bytes(int T, int C, const dinotrk_geom* g, int N,
 size_t dinotrk_infer_max_chunks(int T, int N, int chunk_maps);
 int dinotrk_infer_plan(int kind, int T, int N, const int* anchor_counts, int chunk_maps, int* groups, int* meta,
                        int max_chunks, int* n_chunks);
+/* Host-only helper: the anchor-phase plan of pipeline 1 (coarse pass + exact window), which reads descriptor rows in place
+ * where it can.  Descriptor rows are numbered in one space: row n T + i (< N T) is the unique sample of trajectory point i
+ * of query n; the rows behind belong to a ring of 4 chunks, map j of chunk k at N T + (k % 4) ch + j with
+ * ch = max(chunk_maps, T).  qlist [T][N]: the queries anchored at frame a, ascending, anchor_counts[a] of them;
+ * query_flag [N]: 1 = the query's descriptors depend on the anchor frame, it is never read in place.  Chunks are cut at
+ * whole (query, anchor frame) cells of T items (probe != 0: a first chunk of <= 4096 maps); a frame's span of a chunk is
+ * cut into groups at its runs of consecutive unflagged queries.  A run is read in place (first row = first query * T) when
+ * padding it to 256-row tiles costs at most 1/16 of its rows; the other cells are gathered (first row = the chunk's row of
+ * the group's first map), adjacent ones as one group.  groups [n_chunks][5][gcap] as above with
+ * gcap = dinotrk_infer_anchor_gcap(T, chunk_maps); meta [n_chunks][5] = {maps used, largest m, number of groups, 1 if no
+ * group is thin, gathered maps}.  Either may be NULL to just count. */
+int dinotrk_infer_anchor_gcap(int T, int chunk_maps);
+int dinotrk_infer_plan_anchors(int T, int N, const int* anchor_counts, const int* qlist, const unsigned char* query_flag,
+                               int chunk_maps, int probe, int* groups, int* meta, int max_chunks, int* n_chunks);
 /* Phase 2 pipelining across CUDA streams (process-wide; results are identical in every mode):
  * 0 = everything on the caller's stream; 1 (default) = the descriptor sampling of chunk k+1 runs on an
  * internal side stream under the correlation GEMM of chunk k; 2 = the head's fast path as well;
@@ -199,8 +213,9 @@ int dinotrk_infer_set_overlap(int mode);
  * dinotrk_infer_last_stats (n >= 4 slots): {anchor-phase maps, maps finished by the exact-window path, maps re-done by the
  * full-map path, pipeline used[, of the re-done maps: those queued by the head's certificate rather than by the plan[,
  * contraction: 1 = split fp16 tensor cores, 0 = exact fp32[, coarse pass of pipeline 1: 1 = int8, 0 = fp16 (the pass the
- * phase finished with)[, bits of the float max over frames of feat->q_rho, 0 without int8 operands]]]]} of the last
- * dinotrk_infer call that ran the anchor phase. */
+ * phase finished with)[, bits of the float max over frames of feat->q_rho, 0 without int8 operands[, maps of pipeline 1
+ * whose descriptor the GEMMs read in place from the unique (query, source frame) table, maps whose descriptor was gathered
+ * into the chunk's rows]]]]]} of the last dinotrk_infer call that ran the anchor phase. */
 int dinotrk_infer_set_path(int path);
 /* Coarse pass of pipeline 1:  1 = int8 (feat->q8 required),  0 = fp16 over feat->hi,
  * -1 (default) = int8 when feat->q8 is given and every frame's q_rho is <= 0.03, unless the probe chunk queues more than
