@@ -168,8 +168,8 @@ SIGNATURES = {
     "dinotrk_raft_encode_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dinotrk_raft_encode": (c_int, [_P, c_int, c_int, c_int, c_int, POINTER(RaftWeights), _P, _P, _P, c_size_t, _P]),
     "dinotrk_raft_flow_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
-    "dinotrk_raft_flow": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, POINTER(c_int), c_int, c_int, POINTER(RaftWeights), _P,
-                                  _P, c_size_t, _P]),
+    "dinotrk_raft_flow": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, POINTER(c_int), c_int, c_int,
+                                  POINTER(RaftWeights), _P, _P, c_size_t, _P]),
 }
 
 

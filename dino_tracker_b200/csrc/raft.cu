@@ -604,15 +604,18 @@ size_t dinotrk_raft_flow_workspace_bytes(int H, int W, int n_pairs) {
   return ar.off + 256;
 }
 
-int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_lo, const float* ctx, int T, int H, int W,
-                      const int* pairs, int n_pairs, int num_flow_updates, const dinotrk_raft_weights* w, float* flows,
+int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_lo, const float* ctx, int T, int T_ctx, int H,
+                      int W, const int* pairs, int n_pairs, int num_flow_updates, const dinotrk_raft_weights* w, float* flows,
                       void* workspace, size_t workspace_bytes, void* stream) {
   NvtxRange nvtx_range("dinotrk.raft_flow");
-  DTK_CHECK_ARG(fmap && ctx && pairs && w && flows && T > 0 && n_pairs > 0 && num_flow_updates > 0, "raft_flow: bad arguments");
+  DTK_CHECK_ARG(fmap && ctx && pairs && w && flows && T > 0 && T_ctx > 0 && T_ctx <= T && n_pairs > 0 && num_flow_updates > 0,
+                "raft_flow: bad arguments");
   DTK_CHECK_ARG(!fmap_hi == !fmap_lo, "raft_flow: give both halves of the fmap split or neither");
   DTK_CHECK_ARG(raft_shape_ok(H, W), "raft_flow: frames must be at least 128 x 128 (after padding to a multiple of 8)");
   DTK_CHECK_ARG(raft_weights_ok(w, 32, DINOTRK_RAFT_NCONV), "raft_flow: missing update-block weights");
   for (int g = 0; g < 2 * n_pairs; ++g) DTK_CHECK_ARG(pairs[g] >= 0 && pairs[g] < T, "raft_flow: frame index out of range");
+  for (int g = 0; g < n_pairs; ++g)
+    DTK_CHECK_ARG(pairs[2 * g] < T_ctx, "raft_flow: a flow starts from a frame encoded without its context (i >= T_ctx)");
   DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_raft_flow_workspace_bytes(H, W, n_pairs), "raft_flow: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int Hp = (H + 7) / 8 * 8, Wp = (W + 7) / 8 * 8, h8 = Hp / 8, w8 = Wp / 8, hw = h8 * w8;

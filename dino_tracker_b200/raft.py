@@ -171,7 +171,8 @@ class RaftLarge:
             chunk = pairs[b0:b0 + nb]
             arr = (ctypes.c_int * (2 * len(chunk)))(*[x for p in chunk for x in p])
             _lib.check(self._lib.dinotrk_raft_flow(_lib.ptr(enc.fmap), _lib.ptr(enc.hi), _lib.ptr(enc.lo), _lib.ptr(enc.ctx),
-                                                   enc.T, enc.H, enc.W, arr, len(chunk), n_upd, ctypes.byref(self._w),
+                                                   enc.T, enc.ctx.shape[0], enc.H, enc.W, arr, len(chunk), n_upd,
+                                                   ctypes.byref(self._w),
                                                    _lib.ptr(out[b0:b0 + len(chunk)]), _lib.ptr(ws), ws.numel(), st),
                        "raft_flow")
         return out

@@ -582,14 +582,15 @@ size_t dinotrk_raft_encode_workspace_bytes(int H, int W);
 int dinotrk_raft_encode(const float* frames, int T, int T_ctx, int H, int W, const dinotrk_raft_weights* w, float* fmap,
                         float* ctx, void* workspace, size_t workspace_bytes, void* stream);
 /* Flows [n_pairs][2][H][W] of the pairs (host int32 [n_pairs][2], frames (i, j), the flow i -> j) after
- * num_flow_updates updates: raft_large(frame_i, frame_j, num_flow_updates)[-1], cropped to H x W; every i < T_ctx.  fmap_hi / fmap_lo:
+ * num_flow_updates updates: raft_large(frame_i, frame_j, num_flow_updates)[-1], cropped to H x W.  fmap has T frames, ctx
+ * the first T_ctx of them (1 <= T_ctx <= T); every j < T and every i < T_ctx, else nothing is launched.  fmap_hi / fmap_lo:
  * the fp16 split of fmap for the correlation volume on the F16X3 GEMM (fp32-faithful inside the split's range, see
  * dinotrk_split_faithful), or both NULL for the exact-fp32 GEMM.  A pair's flow does not depend on the other pairs of
  * the call: the same bits in any batch.  The workspace holds each pair's correlation pyramid (4 * h8 w8 * (h8 w8 + the
  * three pooled levels) bytes) and its update-block activations. */
 size_t dinotrk_raft_flow_workspace_bytes(int H, int W, int n_pairs);
-int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_lo, const float* ctx, int T, int H, int W,
-                      const int* pairs, int n_pairs, int num_flow_updates, const dinotrk_raft_weights* w, float* flows,
+int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_lo, const float* ctx, int T, int T_ctx, int H,
+                      int W, const int* pairs, int n_pairs, int num_flow_updates, const dinotrk_raft_weights* w, float* flows,
                       void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- per-kernel-class device timing (CUDA events on the launching stream; bench.py roofline) ------ */

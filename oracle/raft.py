@@ -118,17 +118,23 @@ def flows(sd, enc, pairs, num_flow_updates):
     return torch.sum(mask * up, dim=2).permute(0, 1, 4, 2, 5, 3).reshape(P, 2, 8 * hh, 8 * ww)
 
 
-def torchvision_flow(model, a01, b01, num_flow_updates):
-    """torchvision's ``model((a - 0.5) / 0.5, (b - 0.5) / 0.5, n)[-1]`` in the frames' dtype: its coordinate grids are
-    made in float32, so for float64 they are made in float64 (the only change)."""
+def torchvision_flows(model, a01, b01, num_flow_updates):
+    """torchvision's ``model((a - 0.5) / 0.5, (b - 0.5) / 0.5, n)`` in the frames' dtype: the flows after each of the n
+    updates (the k-th is the flow of k updates).  Its coordinate grids are made in float32, so for float64 they are made
+    in float64 (the only change)."""
     from torchvision.models.optical_flow import raft as tvr
     make = tvr.make_coords_grid
     tvr.make_coords_grid = lambda *a, **k: make(*a, **k).to(a01.dtype)
     try:
         with torch.no_grad():
-            return model((a01 - 0.5) / 0.5, (b01 - 0.5) / 0.5, num_flow_updates=num_flow_updates)[-1]
+            return model((a01 - 0.5) / 0.5, (b01 - 0.5) / 0.5, num_flow_updates=num_flow_updates)
     finally:
         tvr.make_coords_grid = make
+
+
+def torchvision_flow(model, a01, b01, num_flow_updates):
+    """torchvision's ``model((a - 0.5) / 0.5, (b - 0.5) / 0.5, n)[-1]`` (see ``torchvision_flows``)."""
+    return torchvision_flows(model, a01, b01, num_flow_updates)[-1]
 
 
 def seeded_model(seed=0, flow_gain=8.0):

@@ -35,17 +35,23 @@ def padded(x):
     return torch.nn.functional.pad(x, pad, mode="replicate"), pad
 
 
-def tv_flow(model, a, b, n, dtype, tf32=False):
-    """torchvision raft_large on padded frames in ``dtype``, cropped back."""
+def tv_flows(model, a, b, ns, dtype, tf32=False):
+    """torchvision raft_large on padded frames in ``dtype``, cropped back: the flows after each number of updates in
+    ``ns``, from one run of max(ns) updates."""
     (ap, pad), (bp, _) = padded(a), padded(b)
     m = model if dtype == torch.float32 else _copy(model, dtype)
     old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = tf32
     try:
-        f = oraft.torchvision_flow(m, ap.to(dtype), bp.to(dtype), n)
+        fs = oraft.torchvision_flows(m, ap.to(dtype), bp.to(dtype), max(ns))
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
-    return f[..., pad[2]:f.shape[-2] - pad[3], pad[0]:f.shape[-1] - pad[1]].double()
+    return [fs[n - 1][..., pad[2]:fs[n - 1].shape[-2] - pad[3], pad[0]:fs[n - 1].shape[-1] - pad[1]].double() for n in ns]
+
+
+def tv_flow(model, a, b, n, dtype, tf32=False):
+    """torchvision raft_large on padded frames in ``dtype``, cropped back."""
+    return tv_flows(model, a, b, (n,), dtype, tf32)[0]
 
 
 _copies = {}
