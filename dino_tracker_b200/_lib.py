@@ -165,6 +165,12 @@ SIGNATURES = {
     "dinotrk_sampler_count": (c_int, [_P, c_int, c_int, _P, c_int, POINTER(c_int), _P, c_size_t, _P]),
     "dinotrk_sampler_select": (c_int, [_P, c_int, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_size_t, _P]),
     "dinotrk_sampler_gather": (c_int, [_P, c_int, _P, _P, c_int, _P, _P, _P]),
+    "dinotrk_randperm_prefix": (c_int, [_P, c_size_t, ctypes.c_int64, ctypes.c_int64, _P]),
+    "dinotrk_cycle_mask_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dinotrk_cycle_mask_scan": (c_int, [_P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_cycle_select": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P]),
+    "dinotrk_cycle_unnorm": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P]),
+    "dinotrk_cycle_keep": (c_int, [_P, _P, c_int, c_int, c_int, c_float, _P, _P, _P, _P]),
     "dinotrk_raft_encode_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dinotrk_raft_encode": (c_int, [_P, c_int, c_int, c_int, c_int, POINTER(RaftWeights), _P, _P, _P, c_size_t, _P]),
     "dinotrk_raft_flow_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),

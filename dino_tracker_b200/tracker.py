@@ -5,9 +5,9 @@ Same constructor kwargs, attributes, ``forward`` / ``load_weights`` / ``cache_re
 303-325``), so ``dino_tracker.py::get_model`` and ``ModelInference`` use it unchanged.  All arithmetic is
 in the CUDA kernels; this file only owns tensors and forwards calls.  With gradients enabled (the training step of
 ``dino_tracker.py:405-429``) ``forward`` builds a graph: delta-DINO as torch ops, the tracker as one autograd node
-with hand-written forward and backward kernels (``train.py``, ``csrc/train.cu``); ``get_point_predictions`` is the
-primitive the reference's cycle-consistency code (``models/tracker.py:182-301``) is written on.  The cycle-consistency
-sampling itself and the losses / optimiser loop of ``dino_tracker.py`` stay with the reference's trainer.
+with hand-written forward and backward kernels (``train.py``, ``csrc/train.cu``); the cycle-consistency methods
+(``models/tracker.py:182-301``) run all pairs as one batch (``cycle.py``).  The losses / optimiser loop of
+``dino_tracker.py`` stay with the reference's trainer.
 
 Internal layout: features are kept token-major ``[T][P][C]`` (see include/dinotrk.h);
 ``refined_features`` / ``dino_embed_video`` expose zero-copy ``T x C x h x w`` views of them.
@@ -21,6 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from . import cycle as _cycle
 from . import train as _train
 from .networks import DeltaDINO, TrackerHead
 from .range_normalizer import RangeNormalizer
@@ -333,67 +334,29 @@ class Tracker(nn.Module):
         return _train.track_points(self, frame_embeddings, inp)
 
     # ------------------------------------------------------------------ cycle consistency (models/tracker.py:182-301)
+    @_lib.on_device
+    def _cycle_draw(self, frames_set_t, fg_masks):
+        return _cycle.draw(self, frames_set_t, fg_masks, self.frame_embeddings)
+
     @torch.no_grad()
     def get_cycle_consistent_coords(self, frames_set_t, fg_masks):
         """models/tracker.py:182-262.  ``cyc_n_frames`` random (source, target) slots of the frame set; per pair
         ``cyc_batch_size_per_frame`` pixel positions of the source frame (share ``cyc_fg_points_ratio`` inside
         ``fg_masks``), tracked source -> target -> source with the embeddings of the last forward; kept when they
         return within ``cyc_thresh`` px.  Random draws in the reference's order (two ``randint`` on the frame set's
-        device, then per pair a foreground and a background ``randperm``)."""
-        dev = frames_set_t.device                    # the random draws live where the reference makes them:
-        n_set = frames_set_t.shape[0]                 # randint on the frame set's device, randperm on the host
-        src_slots = torch.randint(n_set, (self.cyc_n_frames,), device=dev)
-        tgt_slots = torch.randint(n_set, (self.cyc_n_frames,), device=dev)
-        H, W = fg_masks.shape[-2:]
-        ys = torch.arange(H, device=fg_masks.device).float()
-        xs = torch.arange(W, device=fg_masks.device).float()
-        pixels = torch.stack([xs.repeat(H), ys.repeat_interleave(W)], dim=-1)        # row-major (x, y)
-        n_fg = int(self.cyc_batch_size_per_frame * self.cyc_fg_points_ratio)
-        n_bg = self.cyc_batch_size_per_frame - n_fg
-        emb = self.frame_embeddings
-        rows = {k: [] for k in ("source_points", "target_points", "cycle_points", "source_frame_indices",
-                                "target_frame_indices", "source_times", "target_times")}
-
-        def with_time(xy, t):
-            return torch.cat([xy, torch.full((xy.shape[0], 1), float(t), device=xy.device)], dim=-1)
-
-        def to_px(coords):
-            return self.range_normalizer.unnormalize(coords, src=(-1, 1), dims=[0, 1])
-
-        for s_slot, t_slot in zip(src_slots.to(self._dev), tgt_slots.to(self._dev)):
-            t_src, t_tgt = frames_set_t.to(self._dev)[s_slot], frames_set_t.to(self._dev)[t_slot]
-            is_fg = (fg_masks[int(t_src)] > 0).reshape(-1)
-            fg_px, bg_px = pixels[is_fg], pixels[~is_fg]
-            fg_px = fg_px[torch.randperm(fg_px.shape[0])[:n_fg]]
-            bg_px = bg_px[torch.randperm(bg_px.shape[0])[:n_bg]]
-            start = with_time(torch.cat([fg_px, bg_px], dim=0).to(self._dev), t_src)
-            n = start.shape[0]
-            s_idx, t_idx = s_slot.repeat(n), t_slot.repeat(n)
-            there = with_time(to_px(self.get_point_predictions((start, s_idx, t_idx, frames_set_t), emb)), t_tgt)
-            back = to_px(self.get_point_predictions((there, t_idx, s_idx, frames_set_t), emb))
-            ok = torch.norm(start[:, :2] - back[:, :2], dim=1) <= self.cyc_thresh
-            m = int(ok.sum())
-            rows["source_points"].append(start[ok]); rows["target_points"].append(there[ok]); rows["cycle_points"].append(back[ok])
-            rows["source_frame_indices"].append(s_slot.repeat(m)); rows["target_frame_indices"].append(t_slot.repeat(m))
-            rows["source_times"].append(t_src.repeat(m)); rows["target_times"].append(t_tgt.repeat(m))
-        out = {k: torch.cat(v, dim=0) for k, v in rows.items()}
-        for name in ("source", "target"):
-            t3 = out.pop(f"{name}_times").unsqueeze(1).repeat(1, 3).float()
-            out[f"{name}_times_normalized"] = self.range_normalizer(t3, dst=(-1, 1), dims=[2])[:, 2]
+        device, then per pair a foreground and a background ``randperm``); all pairs tracked as one batch (cycle.py)."""
+        out, _ = self._cycle_draw(frames_set_t, fg_masks)
         return out
 
     def get_cycle_consistent_preds(self, frames_set_t, fg_masks):
         """models/tracker.py:264-301: redraw until at least one point survives the filter, then predict source -> target
-        and target -> source WITH the graph (the cycle-consistency loss of dino_tracker.py:346-353 trains on them)."""
+        and target -> source WITH the graph (the cycle-consistency loss of dino_tracker.py:346-353 trains on them): the
+        survivors' rows of the draw's two legs, as one autograd node."""
         while True:
-            cyc = self.get_cycle_consistent_coords(frames_set_t, fg_masks)
+            cyc, legs = self._cycle_draw(frames_set_t, fg_masks)
             if cyc["source_points"].shape[0] > 0:
                 break
-        emb = self.frame_embeddings
-        fwd = self.get_point_predictions((cyc["source_points"], cyc["source_frame_indices"], cyc["target_frame_indices"],
-                                          frames_set_t), emb)
-        bwd = self.get_point_predictions((cyc["target_points"], cyc["target_frame_indices"], cyc["source_frame_indices"],
-                                          frames_set_t), emb)
+        fwd, bwd = _cycle.predictions(self, self.frame_embeddings, legs)
         return {
             "source_coords": self.range_normalizer(cyc["source_points"], dst=[-1, 1]),
             "target_coords": self.range_normalizer(cyc["target_points"], dst=[-1, 1]),

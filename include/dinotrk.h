@@ -550,6 +550,37 @@ int dinotrk_sampler_select(const uint32_t* bits, int N, int T, const int64_t* fr
 int dinotrk_sampler_gather(const float* rows, int T, const int64_t* row_ids, const int64_t* draws, int m, float* t1,
                            float* t2, void* stream);
 
+/* ---- cycle-consistency term (models/tracker.py:182-301) ------------------------------------------------------------ */
+/* Host only.  The first min(k, n) entries of torch's CPU randperm(n) (int64 out), drawn from the generator state `state`
+ * (the bytes of torch.Generator.get_state(): seed u64, left i32, seeded i32, next u64, mt19937 state[624] as u64, then
+ * the normal-sampling cache), in O(k).  The state is advanced in place past all n - 1 draws randperm makes, so that later
+ * draws are those after torch.randperm(n).  DINOTRK_EINVAL for a state of another size, n < 0, k < 0 or
+ * n >= 2^32 / 20 (torch draws 64-bit numbers there).  No device work. */
+#define DINOTRK_CPU_RNG_STATE_BYTES 5056
+int dinotrk_randperm_prefix(uint8_t* state, size_t state_bytes, int64_t n, int64_t k, int64_t* out);
+/* Foreground masks fg [T][P] uint8 (non-zero = foreground, pixels row-major): off [T][ceil(P / 256)] int32 = foreground
+ * pixels before each block of 256 pixels, n_fg [T] int32 = foreground pixels per frame.  No sync. */
+size_t dinotrk_cycle_mask_workspace_bytes(int T, int P);
+int dinotrk_cycle_mask_scan(const uint8_t* fg, int T, int P, int* off, int* n_fg, void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* One row per drawn point, rows [R][8] int32 = {t_src, is_fg, rank, src_slot, tgt_slot, t_tgt, there_pos, back_pos}:
+ * the point is the rank-th foreground (is_fg != 0) or background pixel of frame t_src (rank below that count);
+ * there_pos / back_pos are its rows in the two legs' batches (permutations of [0, R)).
+ *   select: start [R][3] = (x, y, t_src) and the first leg's input there_pts [there_pos][3] = (x, y, src_slot).
+ *   unnorm: from the first leg's normalised output there_out [R][2] (row order), there_px [R][3] = (x_px, y_px, t_tgt)
+ *           (RangeNormalizer.unnormalize in its fp32 op order) and the second leg's input back_pts [back_pos][3] =
+ *           (x_px, y_px, tgt_slot).
+ *   keep:   back_out [R][2] the second leg's normalised output; row i survives when |start[i].xy - unnormalised
+ *           back_out[i]| <= thresh, the norm evaluated as torch.norm(dim=1) does in fp32.  keep_rows [*n_keep] = the
+ *           surviving rows in order, cycle_px [*n_keep][2] their unnormalised back_out; *n_keep (device int32).
+ * One block for keep: R is a few hundred to a few thousand.  No sync.  Profile class "cycle". */
+int dinotrk_cycle_select(const uint8_t* fg, int T, int H, int W, const int* off, const int* rows, int R, float* start,
+                         float* there_pts, void* stream);
+int dinotrk_cycle_unnorm(const float* there_out, const int* rows, int R, int H, int W, float* there_px, float* back_pts,
+                         void* stream);
+int dinotrk_cycle_keep(const float* start, const float* back_out, int R, int H, int W, float thresh, int* keep_rows,
+                       float* cycle_px, int* n_keep, void* stream);
+
 /* ---- RAFT-large optical flow (torchvision models/optical_flow/raft.py raft_large, eval mode) ---------------------- */
 /* Weights: one entry per convolution in torchvision's parameter order.  w_hi / w_lo are the fp16 split
  * (dinotrk_split_fp16) of the K-major matrix [Np][Kp]: row n = output channel, k = (ky * kw + kx) * C_in + ci with the
