@@ -5,6 +5,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include <nvtx3/nvToolsExt.h>   // header-only; ranges cost nothing unless a profiler injects itself
 
 #include "dinotrk.h"
@@ -112,6 +114,57 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+
+// ---- compaction: count per block (__syncthreads_count), scan the block counts, then emit or select by rank ----------
+// The largest k in [0, n) with key(k) <= x, or 0 if there is none; key (an array or a functor) is ascending.
+template <typename K>
+__device__ __forceinline__ int last_le(int n, int x, K key) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    int k;
+    if constexpr (std::is_pointer<K>::value) k = key[mid]; else k = key(mid);
+    if (k <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// The exclusive rank of this thread's pred among the block's THREADS threads in thread order; *total = the block's
+// count.  One barrier, so every thread of the block calls it; a loop over it needs a barrier before the next call.
+template <int THREADS>
+__device__ __forceinline__ int block_rank(bool pred, int* total = nullptr) {
+  __shared__ int s_warp[THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned ball = __ballot_sync(0xffffffffu, pred);
+  if (lane == 0) s_warp[warp] = __popc(ball);
+  __syncthreads();
+  int rank = __popc(ball & ((1u << lane) - 1u)), sum = 0;
+#pragma unroll
+  for (int k = 0; k < THREADS / 32; ++k) { rank += k < warp ? s_warp[k] : 0; sum += s_warp[k]; }
+  if (total) *total = sum;
+  return rank;
+}
+
+// The index of the n-th (from 0) i in [begin, end) with hit(i), or -1 if there is none.  The whole warp calls it with
+// the same arguments and tests 32 indices at a time.
+template <typename F>
+__device__ __forceinline__ int warp_nth_hit(int begin, int end, int n, F hit) {
+  const int lane = threadIdx.x & 31;
+  for (int base = begin; base < end; base += 32) {
+    const bool h = base + lane < end && hit(base + lane);
+    const unsigned ball = __ballot_sync(0xffffffffu, h);
+    if (n < __popc(ball)) {
+      const unsigned sel = __ballot_sync(0xffffffffu, h && __popc(ball & ((1u << lane) - 1u)) == n);
+      return base + __ffs(sel) - 1;
+    }
+    n -= __popc(ball);
+  }
+  return -1;
+}
+
+// Exclusive scan of `rows` count arrays of nb entries, one block each (features.cu): row r scans cnt + r * nb into
+// off + r * nb and writes its sum to total[r].
+int launch_count_scan(const int* cnt, int nb, int rows, int* off, int* total, cudaStream_t stream);
 
 // ---- exact restatement of the reference's coordinate arithmetic ---------------------------
 // models/tracker.py:84-93: a, b are computed in Python doubles and stored as fp32.

@@ -58,13 +58,9 @@ corr_gemm_kernel(const float* __restrict__ tpc, const float* __restrict__ norms,
   extern __shared__ __align__(16) float smem[];
   const int mt = blockIdx.x;
   if (mt >= tile_start[n_groups]) return;
-  // binary search: last group k with tile_start[k] <= mt and a non-empty tile range
-  int lo = 0, hi = n_groups - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (tile_start[mid] <= mt) lo = mid; else hi = mid - 1;
-  }
-  const int g = lo;  // groups with zero tiles share a start with their successor; "last <=" skips them
+  // last group k with tile_start[k] <= mt and a non-empty tile range: groups with zero tiles share a start with their
+  // successor; "last <=" skips them
+  const int g = last_le(n_groups, mt, tile_start);
   const int m_grp = grp_m[g];
   const int m0 = (mt - tile_start[g]) * BM;
   const int n0 = blockIdx.y * BN;

@@ -17,9 +17,6 @@
 
 namespace dtk {
 
-// exclusive scan of block counts (traj.cu)
-__global__ void scan_counts_kernel(const int* __restrict__ cnt, int n, int* __restrict__ off, int* __restrict__ n_total);
-
 constexpr int CYC_THREADS = 256;   // pixels per count block
 constexpr int CYC_SEL_WARPS = 8;
 constexpr int CYC_KEEP_THREADS = 1024;
@@ -98,23 +95,9 @@ cycle_select_kernel(const uint8_t* __restrict__ fg, int W, int P, int nb, const 
   const uint8_t* m = fg + (size_t)t * P;
   // pixels of the wanted kind before block b: off[b] (foreground) or b * CYC_THREADS - off[b] (background)
   auto before = [&](int b) { return want ? o[b] : b * CYC_THREADS - o[b]; };
-  int lo = 0, hi = nb - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (before(mid) <= r[2]) lo = mid; else hi = mid - 1;
-  }
-  int rank = r[2] - before(lo), pix = -1;
-  for (int base = lo * CYC_THREADS; base < min(lo * CYC_THREADS + CYC_THREADS, P) && pix < 0; base += 32) {
-    const int p = base + lane;
-    const bool hit = p < P && ((m[p] != 0) == (want != 0));
-    const unsigned ball = __ballot_sync(0xffffffffu, hit);
-    if (rank < __popc(ball)) {
-      const unsigned sel = __ballot_sync(0xffffffffu, hit && __popc(ball & ((1u << lane) - 1u)) == rank);
-      pix = base + __ffs(sel) - 1;
-    } else {
-      rank -= __popc(ball);
-    }
-  }
+  const int b = last_le(nb, r[2], before);
+  const int pix = warp_nth_hit(b * CYC_THREADS, min(b * CYC_THREADS + CYC_THREADS, P), r[2] - before(b),
+                               [&](int p) { return (m[p] != 0) == (want != 0); });
   if (lane != 0) return;
   // the host draws ranks below the frame's count, so pix >= 0
   const float x = (float)(pix % W), y = (float)(pix / W);
@@ -149,11 +132,7 @@ __global__ void cycle_unnorm_kernel(const float* __restrict__ there_out, const i
 __global__ void __launch_bounds__(CYC_KEEP_THREADS)
 cycle_keep_kernel(const float* __restrict__ start, const float* __restrict__ back_out, int R, float w_m1, float h_m1,
                   float thresh, int* __restrict__ keep_rows, float* __restrict__ cycle_px, int* __restrict__ n_keep) {
-  __shared__ int s_warp[CYC_KEEP_THREADS / 32];
-  __shared__ int s_base;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_base = 0;
-  __syncthreads();
+  int base = 0;
   for (int i0 = 0; i0 < R; i0 += CYC_KEEP_THREADS) {
     const int i = i0 + threadIdx.x;
     bool keep = false;
@@ -164,21 +143,17 @@ cycle_keep_kernel(const float* __restrict__ start, const float* __restrict__ bac
       const float dx = __fsub_rn(start[3 * i], bx), dy = __fsub_rn(start[3 * i + 1], by);
       keep = __fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy))) <= thresh;
     }
-    const unsigned ball = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) s_warp[warp] = __popc(ball);
-    __syncthreads();
-    int k = s_base + __popc(ball & ((1u << lane) - 1u));
-    for (int w = 0; w < warp; ++w) k += s_warp[w];
+    int total;
+    const int k = base + block_rank<CYC_KEEP_THREADS>(keep, &total);
     if (keep) {
       keep_rows[k] = i;
       cycle_px[2 * k] = bx;
       cycle_px[2 * k + 1] = by;
     }
-    __syncthreads();
-    if (threadIdx.x == CYC_KEEP_THREADS - 1) s_base = k + (keep ? 1 : 0);
-    __syncthreads();
+    base += total;
+    __syncthreads();   // the next chunk's block_rank rewrites the warp counts
   }
-  if (threadIdx.x == 0) *n_keep = s_base;
+  if (threadIdx.x == 0) *n_keep = base;
 }
 
 }  // namespace dtk
@@ -247,11 +222,7 @@ int dinotrk_cycle_mask_scan(const uint8_t* fg, int T, int P, int* off, int* n_fg
   ProfRange pr(PROF_CYCLE, st);
   cycle_mask_count_kernel<<<dim3(nb, T), CYC_THREADS, 0, st>>>(fg, P, nb, cnt);
   DTK_LAUNCHED();
-  for (int t = 0; t < T; ++t) {
-    scan_counts_kernel<<<1, 1024, 0, st>>>(cnt + (size_t)t * nb, nb, off + (size_t)t * nb, n_fg + t);
-    DTK_LAUNCHED();
-  }
-  return DINOTRK_OK;
+  return launch_count_scan(cnt, nb, T, off, n_fg, st);
 }
 
 int dinotrk_cycle_select(const uint8_t* fg, int T, int H, int W, const int* off, const int* rows, int R, float* start,

@@ -34,6 +34,35 @@ void prof_begin(int cls, cudaStream_t st) {
 }
 void prof_end(cudaStream_t st) { cudaEventRecord(g_prof_recs.back().b, st); }
 
+// ---- exclusive scan of block counts: one block per row of nb counts ---------------------------------------------
+constexpr int SCAN_THREADS = 1024;
+__global__ void __launch_bounds__(SCAN_THREADS)
+scan_counts_kernel(const int* __restrict__ cnt, int n, int* __restrict__ off, int* __restrict__ total) {
+  __shared__ int s_sum[SCAN_THREADS];
+  cnt += (size_t)blockIdx.x * n;
+  off += (size_t)blockIdx.x * n;
+  const int per = (n + SCAN_THREADS - 1) / SCAN_THREADS, b = threadIdx.x * per, e = min(b + per, n);
+  int sum = 0;
+  for (int i = b; i < e; ++i) sum += cnt[i];
+  s_sum[threadIdx.x] = sum;
+  __syncthreads();
+  for (int o = 1; o < SCAN_THREADS; o <<= 1) {   // Hillis-Steele inclusive scan
+    const int v = threadIdx.x >= o ? s_sum[threadIdx.x - o] : 0;
+    __syncthreads();
+    s_sum[threadIdx.x] += v;
+    __syncthreads();
+  }
+  int run = s_sum[threadIdx.x] - sum;
+  for (int i = b; i < e; ++i) { off[i] = run; run += cnt[i]; }
+  if (threadIdx.x == SCAN_THREADS - 1) total[blockIdx.x] = s_sum[SCAN_THREADS - 1];
+}
+
+int launch_count_scan(const int* cnt, int nb, int rows, int* off, int* total, cudaStream_t stream) {
+  scan_counts_kernel<<<rows, SCAN_THREADS, 0, stream>>>(cnt, nb, off, total);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
+}
+
 // ---- [T][C][P] <-> [T][P][C] tiled transposes -------------------------------------------------
 __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int R, int S) {
   // per batch item (blockIdx.z): in [R][S] -> out [S][R]

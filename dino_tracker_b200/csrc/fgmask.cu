@@ -20,9 +20,6 @@
 
 namespace dtk {
 
-// exclusive scan of block counts (traj.cu)
-__global__ void scan_counts_kernel(const int* __restrict__ cnt, int n, int* __restrict__ off, int* __restrict__ n_total);
-
 constexpr int PCA_THREADS = 256, PCA_WARPS = PCA_THREADS / 32;
 constexpr int PCA_ROWS = 64;                        // rows a warp accumulates in fp32 before the float64 flush
 constexpr int PCA_TILE = PCA_WARPS * PCA_ROWS;
@@ -315,15 +312,10 @@ split_count_kernel(const float2* __restrict__ traj, int N, int T, const uint8_t*
 __global__ void __launch_bounds__(SPLIT_THREADS)
 split_emit_kernel(const float2* __restrict__ traj, int N, int T, const uint8_t* __restrict__ cls, const int* __restrict__ off,
                   float2* __restrict__ fg, float2* __restrict__ bg) {
-  __shared__ int s_warp[SPLIT_THREADS / 32];
   __shared__ long long s_dst[SPLIT_THREADS];          // fg row, or -1 - bg row
   const int n = blockIdx.x * SPLIT_THREADS + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool is_fg = n < N && cls[n] == 1;
-  const unsigned ball = __ballot_sync(0xffffffffu, is_fg);
-  if (lane == 0) s_warp[warp] = __popc(ball);
-  __syncthreads();
-  int rank = __popc(ball & ((1u << lane) - 1u));
-  for (int k = 0; k < warp; ++k) rank += s_warp[k];
+  const int rank = block_rank<SPLIT_THREADS>(is_fg);
   const int fg0 = off[blockIdx.x], bg0 = blockIdx.x * SPLIT_THREADS - fg0;
   s_dst[threadIdx.x] = is_fg ? (long long)(fg0 + rank) : -1 - (long long)(bg0 + threadIdx.x - rank);
   __syncthreads();
@@ -511,8 +503,7 @@ int dinotrk_traj_split_count(const float* traj, int N, int T, const uint8_t* mas
     split_count_kernel<<<nb, SPLIT_THREADS, 0, st>>>(reinterpret_cast<const float2*>(traj), N, T, masks, Tm, H, W, w.cls,
                                                       w.cnt, w.counts);
     DTK_LAUNCHED();
-    scan_counts_kernel<<<1, 1024, 0, st>>>(w.cnt, nb, w.off, w.counts);
-    DTK_LAUNCHED();
+    if (int rc = launch_count_scan(w.cnt, nb, 1, w.off, w.counts, st)) return rc;
   }
   int host[4];
   DTK_CUDA(cudaMemcpyAsync(host, w.counts, sizeof(host), cudaMemcpyDeviceToHost, st));

@@ -42,11 +42,7 @@ __global__ void index_traj_kernel(const int* __restrict__ grp_frame, const int* 
                                   int* __restrict__ out_index, float* __restrict__ traj) {
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_maps) return;
-  int lo = 0, hi = n_groups - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (grp_map0[mid] <= j) lo = mid; else hi = mid - 1;
-  }
+  const int lo = last_le(n_groups, j, grp_map0);
   int n = grp_row0[lo] + (j - grp_map0[lo]);
   int t = grp_frame[lo];
   out_index[j] = n * T + t;
@@ -88,30 +84,20 @@ __global__ void traj_cos_kernel(const float* __restrict__ tpc, int T, int C, int
 
 // ---------------------------------------------------------------------------------- phase C helpers
 // per anchor frame a: ordered list of the query points n with cos[n][a] >= th, and its length
-__global__ void anchor_lists_kernel(const float* __restrict__ cos_sims, int N, int T, float th,
-                                    int* __restrict__ cnt, int* __restrict__ qlist) {
+constexpr int ANCHOR_LIST_THREADS = 256;
+__global__ void __launch_bounds__(ANCHOR_LIST_THREADS)
+anchor_lists_kernel(const float* __restrict__ cos_sims, int N, int T, float th, int* __restrict__ cnt,
+                    int* __restrict__ qlist) {
   const int a = blockIdx.x;
-  __shared__ int base;
-  __shared__ int wcount[32];
-  if (threadIdx.x == 0) base = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  for (int n0 = 0; n0 < N; n0 += blockDim.x) {
-    int n = n0 + threadIdx.x;
-    bool v = n < N && cos_sims[(size_t)n * T + a] >= th;
-    unsigned bal = __ballot_sync(0xffffffffu, v);
-    if (lane == 0) wcount[warp] = __popc(bal);
-    __syncthreads();
-    int off = base;
-    for (int k = 0; k < warp; ++k) off += wcount[k];
-    if (v) qlist[(size_t)a * N + off + __popc(bal & ((1u << lane) - 1))] = n;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int tot = 0;
-      for (int k = 0; k < nw; ++k) tot += wcount[k];
-      base += tot;
-    }
-    __syncthreads();
+  int base = 0;
+  for (int n0 = 0; n0 < N; n0 += ANCHOR_LIST_THREADS) {
+    const int n = n0 + threadIdx.x;
+    const bool v = n < N && cos_sims[(size_t)n * T + a] >= th;
+    int total;
+    const int rank = block_rank<ANCHOR_LIST_THREADS>(v, &total);
+    if (v) qlist[(size_t)a * N + base + rank] = n;
+    base += total;
+    __syncthreads();   // the next chunk's block_rank rewrites the warp counts
   }
   if (threadIdx.x == 0) cnt[a] = base;
 }
@@ -126,11 +112,7 @@ __global__ void sample_anchor_kernel(const float* __restrict__ tpc, int T, int C
                                      float* __restrict__ desc, float* __restrict__ dnorm, int* __restrict__ out_index,
                                      __half* __restrict__ desc_hi, __half* __restrict__ desc_lo) {
   const int j = blockIdx.x;
-  int lo = 0, hi = n_groups - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (grp_map0[mid] <= j) lo = mid; else hi = mid - 1;
-  }
+  const int lo = last_le(n_groups, j, grp_map0);
   const int a = grp_frame[lo];
   const int u = grp_item0[lo] + (j - grp_map0[lo]);
   const int slot = u / T, i = u - slot * T;
@@ -205,11 +187,7 @@ __global__ void anchor_scalars_kernel(int T, const int* __restrict__ qlist, int 
                                       float* __restrict__ desc_eps) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_maps) return;
-  int lo = 0, hi = n_groups - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (grp_map0[mid] <= j) lo = mid; else hi = mid - 1;
-  }
+  const int lo = last_le(n_groups, j, grp_map0);
   const int a = grp_frame[lo];
   const int uu = grp_item0[lo] + (j - grp_map0[lo]);
   const int slot = uu / T, i = uu - slot * T;
@@ -239,11 +217,7 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
                                      int8_t* __restrict__ desc_q8, float* __restrict__ desc_fac,
                                      float* __restrict__ desc_eps) {
   const int j = map_lo + blockIdx.x;
-  int lo = 0, hi = n_groups - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (grp_map0[mid] <= j) lo = mid; else hi = mid - 1;
-  }
+  const int lo = last_le(n_groups, j, grp_map0);
   if (grp_row0[lo] < n_unique) return;   // read in place
   const int a = grp_frame[lo];
   const int uu = grp_item0[lo] + (j - grp_map0[lo]);
@@ -949,7 +923,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     NvtxRange nv("dinotrk.infer.C.anchors");
     {
       ProfRange pr(PROF_ANCHOR_LIST, st);
-      anchor_lists_kernel<<<T, 256, 0, st>>>(cos_sims, N, T, anchor_th, d_cnt, d_qlist);
+      anchor_lists_kernel<<<T, ANCHOR_LIST_THREADS, 0, st>>>(cos_sims, N, T, anchor_th, d_cnt, d_qlist);
       DTK_LAUNCHED();
     }
     std::vector<int> cnt(T);

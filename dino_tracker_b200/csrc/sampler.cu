@@ -14,9 +14,6 @@
 
 namespace dtk {
 
-// exclusive scan of block counts (traj.cu)
-__global__ void scan_counts_kernel(const int* __restrict__ cnt, int n, int* __restrict__ off, int* __restrict__ n_total);
-
 constexpr int SMP_THREADS = 256;
 constexpr int SMP_MAX_T = 65536;
 
@@ -45,16 +42,11 @@ sampler_prepare_count_kernel(const float2* __restrict__ traj, int N, int T, int*
 __global__ void __launch_bounds__(SMP_THREADS)
 sampler_prepare_emit_kernel(const float2* __restrict__ traj, int N, int T, const int* __restrict__ off,
                             float2* __restrict__ rows, uint32_t* __restrict__ bits) {
-  __shared__ int s_warp[SMP_THREADS / 32];
-  const int n = blockIdx.x * SMP_THREADS + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int n = blockIdx.x * SMP_THREADS + threadIdx.x;
   const float2* src = traj + (size_t)n * T;
   const bool keep = n < N && valid_steps(src, T) > 1;
-  const unsigned ball = __ballot_sync(0xffffffffu, keep);
-  if (lane == 0) s_warp[warp] = __popc(ball);
-  __syncthreads();
+  const int rank = block_rank<SMP_THREADS>(keep);
   if (!keep) return;
-  int rank = __popc(ball & ((1u << lane) - 1u));
-  for (int k = 0; k < warp; ++k) rank += s_warp[k];
   const size_t r = (size_t)off[blockIdx.x] + rank;
   float2* dst = rows + r * T;
   uint32_t* b = bits + r * smp_words(T);
@@ -111,23 +103,9 @@ sampler_select_kernel(const uint32_t* __restrict__ bits, int N, int T, const int
   const int lane = threadIdx.x & 31, i = blockIdx.x * SEL_WARPS + (threadIdx.x >> 5);
   if (i >= m) return;
   const int pos = (int)perm[i];
-  int lo = 0, hi = nb - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (off[mid] <= pos) lo = mid; else hi = mid - 1;
-  }
-  int rank = pos - off[lo], row = -1;
-  for (int base = lo * SMP_THREADS; base < min(lo * SMP_THREADS + SMP_THREADS, N) && row < 0; base += 32) {
-    const int n = base + lane;
-    const bool cand = n < N && is_candidate(bits, s_mask, W, n);
-    const unsigned ball = __ballot_sync(0xffffffffu, cand);
-    if (rank < __popc(ball)) {
-      const unsigned hit = __ballot_sync(0xffffffffu, cand && __popc(ball & ((1u << lane) - 1u)) == rank);
-      row = base + __ffs(hit) - 1;
-    } else {
-      rank -= __popc(ball);
-    }
-  }
+  const int blk = last_le(nb, pos, off);
+  const int row = warp_nth_hit(blk * SMP_THREADS, min(blk * SMP_THREADS + SMP_THREADS, N), pos - off[blk],
+                               [&](int n) { return is_candidate(bits, s_mask, W, n); });
   if (lane == 0) row_ids[i] = row;
   float* out = mat + (size_t)i * T;
   if (row < 0) {   // a position past the candidate total: no row, no weight
@@ -207,8 +185,7 @@ int dinotrk_sampler_prepare_count(const float* traj, int N, int T, int* n_valid,
     ProfRange pr(PROF_SAMPLER, st);
     sampler_prepare_count_kernel<<<nb, SMP_THREADS, 0, st>>>(src, N, T, w.cnt);
     DTK_LAUNCHED();
-    scan_counts_kernel<<<1, 1024, 0, st>>>(w.cnt, nb, w.off, w.total);
-    DTK_LAUNCHED();
+    if (int rc = launch_count_scan(w.cnt, nb, 1, w.off, w.total, st)) return rc;
   }
   return read_total(w, n_valid, st);
 }
@@ -243,8 +220,7 @@ int dinotrk_sampler_count(const uint32_t* bits, int N, int T, const int64_t* fra
     ProfRange pr(PROF_SAMPLER, st);
     sampler_count_kernel<<<nb, SMP_THREADS, smp_words(T) * 4, st>>>(bits, N, T, frames, n_frames, w.cnt);
     DTK_LAUNCHED();
-    scan_counts_kernel<<<1, 1024, 0, st>>>(w.cnt, nb, w.off, w.total);
-    DTK_LAUNCHED();
+    if (int rc = launch_count_scan(w.cnt, nb, 1, w.off, w.total, st)) return rc;
   }
   return read_total(w, n_cand, st);
 }

@@ -145,12 +145,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
   auto decode = [&](int tile, int& g, int& m0, int& n0) {
     int mt = tile / n_tiles_n;
     n0 = (tile - mt * n_tiles_n) * BN;
-    int lo = 0, hi = pb.n_groups - 1;
-    while (lo < hi) {
-      int mid = (lo + hi + 1) >> 1;
-      if (pb.tile_start[mid] <= mt) lo = mid; else hi = mid - 1;
-    }
-    g = lo;
+    g = last_le(pb.n_groups, mt, pb.tile_start);
     m0 = (mt - pb.tile_start[g]) * TM + (int)rank * TC_BM;
   };
 

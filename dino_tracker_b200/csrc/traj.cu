@@ -155,42 +155,15 @@ traj_chain_kernel(ChainArgs a, const uint8_t* __restrict__ occ, int* __restrict_
   if (threadIdx.x == 0) block_cnt[blockIdx.x] = n;
 }
 
-// Exclusive scan of block counts (one block); total -> *n_total.
-constexpr int SCAN_THREADS = 1024;
-__global__ void __launch_bounds__(SCAN_THREADS)
-scan_counts_kernel(const int* __restrict__ cnt, int n, int* __restrict__ off, int* __restrict__ n_total) {
-  __shared__ int s_sum[SCAN_THREADS];
-  const int per = (n + SCAN_THREADS - 1) / SCAN_THREADS, b = threadIdx.x * per, e = min(b + per, n);
-  int sum = 0;
-  for (int i = b; i < e; ++i) sum += cnt[i];
-  s_sum[threadIdx.x] = sum;
-  __syncthreads();
-  for (int o = 1; o < SCAN_THREADS; o <<= 1) {   // Hillis-Steele inclusive scan
-    const int v = threadIdx.x >= o ? s_sum[threadIdx.x - o] : 0;
-    __syncthreads();
-    s_sum[threadIdx.x] += v;
-    __syncthreads();
-  }
-  int run = s_sum[threadIdx.x] - sum;
-  for (int i = b; i < e; ++i) { off[i] = run; run += cnt[i]; }
-  if (threadIdx.x == SCAN_THREADS - 1) *n_total = s_sum[SCAN_THREADS - 1];
-}
-
 // Kept pixel p of block b -> out row off[b] + (rank of p among the block's kept pixels): NaN before s, the walk's
 // positions on [s, s + len), NaN after; marks occ[t][round(y)][round(x)] for t in (s, s + len).
 __global__ void __launch_bounds__(TRAJ_THREADS)
 traj_emit_kernel(const float* __restrict__ fwd, int T, int H, int W, int s, const int* __restrict__ len,
                  const int* __restrict__ off, uint8_t* __restrict__ occ, float* __restrict__ out) {
-  __shared__ int s_warp[TRAJ_THREADS / 32];
   const size_t P = (size_t)H * W, p = (size_t)blockIdx.x * TRAJ_THREADS + threadIdx.x;
   const int L = p < P ? len[p] : 0;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned ball = __ballot_sync(0xffffffffu, L > 0);
-  if (lane == 0) s_warp[warp] = __popc(ball);
-  __syncthreads();
+  const int rank = block_rank<TRAJ_THREADS>(L > 0);
   if (L == 0) return;
-  int rank = __popc(ball & ((1u << lane) - 1u));
-  for (int k = 0; k < warp; ++k) rank += s_warp[k];
   float2* row = reinterpret_cast<float2*>(out) + (size_t)(off[blockIdx.x] + rank) * T;
   const float2 nan2 = make_float2(NAN, NAN);
   for (int t = 0; t < s; ++t) row[t] = nan2;
@@ -232,8 +205,7 @@ traj_nearest_kernel(const float2* __restrict__ posT, int M, int gh, int gw, floa
                     unsigned long long* __restrict__ keys) {
   __shared__ float2 s_pos[NEAR_THREADS];
   __shared__ int s_idx[NEAR_THREADS];
-  __shared__ int s_warp[NEAR_THREADS / 32];
-  const int G = gh * gw, t = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int G = gh * gw, t = blockIdx.y;
   float px[NEAR_PTS], py[NEAR_PTS], best_r[NEAR_PTS], best_s[NEAR_PTS];
   int best_n[NEAR_PTS];
 #pragma unroll
@@ -250,12 +222,8 @@ traj_nearest_kernel(const float2* __restrict__ posT, int M, int gh, int gw, floa
     float2 q = make_float2(NAN, NAN);
     if (n < n1) q = pos[n];
     const bool valid = !isnan(q.x) && !isnan(q.y);
-    const unsigned ball = __ballot_sync(0xffffffffu, valid);
-    if (lane == 0) s_warp[warp] = __popc(ball);
-    __syncthreads();
-    int slot = __popc(ball & ((1u << lane) - 1u)), cnt = 0;
-#pragma unroll
-    for (int k = 0; k < NEAR_THREADS / 32; ++k) { slot += k < warp ? s_warp[k] : 0; cnt += s_warp[k]; }
+    int cnt;
+    const int slot = block_rank<NEAR_THREADS>(valid, &cnt);
     if (valid) { s_pos[slot] = q; s_idx[slot] = n; }
     __syncthreads();
     for (int i = 0; i < cnt; ++i) {
@@ -311,11 +279,7 @@ __global__ void of_filter_kernel(const float* __restrict__ traj, int T, const in
                                  const int* __restrict__ offsets, int n_pairs, int n_pts, uint8_t* __restrict__ keep) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pts) return;
-  int lo = 0, hi = n_pairs - 1;   // pair k: offsets[k] <= i < offsets[k + 1]
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (offsets[mid] <= i) lo = mid; else hi = mid - 1;
-  }
+  const int lo = last_le(n_pairs, i, offsets);   // pair k: offsets[k] <= i < offsets[k + 1]
   const int ts = pair_src[lo], tt = pair_tgt[lo], G = gh * gw;
   const int ns = nearest[(size_t)ts * G + grid_index(src_xy[2 * i + 1], stride, gh) * gw + grid_index(src_xy[2 * i], stride, gw)];
   const int nt = nearest[(size_t)tt * G + grid_index(tgt_xy[2 * i + 1], stride, gh) * gw + grid_index(tgt_xy[2 * i], stride, gw)];
@@ -378,9 +342,7 @@ int dinotrk_traj_chain(const dinotrk_flow_video* fv, const uint8_t* masks, int s
   ProfRange pr(PROF_MISC, st);
   traj_chain_kernel<<<(unsigned)nb, TRAJ_THREADS, 0, st>>>(a, w.occ, w.len, w.cnt);
   DTK_LAUNCHED();
-  scan_counts_kernel<<<1, SCAN_THREADS, 0, st>>>(w.cnt, (int)nb, w.off, n_kept);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
+  return launch_count_scan(w.cnt, (int)nb, 1, w.off, n_kept, st);
 }
 
 int dinotrk_traj_emit(const dinotrk_flow_video* fv, int s, float* out, void* workspace, size_t workspace_bytes, void* stream) {

@@ -139,6 +139,34 @@ def test_cycle_term_matches_per_pair_reference(host_set):
         assert b.abs().max().item() > 0 and _rel(a, b) <= GRAD_TOL
 
 
+def test_mask_scan_batches_frames():
+    """dinotrk_cycle_mask_scan on 5 frames of 476 x 854 (1588 blocks of 256 pixels: each scan thread sums more than one
+    count): every frame's block offsets and foreground count equal numpy's, from one count and one scan launch."""
+    import numpy as np
+    from dino_tracker_b200 import _lib
+    T, P = 5, GEO.H * GEO.W
+    nb = -(-P // 256)
+    assert nb == 1588
+    fg = np.zeros((T, P), np.uint8)                 # frame 0: all background
+    fg[1] = 1                                       # all foreground
+    fg[2] = np.random.default_rng(97).integers(0, 3, P)
+    fg[3, -1] = 1                                   # only the last pixel
+    fg[4, 0] = 2                                    # only pixel 0
+    cnt = np.pad(fg != 0, ((0, 0), (0, nb * 256 - P))).reshape(T, nb, 256).sum(-1)
+    lib = _lib.load()
+    d_fg = torch.from_numpy(fg).to(DEV)
+    off = torch.full((T, nb), -1, device=DEV, dtype=torch.int32)
+    n_fg = torch.full((T,), -1, device=DEV, dtype=torch.int32)
+    ws_bytes = lib.dinotrk_cycle_mask_workspace_bytes(T, P)
+    ws = torch.empty(ws_bytes, device=DEV, dtype=torch.uint8)
+    before = _lib.launch_count()
+    _lib.check(lib.dinotrk_cycle_mask_scan(_lib.ptr(d_fg), T, P, _lib.ptr(off), _lib.ptr(n_fg), _lib.ptr(ws), ws_bytes,
+                                           _lib.stream_ptr()), "cycle_mask_scan")
+    assert _lib.launch_count() - before == 2        # the count and one scan over all frames
+    np.testing.assert_array_equal(off.cpu().numpy(), np.cumsum(cnt, 1) - cnt)
+    np.testing.assert_array_equal(n_fg.cpu().numpy(), cnt.sum(1))
+
+
 def test_keep_decides_as_torch_norm_at_the_threshold():
     """Points whose way back ends within a few ulps of the 4 px circle: the kernel's keep flags equal
     torch.norm(start - unnormalize(back), dim=1) <= 4 evaluated on the device."""
