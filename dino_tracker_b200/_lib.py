@@ -29,7 +29,8 @@ class Features(Structure):
 
 class VitConfig(Structure):
     _fields_ = [("depth", c_int), ("dim", c_int), ("heads", c_int), ("tap_layer", c_int), ("patch", c_int), ("stride", c_int),
-                ("attn_materialized", c_int), ("gemm_f16", c_int), ("gemm_pair", c_int)]
+                ("attn_materialized", c_int), ("gemm_f16", c_int), ("gemm_pair", c_int), ("swiglu_hidden", c_int),
+                ("facet", c_int)]
 
 
 class VitWeights(Structure):

@@ -1,7 +1,8 @@
 // DINOv2 ViT feature extractor (SURVEY.md 8a row a1): ImageNet normalisation, 14x14 / stride-7 patch embedding,
 // cls + interpolated position embedding, pre-LN blocks (LayerNorm eps 1e-6, MHA scale 1/8, LayerScale, MLP 4x with
-// exact GELU), tap = output of block `layer` before the final norm, cls dropped, written straight into the
-// token-major feature video [T][P][C]   (models/extractor.py:41-85,137-150; utils.py:32-72; the block arithmetic is
+// exact GELU, or ViT-g/14's SwiGLU MLP), tap = output of block `layer` before the final norm -- or that block's query /
+// key / value facet, its qkv Linear output -- cls dropped, written straight into the
+// token-major feature video [T][P][C]   (models/extractor.py:41-85,137-150,224-266; utils.py:32-72; the block arithmetic is
 // facebookresearch/dinov2's -- parity unpinned, see DESIGN.md).
 //
 // Default path (gemm_f16 = 1, attn_materialized = 0): fp16 operands / fp32 accumulation everywhere.  The linear layers
@@ -355,6 +356,88 @@ struct EpiGelu : EpiBase {
   }
 };
 
+// silu(a) b.  fp16 path: a / (1 + 2^(-a log2 e)) with one ex2.approx and one rcp.approx (MUFU; relative error
+// ~2^-21 + |a| 2^-24 from the rounded exponent argument, below the fp16 rounding of h right after); a -> -inf gives
+// 2^+inf = inf and a * 0 = -0.  Explicit roundings keep the coalesced and thread-per-row calls bit-identical.
+template <typename OutT>
+__device__ __forceinline__ float swiglu_gate(float a, float b) {
+  if constexpr (sizeof(OutT) == 4) return __fmul_rn(__fdiv_rn(a, __fadd_rn(1.f, expf(-a))), b);
+  const float e = fast_exp2(__fmul_rn(-1.4426950408889634f, a));
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(__fadd_rn(1.f, e)));
+  return __fmul_rn(__fmul_rn(a, r), b);
+}
+
+// SwiGLU MLP: h[r][j] = silu(x1_j + b1_j) * (x2_j + b2_j) from the w12 GEMM of width 2 Hd, whose rows (and bias) the
+// host interleaves per pair of hidden units: GEMM columns 4q .. 4q+3 = x1 of units 2q, 2q+1, then x2 of the same two.
+// So every 4-column group (vec4) and every 32-column block (thread-per-row) holds whole (x1, x2) pairs, and output
+// column = GEMM column / 2.  The 2 Hd-wide product never leaves the SM.  Hd % 8 == 0, so N = 2 Hd and every column
+// count the GEMM passes are multiples of 16: a block's 8 or 16 outputs are one or two 16-byte fp16 stores.
+template <typename OutT>
+struct EpiSwiGLU : EpiBase {
+  static constexpr bool kCoalesced = true;
+  OutT* h; const float* bias; int ld;   // ld = Hd
+  int all_direct = 0;
+  __device__ __forceinline__ bool direct(int) const { return all_direct != 0; }
+  __device__ __forceinline__ void vec4(int, int r, int col, float4 v) const {
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col));
+    const float g0 = swiglu_gate<OutT>(__fadd_rn(v.x, bb.x), __fadd_rn(v.z, bb.z));
+    const float g1 = swiglu_gate<OutT>(__fadd_rn(v.y, bb.y), __fadd_rn(v.w, bb.w));
+    OutT* o = h + (size_t)r * ld + (col >> 1);
+    if constexpr (sizeof(OutT) == 4) *reinterpret_cast<float2*>(o) = make_float2(g0, g1);
+    else *reinterpret_cast<__half2*>(o) = __floats2half2_rn(g0, g1);
+  }
+  __device__ __forceinline__ void operator()(State&, int, int r, int col0, const float (&f)[32], int ncols) const {
+    OutT* o = h + (size_t)r * ld + (col0 >> 1);
+    float gl[16];
+#pragma unroll
+    for (int i = 0; i < 32; i += 4) {
+      const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col0 + (i < ncols ? i : 0)));
+      gl[i / 2] = swiglu_gate<OutT>(__fadd_rn(f[i], bb.x), __fadd_rn(f[i + 2], bb.z));
+      gl[i / 2 + 1] = swiglu_gate<OutT>(__fadd_rn(f[i + 1], bb.y), __fadd_rn(f[i + 3], bb.w));
+    }
+    if constexpr (sizeof(OutT) == 4) {
+#pragma unroll
+      for (int i = 0; i < 16; i += 4)
+        if (2 * i + 8 <= ncols) *reinterpret_cast<float4*>(o + i) = make_float4(gl[i], gl[i + 1], gl[i + 2], gl[i + 3]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 16; i += 8)
+        if (2 * i + 16 <= ncols) {
+          __half2 h0 = __floats2half2_rn(gl[i], gl[i + 1]), h1 = __floats2half2_rn(gl[i + 2], gl[i + 3]);
+          __half2 h2 = __floats2half2_rn(gl[i + 4], gl[i + 5]), h3 = __floats2half2_rn(gl[i + 6], gl[i + 7]);
+          *reinterpret_cast<uint4*>(o + i) = make_uint4(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1),
+                                                        *reinterpret_cast<uint32_t*>(&h2), *reinterpret_cast<uint32_t*>(&h3));
+        }
+    }
+  }
+};
+
+// query / key / value facet of the tap block: out[b][n - 1][col] = acc + bias[col] for token n >= 1 of frame b
+// (row r = b N1 + n), fp32, token-major; the cls row (n = 0) is dropped
+struct EpiFacet : EpiBase {
+  static constexpr bool kCoalesced = true;
+  float* out; const float* bias; int N1, D;
+  __device__ __forceinline__ void vec4(int, int r, int col, float4 v) const {
+    const int b = fast_div(r, N1), n = r - b * N1;
+    if (n == 0) return;
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col));
+    *reinterpret_cast<float4*>(out + ((size_t)b * (N1 - 1) + n - 1) * D + col) =
+        make_float4(v.x + bb.x, v.y + bb.y, v.z + bb.z, v.w + bb.w);
+  }
+  __device__ __forceinline__ void operator()(State&, int, int r, int col0, const float (&f)[32], int ncols) const {
+    const int b = r / N1, n = r - b * N1;
+    if (n == 0) return;
+    float* o = out + ((size_t)b * (N1 - 1) + n - 1) * D + col0;
+#pragma unroll
+    for (int i = 0; i < 32; i += 4)
+      if (i < ncols) {   // ncols is a multiple of 4 (D % 64 == 0)
+        const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col0 + i));
+        *reinterpret_cast<float4*>(o + i) = make_float4(f[i] + bb.x, f[i + 1] + bb.y, f[i + 2] + bb.z, f[i + 3] + bb.w);
+      }
+  }
+};
+
 // group tables for the GEMMs: one group of `rows` rows, or `heads` groups (attention)
 static int plan(const TcPlan& pl, int n_groups, int rows, int row_stride, int row_base, int batch_base, cudaStream_t st,
                 int tile_rows = TC_BM) {
@@ -487,6 +570,38 @@ static int vit_fc1(const VitShape& s, const TcPlan& pl, const void* y, const voi
                                                  PROF_VIT_GEMM);
 }
 
+// h = silu(x1) * x2, [x1 x2] = y . w12^T + bias (rows interleaved, see EpiSwiGLU), y [rows][D] -> h [rows][Hd]
+static int vit_swiglu(const VitShape& s, const TcPlan& pl, const void* y, const void* w, const float* bias, int Hd, void* h,
+                      cudaStream_t st) {
+  const TcOperands op = linear_operands(y, s.rows, w);
+  const TcProblem pb = pl.problem(1, 2 * Hd, s.D);
+  const int tiles = cdiv((int)s.rows, TC_BM);
+  if (s.pairs) {
+    EpiSwiGLU<__half> eg{{}, reinterpret_cast<__half*>(h), bias, Hd};
+    eg.all_direct = 1;   // as fc1 on CTA pairs: each thread writes its row's 16 outputs per 32 columns as whole sectors
+    return tc_launch<TcMode::F16, EpiSwiGLU<__half>, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), eg, st, PROF_VIT_GEMM);
+  }
+  if (s.f16)
+    return tc_launch<TcMode::F16, EpiSwiGLU<__half>>(op, pb, tiles, EpiSwiGLU<__half>{{}, reinterpret_cast<__half*>(h), bias, Hd},
+                                                     st, PROF_VIT_GEMM);
+  return tc_launch<TcMode::TF32, EpiSwiGLU<float>>(op, pb, tiles, EpiSwiGLU<float>{{}, reinterpret_cast<float*>(h), bias, Hd},
+                                                   st, PROF_VIT_GEMM);
+}
+
+// facet f of the tap block: out_tpc [B][P][D] = (y . qkv_w[(f-1) D : f D]^T + qkv_b[(f-1) D : f D]) without the cls rows.
+// The weight slice starts (f-1) D^2 elements into qkv_w; the caller checks that it and the bias slice are 16-byte aligned
+// (the TMA base and the epilogue's float4 bias reads).
+static int vit_facet(const VitShape& s, const TcPlan& pl, const void* y, const void* w_slice, const float* bias_slice,
+                     float* out_tpc, cudaStream_t st) {
+  const EpiFacet ef{{}, out_tpc, bias_slice, s.N1, s.D};
+  const TcOperands op = linear_operands(y, s.rows, w_slice);
+  const TcProblem pb = pl.problem(1, s.D, s.D);
+  const int tiles = cdiv((int)s.rows, TC_BM);
+  return s.pairs ? tc_launch<TcMode::F16, EpiFacet, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), ef, st, PROF_VIT_GEMM)
+       : s.f16 ? tc_launch<TcMode::F16, EpiFacet>(op, pb, tiles, ef, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, EpiFacet>(op, pb, tiles, ef, st, PROF_VIT_GEMM);
+}
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -500,7 +615,8 @@ size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_ge
   const size_t N1p = align_up(N1, 4);
   b += align_up(B * N1 * D * 4, 256) * 2;                                  // x, y
   b += align_up(B * N1 * D * 4, 256) * 2 + align_up(B * N1p * D * 4, 256); // q, k, vT
-  size_t hid = B * N1 * 4 * D * 4, col = B * P * (size_t)vit_kp(c) * 4;
+  const size_t hid_w = c->swiglu_hidden > 0 ? (size_t)c->swiglu_hidden : 4 * D;   // MLP hidden width
+  size_t hid = B * N1 * hid_w * 4, col = B * P * (size_t)vit_kp(c) * 4;
   b += align_up(hid > col ? hid : col, 256);                               // MLP hidden / im2col (aliased)
   b += align_up((size_t)c->heads * VIT_ROW_CHUNK * N1p * 4, 256);          // attention scores of one row chunk
   b += 4 * align_up((size_t)(c->heads + 2) * 4, 256) + 4096;               // plan tables
@@ -527,11 +643,14 @@ int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom
                       const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
                       size_t workspace_bytes, void* stream) {
   DTK_CHECK_ARG(c && g && in && p0 && out0, "vit_stage: null pointer");
-  DTK_CHECK_ARG(stage >= DINOTRK_VIT_LAYERNORM && stage <= DINOTRK_VIT_FC2, "vit_stage: unknown stage %d", stage);
+  DTK_CHECK_ARG(stage >= DINOTRK_VIT_LAYERNORM && stage <= DINOTRK_VIT_SWIGLU, "vit_stage: unknown stage %d", stage);
   DTK_CHECK_ARG(c->gemm_f16 != 0 && c->attn_materialized == 0, "vit_stage: fp16 operand mode only");
   DTK_CHECK_ARG(B > 0 && c->dim == c->heads * HD && c->dim <= 2048, "vit_stage: dim must be heads x 64 (<= 2048)");
+  DTK_CHECK_ARG(c->swiglu_hidden >= 0 && c->swiglu_hidden % 8 == 0, "vit_stage: swiglu_hidden must be a multiple of 8");
+  DTK_CHECK_ARG(stage != DINOTRK_VIT_SWIGLU || c->swiglu_hidden > 0, "vit_stage: the SwiGLU stage needs swiglu_hidden > 0");
   DTK_CHECK_ARG(stage == DINOTRK_VIT_LAYERNORM || w, "vit_stage: null weight");
-  DTK_CHECK_ARG(stage == DINOTRK_VIT_QKV || stage == DINOTRK_VIT_FC1 || p1, "vit_stage: null second parameter vector");
+  DTK_CHECK_ARG(stage == DINOTRK_VIT_QKV || stage == DINOTRK_VIT_FC1 || stage == DINOTRK_VIT_SWIGLU || p1,
+                "vit_stage: null second parameter vector");
   DTK_CHECK_ARG(stage != DINOTRK_VIT_QKV || (out1 && out2), "vit_stage: qkv needs q, k and v^T");
   DTK_CHECK_ARG(workspace && workspace_bytes >= DINOTRK_VIT_STAGE_WORKSPACE_BYTES, "vit_stage: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
@@ -549,7 +668,9 @@ int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom
                            reinterpret_cast<__half*>(out2), st);
     case DINOTRK_VIT_PROJ: return vit_residual(s, pl, in, w, s.D, p0, p1, reinterpret_cast<float*>(out0), st);
     case DINOTRK_VIT_FC1: return vit_fc1(s, pl, in, w, p0, out0, st);
-    default: return vit_residual(s, pl, in, w, 4 * s.D, p0, p1, reinterpret_cast<float*>(out0), st);
+    case DINOTRK_VIT_SWIGLU: return vit_swiglu(s, pl, in, w, p0, c->swiglu_hidden, out0, st);
+    default:
+      return vit_residual(s, pl, in, w, c->swiglu_hidden ? c->swiglu_hidden : 4 * s.D, p0, p1, reinterpret_cast<float*>(out0), st);
   }
 }
 
@@ -561,8 +682,29 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   const int D = c->dim, heads = c->heads, P = g->h * g->w, N1 = P + 1, Kp = vit_kp(c);
   DTK_CHECK_ARG(D == heads * HD && D % 64 == 0 && D <= 2048, "vit_forward: dim must be heads x 64 (<= 2048)");
   DTK_CHECK_ARG(c->tap_layer >= 0 && c->tap_layer < c->depth, "vit_forward: tap layer out of range");
+  DTK_CHECK_ARG(c->swiglu_hidden >= 0 && c->swiglu_hidden % 8 == 0, "vit_forward: swiglu_hidden must be a multiple of 8");
+  DTK_CHECK_ARG(c->facet >= 0 && c->facet <= 3, "vit_forward: facet must be 0 (tokens), 1 (queries), 2 (keys) or 3 (values)");
+  const int Hd = c->swiglu_hidden, hid_k = Hd ? Hd : 4 * D;   // MLP hidden width: the K of fc2 / w3
   const int N1p = (int)align_up((size_t)N1, 4);   // row pitch of the score / v^T arrays (TMA strides are 16-byte multiples)
   DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_vit_workspace_bytes(c, g, B), "vit_forward: workspace too small");
+  // fp16 operand mode (default): LayerNorm / GELU / attention write fp16 activations, weights are fp16 (11-bit
+  // significand like TF32, twice the tensor rate, half the operand traffic).  The validation path
+  // (attn_materialized) keeps every operand fp32 / TF32.
+  const VitShape s = vit_shape(c, g, B);
+  const bool f16 = s.f16;
+  // facet > 0: the features are the tap block's qkv Linear output (what the reference's qkv hook records), rows
+  // [(f-1) D, f D) of qkv.w and qkv.b -- one N = D GEMM after that block's LayerNorm 1, written straight into out_tpc;
+  // the block's attention and MLP do not run.  The slices are the GEMM's TMA base and its float4 bias reads.
+  const void* facet_w = nullptr;
+  const float* facet_b = nullptr;
+  if (c->facet) {
+    const float* const* wtap = wt->blocks + (size_t)c->tap_layer * 14;
+    const size_t off = (size_t)(c->facet - 1) * D;
+    facet_w = reinterpret_cast<const char*>(wtap[2]) + off * D * (f16 ? sizeof(__half) : sizeof(float));
+    facet_b = wtap[3] + off;
+    DTK_CHECK_ARG(wtap[2] && wtap[3] && ((uintptr_t)facet_w & 15) == 0 && ((uintptr_t)facet_b & 15) == 0,
+                  "vit_forward: qkv weight / bias of the tap block not 16-byte aligned");
+  }
   cudaStream_t st = (cudaStream_t)stream;
   Arena ar(workspace, workspace_bytes);
   const size_t rows = (size_t)B * N1;
@@ -571,18 +713,12 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   float* q = ar.take<float>(rows * D);
   float* k = ar.take<float>(rows * D);
   float* vT = ar.take<float>((size_t)B * N1p * D);
-  size_t hid = rows * 4 * D, col = (size_t)B * P * Kp;
+  size_t hid = rows * hid_k, col = (size_t)B * P * Kp;
   float* hbuf = ar.take<float>(hid > col ? hid : col);
   float* S = ar.take<float>((size_t)heads * VIT_ROW_CHUNK * N1p);
   TcPlan pl{ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2)};
   DTK_CHECK_ARG(ar.ok(), "vit_forward: workspace arena overflow");
   int rc;
-
-  // fp16 operand mode (default): LayerNorm / GELU / attention write fp16 activations, weights are fp16 (11-bit
-  // significand like TF32, twice the tensor rate, half the operand traffic).  The validation path
-  // (attn_materialized) keeps every operand fp32 / TF32.
-  const VitShape s = vit_shape(c, g, B);
-  const bool f16 = s.f16;
   // y and hbuf hold fp16 activations in fp16 operand mode, fp32 ones otherwise
   __half* h16 = reinterpret_cast<__half*>(hbuf);
 
@@ -604,9 +740,10 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   for (int l = 0; l <= c->tap_layer; ++l) {
     const float* const* w = wt->blocks + (size_t)l * 14;
     // w: 0 norm1.w 1 norm1.b 2 qkv.w 3 qkv.b 4 proj.w 5 proj.b 6 ls1 7 norm2.w 8 norm2.b 9 fc1.w 10 fc1.b 11 fc2.w 12 fc2.b 13 ls2
-    // (the four weight matrices are fp16 arrays in fp16 operand mode)
+    // (the four weight matrices are fp16 arrays in fp16 operand mode; SwiGLU: 9-12 are w12.w, w12.b, w3.w, w3.b)
     if ((rc = vit_layernorm(s, x, w[0], w[1], y, st))) return rc;
     if ((rc = vit_row_plan(s, pl, st))) return rc;
+    if (facet_w && l == c->tap_layer) return vit_facet(s, pl, y, facet_w, facet_b, out_tpc, st);
     if (c->attn_materialized == 0) {
       // fused attention: fp16 q / k / v^T, scores stay in registers
       __half* q16 = reinterpret_cast<__half*>(q);
@@ -641,8 +778,12 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
     if ((rc = vit_row_plan(s, pl, st))) return rc;
     if ((rc = vit_residual(s, pl, y, w[4], D, w[5], w[6], x, st))) return rc;              // proj + LayerScale + residual
     if ((rc = vit_layernorm(s, x, w[7], w[8], y, st))) return rc;
-    if ((rc = vit_fc1(s, pl, y, w[9], w[10], hbuf, st))) return rc;
-    if ((rc = vit_residual(s, pl, hbuf, w[11], 4 * D, w[12], w[13], x, st))) return rc;   // fc2 + LayerScale + residual
+    if (Hd) {
+      if ((rc = vit_swiglu(s, pl, y, w[9], w[10], Hd, hbuf, st))) return rc;
+    } else {
+      if ((rc = vit_fc1(s, pl, y, w[9], w[10], hbuf, st))) return rc;
+    }
+    if ((rc = vit_residual(s, pl, hbuf, w[11], hid_k, w[12], w[13], x, st))) return rc;   // fc2 / w3 + LayerScale + residual
   }
   {
     ProfRange pr(PROF_VIT_MISC, st);

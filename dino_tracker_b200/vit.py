@@ -7,7 +7,9 @@ interpolation (``:41-85``), runs the video one frame at a time and keeps the out
 before the final norm, cls token dropped (``:137-150``, ``utils.py:54-67``).  Here the weights come from a
 DINOv2 state dict (hub key names, so real checkpoints load unchanged), the position embedding is
 interpolated once at load time with the reference's formula, and every frame batch is one
-``dinotrk_vit_forward`` call that writes token-major features ``[T][P][C]`` directly.
+``dinotrk_vit_forward`` call that writes token-major features ``[T][P][C]`` directly.  The query / key / value
+facets (the reference's qkv hook, ``models/extractor.py:224-266``) and ViT-g/14's SwiGLU feed-forward run on the same
+call.
 """
 import ctypes
 import math
@@ -26,6 +28,18 @@ CONFIGS = {  # name: (depth, dim, heads)
 _BLOCK_KEYS = ("norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.bias", "attn.proj.weight",
                "attn.proj.bias", "ls1.gamma", "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias",
                "mlp.fc2.weight", "mlp.fc2.bias", "ls2.gamma")
+# ViT-g/14's SwiGLU feed-forward (hub keys mlp.w12.* / mlp.w3.*) takes slots 9-12 of the weight table
+_SWIGLU_KEYS = _BLOCK_KEYS[:9] + ("mlp.w12.weight", "mlp.w12.bias", "mlp.w3.weight", "mlp.w3.bias", "ls2.gamma")
+FACETS = {"tokens": 0, "queries": 1, "keys": 2, "values": 3}   # dinotrk_vit_config.facet
+
+
+def interleave_w12(t):
+    """SwiGLU w12 rows (or its bias) from the hub layout [x1 (Hd rows); x2 (Hd rows)] to pairs of hidden units:
+    rows 4q .. 4q+3 = x1[2q], x1[2q+1], x2[2q], x2[2q+1].  The CUDA epilogue then finds both halves of an output
+    in the same four GEMM columns (dinotrk_vit_weights)."""
+    hd = t.shape[0] // 2
+    x1, x2 = t[:hd].reshape(hd // 2, 1, 2, *t.shape[1:]), t[hd:].reshape(hd // 2, 1, 2, *t.shape[1:])
+    return torch.cat((x1, x2), dim=1).reshape(t.shape).contiguous()
 
 
 def interpolate_pos_embed(pos_embed, n_h, n_w):
@@ -47,11 +61,17 @@ def interpolate_pos_embed(pos_embed, n_h, n_w):
 
 
 class DinoV2Features(torch.nn.Module):
-    """``VitExtractor`` replacement: ``forward(video01)`` -> token-major features [T][P][C] on the GPU."""
+    """``VitExtractor`` replacement: ``forward(video01)`` -> token-major features [T][P][C] on the GPU.
+
+    ``facet``: 'tokens' (block ``layer``'s output), or 'queries' / 'keys' / 'values' (that block's qkv Linear
+    output, the reference's qkv hook, ``models/extractor.py:124-128,224-266``).  A state dict whose blocks carry
+    ``mlp.w12.*`` / ``mlp.w3.*`` (ViT-g/14) runs the SwiGLU feed-forward; its hidden width is read from ``w3``."""
 
     def __init__(self, state_dict, heads, layer=None, stride=7, patch=14, device="cuda:0", frames_per_call=2,
-                 attention="fused", cta_pairs=True):
+                 attention="fused", cta_pairs=True, facet="tokens"):
         super().__init__()
+        if facet not in FACETS:
+            raise ValueError(f"facet {facet} not supported")
         self._dev = _lib.require_cuda(device)
         self._lib = _lib.load()
         sd = {k: v.detach().to(self._dev, torch.float32).contiguous() for k, v in state_dict.items()}
@@ -64,20 +84,41 @@ class DinoV2Features(torch.nn.Module):
         assert attention in ("fused", "materialized")
         self.attention = attention
         self.cta_pairs = cta_pairs
+        self.facet = facet
+        self.swiglu_hidden = self._swiglu_hidden(sd) if "blocks.0.mlp.w12.weight" in sd else 0
+        if self.swiglu_hidden:
+            for i in range(self.depth):
+                for k in ("mlp.w12.weight", "mlp.w12.bias"):
+                    sd[f"blocks.{i}.{k}"] = interleave_w12(sd[f"blocks.{i}.{k}"])
         self._sd = sd
         # fused mode: weight matrices in fp16 (fp16 MMAs); materialized (validation) mode: fp32 / TF32
         self._f16 = attention == "fused"
         wdt = torch.float16 if self._f16 else torch.float32
-        mats = ("attn.qkv.weight", "attn.proj.weight", "mlp.fc1.weight", "mlp.fc2.weight")
+        mats = ("attn.qkv.weight", "attn.proj.weight", "mlp.fc1.weight", "mlp.fc2.weight", "mlp.w12.weight", "mlp.w3.weight")
         pw = sd["patch_embed.proj.weight"].reshape(self.dim, -1)
         mult = 8 if self._f16 else 4
         if pw.shape[1] % mult:
             pw = F.pad(pw, (0, mult - pw.shape[1] % mult))
         self._patch_w = pw.to(wdt).contiguous()
+        keys = _SWIGLU_KEYS if self.swiglu_hidden else _BLOCK_KEYS
         self._blocks = [sd[f"blocks.{i}.{k}"].to(wdt).contiguous() if k in mats else sd[f"blocks.{i}.{k}"]
-                        for i in range(self.depth) for k in _BLOCK_KEYS]
+                        for i in range(self.depth) for k in keys]
         self._block_ptrs = (ctypes.c_void_p * len(self._blocks))(*[t.data_ptr() for t in self._blocks])
         self._pos_cache = {}
+
+    def _swiglu_hidden(self, sd):
+        """Hd from w3 [D][Hd] (the hub's SwiGLUFFNFused rounds 2/3 of 4 D up to a multiple of 8; not recomputed
+        here), and every block's w12 [2 Hd][D] / w3 shapes checked against it."""
+        D, hd = self.dim, sd["blocks.0.mlp.w3.weight"].shape[1]
+        if hd % 8:
+            raise ValueError(f"SwiGLU hidden width {hd} is not a multiple of 8")
+        for i in range(self.depth):
+            p = f"blocks.{i}.mlp."
+            shapes = {k: tuple(sd[p + k].shape) if p + k in sd else None for k in ("w12.weight", "w12.bias", "w3.weight", "w3.bias")}
+            want = {"w12.weight": (2 * hd, D), "w12.bias": (2 * hd,), "w3.weight": (D, hd), "w3.bias": (D,)}
+            if shapes != want:
+                raise ValueError(f"block {i}: SwiGLU weights {shapes}, expected {want}")
+        return hd
 
     @classmethod
     def from_name(cls, model_name, state_dict, **kw):
@@ -101,7 +142,8 @@ class DinoV2Features(torch.nn.Module):
         geom = _lib.make_geom(H, W, self.patch, self.stride, 35)
         P = geom.h * geom.w
         cfg = _lib.VitConfig(self.depth, self.dim, self.heads, self.layer, self.patch, self.stride,
-                             0 if self.attention == "fused" else 1, 1 if self._f16 else 0, 1 if self.cta_pairs else 0)
+                             0 if self.attention == "fused" else 1, 1 if self._f16 else 0, 1 if self.cta_pairs else 0,
+                             self.swiglu_hidden, FACETS[self.facet])
         cls_pos, pos = self._pos(geom.h, geom.w)
         wt = _lib.VitWeights()
         wt.patch_w, wt.patch_b = self._patch_w.data_ptr(), self._sd["patch_embed.proj.bias"].data_ptr()
@@ -129,9 +171,12 @@ class DinoV2Features(torch.nn.Module):
 @torch.no_grad()
 def get_dino_features_video(video, model_name="dinov2_vitb14", facet="tokens", stride=7, layer=None,
                             device="cuda:0", state_dict=None):
-    """``utils.py::get_dino_features_video`` (facet 'tokens'): T x C x h x w on the CPU like the reference
-    (``utils.py:53,67``).  ``state_dict``: DINOv2 weights (the reference downloads them with torch.hub)."""
-    assert facet == "tokens", "only the 'tokens' facet is on the shipped path (config/preprocessing.yaml:12)"
+    """``utils.py::get_dino_features_video``: T x C x h x w on the CPU like the reference (``utils.py:53,67``), for
+    ``facet`` in tokens / queries / keys / values (anything else raises ``ValueError`` as the reference does) and any
+    backbone of ``CONFIGS``.  ``layer=None``: the last block of ``state_dict``.  ``state_dict``: DINOv2 weights with hub
+    key names (the reference downloads them with torch.hub)."""
+    if facet not in FACETS:
+        raise ValueError(f"facet {facet} not supported")
     assert state_dict is not None, "pass the DINOv2 state dict (no network access here)"
-    ex = DinoV2Features.from_name(model_name, state_dict, layer=layer, stride=stride, device=device)
+    ex = DinoV2Features.from_name(model_name, state_dict, layer=layer, stride=stride, device=device, facet=facet)
     return ex.features_chw(video).cpu()

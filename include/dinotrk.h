@@ -347,18 +347,27 @@ typedef struct dinotrk_vit_config {
                               0 (or attn_materialized): fp32 arrays, TF32 MMAs */
   int gemm_pair;           /* with gemm_f16: 1 = linear layers on CTA pairs (two-CTA clusters, 256 x 256 tiles, each CTA
                               loads half of the weight tile and multicasts it to both), 0 = single-CTA 128 x 256 tiles */
+  int swiglu_hidden;       /* 0: GELU MLP (fc1 [4D][D], fc2 [D][4D]); Hd > 0 (a multiple of 8): SwiGLU MLP of hidden width Hd
+                              (ViT-g/14: 4096), h = silu(x1) * x2 with [x1 x2] = y . w12^T + b12, then w3 [D][Hd] */
+  int facet;               /* 0 tokens (block tap_layer's output); 1 queries, 2 keys, 3 values: rows [(f-1) D, f D) of
+                              block tap_layer's qkv Linear output (no 1/8 scale), that block's attention and MLP skipped */
 } dinotrk_vit_config;
 /* Device fp32 (weight matrices fp16 when gemm_f16).  patch_w: patch-embedding conv weight flattened K-major
  * [dim][Kp], Kp = 3*patch*patch zero-padded to a multiple of 4 (fp32) / 8 (fp16) elements; cls_pos [dim] =
  * cls_token + pos_embed[0]; pos [h*w][dim] = bicubic-interpolated patch position embedding (extractor.py:57-85);
  * blocks: HOST array of depth x 14 device pointers in the order norm1.w, norm1.b, qkv.w [3D][D], qkv.b, proj.w,
- * proj.b, ls1.gamma, norm2.w, norm2.b, fc1.w [4D][D], fc1.b, fc2.w [D][4D], fc2.b, ls2.gamma. */
+ * proj.b, ls1.gamma, norm2.w, norm2.b, fc1.w [4D][D], fc1.b, fc2.w [D][4D], fc2.b, ls2.gamma.  With swiglu_hidden = Hd
+ * slots 9-12 hold w12.w [2Hd][D], w12.b [2Hd], w3.w [D][Hd], w3.b [D], where the rows of w12 (and its bias) are
+ * interleaved in pairs of hidden units: rows 4q .. 4q+3 = x1 rows 2q, 2q+1, then x2 rows 2q, 2q+1 (hub layout: x1 rows
+ * 0..Hd-1, x2 rows Hd..2Hd-1).  Every pointer is 16-byte aligned. */
 typedef struct dinotrk_vit_weights {
   const void* patch_w; const float* patch_b; const float* cls_pos; const float* pos;
   const float* const* blocks;
 } dinotrk_vit_weights;
 size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_geom* g, int B);
-/* frames [B][3][H][W] RGB in [0,1] -> out_tpc [B][h*w][dim] (token-major features of block tap_layer). */
+/* frames [B][3][H][W] RGB in [0,1] -> out_tpc [B][h*w][dim] (token-major features of block tap_layer: its output, or
+ * its query / key / value facet), cls token dropped.  The workspace holds the MLP hidden activations at the config's
+ * width (4 dim, or swiglu_hidden). */
 int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const dinotrk_vit_config* c,
                         const dinotrk_vit_weights* wt, float* out_tpc, void* workspace,
                         size_t workspace_bytes, void* stream);
@@ -385,7 +394,11 @@ int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16
  *   PROJ       y [rows][D] fp16, proj_w [D][D], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (y . proj_w + bias)
  *   FC1        y [rows][D] fp16, fc1_w [4D][D], bias [4D], -  -> h [rows][4D] fp16 = gelu(y . fc1_w + bias) (exact GELU
  *              with erf to 1.5e-7)
- *   FC2        h [rows][4D] fp16, fc2_w [D][4D], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (h . fc2_w + bias)
+ *   FC2        h [rows][Kh] fp16, fc2_w [D][Kh], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (h . fc2_w + bias), with
+ *              Kh = 4D, or Kh = c->swiglu_hidden when that is non-zero (the SwiGLU MLP's w3)
+ *   SWIGLU     y [rows][D] fp16, w12_w [2Hd][D] (rows interleaved as in dinotrk_vit_weights), bias [2Hd] (interleaved
+ *              alike), -  -> h [rows][Hd] fp16 = silu(x1) * x2, Hd = c->swiglu_hidden (> 0); the 2Hd-wide product is
+ *              never stored
  * workspace: DINOTRK_VIT_STAGE_WORKSPACE_BYTES of device memory (tile plan).  Rows past `rows` are not touched. */
 #define DINOTRK_VIT_LAYERNORM 0
 #define DINOTRK_VIT_PATCH 1
@@ -393,6 +406,7 @@ int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16
 #define DINOTRK_VIT_PROJ 3
 #define DINOTRK_VIT_FC1 4
 #define DINOTRK_VIT_FC2 5
+#define DINOTRK_VIT_SWIGLU 6
 #define DINOTRK_VIT_STAGE_WORKSPACE_BYTES 4096
 int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom* g, int B, const void* in, const void* w,
                       const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
