@@ -90,10 +90,14 @@ template <class E> struct EpiPrefetch<E, std::enable_if_t<E::kPrefetch>> { stati
 
 // Fragment epilogues (`static constexpr bool kFragment = true`) skip the shared-memory round trip: right after the tile's
 // last wgmma has completed, every consumer thread calls
-//   fragment(g, r, m, n0, fc, acc)
+//   fragment(g, r, m, n0, fc, acc, cols)
 // with its own accumulator registers (float, or int in S8 mode): acc[4 i + {0, 1}] are row r, acc[4 i + {2, 3}] row r + 8 (rows inside group g, which
 // has m rows: rows >= m are padding), columns n0 + 8 i + fc + {0, 1}.  The 4 lanes of a quad (lane & 3) hold the same
-// two rows.  No barrier, no shared memory.
+// two rows.  cols[c] (shared memory, c < BN = 256) holds
+//   float2 column(g, n0, t)
+// of the same tile: consumer thread t of each warpgroup calls it when the tile starts, for columns n0 + t (.x) and
+// n0 + t + 128 (.y), so that the global reads are in flight during the tile's K loop and the epilogue reads its per-column
+// values from shared memory with constant offsets.
 template <class E, class = void> struct EpiFragment { static constexpr bool value = false; };
 template <class E> struct EpiFragment<E, std::enable_if_t<E::kFragment>> { static constexpr bool value = true; };
 
@@ -192,9 +196,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
     };
     int stage = 0, phase = 0;
     typename Cfg::Acc acc[BN / 2];
+    // fragment epilogues: the warpgroup's per-column values of the tile in one of two buffers, used by alternate tiles (a
+    // thread rewrites a buffer only after the next tile's barrier, which every thread passes after its epilogue's reads)
+    int cbuf = 0;
+    static_assert(!EpiFragment<Epi>::value || (BN == 256 && 4 * BN * 4 <= Cfg::kEpiBytes), "fragment epilogue: column buffers");
     for (int tile = unit; tile < total_tiles; tile += n_units) {
       int g, m0, n0;
       decode(tile, g, m0, n0);
+      float2 col_v;
+      if constexpr (EpiFragment<Epi>::value) col_v = epi.column(g, n0, t);
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
       int prev = -1;
@@ -232,7 +242,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
 
       const int rbase = m0 + cw * 64;        // row (inside the group) of the warpgroup's first row
       if constexpr (EpiFragment<Epi>::value) {
-        epi.fragment(g, rbase + fr, pb.grp_m[g], n0, fc, acc);
+        float* cols = epi_scratch + (2 * cw + cbuf) * BN;
+        cbuf ^= 1;
+        cols[t] = col_v.x;
+        cols[t + 128] = col_v.y;
+        tc::named_sync(1 + cw, 128);
+        epi.fragment(g, rbase + fr, pb.grp_m[g], n0, fc, acc, cols);
       } else if constexpr (!Cfg::kS8) {
         // ---- epilogue: 32-column blocks through shared memory ----
         const int r = rbase + t;

@@ -15,9 +15,9 @@ namespace dtk {
 // error is part of XW_EPS).  The int8 pass forms the same statistics of acc * fac_x * fac_d from its exact int32
 // accumulators (converted exactly: C <= XW_S8_MAX_C).
 //
-// A fragment epilogue (tcgemm.cuh): it works on the accumulator registers of all eight consumer warps, with no shared
-// memory and no barrier.  Per element only u = acc * (1 / |F|) is formed; the row's positive factor 1 / |d| (and the ReLU)
-// are applied to the two statistics at the end -- multiplication by a positive constant does not change which token holds
+// A fragment epilogue (tcgemm.cuh): it works on the accumulator registers of all eight consumer warps; the tile's token
+// factors come from shared memory, where the GEMM body staged them (column()).  Per element only u = acc * (1 / |F|) is
+// formed; the row's positive factor 1 / |d| (and the ReLU) are applied to the two statistics at the end -- multiplication by a positive constant does not change which token holds
 // the maximum.  The statistics -- the maximum, the first token holding it, the second largest value of the multiset -- do
 // not depend on the order the values are folded in: a thread folds its 32 values per (row, key tile) in increasing column
 // order, then the 4 lanes of the quad merge theirs by shuffles.
@@ -49,25 +49,33 @@ struct CoarseEpi {
     s.tok = take ? tok : s.tok;
     s.m1 = fmaxf(s.m1, m1);
   }
-  // folds key tile kh of the thread's two rows into s[0], s[1].  EDGE: the GEMM tile reaches past the end of the map
+  // the token factors of columns n0 + t and n0 + t + 128 (0 past the end of the map)
+  __device__ __forceinline__ float2 column(int g, int n0, int t) const {
+    const float* rn = rnorms + (size_t)grp_frame[g] * P;
+    const int c0 = n0 + t, c1 = c0 + XW_TILE;
+    return make_float2(c0 < P ? __ldg(rn + c0) : 0.f, c1 < P ? __ldg(rn + c1) : 0.f);
+  }
+  // folds key tile kh of the thread's two rows into s[0], s[1]; cols: the tile's token factors.  EDGE: the GEMM tile
+  // reaches past the end of the map
   template <bool EDGE>
-  __device__ __forceinline__ void fold(Top2 (&s)[2], int kh, const float* rn, int n0, int fc,
+  __device__ __forceinline__ void fold(Top2 (&s)[2], int kh, const float* cols, int n0, int fc,
                                        const Acc (&acc)[XW_GEMM_BN / 2]) const {
 #pragma unroll
     for (int ii = 0; ii < XW_TILE / 8; ++ii) {   // (constant trip count: acc must stay in registers)
       const int i = kh * XW_TILE / 8 + ii;
+      const float2 rnv = tc::lds_f2(tc::smem_u32(cols + fc + 8 * i));
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         const int col = n0 + 8 * i + fc + j;
         const bool ok = !EDGE || col < P;                // columns past the end of the map never win
-        const float rnv = __ldg(rn + (ok ? col : 0));
-        push(s[0], ok ? (float)acc[4 * i + j] * rnv : -INFINITY, col);
-        push(s[1], ok ? (float)acc[4 * i + 2 + j] * rnv : -INFINITY, col);
+        const float f = j ? rnv.y : rnv.x;
+        push(s[0], ok ? (float)acc[4 * i + j] * f : -INFINITY, col);
+        push(s[1], ok ? (float)acc[4 * i + 2 + j] * f : -INFINITY, col);
       }
     }
   }
-  __device__ __forceinline__ void fragment(int g, int r, int m, int n0, int fc, const Acc (&acc)[XW_GEMM_BN / 2]) const {
-    const float* rn = rnorms + (size_t)grp_frame[g] * P;
+  __device__ __forceinline__ void fragment(int g, int r, int m, int n0, int fc, const Acc (&acc)[XW_GEMM_BN / 2],
+                                           const float* cols) const {
     // after the quad's merge every lane holds all four results; lane q keeps and writes row r + 8 (q >> 1) of key tile
     // 2 (n0 / 256) + (q & 1)
     const int q = threadIdx.x & 3;
@@ -76,8 +84,8 @@ struct CoarseEpi {
 #pragma unroll
     for (int kh = 0; kh < 2; ++kh) {
       Top2 s[2] = {{-INFINITY, -INFINITY, 0x7fffffff}, {-INFINITY, -INFINITY, 0x7fffffff}};   // rows r, r + 8
-      if (edge) fold<true>(s, kh, rn, n0, fc, acc);
-      else fold<false>(s, kh, rn, n0, fc, acc);
+      if (edge) fold<true>(s, kh, cols, n0, fc, acc);
+      else fold<false>(s, kh, cols, n0, fc, acc);
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll

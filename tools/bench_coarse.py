@@ -1,12 +1,13 @@
 """The anchor phase's coarse pass (xw_coarse_gemm: CTA-pair fp16 wgmma GEMM + tile-key epilogue) on its own, at the
 shapes one steady-state chunk of BASELINE config 2 gives it.  GPU only.
 
-  python tools/bench_coarse.py [--launches 100] [--windows 5]
+  python tools/bench_coarse.py [--launches 100] [--windows 5] [--C 1024]
 
-Inputs: seeded feature video T = 50, P = 67 x 121 = 8107 tokens, C = 1024; one anchor-phase chunk of 32,750 descriptor
-rows.  With 256 queries that anchor in every frame, every anchor frame holds 256 x 50 = 12,800 work items; the chunk cap of
-32,768 maps cut at whole cells (multiples of T) is 32,750, and the probe chunk (4,050 items) takes the start of frame 0.
-So the first full chunk is frame 0's remaining 8,750 rows, all 12,800 of frame 1 and 11,200 of frame 2.
+Inputs: seeded feature video T = 50, P = 67 x 121 = 8107 tokens, C = 1024 (--C: another channel count, a multiple of
+16 up to 1040, so that the time per launch can be fitted against the reduction length: the intercept is the cost per tile
+that does not scale with K); one anchor-phase chunk of 32,750 descriptor rows.  With 256 queries that anchor in every
+frame, every anchor frame holds 256 x 50 = 12,800 work items; the chunk cap of 32,768 maps cut at whole cells (multiples
+of T) is 32,750, and the probe chunk (4,050 items) takes the start of frame 0.  So the first full chunk is frame 0's remaining 8,750 rows, all 12,800 of frame 1 and 11,200 of frame 2.
 
 Prints one JSON line:
   ms_per_launch     CUDA events around dinotrk_xw_coarse_keys, median over the windows, with min and max.  Besides the
@@ -22,8 +23,10 @@ Prints one JSON line:
   gpu               card name, power limit and the SM clock (NVML, sampled during the timed windows)
   keys_sha256       digest of the keys, to compare builds bit for bit
   int8              the same chunk on the int8 pass (dinotrk_xw_coarse_keys_i8 on dinotrk_quantise_s8 operands): ms, tops
-                    (2 * rows * P * C over its time), speedup over the fp16 pass, the largest per-map eps, and the SM
-                    clock sampled during its own timed windows
+                    (2 * rows * P * C over its time), speedup over the fp16 pass, the largest per-map eps, the SM
+                    clock sampled during its own timed windows, and clocks_per_mma_block: ms x SM clock x CTAs over the
+                    launch's 128 x 128 x 128 MMA blocks (128 descriptor rows of a CTA, 128 tokens, one 128-channel K
+                    block; padding rows, tokens and channels included), 512 clocks at the full int8 rate
 """
 import argparse
 import ctypes
@@ -40,7 +43,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
-T, GH, GW, C = 50, bench.GEO_H, bench.GEO_W, 1024
+T, GH, GW = 50, bench.GEO_H, bench.GEO_W
 P = GH * GW
 GROUPS = ((0, 8750), (1, 12800), (2, 11200))   # (anchor frame, descriptor rows)
 BM_PAIR, BN, BK = 256, 256, 64                  # CTA-pair tile of the coarse GEMM, fp16 K block (tcgemm.cuh)
@@ -80,8 +83,11 @@ def main():
     ap.add_argument("--launches", type=int, default=100, help="launches per timed window (>= 20)")
     ap.add_argument("--windows", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--C", type=int, default=1024, help="feature channels (a multiple of 16, <= 1040)")
     a = ap.parse_args()
     assert a.launches >= 20
+    assert a.C > 0 and a.C % 16 == 0 and a.C <= 1040, "--C: a multiple of 16 up to 1040 (the int8 pass's limits)"
+    C = a.C
     assert torch.cuda.is_available(), "bench_coarse.py needs a CUDA device"
     dev = "cuda:0"
     torch.cuda.set_device(0)
@@ -164,8 +170,10 @@ def main():
     mm_ms = time_windows(lambda: torch.matmul(w, x.t()), a.launches, a.windows)
 
     flop = 2.0 * rows * P * C
+    # int8: CTA row blocks of 128 x token blocks of 128 x K blocks of 128 channels
+    mma_blocks8 = 2 * sum(-(-n // BM_PAIR) for _, n in GROUPS) * -(-P // 128) * -(-C // 128)
     pair_tiles = sum(-(-n // BM_PAIR) for _, n in GROUPS) * -(-P // BN)
-    kblocks = 2 * pair_tiles * (C // BK)                       # CTA K blocks per launch
+    kblocks = 2 * pair_tiles * -(-C // BK)                     # CTA K blocks per launch
     l2_bytes = kblocks * 2 * 128 * BK * 2                      # A (128 rows) + B half (128 rows), fp16
     ctas = 2 * (torch.cuda.get_device_properties(0).multi_processor_count // 2)
     mhz = clocks["sm_mhz"]
@@ -187,7 +195,9 @@ def main():
         "gpu": dict(gpu, sm_mhz=mhz, clock_reasons=clocks["reasons"], clock_samples=clocks["samples"]),
         "keys_sha256": digest,
         "int8": {"ms_per_launch": s8_med, "ms_min": min(s8_ms), "ms_max": max(s8_ms), "tops": flop / (s8_med / 1e3) / 1e12,
-                 "speedup_vs_fp16": med / s8_med, "eps_max": eps.max().item(),
+                 "speedup_vs_fp16": med / s8_med, "eps_max": eps.max().item(), "mma_blocks": mma_blocks8,
+                 "clocks_per_mma_block": (s8_med / 1e3 * clocks8["sm_mhz"] * 1e6 * ctas / mma_blocks8)
+                 if clocks8["sm_mhz"] else None,
                  "gpu": {"sm_mhz": clocks8["sm_mhz"], "clock_reasons": clocks8["reasons"], "clock_samples": clocks8["samples"]}},
     }))
 
