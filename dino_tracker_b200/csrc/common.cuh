@@ -24,6 +24,16 @@ extern unsigned long long g_launches;
     }                                         \
   } while (0)
 
+// Supported token grids of the tracker's entry points (head, inference, training backward): h <= 256, w <= 256 and
+// h * w <= 32,768 (1274 x 1274 px at patch 14 / stride 7).  Shared-memory map buffers and per-map key arrays are sized
+// for it.
+constexpr int DTK_GRID_MAX_SIDE = 256, DTK_GRID_MAX_TOKENS = 32768;
+#define DTK_CHECK_GRID(g, what)                                                                                          \
+  DTK_CHECK_ARG((g).h > 0 && (g).w > 0 && (g).h <= dtk::DTK_GRID_MAX_SIDE && (g).w <= dtk::DTK_GRID_MAX_SIDE &&          \
+                    (g).h * (g).w <= dtk::DTK_GRID_MAX_TOKENS,                                                           \
+                "%s: token grid %d x %d outside the supported envelope (h, w <= %d, h * w <= %d tokens)", what, (g).h,  \
+                (g).w, dtk::DTK_GRID_MAX_SIDE, dtk::DTK_GRID_MAX_TOKENS)
+
 #define DTK_CUDA(call)                                                              \
   do {                                                                              \
     cudaError_t e__ = (call);                                                       \

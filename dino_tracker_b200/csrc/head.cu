@@ -17,6 +17,11 @@
 // cross-warp traffic), takes the side/corner halo from its lane neighbours by shuffle and
 // accumulates the second convolution into 16 registers.  The next map is prefetched with cp.async
 // while the current one is being refined.
+//
+// Grids wider or taller than 128 tokens take head_big_kernel for the full map instead (thread = 4x4 tile recomputing its
+// hidden halo, one map buffer); both fast-path kernels work on any grid of the envelope.
+#include <algorithm>
+
 #include "common.cuh"
 #include "corr.cuh"
 
@@ -661,6 +666,184 @@ head_tm_kernel(const float* __restrict__ maps, const unsigned long long* __restr
   }
 }
 
+// ------------------------------------------------------------------------------------------------------
+// Full map on grids beyond head_kernel's band layout (w > 128 or h > 128, up to the DTK_GRID_MAX_* envelope): one CTA per
+// map with the map once in shared memory (32,768 tokens = 128 KiB leave no room for a second buffer; several CTAs per SM
+// hide the load instead).  Thread = 4 x 4 output tile.  Per hidden channel it recomputes its 6 x 6 hidden window from the
+// 8 x 8 input window it keeps in registers, so no halo crosses threads and any grid shape works.  Every hidden value and
+// logit is formed by the same operation sequence as in head_kernel (b1 then the 9 taps in (ky, kx) order; b2 then the
+// channels).  The logits of the (2 box_r + 1)^2 box around the arg-max are kept for the disc soft-argmax.
+constexpr int HB_THREADS = 256;
+constexpr int HB_WARPS = HB_THREADS / 32;
+
+__global__ void __launch_bounds__(HB_THREADS, 2)
+head_big_kernel(const float* __restrict__ maps, int n_maps_arg, const int* __restrict__ map_list,
+                const int* __restrict__ list_count, HeadParams hp, dinotrk_head_weights wts, int box_r,
+                const int* __restrict__ out_index, float* __restrict__ out, int* __restrict__ aux) {
+  extern __shared__ __align__(16) float smem[];
+  const int n_maps = map_list ? *list_count : n_maps_arg;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int h = hp.h, w = hp.w, P = hp.P;
+  const int lin_elems = (hp.map_stride + 3) & ~3;
+  const int box_s = 2 * box_r + 1;
+  float* lin = smem;
+  float* sm_box = smem + lin_elems;                        // [box_s][box_s] logits around the arg-max
+  float* sm_red = sm_box + ((box_s * box_s + 3) & ~3);     // [6][HB_WARPS]
+  unsigned long long* sm_red64 = reinterpret_cast<unsigned long long*>(sm_red + 6 * HB_WARPS);  // [HB_WARPS]
+  const int nchunks = hp.map_stride / 4;
+  const int tiles_x = (w + 3) >> 2, n_tiles = tiles_x * ((h + 3) >> 2);
+
+  for (int mk = blockIdx.x; mk < n_maps; mk += gridDim.x) {
+    const int map = map_list ? map_list[mk] : mk;
+    {
+      const float4* src = reinterpret_cast<const float4*>(maps + (size_t)map * hp.map_stride);
+      for (int i = tid; i < nchunks; i += HB_THREADS) cp_async16_head(lin + 4 * i, src + i);
+      asm volatile("cp.async.commit_group;\n" ::);
+      asm volatile("cp.async.wait_group 0;\n" ::);
+    }
+    __syncthreads();
+
+    // ---- arg-max of the (already ReLU'd) map: first maximal index ----
+    unsigned long long key = 0ull;
+    for (int i = tid; i < P; i += HB_THREADS) {
+      float v = lin[i] + 0.f;
+      unsigned long long k = ((unsigned long long)__float_as_uint(v) << 32) | (unsigned)(0x7fffffff - i);
+      key = k > key ? k : key;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o); key = t > key ? t : key; }
+    if (lane == 0) sm_red64[warp] = key;
+    __syncthreads();
+    unsigned long long kbest = sm_red64[0];
+#pragma unroll
+    for (int k = 1; k < HB_WARPS; ++k) { unsigned long long t = sm_red64[k]; kbest = t > kbest ? t : kbest; }
+    const int amax = 0x7fffffff - (int)(kbest & 0xffffffffu);
+    const int arow = amax / w, acol = amax - arow * w;
+
+    // ---- refiner, tile by tile; online (max, sum) of the softmax over the whole map ----
+    MS ms{-INFINITY, 0.f};
+    for (int t = tid; t < n_tiles; t += HB_THREADS) {
+      const int r0 = (t / tiles_x) * 4, c0 = (t - (t / tiles_x) * tiles_x) * 4;
+      float m[8][8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = r0 - 2 + i;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = c0 - 2 + j;
+          m[i][j] = (r >= 0 && r < h && c >= 0 && c < w) ? lin[r * w + c] : 0.f;
+        }
+      }
+      bool hin[6][6];   // hidden position inside the map (outside: 0, the zero padding of the second convolution)
+#pragma unroll
+      for (int i = 0; i < 6; ++i)
+#pragma unroll
+        for (int j = 0; j < 6; ++j) hin[i][j] = r0 - 1 + i >= 0 && r0 - 1 + i < h && c0 - 1 + j >= 0 && c0 - 1 + j < w;
+      float acc[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = wts.b2;
+#pragma unroll 1
+      for (int o = 0; o < 16; ++o) {
+        float hid[6][6];
+#pragma unroll
+        for (int i = 0; i < 6; ++i)
+#pragma unroll
+          for (int j = 0; j < 6; ++j) {
+            float a = wts.b1[o];
+#pragma unroll
+            for (int ki = 0; ki < 3; ++ki)
+#pragma unroll
+              for (int kj = 0; kj < 3; ++kj) a = fmaf(wts.w1[o][ki * 3 + kj], m[i + ki][j + kj], a);
+            hid[i][j] = hin[i][j] ? fmaxf(a, 0.f) : 0.f;
+          }
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            float a = acc[i][j];
+#pragma unroll
+            for (int ki = 0; ki < 3; ++ki)
+#pragma unroll
+              for (int kj = 0; kj < 3; ++kj) a = fmaf(wts.w2[o][ki * 3 + kj], hid[i + ki][j + kj], a);
+            acc[i][j] = a;
+          }
+      }
+      MS tm{-INFINITY, 0.f};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (r0 + i < h && c0 + j < w) tm.m = fmaxf(tm.m, acc[i][j]);
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int r = r0 + i, c = c0 + j;
+          if (r < h && c < w) {
+            tm.s += __expf(acc[i][j] - tm.m);
+            if (abs(r - arow) <= box_r && abs(c - acol) <= box_r) sm_box[(r - arow + box_r) * box_s + c - acol + box_r] = acc[i][j];
+          }
+        }
+      ms = ms_merge(ms, tm);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      MS t{__shfl_xor_sync(0xffffffffu, ms.m, o), __shfl_xor_sync(0xffffffffu, ms.s, o)};
+      ms = ms_merge(ms, t);
+    }
+    if (lane == 0) { sm_red[warp] = ms.m; sm_red[HB_WARPS + warp] = ms.s; }
+    __syncthreads();   // also publishes sm_box
+
+    // ---- disc-masked soft-argmax (warp 0) with the stability branch, as head_kernel ----
+    if (warp == 0) {
+      float zmax = -INFINITY;
+#pragma unroll
+      for (int k = 0; k < HB_WARPS; ++k) zmax = fmaxf(zmax, sm_red[k]);
+      float s = 0.f, sx = 0.f, sy = 0.f, gx = 0.f, gy = 0.f, cnt = 0.f;
+      for (int q = lane; q < box_s * box_s; q += 32) {
+        const int r = arow - box_r + q / box_s, c = acol - box_r + q % box_s;
+        const int dr = (r - arow) * hp.stride_px, dc = (c - acol) * hp.stride_px;
+        if (r >= 0 && r < h && c >= 0 && c < w && dr * dr + dc * dc <= hp.radius2) {
+          const float e = expf(sm_box[q] - zmax);
+          const float x = (float)(hp.half_patch + c * hp.stride_px), y = (float)(hp.half_patch + r * hp.stride_px);
+          s += e; sx = fmaf(x, e, sx); sy = fmaf(y, e, sy);
+          gx += x; gy += y; cnt += 1.f;
+        }
+      }
+      float vals[6] = {s, sx, sy, gx, gy, cnt};
+#pragma unroll
+      for (int q = 0; q < 6; ++q) vals[q] = warp_sum(vals[q]);
+      if (lane == 0) {
+        float ssum = 0.f;
+#pragma unroll
+        for (int k = 0; k < HB_WARPS; ++k) {
+          const float mk_ = sm_red[k];
+          if (mk_ != -INFINITY) ssum += sm_red[HB_WARPS + k] * expf(mk_ - zmax);
+        }
+        float sp = __fdiv_rn(vals[0], ssum), spx = __fdiv_rn(vals[1], ssum), spy = __fdiv_rn(vals[2], ssum);
+        const bool fallback = sp < 1e-8f;
+        if (fallback) {  // heatmap <- (heatmap + 1/|mask|) * mask  (tracker_head.py:87-94)
+          float u = __fdiv_rn(1.f, vals[5]);
+          sp = fmaf(vals[5], u, sp); spx = fmaf(vals[3], u, spx); spy = fmaf(vals[4], u, spy);
+        }
+        float px = __fdiv_rn(spx, sp), py = __fdiv_rn(spy, sp);
+        float nx = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(px, hp.normW)), -1.f);
+        float ny = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(py, hp.normH)), -1.f);
+        if (hp.out_mode == 0) {
+          nx = __fmul_rn(__fdiv_rn(__fadd_rn(nx, 1.f), 2.f), hp.normW);
+          ny = __fmul_rn(__fdiv_rn(__fadd_rn(ny, 1.f), 2.f), hp.normH);
+        }
+        size_t oi = (size_t)(out_index ? out_index[map] : map) * hp.out_stride;
+        out[oi] = nx; out[oi + 1] = ny;
+        if (aux) { aux[2 * map] = amax; aux[2 * map + 1] = fallback ? 1 : 0; }
+      }
+    }
+    __syncthreads();  // lin / sm_box / sm_red are reused by the next map
+  }
+}
+
 __global__ void zero_int_kernel(int* p) { *p = 0; }
 
 int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geom& g,
@@ -668,8 +851,7 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
                 int* aux, int* scratch, cudaStream_t st, const unsigned long long* tkeys, bool counter_zeroed,
                 int ctas_per_sm, int parts) {
   if (n_maps <= 0) return DINOTRK_OK;
-  DTK_CHECK_ARG(g.w <= HEAD_MAX_W && g.h <= HEAD_MAX_H, "head: token grid %dx%d exceeds the supported %dx%d",
-                g.h, g.w, HEAD_MAX_H, HEAD_MAX_W);
+  DTK_CHECK_GRID(g, "head");
   HeadParams hp;
   hp.h = g.h; hp.w = g.w; hp.P = g.h * g.w; hp.map_stride = map_stride;
   hp.stride_px = g.stride; hp.half_patch = g.patch / 2; hp.radius2 = g.radius * g.radius;
@@ -683,7 +865,7 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
   const int sms = num_sms();
   const int lin_elems = (map_stride + 3) & ~3;
   // the window fast path needs the disc inside the 11 x 11 box and a scratch list for the uncertified maps
-  const bool window_ok = scratch != nullptr && g.radius <= 5 * g.stride && g.w <= HEAD_MAX_W;
+  const bool window_ok = scratch != nullptr && g.radius <= 5 * g.stride;
   int* slow_count = scratch;
   int* slow_list = scratch ? scratch + 1 : nullptr;
   if (window_ok && (parts & 1)) {
@@ -724,6 +906,29 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
   }
   if (!(parts & 2)) return DINOTRK_OK;
   // full-map kernel: every map (no scratch) or only the maps the window kernel could not certify
+  if (g.w > HEAD_MAX_W || g.h > HEAD_MAX_H) {
+    const int box_r = std::min(g.radius / g.stride, std::max(g.h, g.w));   // the disc lies in the box around the arg-max
+    const int box_s = 2 * box_r + 1;
+    const size_t smem = (size_t)(lin_elems + ((box_s * box_s + 3) & ~3) + 6 * HB_WARPS) * sizeof(float) +
+                        HB_WARPS * sizeof(unsigned long long);
+    DTK_CHECK_ARG(smem <= 227 * 1024, "head: disc radius %d px at stride %d does not fit the full-map kernel", g.radius, g.stride);
+    static PerDev<size_t> attr_big_dev;
+    static PerDev<int> per_sm_big_dev;   // occupancy at the smem of attr_big_dev
+    size_t& attr_big = attr_big_dev.get();
+    int& per_sm_big = per_sm_big_dev.get();
+    if (smem != attr_big) {
+      DTK_CUDA(cudaFuncSetAttribute(head_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      DTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_big, head_big_kernel, HB_THREADS, smem));
+      if (per_sm_big < 1) per_sm_big = 1;
+      attr_big = smem;
+    }
+    const int grid = n_maps < sms * per_sm_big ? n_maps : sms * per_sm_big;
+    ProfRange pr(PROF_HEAD_FULL, st);
+    head_big_kernel<<<grid, HB_THREADS, smem, st>>>(maps, n_maps, window_ok ? slow_list : nullptr, window_ok ? slow_count : nullptr,
+                                                   hp, hw, box_r, out_index, out, aux);
+    DTK_LAUNCHED();
+    return DINOTRK_OK;
+  }
   const int nwarps = cdiv(g.h, 4);
   const int threads = nwarps * 32;
   size_t smem = (size_t)(2 * lin_elems + 2 * nwarps * 2 * 128 + 6 * 32) * sizeof(float) + 32 * sizeof(unsigned long long);

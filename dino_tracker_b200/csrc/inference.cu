@@ -761,6 +761,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   const float* tpc = feat->tpc;
   const int T = feat->T, C = feat->C;
   DTK_CHECK_ARG(T > 0 && C > 0 && C % 4 == 0 && N >= 0, "infer: bad sizes");
+  DTK_CHECK_GRID(*g, "infer");
   DTK_CHECK_ARG((feat->hi == nullptr) == (feat->lo == nullptr), "infer: hi and lo must be given together");
   const FeatView fv = make_view(*feat, *g);
   DTK_CHECK_ARG(start_phase >= 0 && start_phase <= stop_after && stop_after <= 3,
@@ -928,7 +929,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     }
     std::vector<int> cnt(T);
     // pipeline of the anchor phase: coarse pass + exact window (xwin.cuh) on the tensor path, unless disabled
-    bool use_xw = tensor && g->radius <= 5 * g->stride && n_tiles_map <= 64;
+    bool use_xw = tensor && g->radius <= 5 * g->stride;
     int pathsel = g_xw_path;
     if (pathsel < 0) { const char* e = getenv("DTK_XW"); if (e) pathsel = atoi(e) != 0 ? 1 : 0; }
     if (pathsel == 0) use_xw = false;

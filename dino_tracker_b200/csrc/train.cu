@@ -4,10 +4,12 @@
 // dino_tracker.py:405-429) and to the refiner's (normalised) weights.  The forward of a training step is the inference
 // forward with the maps kept (dinotrk_sample_descriptors + dinotrk_corr_maps + dinotrk_head with aux); this file is the
 // reverse pass, three kernels:
-//   1. track_head_bwd_kernel  one block per map, the whole map in shared memory: refiner recomputed channel by channel,
+//   1. track_head_bwd_kernel  one block per map, the whole map in shared memory (in a workspace slice in global memory on
+//                             grids whose five map buffers do not fit, P > 11,560 tokens): refiner recomputed channel by channel,
 //                             softmax / disc soft-argmax (tracker_head.py:68-105, both branches), then d/dlogits,
 //                             conv2^T, ReLU', conv1^T -> d/dmap, and the weight gradients (block reductions + atomics).
-//   2. track_corr_bwd_kernel  one block per map: cosine-correlation backward (tracker.py:158-169) on the tokens that
+//   2. track_corr_bwd_kernel  one block per map (token list in shared memory, or in the workspace beyond 19,366 tokens):
+//                             cosine-correlation backward (tracker.py:158-169) on the tokens that
 //                             carry gradient -> d/ddescriptor and atomic adds into d/dE[target frame].
 //   3. track_sample_bwd_kernel one block per point: the trilinear sampling weights of the forward (utils.py:75-101,
 //                             including the fp32 temporal leak) scatter d/ddescriptor into d/dE.
@@ -72,19 +74,23 @@ __device__ __forceinline__ float conv3t(const float* __restrict__ src, int r, in
   return a;
 }
 
+// kGlobal: the five map buffers of block b are gbuf[b * 5 P ...] in global memory (grids whose 5 P floats exceed shared
+// memory); shared memory then holds the reduction slots only.  Same arithmetic either way.
+template <bool kGlobal>
 __global__ void __launch_bounds__(TB_THREADS, 1)
 track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ aux, const float* __restrict__ grad_out,
-                      TrainGeom tg, dinotrk_head_weights wts, float* __restrict__ dcorr, float* __restrict__ grad_w) {
+                      TrainGeom tg, dinotrk_head_weights wts, float* __restrict__ dcorr, float* __restrict__ grad_w,
+                      float* __restrict__ gbuf) {
   extern __shared__ __align__(16) float tb_smem[];
   const int P = tg.P, h = tg.h, w = tg.w;
-  float* m = tb_smem;            // relu(corr)
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  float* m = kGlobal ? gbuf + (size_t)b * 5 * P : tb_smem;   // relu(corr)
   float* z = m + P;              // logits, then d/dlogits
   float* ho = z + P;             // hidden channel o
   float* dho = ho + P;           // its gradient
   float* dm = dho + P;           // d/dmap
-  float* red = dm + P;           // [TB_WARPS * TB_NRED]
+  float* red = kGlobal ? tb_smem : dm + P;   // [TB_WARPS * TB_NRED]
   __shared__ float sc[8];        // px, py, s', count, dot
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const float* mp = maps + (size_t)b * tg.map_stride;
   const int amax = aux[2 * b], fb = aux[2 * b + 1];
   const int arow = amax / w, acol = amax - arow * w;
@@ -240,19 +246,22 @@ track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ au
 
 // corr = <s, F> / max(|s| |F|, 1e-8):  d/ds = g (F / D - corr s / |s|^2),  d/dF = g (s / D - corr F / |F|^2)  (the
 // second terms only where the clamp is inactive).  The map holds relu(corr); where it is 0 the incoming gradient is 0 too.
+// kGlobal: the token list of block b is gbuf[b * 3 P ...] in global memory (grids whose 3 P words exceed shared memory).
 constexpr int TC_THREADS_BWD = 256;
+template <bool kGlobal>
 __global__ void __launch_bounds__(TC_THREADS_BWD)
 track_corr_bwd_kernel(const float* __restrict__ tpc, const float* __restrict__ norms, int C, int P, int map_stride,
                       const float* __restrict__ maps, const float* __restrict__ dcorr, const float* __restrict__ desc,
                       const float* __restrict__ desc_norm, const int* __restrict__ tgt_frame, float* __restrict__ ddesc,
-                      float* __restrict__ grad_tpc) {
+                      float* __restrict__ grad_tpc, float* __restrict__ gbuf) {
   extern __shared__ __align__(16) float tcb_smem[];
-  int* l_tok = reinterpret_cast<int*>(tcb_smem);       // [P]
-  float* l_a = tcb_smem + P;                            // g / D
+  const int b = blockIdx.x, tid = threadIdx.x;
+  float* lbuf = kGlobal ? gbuf + (size_t)b * 3 * P : tcb_smem;
+  int* l_tok = reinterpret_cast<int*>(lbuf);           // [P]
+  float* l_a = lbuf + P;                                // g / D
   float* l_b = l_a + P;                                 // g corr / |F|^2 (0 under the clamp)
   __shared__ int n_list;
   __shared__ float red[TC_THREADS_BWD / 32];
-  const int b = blockIdx.x, tid = threadIdx.x;
   const int f = tgt_frame[b];
   const float sn = desc_norm[b];
   const float* fn = norms + (size_t)f * P;
@@ -326,9 +335,32 @@ using namespace dtk;
 
 extern "C" {
 
+// shared memory of the map buffers of the two per-map kernels; above the limit they live in the workspace instead
+static size_t head_bwd_smem(int P) { return ((size_t)5 * P + TB_WARPS * TB_NRED) * sizeof(float); }
+static size_t corr_bwd_smem(int P) { return (size_t)3 * P * sizeof(float); }
+// The shared-memory variant runs when its dynamic buffers plus the kernel's static shared memory fit the per-block opt-in
+// limit (227 KiB on sm_90: P <= 11,560 for the head kernel, P <= 19,366 for the correlation kernel).  A failed query
+// counts as "does not fit": the workspace variant runs on every grid.
+static bool bwd_smem_fits(const void* kernel, size_t dyn) {
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa{};
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+      cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return dyn + fa.sharedSizeBytes <= (size_t)optin;
+}
+static bool head_bwd_global(int P) { return !bwd_smem_fits((const void*)track_head_bwd_kernel<false>, head_bwd_smem(P)); }
+static bool corr_bwd_global(int P) { return !bwd_smem_fits((const void*)track_corr_bwd_kernel<false>, corr_bwd_smem(P)); }
+
 size_t dinotrk_track_backward_workspace_bytes(int B, int C, const dinotrk_geom* g) {
   if (!g || B <= 0) return 0;
-  return align_up((size_t)B * dinotrk_map_stride(g) * sizeof(float), 256) + align_up((size_t)B * C * sizeof(float), 256) + 1024;
+  const int P = g->h * g->w;
+  size_t b = align_up((size_t)B * dinotrk_map_stride(g) * sizeof(float), 256) + align_up((size_t)B * C * sizeof(float), 256) + 1024;
+  if (head_bwd_global(P)) b += align_up((size_t)B * 5 * P * sizeof(float), 256);
+  if (corr_bwd_global(P)) b += align_up((size_t)B * 3 * P * sizeof(float), 256);
+  return b;
 }
 
 int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, const dinotrk_head_weights* hw,
@@ -339,6 +371,7 @@ int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, 
                     aux && grad_out && grad_w && workspace,
                 "track_backward: null pointer");
   DTK_CHECK_ARG(B >= 0 && N > 0 && feat->C > 0, "track_backward: bad sizes");
+  DTK_CHECK_GRID(*g, "track_backward");
   DTK_CHECK_ARG(g->radius <= 5 * g->stride, "track_backward: disc radius %d exceeds 5 tokens", g->radius);
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_track_backward_workspace_bytes(B, feat->C, g), "track_backward: workspace too small");
   if (B == 0) return DINOTRK_OK;
@@ -351,24 +384,28 @@ int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, 
   tg.h = g->h; tg.w = g->w; tg.P = P; tg.stride = g->stride; tg.half_patch = g->patch / 2; tg.radius2 = g->radius * g->radius;
   tg.map_stride = dinotrk_map_stride(g);
   tg.normW = (float)(g->W - 1); tg.normH = (float)(g->H - 1);
-  const size_t smem1 = ((size_t)5 * P + TB_WARPS * TB_NRED) * sizeof(float);
-  const size_t smem2 = (size_t)3 * P * sizeof(float);
-  DTK_CHECK_ARG(smem1 <= 227 * 1024, "track_backward: token grid of %d tokens does not fit the shared-memory map buffers", P);
+  const bool g1 = head_bwd_global(P), g2 = corr_bwd_global(P);
+  float* gbuf1 = g1 ? ar.take<float>((size_t)B * 5 * P) : nullptr;
+  float* gbuf2 = g2 ? ar.take<float>((size_t)B * 3 * P) : nullptr;
+  DTK_CHECK_ARG(ar.ok(), "track_backward: workspace arena overflow");
+  const size_t smem1 = g1 ? TB_WARPS * TB_NRED * sizeof(float) : head_bwd_smem(P);
+  const size_t smem2 = g2 ? 0 : corr_bwd_smem(P);
   static PerDev<size_t> attr1_dev, attr2_dev;
-  if (attr1_dev.get() < smem1) {
-    DTK_CUDA(cudaFuncSetAttribute(track_head_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+  if (!g1 && attr1_dev.get() < smem1) {
+    DTK_CUDA(cudaFuncSetAttribute(track_head_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
     attr1_dev.get() = smem1;
   }
-  if (attr2_dev.get() < smem2) {
-    DTK_CUDA(cudaFuncSetAttribute(track_corr_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+  if (!g2 && attr2_dev.get() < smem2) {
+    DTK_CUDA(cudaFuncSetAttribute(track_corr_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
     attr2_dev.get() = smem2;
   }
   NvtxRange nv("dinotrk_track_backward");
   ProfRange pr(PROF_TRAIN_BWD, st);
-  track_head_bwd_kernel<<<B, TB_THREADS, smem1, st>>>(maps, aux, grad_out, tg, *hw, dcorr, grad_w);
+  (g1 ? track_head_bwd_kernel<true> : track_head_bwd_kernel<false>)<<<B, TB_THREADS, smem1, st>>>(maps, aux, grad_out, tg, *hw,
+                                                                                              dcorr, grad_w, gbuf1);
   DTK_LAUNCHED();
-  track_corr_bwd_kernel<<<B, TC_THREADS_BWD, smem2, st>>>(feat->tpc, feat->norms, C, P, tg.map_stride, maps, dcorr, desc, desc_norm,
-                                                        tgt_frame, ddesc, grad_tpc);
+  (g2 ? track_corr_bwd_kernel<true> : track_corr_bwd_kernel<false>)<<<B, TC_THREADS_BWD, smem2, st>>>(
+      feat->tpc, feat->norms, C, P, tg.map_stride, maps, dcorr, desc, desc_norm, tgt_frame, ddesc, grad_tpc, gbuf2);
   DTK_LAUNCHED();
   if (grad_tpc) {
     track_sample_bwd_kernel<<<B, SAMPLE_THREADS, 0, st>>>(C, P, g->h, g->w, make_point_affine(*g), points, frames_set, N, 0, ddesc, grad_tpc);

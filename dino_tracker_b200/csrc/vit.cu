@@ -763,8 +763,15 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
                                                       pl.problem(heads, N1, HD), heads * cdiv(rc_rows, TC_BM),
                                                       EpiStore{{}, S, N1p, VIT_ROW_CHUNK}, st, PROF_VIT_ATTN))) return rc;
           {
+            const size_t smem = (size_t)N1 * 4;   // one score row; above 48 KiB from 12,288 tokens (e.g. 714 x 1274 frames)
+            static PerDev<size_t> attr_dev;
+            if (smem > 48 * 1024 && smem > attr_dev.get()) {
+              DTK_CHECK_ARG(smem <= 227 * 1024, "vit: %d tokens exceed the materialized attention's score row", N1);
+              DTK_CUDA(cudaFuncSetAttribute(vit_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+              attr_dev.get() = smem;
+            }
             ProfRange pr(PROF_VIT_ATTN, st);  // rows of S live at (head * VIT_ROW_CHUNK + r)
-            vit_softmax_kernel<<<dim3(rc_rows, heads), 256, (size_t)N1 * 4, st>>>(S, N1, N1p, (size_t)VIT_ROW_CHUNK * N1p);
+            vit_softmax_kernel<<<dim3(rc_rows, heads), 256, smem, st>>>(S, N1, N1p, (size_t)VIT_ROW_CHUNK * N1p);
             DTK_LAUNCHED();
           }
           if ((rc = plan(pl, heads, rc_rows, VIT_ROW_CHUNK, 0, b * heads, st))) return rc;

@@ -150,7 +150,9 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
 //     pinfo[map] = coarse arg-max token, or -1 - token if the map is ambiguous.
 // (b) one warp per CELL: the lower medians of the unambiguous maps' coarse arg-max row / column give the box centre; a map
 //     fits if every candidate lies within +-XW_SLACK of it.
+//     KPL = cdiv(n_tiles, 32) keys per lane, tile t = lane + 32 q: candidates are ranked in tile order for any KPL.
 constexpr int PLAN_WARPS = 8;
+template <int KPL>
 __global__ void __launch_bounds__(PLAN_WARPS * 32)
 xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, int n_groups, int n_tiles,
                const unsigned long long* __restrict__ key1, const float* __restrict__ eps_map,
@@ -162,14 +164,16 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, 
   for (int map = gw; map < n_maps; map += nw) {
     const unsigned long long* k1 = key1 + (size_t)map * n_tiles;
     const float* k2 = max2 + (size_t)map * n_tiles;
-    unsigned long long kk[2] = {0ull, 0ull};
-    float v2[2] = {0.f, 0.f};
+    unsigned long long kk[KPL] = {};
+    float v2[KPL] = {};
 #pragma unroll
-    for (int q = 0; q < 2; ++q) {
+    for (int q = 0; q < KPL; ++q) {
       const int t = lane + 32 * q;
       if (t < n_tiles) { kk[q] = __ldg(k1 + t); v2[q] = __ldg(k2 + t); }
     }
-    unsigned long long gk = kk[0] > kk[1] ? kk[0] : kk[1];
+    unsigned long long gk = kk[0];
+#pragma unroll
+    for (int q = 1; q < KPL; ++q) gk = gk > kk[q] ? gk : kk[q];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { unsigned long long t = __shfl_xor_sync(0xffffffffu, gk, o); gk = t > gk ? t : gk; }
     const float gmax = __uint_as_float((unsigned)(gk >> 32));
@@ -179,7 +183,7 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, 
     bool amb = false;
     int ncand = 0;
 #pragma unroll
-    for (int q = 0; q < 2; ++q) {
+    for (int q = 0; q < KPL; ++q) {
       const int t = lane + 32 * q;
       const bool in = t < n_tiles;
       const bool isc = in && __uint_as_float((unsigned)(kk[q] >> 32)) >= th;
@@ -268,13 +272,15 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
                    cudaStream_t st, int n_maps, float min_norm, const float* eps) {
   static_assert(XW_MAX_CAND == 4, "candidates are read as one int4");
   const int n_tiles = cdiv(g.h * g.w, XW_TILE);
-  DTK_CHECK_ARG(n_tiles <= 64, "exact-window path: token grid too large (%d tiles)", n_tiles);
+  DTK_CHECK_GRID(g, "exact-window path");
+  static_assert(DTK_GRID_MAX_TOKENS <= 256 * XW_TILE, "xw_cand_kernel keeps at most 8 keys per lane");
   DTK_CHECK_ARG(cells.max_m <= XW_MAX_CELL, "exact-window path: cell of %d rows", cells.max_m);
   if (cells.n_cells <= 0 || n_maps <= 0) return DINOTRK_OK;
   ProfRange pr(PROF_XW_PLAN, st);
   int grid = cdiv(n_maps, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;
-  xw_cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, min_norm, n_groups, n_tiles, xc.key1, eps, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
+  auto cand_kernel = n_tiles <= 64 ? xw_cand_kernel<2> : n_tiles <= 128 ? xw_cand_kernel<4> : xw_cand_kernel<8>;
+  cand_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(n_maps, desc_norm, min_norm, n_groups, n_tiles, xc.key1, eps, xc.max2, xc.cand, xc.pinfo, xc.slow_cnt);
   DTK_LAUNCHED();
   grid = cdiv(cells.n_cells, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;

@@ -15,7 +15,10 @@ from . import _lib
 from .range_normalizer import RangeNormalizer
 from .tracker import Tracker
 
-DEFAULT_CHUNK_MAPS = 32768   # maps per correlation/head chunk (32 KB each at 854x476); clamped to the work of the call
+# maps per correlation/head chunk, clamped to the work of the call.  A map is 4 bytes per token (32 KB at 854x476, 73 KB at
+# 1274x714, 128 KB at 32,768 tokens) and two chunks are in flight, so the workspace grows with the grid: about 2 GiB at
+# 854x476, 4.8 GiB at 1274x714 and 8 GiB at 1274x1274 for the maps alone.
+DEFAULT_CHUNK_MAPS = 32768
 
 
 # ---- module-level helpers (models/model_inference.py:8-74) -------------------------------------

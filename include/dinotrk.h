@@ -133,7 +133,9 @@ int dinotrk_corr_maps(const dinotrk_features* feat, const dinotrk_geom* g,
 /* Head only: maps -> (x, y) (tracker_head.py:107-121).  aux (may be NULL) receives per map
  * {argmax index, fallback flag} as int32[2].  scratch: device int32[n_maps + 1] enabling the windowed
  * fast path (exact refiner on the 11x11 box around the arg-max + certified absence of the stability
- * branch; uncertified maps go to the full-map kernel); NULL: full-map kernel for every map. */
+ * branch; uncertified maps go to the full-map kernel); NULL: full-map kernel for every map.
+ * Token grids: h <= 256, w <= 256 and h * w <= 32,768 (e.g. 1274 x 714 or 1274 x 1274 px at patch 14 / stride 7);
+ * larger grids return DINOTRK_EINVAL.  Grids wider or taller than 128 tokens take a separate full-map kernel. */
 int dinotrk_head(const float* maps, int n_maps, const dinotrk_geom* g,
                  const dinotrk_head_weights* hw, const int* out_index, float* out,
                  int out_stride, int out_mode, int* aux, int* scratch, void* stream);
@@ -148,7 +150,10 @@ int dinotrk_head(const float* maps, int n_maps, const dinotrk_geom* g,
  *            source descriptors (tracker.py:96-111); NULL: embeddings without gradient (cached refined features).
  * points [B][3] = (x_px, y_px, set slot) and frames_set [N] as given to dinotrk_sample_descriptors; tgt_frame [B] =
  * the FRAME (index into feat) each map correlates against.  arg-max and disc mask carry no gradient (as in autograd).
- * Accumulates with atomics: the caller zeroes grad_w / grad_tpc.  Syncs: no. */
+ * Accumulates with atomics: the caller zeroes grad_w / grad_tpc.  Syncs: no.
+ * Token grids as dinotrk_head (h, w <= 256, h * w <= 32,768; else DINOTRK_EINVAL).  Beyond 11,560 tokens the per-map
+ * buffers of the reverse pass live in the workspace (5 P floats per map, 3 P more beyond 19,366 tokens), which
+ * dinotrk_track_backward_workspace_bytes includes. */
 size_t dinotrk_track_backward_workspace_bytes(int B, int C, const dinotrk_geom* g);
 int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, const dinotrk_head_weights* hw,
                            const float* points, const int* frames_set, int N, const float* desc,
@@ -168,7 +173,10 @@ int dinotrk_sample_backward(int T, int C, const dinotrk_geom* g, const float* po
  * together with stop_after < 3 / 2 / 1.  Phases 0 = trajectories (compute_trajectories),
  * 1 = cos-sims, 2 = anchors, 3 = occlusion; phases start_phase..stop_after run (0..3 = infer), and
  * the outputs of earlier phases are then inputs.  SYNCS the stream once when phase 2 runs (reads
- * the per-frame anchor counts back to size the anchor work lists). */
+ * the per-frame anchor counts back to size the anchor work lists).
+ * Token grids as dinotrk_head (h, w <= 256, h * w <= 32,768; else DINOTRK_EINVAL).  Both anchor pipelines run on every
+ * grid of that envelope; at 32,768 tokens one chunk of maps is 128 KiB per map, so a chunk of 32,768 maps takes 4 GiB
+ * of the workspace and two are in flight. */
 size_t dinotrk_infer_workspace_bytes(int T, int C, const dinotrk_geom* g, int N, int chunk_maps);
 /* Host-only helper (no GPU needed): the chunk plan dinotrk_infer uses.  kind 0 = trajectory phase (items = every
  * (frame, query row) pair), kind 1 = anchor phase (anchor_counts[a] * T items per anchor frame a).  Chunks hold
