@@ -24,7 +24,7 @@ class HeadWeights(Structure):
 
 class Features(Structure):
     _fields_ = [("tpc", c_void_p), ("norms", c_void_p), ("hi", c_void_p), ("lo", c_void_p), ("T", c_int), ("C", c_int),
-                ("q8", c_void_p), ("q_fac", c_void_p), ("q_rho", c_void_p)]
+                ("q8", c_void_p), ("q_fac", c_void_p), ("q_rho", c_void_p), ("hilo", c_void_p)]
 
 
 class VitConfig(Structure):
@@ -66,6 +66,7 @@ SIGNATURES = {
     "dinotrk_token_norms": (c_int, [_P, _P, c_int, c_int, c_int, _P]),
     "dinotrk_sample_descriptors": (c_int, [_P, c_int, c_int, POINTER(Geom), _P, c_int, _P, c_int, c_int, _P, _P, _P]),
     "dinotrk_split_fp16": (c_int, [_P, _P, _P, c_size_t, _P]),
+    "dinotrk_split_hilo": (c_int, [_P, _P, c_size_t, c_int, _P]),
     "dinotrk_quantise_s8": (c_int, [_P, _P, c_size_t, c_int, c_int, _P, _P, _P, _P, _P]),
     "dinotrk_split_range": (c_int, [_P, c_size_t, _P, c_size_t, _P, _P]),
     "dinotrk_split_faithful": (c_int, [c_float, c_float, c_int]),
@@ -244,8 +245,9 @@ def require_cuda(device):
     return dev
 
 
-def make_features(tpc, norms, hi=None, lo=None, quant=None):
-    """quant: (q8, fac, rho_f) of quantise_features, or None (the anchor phase's coarse pass then runs on fp16)."""
+def make_features(tpc, norms, hi=None, lo=None, quant=None, hilo=None):
+    """quant: (q8, fac, rho_f) of quantise_features, or None (the anchor phase's coarse pass then runs on fp16).
+    hilo: split_hilo of tpc, or None (the exact box GEMM then reads hi and lo as separate 64-byte rows)."""
     f = Features()
     f.tpc, f.norms = tpc.data_ptr(), norms.data_ptr()
     f.hi = hi.data_ptr() if hi is not None else None
@@ -253,7 +255,8 @@ def make_features(tpc, norms, hi=None, lo=None, quant=None):
     f.T, f.C = tpc.shape[0], tpc.shape[2]
     if quant is not None:
         f.q8, f.q_fac, f.q_rho = (t.data_ptr() for t in quant)
-    f._keep = (tpc, norms, hi, lo, quant)  # keep the tensors alive as long as the struct
+    f.hilo = hilo.data_ptr() if hilo is not None else None
+    f._keep = (tpc, norms, hi, lo, quant, hilo)  # keep the tensors alive as long as the struct
     return f
 
 
@@ -296,6 +299,15 @@ def split_fp16(x, stream):
     lo = torch.empty(x.shape, device=x.device, dtype=torch.float16)
     check(load().dinotrk_split_fp16(ptr(x), ptr(hi), ptr(lo), x.numel(), stream), "split_fp16")
     return hi, lo
+
+
+def split_hilo(x, stream):
+    """The fp16 split of a [..., C] fp32 tensor interleaved per 32 channels (include/dinotrk.h: dinotrk_split_hilo):
+    fp16 [..., 64 * ceil(C / 32)], hi and lo of channels 32 b .. 32 b + 31 at 64 b and 64 b + 32."""
+    C = x.shape[-1]
+    hilo = torch.empty(x.shape[:-1] + (64 * (-(-C // 32)),), device=x.device, dtype=torch.float16)
+    check(load().dinotrk_split_hilo(ptr(x), ptr(hilo), x.numel() // C, C, stream), "split_hilo")
+    return hilo
 
 
 def split_features(tpc, norms, stream):

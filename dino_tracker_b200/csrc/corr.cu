@@ -265,7 +265,7 @@ int launch_corr_maps(const FeatView& fv, const float* desc, int desc_rows, const
     if (fv.tensor()) {
       int rc = launch_corr_gemm_tc(fv.hi, fv.lo, norms, fv.T, C, P, desc, desc_rows, desc_norm, grp_frame, grp_row0,
                                    grp_m, grp_map0, tile_start, n_groups, max_tiles, maps, map_stride, split_ws, st, tkeys,
-                                   assist.split_ready, tile_rows);
+                                   assist.split_ready, tile_rows, true, nullptr, corr_hilo(fv) ? fv.hilo : nullptr);
       if (rc) return rc;
     } else {
       static PerDev<bool> attr_dev;

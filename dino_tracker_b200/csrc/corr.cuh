@@ -10,12 +10,18 @@ struct FeatView {
   const float* tpc; const float* norms; const void* hi; const void* lo;
   int T, C, P;
   const void* q8; const float* q_fac; const float* q_rho;   // int8 coarse operands (optional, dinotrk_features)
+  const void* hilo;   // [T][P][ceil(C / 32)][64] hi / lo interleaved per 32 channels (optional, with hi / lo)
   bool tensor() const { return hi != nullptr && lo != nullptr; }
   bool s8() const { return q8 != nullptr && q_fac != nullptr && q_rho != nullptr; }
 };
 static inline FeatView make_view(const dinotrk_features& f, const dinotrk_geom& g) {
-  return FeatView{f.tpc, f.norms, f.hi, f.lo, f.T, f.C, g.h * g.w, f.q8, f.q_fac, f.q_rho};
+  return FeatView{f.tpc, f.norms, f.hi, f.lo, f.T, f.C, g.h * g.w, f.q8, f.q_fac, f.q_rho, f.hi && f.lo ? f.hilo : nullptr};
 }
+// fp16 elements per row of the interleaved split: 64 per 32-channel block (the last one zero-padded)
+__host__ __device__ inline int hilo_row(int C) { return 64 * ((C + 31) / 32); }
+// The full-map GEMM runs on the interleaved split (TcMode::F16X3I) when the features carry it and C % 32 == 0 (the
+// descriptors' interleaved rows then fill exactly the workspace of their separate halves).
+static inline bool corr_hilo(const FeatView& fv) { return fv.hilo != nullptr && fv.C % 32 == 0; }
 
 constexpr int CORR_TILE = 256;   // token tile of the tensor-core correlation GEMM (= TC_BN); unit of the tile maxima
 
@@ -25,7 +31,9 @@ constexpr int CORR_TILE = 256;   // token tile of the tensor-core correlation GE
 //               first arg-max.  Maps of thin groups (streaming kernel) get ~0 in tile 0 = "no keys".  Only produced on
 //               the tensor path (fv.tensor()).
 //   zero_word   an int the plan kernel sets to 0 (the head's counter of uncertified maps: saves a launch)
-//   split_ready the fp16 hi/lo copies of `desc` are already in split_ws (written by the sampler): skip the split kernel
+//   split_ready the fp16 hi/lo copies of `desc` are already in split_ws (written by the sampler): skip the split kernel.
+//               With corr_hilo(fv) they must be interleaved ([rows][2 C], dinotrk_split_hilo's layout), else hi rows then
+//               lo rows at the next 256-byte boundary
 //   no_thin     the caller knows that no group has <= STREAM_MAX_M descriptors: skip the streaming kernel launch
 struct CorrAssist {
   unsigned long long* tkeys = nullptr;
@@ -51,8 +59,11 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
                         int max_tiles, float* maps, int map_stride, float* desc_split_ws, cudaStream_t st,
                         unsigned long long* tkeys = nullptr, bool split_ready = false, int tile_rows = 0 /* 0: default */,
                         bool relu = true /* false: signed cosines (no tile keys) */,
-                        const float* clamp = nullptr /* [desc_rows]: per-row replacement of the norm product's 1e-8 (signed only) */);
+                        const float* clamp = nullptr /* [desc_rows]: per-row replacement of the norm product's 1e-8 (signed only) */,
+                        const void* tpc_hilo = nullptr /* interleaved features (corr_hilo): the F16X3I GEMM; a ready split in
+                                                          desc_split_ws is then interleaved too */);
 int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t st);
+int launch_split_hilo(const float* x, void* hilo, size_t rows, int C, cudaStream_t st);
 
 // Faithful range of the fp16 hi/lo split (DESIGN.md 3.1).  Per element, x - hi - lo is at most 2^-22 |x| while lo is an fp16
 // normal and at most 2^-25 (half the smallest subnormal step) otherwise, so the split contraction's cosine error is

@@ -101,18 +101,45 @@ int make_tmap_4d(CUtensorMap* map, const void* base, const uint64_t dims[4], con
 }
 
 // x = hi + lo (+ residual <= 2^-22 |x| in the fp16 normal range): hi = rn_fp16(x), lo = rn_fp16(x - hi)
+__device__ __forceinline__ void split4(const float4& v, uint2& hi, uint2& lo) {
+  __half h0 = __float2half_rn(v.x), h1 = __float2half_rn(v.y), h2 = __float2half_rn(v.z), h3 = __float2half_rn(v.w);
+  __half l0 = __float2half_rn(v.x - __half2float(h0)), l1 = __float2half_rn(v.y - __half2float(h1));
+  __half l2 = __float2half_rn(v.z - __half2float(h2)), l3 = __float2half_rn(v.w - __half2float(h3));
+  __half2 a = __halves2half2(h0, h1), b2 = __halves2half2(h2, h3), c = __halves2half2(l0, l1), d = __halves2half2(l2, l3);
+  hi = make_uint2(*reinterpret_cast<unsigned*>(&a), *reinterpret_cast<unsigned*>(&b2));
+  lo = make_uint2(*reinterpret_cast<unsigned*>(&c), *reinterpret_cast<unsigned*>(&d));
+}
+
 __global__ void split_f16_kernel(const float4* __restrict__ x, uint2* __restrict__ hi, uint2* __restrict__ lo, size_t n4) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (; i < n4; i += stride) {
-    float4 v = __ldg(x + i);
-    __half h0 = __float2half_rn(v.x), h1 = __float2half_rn(v.y), h2 = __float2half_rn(v.z), h3 = __float2half_rn(v.w);
-    __half l0 = __float2half_rn(v.x - __half2float(h0)), l1 = __float2half_rn(v.y - __half2float(h1));
-    __half l2 = __float2half_rn(v.z - __half2float(h2)), l3 = __float2half_rn(v.w - __half2float(h3));
-    __half2 a = __halves2half2(h0, h1), b2 = __halves2half2(h2, h3), c = __halves2half2(l0, l1), d = __halves2half2(l2, l3);
-    hi[i] = make_uint2(*reinterpret_cast<unsigned*>(&a), *reinterpret_cast<unsigned*>(&b2));
-    lo[i] = make_uint2(*reinterpret_cast<unsigned*>(&c), *reinterpret_cast<unsigned*>(&d));
+  for (; i < n4; i += stride) split4(__ldg(x + i), hi[i], lo[i]);
+}
+
+// the split interleaved per 32 channels (dinotrk_split_hilo): thread = 4 channels of a row; in a 32-channel block, hi of
+// channels 4 q .. 4 q + 3 goes to the block's 8-byte word q and lo to word 8 + q
+__global__ void split_hilo_kernel(const float* __restrict__ x, uint2* __restrict__ hilo, size_t rows, int C) {
+  const int nb = (C + 31) / 32;
+  const size_t n = rows * nb * 8;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const size_t rb = i >> 3, row = rb / nb;
+    const int q = (int)(i & 7), c = 32 * (int)(rb - row * nb) + 4 * q;
+    const float4 v = c < C ? __ldg(reinterpret_cast<const float4*>(x + row * C + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    split4(v, hilo[16 * rb + q], hilo[16 * rb + 8 + q]);
   }
+}
+
+int launch_split_hilo(const float* x, void* hilo, size_t rows, int C, cudaStream_t st) {
+  DTK_CHECK_ARG(C > 0 && C % 4 == 0, "split_hilo: C must be a positive multiple of 4");
+  const size_t n = rows * ((C + 31) / 32) * 8;
+  if (n == 0) return DINOTRK_OK;
+  unsigned grid = (unsigned)((n + 255) / 256);
+  if (grid > (unsigned)num_sms() * 16) grid = num_sms() * 16;
+  ProfRange pr(PROF_MISC, st);
+  split_hilo_kernel<<<grid, 256, 0, st>>>(x, reinterpret_cast<uint2*>(hilo), rows, C);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
 }
 
 int launch_split_f16(const float* x, void* hi, void* lo, size_t n, cudaStream_t st) {
@@ -274,17 +301,28 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
                         const float* desc, int desc_rows, const float* desc_norm, const int* grp_frame,
                         const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                         int max_tiles, float* maps, int map_stride, float* desc_split_ws, cudaStream_t st,
-                        unsigned long long* tkeys, bool split_ready, int tile_rows, bool relu, const float* clamp) {
+                        unsigned long long* tkeys, bool split_ready, int tile_rows, bool relu, const float* clamp,
+                        const void* tpc_hilo) {
   static_assert(TC_BN == CORR_TILE, "the tile maxima are per GEMM N tile");
   DTK_CHECK_ARG(C % 8 == 0, "corr (tensor path): C must be a multiple of 8");
   DTK_CHECK_ARG(relu || tkeys == nullptr, "corr (tensor path): tile keys need the ReLU maps");
+  DTK_CHECK_ARG(!tpc_hilo || (relu && C % 32 == 0), "corr (tensor path): interleaved operands need C %% 32 == 0 and ReLU maps");
+  const bool pairs = (tile_rows > 0 ? tile_rows : corr_tc_tile_rows()) == TC2_BM;   // tile_start was planned with this M tile
+  const TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
+  if (tpc_hilo) {   // descriptors interleaved like the features: [desc_rows][2 C] at the start of the workspace
+    int rc = split_ready ? DINOTRK_OK : launch_split_hilo(desc, desc_split_ws, desc_rows, C, st);
+    if (rc) return rc;
+    const TcOperands op{desc_split_ws, nullptr, (uint64_t)desc_rows, 0, tpc_hilo, nullptr, (uint64_t)T, 0};
+    using Epi = CorrEpi<true>;
+    const Epi epi{norms, desc_norm, grp_frame, grp_row0, grp_map0, maps, map_stride, P, tkeys, cdiv(P, CORR_TILE)};
+    return pairs ? tc_launch<TcMode::F16X3I, Epi, TC_BN, true>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM)
+                 : tc_launch<TcMode::F16X3I, Epi>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM);
+  }
   char* d_hi = reinterpret_cast<char*>(desc_split_ws);
   char* d_lo = d_hi + align_up((size_t)desc_rows * C * 2, 256);
   int rc = split_ready ? DINOTRK_OK : launch_split_f16(desc, d_hi, d_lo, (size_t)desc_rows * C, st);
   if (rc) return rc;
-  const bool pairs = (tile_rows > 0 ? tile_rows : corr_tc_tile_rows()) == TC2_BM;   // tile_start was planned with this M tile
   const TcOperands op{d_hi, d_lo, (uint64_t)desc_rows, 0, tpc_hi, tpc_lo, (uint64_t)T, 0};
-  const TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
   auto run = [&](const auto& epi) {
     using Epi = std::decay_t<decltype(epi)>;
     return pairs ? tc_launch<TcMode::F16X3, Epi, TC_BN, true>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM)
@@ -303,6 +341,11 @@ using namespace dtk;
 extern "C" int dinotrk_split_fp16(const float* x, void* hi, void* lo, size_t n, void* stream) {
   DTK_CHECK_ARG(x && hi && lo, "split_fp16: null pointer");
   return launch_split_f16(x, hi, lo, n, (cudaStream_t)stream);
+}
+
+extern "C" int dinotrk_split_hilo(const float* x, void* hilo, size_t rows, int C, void* stream) {
+  DTK_CHECK_ARG(x && hilo, "split_hilo: null pointer");
+  return launch_split_hilo(x, hilo, rows, C, (cudaStream_t)stream);
 }
 
 extern "C" int dinotrk_split_range(const float* x, size_t n, const float* norms, size_t n_tok, float* range, void* stream) {

@@ -846,6 +846,8 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   DTK_CHECK_ARG(ar.ok(), "infer: workspace arena overflow");
   DTK_CHECK_ARG(xw_rows <= 0x7fffffffu, "infer: %zu descriptor rows exceed the row index", xw_rows);
   const bool tensor = fv.tensor();   // tensor-core GEMM: tile keys for the head, fp16 split fused into the samplers
+  FeatView fv_split = fv;            // the full-map pipeline's sampler writes the separate halves: F16X3 there
+  fv_split.hilo = nullptr;
 
   // The chunks of a phase are planned on the host in one go and their group arrays uploaded with ONE copy, so the
   // per-chunk launches below never block the host (a pageable cudaMemcpyAsync per chunk would).
@@ -876,7 +878,8 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     if (tensor) {   // the query descriptors are reused by every chunk: split them once (layout of desc_rows = N)
       for (int k = 0; k < 2; ++k) {
         char* a_hi = reinterpret_cast<char*>(cb[k].split);
-        int rc = launch_split_f16(descA, a_hi, a_hi + align_up((size_t)N * C * 2, 256), (size_t)N * C, st);
+        int rc = corr_hilo(fv) ? launch_split_hilo(descA, a_hi, N, C, st)
+                               : launch_split_f16(descA, a_hi, a_hi + align_up((size_t)N * C * 2, 256), (size_t)N * C, st);
         if (rc) return rc;
       }
     }
@@ -1085,7 +1088,8 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
           char* c_hi = reinterpret_cast<char*>(b.split);
           char* c_lo = c_hi + align_up((size_t)ch * C * 2, 256);          // layout of a descriptor array of `ch` rows
           int rc2 = launch_xw_compact(nullptr, u_hi, u_lo, x.arow, x.norm, x.out_index, C, gp.f, gp.map0, cm.n_groups,
-                                      n_slow, x.xc, nullptr, c_hi, c_lo, b.norm, out_index_ring[0], d_cgrp, sg_cap, st, q_rows, q_groups);
+                                      n_slow, x.xc, nullptr, c_hi, c_lo, b.norm, out_index_ring[0], d_cgrp, sg_cap, st, q_rows, q_groups,
+                                      corr_hilo(fv));
           if (rc2) return rc2;
           q_rows += n_slow; q_groups += cm.n_groups;
         }
@@ -1195,7 +1199,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       if (k >= k0 + 2 && (rc = head_full(k - 2))) return rc;   // last reader of maps / keys / list of this buffer set
       CorrAssist as;
       as.tkeys = tensor ? b.tkeys : nullptr; as.zero_word = b.hscratch; as.split_ready = tensor; as.no_thin = cm.no_thin;
-      rc = launch_corr_maps(fv, b.desc, cm.used, b.norm, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, ms,
+      rc = launch_corr_maps(fv_split, b.desc, cm.used, b.norm, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, ms,
                             b.plan, b.split, st, as);
       if (rc) return rc;
       if (ovl) DTK_CUDA(cudaEventRecord(ia->gemm[k & 1], st));

@@ -15,6 +15,10 @@
 // Modes:
 //   F16X3  : fp32-faithful split-precision: operands pre-split into fp16 hi + fp16 lo (x = hi + lo up to 2^-22),
 //            lo*hi + hi*lo + hi*hi on the f16 tensor pipe (twice the TF32 rate), fp32 accumulation
+//   F16X3I : F16X3 on operands whose hi and lo are interleaved per 32 channels ([rows][ceil(K / 32)][64] fp16, one
+//            128-byte row = [hi 32 | lo 32], dinotrk_split_hilo): K blocks of 32 channels, one TMA per operand and stage,
+//            hi read at 0 / 32 bytes into the row and lo at 64 / 96.  The same wgmma sequence as F16X3 (bit-identical
+//            results) on half the bytes per stage, so twice the stages fit.  The "hi" operands carry the interleaved arrays
 //   TF32X3 : the same scheme with TF32 parts (fp32 storage)
 //   TF32   : single pass on fp32 data (the tensor core reads the top 19 bits)
 //   BF16   : single pass on bf16 data
@@ -33,7 +37,7 @@
 
 namespace dtk {
 
-enum class TcMode { TF32X3 = 0, TF32 = 1, BF16 = 2, F16X3 = 3, F16 = 4, S8 = 5 };
+enum class TcMode { TF32X3 = 0, TF32 = 1, BF16 = 2, F16X3 = 3, F16 = 4, S8 = 5, F16X3I = 6 };
 
 constexpr int TC_BM = 128, TC_BN = 256;   // TC_BN: default N tile (template parameter BN overrides it)
 constexpr int TC2_BM = 256;               // M tile of a CTA pair
@@ -44,8 +48,10 @@ constexpr int TC_SMEM_MAX = 227 * 1024;
 template <TcMode MODE, int BN = TC_BN>
 struct TcCfg {
   static_assert(BN == 64 || BN == 128 || BN == 256, "N tile must be 64, 128 or 256");
-  static constexpr int kElem = MODE == TcMode::S8 ? 1 : (MODE == TcMode::BF16 || MODE == TcMode::F16X3 || MODE == TcMode::F16) ? 2 : 4;
-  static constexpr int kBK = 128 / kElem;                         // elements per 128-byte swizzle row
+  static constexpr bool kIL = MODE == TcMode::F16X3I;             // hi / lo interleaved in each 128-byte row
+  static constexpr int kElem = MODE == TcMode::S8 ? 1 : (MODE == TcMode::BF16 || MODE == TcMode::F16X3 || MODE == TcMode::F16 || kIL) ? 2 : 4;
+  static constexpr int kRowElems = 128 / kElem;                   // elements per 128-byte swizzle row
+  static constexpr int kBK = kIL ? kRowElems / 2 : kRowElems;     // K (channels) per K block
   static constexpr int kOps = (MODE == TcMode::TF32X3 || MODE == TcMode::F16X3) ? 2 : 1;   // hi (+ lo) tiles per operand
   static constexpr int kMmaK = 32 / kElem;                        // K per wgmma
   static constexpr int kABytes = TC_BM * 128, kBBytes = BN * 128;
@@ -166,7 +172,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
           tc::mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* st = smem + stage * Cfg::kStageBytes;
           tc::mbar_expect_tx(&full[stage], Cfg::kStageBytes);
-          const int k0 = kb * Cfg::kBK;
+          const int k0 = kb * Cfg::kRowElems;   // (interleaved: 32 channels = one whole row)
           tc::tma_load_2d(&tmA_hi, &full[stage], st, k0, arow);
           if (Cfg::kOps == 2) tc::tma_load_2d(&tmA_lo, &full[stage], st + Cfg::kABytes, k0, arow);
           uint8_t* sb = st + Cfg::kOps * Cfg::kABytes;
@@ -219,6 +225,11 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
           const uint64_t a_hi = tc::smem_desc_sw128(sa + koff), b_hi = tc::smem_desc_sw128(sb + koff);
           if constexpr (Cfg::kS8) {
             tc::wgmma_ss_s8<BN>(acc, a_hi, b_hi, 1u);
+          } else if constexpr (Cfg::kIL) {   // lo 64 bytes after hi in the same row; F16X3's product order
+            const uint64_t a_lo = tc::smem_desc_sw128(sa + 64 + koff), b_lo = tc::smem_desc_sw128(sb + 64 + koff);
+            tc::wgmma_ss<false, BN>(acc, a_lo, b_hi, 1u);
+            tc::wgmma_ss<false, BN>(acc, a_hi, b_lo, 1u);
+            tc::wgmma_ss<false, BN>(acc, a_hi, b_hi, 1u);
           } else if (Cfg::kOps == 2) {
             const uint64_t a_lo = tc::smem_desc_sw128(sa + Cfg::kABytes + koff);
             const uint64_t b_lo = tc::smem_desc_sw128(sb + Cfg::kBBytes + koff);
@@ -346,7 +357,7 @@ int launch_tc_plan(const TcPlan& pl, int n_groups, int rows, int row_stride, int
 int launch_amax(const float* x, size_t n, unsigned* amax, unsigned grid, cudaStream_t st);
 
 // Operands: A [a_rows][K], B [b_batch][N][K], row pitches lda / ldb in elements (0: dense).  The lo parts are read in the
-// split modes only (TcCfg::kOps == 2).
+// split modes only (TcCfg::kOps == 2).  F16X3I: a_hi / b_hi are the interleaved arrays, rows of 64 ceil(K / 32) elements.
 struct TcOperands {
   const void* a_hi; const void* a_lo; uint64_t a_rows, lda;
   const void* b_hi; const void* b_lo; uint64_t b_batch, ldb;
@@ -360,9 +371,11 @@ int tc_launch(const TcOperands& op, const TcProblem& pb, int m_tiles, const Epi&
   using Cfg = TcCfg<MODE, BN>;
   constexpr int elem = MODE == TcMode::S8 ? TMAP_S8 : MODE == TcMode::BF16 ? TMAP_BF16 : Cfg::kElem == 2 ? TMAP_F16 : TMAP_F32;
   CUtensorMap ta[2], tb[2];
+  const uint64_t cols = Cfg::kIL ? 64 * (uint64_t)((pb.K + 31) / 32) : (uint64_t)pb.K;   // elements per operand row
   for (int i = 0; i < Cfg::kOps; ++i) {   // single-pass modes pass the hi maps twice
-    if (int rc = make_tmap_2d(&ta[i], i ? op.a_lo : op.a_hi, op.a_rows, pb.K, TC_BM, Cfg::kBK, elem, op.lda)) return rc;
-    if (int rc = make_tmap_3d(&tb[i], i ? op.b_lo : op.b_hi, op.b_batch, pb.N, pb.K, PAIR ? BN / 2 : BN, Cfg::kBK, elem, op.ldb))
+    if (int rc = make_tmap_2d(&ta[i], i ? op.a_lo : op.a_hi, op.a_rows, cols, TC_BM, Cfg::kRowElems, elem, op.lda)) return rc;
+    if (int rc = make_tmap_3d(&tb[i], i ? op.b_lo : op.b_hi, op.b_batch, pb.N, cols, PAIR ? BN / 2 : BN, Cfg::kRowElems, elem,
+                              op.ldb))
       return rc;
   }
   const auto kern = [] {   // if constexpr: only the kernel launched here is instantiated

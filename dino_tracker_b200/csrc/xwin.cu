@@ -299,34 +299,44 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
 //             loaded once per cell and each warpgroup drains its pipeline once per cell.
 //   MB = 128  cells of up to 128 maps: warpgroup 1 takes descriptor rows 0-63 and warpgroup 2 rows 64-127 of the same part;
 //             the two parts run one after the other, a stage holding the descriptor K-block and one part.
-// K blocks of 32 channels in 64-byte-swizzled rows (a MB = 64 stage is 64 KiB: three fit).  Split precision: lo*hi + hi*lo
-// + hi*hi per K step of 16, K ascending -- the full-map GEMM's sequence of products.  The box rows arrive as 4-D TMA boxes
-// {32 channels, 21 columns, 12 or 9 rows, 1 frame} of the [T][h][w][C] feature video, zero-filled outside the token grid.
+// K blocks of 32 channels.  Split precision: lo*hi + hi*lo + hi*hi per K step of 16, K ascending -- the full-map GEMM's
+// sequence of products.  The descriptor K-block is two tiles (hi, lo) of 64-byte-swizzled rows.  The box rows arrive as 4-D
+// TMA boxes {channels, 21 columns, 12 or 9 rows, 1 frame} of the feature video, zero-filled outside the token grid, in one
+// of two row layouts (HILO):
+//   false  the separate hi and lo halves [T][h][w][C]: two boxes of 64-byte rows (32 channels) per part and K block.
+//   true   the interleaved split [T][h][w][ceil(C / 32)][64] (FeatView::hilo): one box of 128-byte rows [hi 32 | lo 32] in
+//          the 128-byte swizzle; a K step reads hi 0 / 32 and lo 64 / 96 bytes into the row.  Same bytes in half as many
+//          rows: the TMA's cost per row, not the MMA, bounds the 64-byte layout (DESIGN.md 4.3).
+// A MB = 64 stage is 64 KiB in either layout (three fit), a MB = 128 stage 48 KiB (four).
 // Epilogue: straight from the accumulator fragment to xbox[map][token] (a quad holds 8 consecutive tokens of one map).
-template <int MB>
+template <int MB, bool HILO>
 struct XwCfg {
-  static constexpr int kBK = 32;                                  // fp16 channels per 64-byte swizzle row
-  static constexpr int kRow = 2 * kBK;                            // bytes per operand row
+  static constexpr int kBK = 32;                                  // channels per K block
+  static constexpr int kRow = 2 * kBK;                            // bytes per descriptor row of one half (64-byte swizzle)
+  static constexpr int kTokRow = HILO ? 2 * kRow : kRow;          // bytes per token row of one TMA box
+  static constexpr int kBoxes = HILO ? 1 : 2;                     // token boxes per part and K block
   static constexpr int kDescBytes = MB * kRow;                    // one operand half (hi or lo) of the descriptor K-block
-  static constexpr int kTok0Bytes = XW_N0 * kRow, kTok1Bytes = XW_N1 * kRow;   // one half of a part's token tile
-  static constexpr int kTok0Tx = XW_ROWS0 * XW_BOX * kRow, kTok1Tx = XW_ROWS1 * XW_BOX * kRow;   // bytes the TMA box lands
-  // stage: [desc hi | desc lo | part 0 hi | part 0 lo (| part 1 hi | part 1 lo, MB = 64)]; with MB = 128 either part uses
-  // the part 0 slots
+  static constexpr int kTok0Bytes = XW_N0 * kTokRow, kTok1Bytes = XW_N1 * kTokRow;   // one token box's slot
+  static constexpr int kTok0Tx = XW_ROWS0 * XW_BOX * kTokRow, kTok1Tx = XW_ROWS1 * XW_BOX * kTokRow;   // bytes a box lands
+  // stage: [desc hi | desc lo | part 0 boxes (| part 1 boxes, MB = 64)]; with MB = 128 either part uses the part 0 slots.
+  // Every token box starts 1024-byte aligned (the 128-byte swizzle's atom).
   static constexpr int kTokOff = 2 * kDescBytes;
-  static constexpr int kStageBytes = MB == 64 ? 2 * (kDescBytes + kTok0Bytes + kTok1Bytes) : 2 * (kDescBytes + kTok0Bytes);
+  static constexpr int kStageBytes = kTokOff + kBoxes * (MB == 64 ? kTok0Bytes + kTok1Bytes : kTok0Bytes);
   static constexpr int kStages = MB == 64 ? 3 : 4;
   static constexpr int kSmem = kStages * kStageBytes + 1024 + 256;
   static_assert(kStages * kStageBytes + 1024 + 256 <= 227 * 1024, "shared-memory ring too large");
+  static_assert(kTokOff % 1024 == 0 && kTok0Bytes % 1024 == 0 && kTok1Bytes % 1024 == 0 && kStageBytes % 1024 == 0,
+                "token boxes must start 1024-byte aligned");
 };
 
 // One part of a cell on one consumer warpgroup: the K loop over the ring, then rows [r0, r0 + 64) of the cell x the part's
-// tokens into xbox.  d_off / t_off: byte offsets of the warpgroup's descriptor rows / the part's token tile in a stage,
-// t_half: distance from a token tile's hi half to its lo half.
-template <int MB, int N>
+// tokens into xbox.  d_off / t_off: byte offsets of the warpgroup's descriptor rows / the part's token box(es) in a stage,
+// t_half: distance from a token box's hi half to its lo half (separate halves only).
+template <int MB, bool HILO, int N>
 __device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t* empty, int& stage, int& phase, int KB,
                                         uint32_t d_off, uint32_t t_off, uint32_t t_half, float* __restrict__ xbox, int map0,
                                         int r0, int m) {
-  using Cfg = XwCfg<MB>;
+  using Cfg = XwCfg<MB, HILO>;
   constexpr int kTok = (N == XW_N0 ? XW_ROWS0 : XW_ROWS1) * XW_BOX;   // tokens of the part
   constexpr int kCol0 = N == XW_N0 ? 0 : XW_ROWS0 * XW_BOX;           // its first column in xbox
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = threadIdx.x & 127;
@@ -343,7 +353,8 @@ __device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t*
     for (int ks = 0; ks < Cfg::kBK / 16; ++ks) {
       const uint32_t koff = ks * 32;
       const uint64_t d_hi = tc::smem_desc_sw64(sd + koff), d_lo = tc::smem_desc_sw64(sd + Cfg::kDescBytes + koff);
-      const uint64_t t_hi = tc::smem_desc_sw64(st + koff), t_lo = tc::smem_desc_sw64(st + t_half + koff);
+      const uint64_t t_hi = HILO ? tc::smem_desc_sw128(st + koff) : tc::smem_desc_sw64(st + koff);
+      const uint64_t t_lo = HILO ? tc::smem_desc_sw128(st + Cfg::kRow + koff) : tc::smem_desc_sw64(st + t_half + koff);
       tc::wgmma_ss<false, N>(acc, d_lo, t_hi, 1u);   // desc_lo * tok_hi, desc_hi * tok_lo, desc_hi * tok_hi:
       tc::wgmma_ss<false, N>(acc, d_hi, t_lo, 1u);   // the product order of tc_gemm_kernel (F16X3)
       tc::wgmma_ss<false, N>(acc, d_hi, t_hi, 1u);
@@ -373,13 +384,14 @@ __device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t*
   }
 }
 
-template <int MB>
+// tm0 / tm1: token boxes of part 0 / 1 ([0] hi or the interleaved split, [1] lo; [1] unused with HILO)
+template <int MB, bool HILO>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant__ CUtensorMap tmD_lo,
                const __grid_constant__ CUtensorMap tm0_hi, const __grid_constant__ CUtensorMap tm0_lo,
                const __grid_constant__ CUtensorMap tm1_hi, const __grid_constant__ CUtensorMap tm1_lo, XwCells cells,
                const int2* __restrict__ box_org, float* __restrict__ xbox, int K) {
-  using Cfg = XwCfg<MB>;
+  using Cfg = XwCfg<MB, HILO>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);   // [kStages]
@@ -389,8 +401,10 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
   const int KB = (K + Cfg::kBK - 1) / Cfg::kBK;
 
   if (threadIdx.x == 0) {
-    tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo); tc::prefetch_tmap(&tm0_hi); tc::prefetch_tmap(&tm0_lo);
-    tc::prefetch_tmap(&tm1_hi); tc::prefetch_tmap(&tm1_lo);
+    tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo); tc::prefetch_tmap(&tm0_hi);
+    if (!HILO) tc::prefetch_tmap(&tm0_lo);
+    tc::prefetch_tmap(&tm1_hi);
+    if (!HILO) tc::prefetch_tmap(&tm1_lo);
     for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 2); }   // 2 consumer warpgroups
     tc::mbar_fence_init();
   }
@@ -407,22 +421,22 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
         const int drow = cells.arow[cell], frame = cells.frame[cell];
         for (int part = 0; part < (MB == 64 ? 1 : 2); ++part) {
           for (int kb = 0; kb < KB; ++kb) {
-            const int k0 = kb * Cfg::kBK;
+            const int k0 = kb * Cfg::kBK, kt = HILO ? 2 * k0 : k0;   // channel / token-row element of the K block
             tc::mbar_wait(&empty[stage], phase ^ 1);
             uint8_t* st = smem + stage * Cfg::kStageBytes;
             uint8_t* s0 = st + Cfg::kTokOff;
             if constexpr (MB == 64) {   // the descriptors and both parts
-              tc::mbar_expect_tx(&full[stage], 2 * (Cfg::kDescBytes + Cfg::kTok0Tx + Cfg::kTok1Tx));
-              uint8_t* s1 = s0 + 2 * Cfg::kTok0Bytes;
-              tc::tma_load_4d(&tm0_hi, &full[stage], s0, k0, org.y, org.x, frame);
-              tc::tma_load_4d(&tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, k0, org.y, org.x, frame);
-              tc::tma_load_4d(&tm1_hi, &full[stage], s1, k0, org.y, org.x + XW_ROWS0, frame);
-              tc::tma_load_4d(&tm1_lo, &full[stage], s1 + Cfg::kTok1Bytes, k0, org.y, org.x + XW_ROWS0, frame);
+              tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + Cfg::kBoxes * (Cfg::kTok0Tx + Cfg::kTok1Tx));
+              uint8_t* s1 = s0 + Cfg::kBoxes * Cfg::kTok0Bytes;
+              tc::tma_load_4d(&tm0_hi, &full[stage], s0, kt, org.y, org.x, frame);
+              if (!HILO) tc::tma_load_4d(&tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, kt, org.y, org.x, frame);
+              tc::tma_load_4d(&tm1_hi, &full[stage], s1, kt, org.y, org.x + XW_ROWS0, frame);
+              if (!HILO) tc::tma_load_4d(&tm1_lo, &full[stage], s1 + Cfg::kTok1Bytes, kt, org.y, org.x + XW_ROWS0, frame);
             } else {                    // the descriptors and part `part`
-              tc::mbar_expect_tx(&full[stage], 2 * (Cfg::kDescBytes + (part ? Cfg::kTok1Tx : Cfg::kTok0Tx)));
+              tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + Cfg::kBoxes * (part ? Cfg::kTok1Tx : Cfg::kTok0Tx));
               const int by = org.x + (part ? XW_ROWS0 : 0);
-              tc::tma_load_4d(part ? &tm1_hi : &tm0_hi, &full[stage], s0, k0, org.y, by, frame);
-              tc::tma_load_4d(part ? &tm1_lo : &tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, k0, org.y, by, frame);
+              tc::tma_load_4d(part ? &tm1_hi : &tm0_hi, &full[stage], s0, kt, org.y, by, frame);
+              if (!HILO) tc::tma_load_4d(part ? &tm1_lo : &tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, kt, org.y, by, frame);
             }
             tc::tma_load_2d(&tmD_hi, &full[stage], st, k0, drow);
             tc::tma_load_2d(&tmD_lo, &full[stage], st + Cfg::kDescBytes, k0, drow);
@@ -441,52 +455,61 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
       const int m = cells.m[cell], map0 = cells.row0[cell];
       if constexpr (MB == 64) {   // warpgroup 1: part 0, warpgroup 2: part 1, all 64 descriptor rows
         if (cw == 0)
-          xw_part<MB, XW_N0>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 0, m);
+          xw_part<MB, HILO, XW_N0>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 0, m);
         else
-          xw_part<MB, XW_N1>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff + 2 * Cfg::kTok0Bytes, Cfg::kTok1Bytes,
-                             xbox, map0, 0, m);
+          xw_part<MB, HILO, XW_N1>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff + Cfg::kBoxes * Cfg::kTok0Bytes,
+                                   Cfg::kTok1Bytes, xbox, map0, 0, m);
       } else {                    // warpgroup cw: descriptor rows [64 cw, 64 cw + 64) of both parts
         const uint32_t d_off = cw * 64 * Cfg::kRow;
-        xw_part<MB, XW_N0>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
-        xw_part<MB, XW_N1>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
+        xw_part<MB, HILO, XW_N0>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
+        xw_part<MB, HILO, XW_N1>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
       }
     }
   }
+}
+
+template <int MB, bool HILO>
+static int run_xw_gemm(const CUtensorMap (&tm)[6], const XwCells& cells, const XwChunk& xc, int C, cudaStream_t st) {
+  static PerDev<bool> attr_dev;
+  bool& attr = attr_dev.get();
+  if (!attr) {
+    DTK_CUDA(cudaFuncSetAttribute(xw_gemm_kernel<MB, HILO>, cudaFuncAttributeMaxDynamicSharedMemorySize, XwCfg<MB, HILO>::kSmem));
+    attr = true;
+  }
+  const int sms = num_sms();
+  const int grid = cells.n_cells < sms ? cells.n_cells : sms;
+  ProfRange pr(PROF_XW_GEMM, st);
+  xw_gemm_kernel<MB, HILO><<<grid, TC_THREADS, XwCfg<MB, HILO>::kSmem, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], cells,
+                                                                              xc.box_org, xc.xbox, C);
+  DTK_LAUNCHED();
+  return DINOTRK_OK;
 }
 
 int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_hi, const void* desc_lo, int desc_rows,
                    const XwCells& cells, const XwChunk& xc, cudaStream_t st) {
   if (cells.n_cells <= 0) return DINOTRK_OK;
   DTK_CHECK_ARG(fv.C % 8 == 0 && cells.max_m <= XW_MAX_CELL, "exact-window GEMM: bad sizes");
-  const bool small = cells.max_m <= 64;
-  constexpr int BK = XwCfg<64>::kBK, SW = 2 * BK;   // 32-channel K blocks, 64-byte swizzle
-  CUtensorMap tD_hi, tD_lo, t0_hi, t0_lo, t1_hi, t1_lo;
+  const bool small = cells.max_m <= 64, hilo = fv.hilo != nullptr;
+  constexpr int BK = XwCfg<64, false>::kBK, SW = 2 * BK;   // 32-channel K blocks; descriptors in 64-byte swizzle
+  CUtensorMap tm[6];   // desc hi, desc lo, part 0 [hi | hilo], part 0 lo, part 1 [hi | hilo], part 1 lo
   int rc;
-  if ((rc = make_tmap_2d(&tD_hi, desc_hi, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
-  if ((rc = make_tmap_2d(&tD_lo, desc_lo, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
-  const uint64_t dims[4] = {(uint64_t)fv.C, (uint64_t)g.w, (uint64_t)g.h, (uint64_t)fv.T};
-  const uint64_t strides[3] = {(uint64_t)fv.C * 2, (uint64_t)g.w * fv.C * 2, (uint64_t)fv.P * fv.C * 2};
-  const uint32_t box0[4] = {BK, XW_BOX, XW_ROWS0, 1}, box1[4] = {BK, XW_BOX, XW_ROWS1, 1};
-  if ((rc = make_tmap_4d(&t0_hi, fv.hi, dims, strides, box0, TMAP_F16, SW))) return rc;
-  if ((rc = make_tmap_4d(&t0_lo, fv.lo, dims, strides, box0, TMAP_F16, SW))) return rc;
-  if ((rc = make_tmap_4d(&t1_hi, fv.hi, dims, strides, box1, TMAP_F16, SW))) return rc;
-  if ((rc = make_tmap_4d(&t1_lo, fv.lo, dims, strides, box1, TMAP_F16, SW))) return rc;
-  static PerDev<bool> attr_dev;
-  bool& attr = attr_dev.get();
-  if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(xw_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, XwCfg<64>::kSmem));
-    DTK_CUDA(cudaFuncSetAttribute(xw_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, XwCfg<128>::kSmem));
-    attr = true;
+  if ((rc = make_tmap_2d(&tm[0], desc_hi, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
+  if ((rc = make_tmap_2d(&tm[1], desc_lo, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
+  const uint64_t row = hilo ? (uint64_t)hilo_row(fv.C) : (uint64_t)fv.C;   // fp16 elements per token row
+  const uint64_t dims[4] = {row, (uint64_t)g.w, (uint64_t)g.h, (uint64_t)fv.T};
+  const uint64_t strides[3] = {row * 2, (uint64_t)g.w * row * 2, (uint64_t)fv.P * row * 2};
+  const uint32_t ib = hilo ? 2 * BK : BK, tsw = hilo ? 128 : SW;
+  const uint32_t box0[4] = {ib, XW_BOX, XW_ROWS0, 1}, box1[4] = {ib, XW_BOX, XW_ROWS1, 1};
+  if ((rc = make_tmap_4d(&tm[2], hilo ? fv.hilo : fv.hi, dims, strides, box0, TMAP_F16, tsw))) return rc;
+  if ((rc = make_tmap_4d(&tm[4], hilo ? fv.hilo : fv.hi, dims, strides, box1, TMAP_F16, tsw))) return rc;
+  if (hilo) {
+    tm[3] = tm[2];
+    tm[5] = tm[4];
+    return small ? run_xw_gemm<64, true>(tm, cells, xc, fv.C, st) : run_xw_gemm<128, true>(tm, cells, xc, fv.C, st);
   }
-  const int sms = num_sms();
-  const int grid = cells.n_cells < sms ? cells.n_cells : sms;
-  ProfRange pr(PROF_XW_GEMM, st);
-  if (small)
-    xw_gemm_kernel<64><<<grid, TC_THREADS, XwCfg<64>::kSmem, st>>>(tD_hi, tD_lo, t0_hi, t0_lo, t1_hi, t1_lo, cells, xc.box_org, xc.xbox, fv.C);
-  else
-    xw_gemm_kernel<128><<<grid, TC_THREADS, XwCfg<128>::kSmem, st>>>(tD_hi, tD_lo, t0_hi, t0_lo, t1_hi, t1_lo, cells, xc.box_org, xc.xbox, fv.C);
-  DTK_LAUNCHED();
-  return DINOTRK_OK;
+  if ((rc = make_tmap_4d(&tm[3], fv.lo, dims, strides, box0, TMAP_F16, tsw))) return rc;
+  if ((rc = make_tmap_4d(&tm[5], fv.lo, dims, strides, box1, TMAP_F16, tsw))) return rc;
+  return small ? run_xw_gemm<64, false>(tm, cells, xc, fv.C, st) : run_xw_gemm<128, false>(tm, cells, xc, fv.C, st);
 }
 
 // ====================================================================================================== 4. head
@@ -844,6 +867,8 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
 // ====================================================================================================== 5. full-map queue
 // One block per queued map: copies its descriptor (fp32 + fp16 hi / lo), norm and output slot to compact row b; block 0
 // also writes the compact group arrays.  Rows of a group keep their queue order (arbitrary, results do not depend on it).
+// HILO: the fp16 row goes to c_hi interleaved per 32 channels ([rows][2 C], C % 32 == 0; c_lo unused).
+template <bool HILO>
 __global__ void __launch_bounds__(128)
 xw_compact_kernel(const float4* __restrict__ desc, const uint4* __restrict__ dhi, const uint4* __restrict__ dlo,
                   const int* __restrict__ arow, const float* __restrict__ desc_norm, const int* __restrict__ out_index, int C, const int* __restrict__ grp_frame,
@@ -875,8 +900,14 @@ xw_compact_kernel(const float4* __restrict__ desc, const uint4* __restrict__ dhi
     for (int i = threadIdx.x; i < C / 4; i += blockDim.x) c_desc[(size_t)b * (C / 4) + i] = desc[srow * (C / 4) + i];
   if (dhi != nullptr)
     for (int i = threadIdx.x; i < C / 8; i += blockDim.x) {
-      c_hi[(size_t)b * (C / 8) + i] = dhi[srow * (C / 8) + i];
-      c_lo[(size_t)b * (C / 8) + i] = dlo[srow * (C / 8) + i];
+      if (HILO) {   // 8 channels = a quarter of a 32-channel block: hi at uint4 (i / 4) 8 + i % 4, lo 4 further
+        const size_t o = (size_t)b * (C / 4) + (i >> 2) * 8 + (i & 3);
+        c_hi[o] = dhi[srow * (C / 8) + i];
+        c_hi[o + 4] = dlo[srow * (C / 8) + i];
+      } else {
+        c_hi[(size_t)b * (C / 8) + i] = dhi[srow * (C / 8) + i];
+        c_lo[(size_t)b * (C / 8) + i] = dlo[srow * (C / 8) + i];
+      }
     }
   if (threadIdx.x == 0) { c_norm[b] = desc_norm[src]; c_out_index[b] = out_index[src]; }
 }
@@ -884,10 +915,11 @@ xw_compact_kernel(const float4* __restrict__ desc, const uint4* __restrict__ dhi
 int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const int* arow, const float* desc_norm,
                       const int* out_index, int C, const int* grp_frame, const int* grp_map0, int n_groups, int n_slow,
                       const XwChunk& xc, float* c_desc, void* c_hi, void* c_lo, float* c_norm, int* c_out_index, int* cgrp,
-                      int gcap, cudaStream_t st, int row_base, int grp_base) {
+                      int gcap, cudaStream_t st, int row_base, int grp_base, bool hilo) {
   if (n_slow <= 0) return DINOTRK_OK;
+  DTK_CHECK_ARG(!hilo || C % 32 == 0, "xw_compact: interleaved rows need C %% 32 == 0");
   ProfRange pr(PROF_MISC, st);
-  xw_compact_kernel<<<n_slow, 128, 0, st>>>(reinterpret_cast<const float4*>(desc), reinterpret_cast<const uint4*>(desc_hi),
+  (hilo ? xw_compact_kernel<true> : xw_compact_kernel<false>)<<<n_slow, 128, 0, st>>>(reinterpret_cast<const float4*>(desc), reinterpret_cast<const uint4*>(desc_hi),
                                             reinterpret_cast<const uint4*>(desc_lo), arow, desc_norm, out_index, C, grp_frame, grp_map0,
                                             n_groups, xc.slow_cnt, xc.slow_list, reinterpret_cast<float4*>(c_desc),
                                             reinterpret_cast<uint4*>(c_hi), reinterpret_cast<uint4*>(c_lo), c_norm, c_out_index, cgrp,

@@ -138,6 +138,7 @@ int launch_xw_rnorms(const FeatView& fv, float* rnorms, unsigned* min_bits, cuda
 // eps: per-map bound on |coarse - exact| of the int8 pass (xw_eps_s8), nullptr for the fp16 pass (XW_EPS)
 int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, const dinotrk_geom& g, const XwChunk& xc,
                    cudaStream_t st, int n_maps, float min_norm, const float* eps);
+// box tokens from fv.hilo (128-byte rows) when given, else from fv.hi / fv.lo (64-byte rows)
 int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_hi, const void* desc_lo, int desc_rows,
                    const XwCells& cells, const XwChunk& xc, cudaStream_t st);
 int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head_weights& hw, const XwCells& cells,
@@ -146,9 +147,10 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
 // Appends the queued maps' descriptor rows (fp32 optional, hi, lo, norm, out_index) to compact arrays at row_base and their
 // group arrays ([frame | row0 | m | map0] x gcap, entries grp_base ..) to cgrp.  n_slow = host copy of slow_cnt[n_groups].
 // arow[map] = the map's row in desc / desc_hi / desc_lo (nullptr: the map index); norm and out_index are per map.
+// hilo: the fp16 rows go to c_hi interleaved per 32 channels (the full-map GEMM's F16X3I operand; c_lo unused).
 int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_lo, const int* arow, const float* desc_norm,
                       const int* out_index, int C, const int* grp_frame, const int* grp_map0, int n_groups, int n_slow,
                       const XwChunk& xc, float* c_desc, void* c_hi, void* c_lo, float* c_norm, int* c_out_index, int* cgrp,
-                      int gcap, cudaStream_t st, int row_base = 0, int grp_base = 0);
+                      int gcap, cudaStream_t st, int row_base = 0, int grp_base = 0, bool hilo = false);
 
 }  // namespace dtk

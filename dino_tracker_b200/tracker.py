@@ -103,8 +103,8 @@ class Tracker(nn.Module):
     def features_struct(self, tpc, norms, quant=False):
         """C struct for a [T][P][C] feature video (+ its cached fp16 hi/lo split in fp16x3 mode).  A video outside the
         split's faithful range gets no split: its contractions run on the exact-fp32 path (with a RuntimeWarning).
-        quant: also the int8 operands of the anchor phase's coarse pass (dinotrk_infer only; computed on first request and
-        cached with the split)."""
+        quant: also the anchor phase's own operands, the int8 rows of the coarse pass and the interleaved split of the exact
+        box GEMM (dinotrk_infer only; computed on first request and cached with the split)."""
         if self.corr_precision != "fp16x3" or tpc.shape[-1] % 8:
             return _lib.make_features(tpc, norms)
         # The split lives ON the tensor object it was computed from: a fresh feature tensor (uncached forward,
@@ -113,11 +113,13 @@ class Tracker(nn.Module):
         split = getattr(tpc, "_dtk_split", None)
         if split is None or split[0] != tpc._version:
             hi, lo = _lib.split_features(tpc, norms, _lib.stream_ptr(self._dev))
-            split = [tpc._version, hi, lo, None]
+            split = [tpc._version, hi, lo, None, None]
             tpc._dtk_split = split
         if quant and split[3] is None and split[1] is not None:
             split[3] = _lib.quantise_features(tpc, norms, _lib.stream_ptr(self._dev))
-        return _lib.make_features(tpc, norms, split[1], split[2], split[3] if quant else None)
+        if quant and split[4] is None and split[1] is not None:
+            split[4] = _lib.split_hilo(tpc, _lib.stream_ptr(self._dev))
+        return _lib.make_features(tpc, norms, split[1], split[2], split[3] if quant else None, split[4] if quant else None)
 
     def _set_dino(self, chw):
         self._dino_tpc, self._dino_norms = self._pack(chw)

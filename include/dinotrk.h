@@ -57,7 +57,9 @@ typedef struct dinotrk_head_weights {
  * fp32-faithful), otherwise on the exact-fp32 FFMA GEMM.  C must then be a multiple of 8.
  * q8 / q_fac / q_rho (optional, all or none; C a multiple of 16 and <= 1040): the int8 operands of the anchor phase's
  * coarse pass, written by dinotrk_quantise_s8 with rows_per_group = h*w (q8 [T][P][C] int8, q_fac [T][P], q_rho [T] =
- * the largest relative residual of each frame). */
+ * the largest relative residual of each frame).
+ * hilo (optional, with hi / lo): the same split interleaved per 32 channels, written by dinotrk_split_hilo; the exact box
+ * GEMM of the anchor phase then reads hi and lo of a token as one 128-byte row per 32 channels. */
 typedef struct dinotrk_features {
   const float* tpc;
   const float* norms;
@@ -67,6 +69,7 @@ typedef struct dinotrk_features {
   const void* q8;
   const float* q_fac;
   const float* q_rho;
+  const void* hilo;
 } dinotrk_features;
 
 int dinotrk_version(void);
@@ -89,6 +92,9 @@ int dinotrk_quantise_s8(const float* x, const float* norms, size_t rows, int C, 
                         float* rho, float* rho_max, void* stream);
 /* x = hi + lo with hi = rn_fp16(x), lo = rn_fp16(x - hi) (fp16 arrays of n elements); n % 4 == 0. */
 int dinotrk_split_fp16(const float* x, void* hi, void* lo, size_t n, void* stream);
+/* The same split of x [rows][C] (C % 4 == 0) interleaved per 32 channels: hilo [rows][ceil(C / 32)][64] fp16, where
+ * element 64 b + j of a row is hi[32 b + j] and 64 b + 32 + j is lo[32 b + j]; channels past C are zero. */
+int dinotrk_split_hilo(const float* x, void* hilo, size_t rows, int C, void* stream);
 /* The numbers the split's faithful range is stated in: range (device float[2]) = {max |x| over the n elements of x,
  * smallest non-zero value of the n_tok token norms (3.4e38 if there is none)}.  dinotrk_split_faithful (host only) is 1
  * when they are in range for C channels: the split contraction is then fp32-faithful (max |x| <= 65504, every non-zero
@@ -254,7 +260,8 @@ int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* 
  * against the 21 x 21 token box of frame cell_frame[k] whose first row / column is box_org[k] = {row, column} (int32
  * [n_cells][2]; tokens outside the grid count as zero; column INT_MIN: skip the cell).  Writes the raw accumulators
  * xbox[row][by * 21 + bx] (fp32, [desc_rows][448]); columns 441..447, rows outside every cell and the rows of skipped cells
- * are not written.  max_m = the largest cell_m (<= 128).  feat->hi and feat->lo are required.  Syncs: no. */
+ * are not written.  max_m = the largest cell_m (<= 128).  feat->hi and feat->lo are required; with feat->hilo the box
+ * tokens are read from it instead (the same bits).  Syncs: no. */
 int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
                         int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
                         int n_cells, int max_m, float* xbox, void* stream);

@@ -3,20 +3,24 @@ token box) on its own, at the shapes one steady-state chunk of BASELINE config 2
 
   python tools/bench_xw_gemm.py [--launches 1000] [--windows 5]
 
-Inputs: seeded features of the chunk's three anchor frames (P = 67 x 121 = 8107 tokens, C = 1024, split into fp16 hi / lo);
+Inputs: seeded features of the chunk's three anchor frames (P = 67 x 121 = 8107 tokens, C = 1024, split into fp16 hi / lo,
+and the same split interleaved per 32 channels);
 655 cells of T = 50 maps (32,750 descriptor rows), as in the first full anchor chunk of config 2 (tools/bench_coarse.py):
 175 cells anchored in frame 0, 256 in frame 1, 224 in frame 2.  Box origins are drawn from a seed, about a quarter of the
 boxes hanging over the border of the token grid (zero-filled there).
 
-Prints one JSON line:
+Both token-row layouts are timed, alternating window by window: `split` (separate hi / lo halves, 64-byte rows) and
+`hilo` (the interleaved split in the feature struct, 128-byte rows).  Prints one JSON line; per layout:
   ms_per_launch        CUDA events around dinotrk_xw_box_gemm, median over the windows, with min and max
   useful_tflops        2 * maps * 441 * C * 3 (three split-precision products per box token) over ms_per_launch
   executed_tflops      the MMA work the kernel issues: per cell of T <= 64 maps, 64 descriptor rows x 448 box columns
                        (m64n256 + m64n192) x C x 3
   clocks_per_64ch      ms_per_launch x SM clock x CTAs / (cells x C / 64): the period of 64 channels of one cell on one
-                       SM, epilogue included (1,344 clocks of MMA at the full fp16 rate of 2,048 FMA per clock per SM)
+                       SM, epilogue included (2,688 clocks of MMA at the full fp16 rate of 2,048 FMA per clock per SM)
+  clocks_per_stage     the same per 32-channel ring stage (1,344 clocks of MMA)
+  xbox_sha256          digest of the accumulators, to compare builds and layouts bit for bit
+and once:
   gpu                  card name, power limit and the SM clock (NVML, sampled during the timed windows)
-  xbox_sha256          digest of the accumulators, to compare builds bit for bit
 """
 import argparse
 import ctypes
@@ -62,7 +66,8 @@ def main():
     feats = torch.randn(n_frames, P, C, device=dev, generator=g)
     norms = feats.norm(dim=2).contiguous()
     f_hi, f_lo = _lib.split_fp16(feats, st)
-    fs = _lib.make_features(feats, norms, f_hi, f_lo)
+    layouts = {"split": _lib.make_features(feats, norms, f_hi, f_lo),
+               "hilo": _lib.make_features(feats, norms, f_hi, f_lo, hilo=_lib.split_hilo(feats, st))}
     n_cells = sum(n for _, n in CELLS)
     rows = n_cells * T
     desc = torch.randn(rows, C, device=dev, generator=g)
@@ -77,42 +82,55 @@ def main():
     org_d = torch.from_numpy(org).to(dev).contiguous()
     geom = _lib.make_geom(14 + 7 * (GH - 1), 14 + 7 * (GW - 1))
     xbox = torch.zeros(rows, COLS, dtype=torch.float32, device=dev)
-    args = (ctypes.byref(fs), ctypes.byref(geom), _lib.ptr(d_hi), _lib.ptr(d_lo), rows, _lib.ptr(row0), _lib.ptr(m),
-            _lib.ptr(frame), _lib.ptr(org_d), n_cells, T, _lib.ptr(xbox), st)
 
-    def gemm():
-        _lib.check(lib.dinotrk_xw_box_gemm(*args), "xw_box_gemm")
+    def gemm_of(fs):
+        args = (ctypes.byref(fs), ctypes.byref(geom), _lib.ptr(d_hi), _lib.ptr(d_lo), rows, _lib.ptr(row0), _lib.ptr(m),
+                _lib.ptr(frame), _lib.ptr(org_d), n_cells, T, _lib.ptr(xbox), st)
+        return lambda: _lib.check(lib.dinotrk_xw_box_gemm(*args), "xw_box_gemm")
 
-    for _ in range(a.warmup):
-        gemm()
-    torch.cuda.synchronize()
-    digest = hashlib.sha256(xbox[:, :BOX * BOX].cpu().numpy().tobytes()).hexdigest()
+    gemms = {name: gemm_of(fs) for name, fs in layouts.items()}
+    digest = {}
+    for name, gemm in gemms.items():
+        xbox.zero_()
+        for _ in range(a.warmup):
+            gemm()
+        torch.cuda.synchronize()
+        digest[name] = hashlib.sha256(xbox[:, :BOX * BOX].cpu().numpy().tobytes()).hexdigest()
 
     gpu = card_info()
     sampler = bench.ClockSampler(0)
     sampler.start()
     time.sleep(0.1)
     t0 = time.perf_counter()
-    call_ms = time_windows(gemm, a.launches, a.windows)
+    call_ms = {name: [] for name in gemms}
+    for _ in range(a.windows):   # the layouts alternate window by window
+        for name, gemm in gemms.items():
+            call_ms[name] += time_windows(gemm, a.launches, 1)
     t1 = time.perf_counter()
     clocks = sampler.stop(t0, t1)
 
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     ctas = min(n_cells, sms)
     mhz = clocks["sm_mhz"]
-    med = sorted(call_ms)[len(call_ms) // 2]
-    sec = med / 1e3
     useful = 2.0 * rows * BOX * BOX * C * 3
     executed = 2.0 * n_cells * EXEC_ROWS * EXEC_COLS * C * 3
+    legs = {}
+    for name, ms in call_ms.items():
+        med = sorted(ms)[len(ms) // 2]
+        sec = med / 1e3
+        legs[name] = {
+            "ms_per_launch": med, "ms_per_launch_min": min(ms), "ms_per_launch_max": max(ms),
+            "useful_tflops": useful / sec / 1e12, "executed_tflops": executed / sec / 1e12,
+            "clocks_per_64ch": (sec * mhz * 1e6 * ctas / (n_cells * C / 64)) if mhz else None,
+            "clocks_per_stage": (sec * mhz * 1e6 * ctas / (n_cells * -(-C // 32))) if mhz else None,
+            "xbox_sha256": digest[name],
+        }
     print(json.dumps({
-        "kernel": "xw_exact_gemm (xw_gemm_kernel<64>)",
+        "kernel": "xw_exact_gemm (xw_gemm_kernel<64, HILO>)",
         "shape": {"T": T, "P": P, "C": C, "cells": n_cells, "rows": rows, "boxes_over_the_border": border, "ctas": ctas},
         "launches_per_window": a.launches, "windows": a.windows,
-        "ms_per_launch": med, "ms_per_launch_min": min(call_ms), "ms_per_launch_max": max(call_ms),
-        "useful_tflops": useful / sec / 1e12, "executed_tflops": executed / sec / 1e12,
-        "clocks_per_64ch": (sec * mhz * 1e6 * ctas / (n_cells * C / 64)) if mhz else None,
+        "layouts": legs, "same_xbox": digest["split"] == digest["hilo"],
         "gpu": dict(gpu, sm_mhz=mhz, clock_reasons=clocks["reasons"], clock_samples=clocks["samples"]),
-        "xbox_sha256": digest,
     }))
 
 
