@@ -94,18 +94,27 @@ template <class E> struct EpiCoalesced<E, std::enable_if_t<E::kCoalesced>> { sta
 template <class E, class = void> struct EpiPrefetch { static constexpr bool value = false; };
 template <class E> struct EpiPrefetch<E, std::enable_if_t<E::kPrefetch>> { static constexpr bool value = true; };
 
-// Fragment epilogues (`static constexpr bool kFragment = true`) skip the shared-memory round trip: right after the tile's
-// last wgmma has completed, every consumer thread calls
-//   fragment(g, r, m, n0, fc, acc, cols)
-// with its own accumulator registers (float, or int in S8 mode): acc[4 i + {0, 1}] are row r, acc[4 i + {2, 3}] row r + 8 (rows inside group g, which
-// has m rows: rows >= m are padding), columns n0 + 8 i + fc + {0, 1}.  The 4 lanes of a quad (lane & 3) hold the same
-// two rows.  cols[c] (shared memory, c < BN = 256) holds
-//   float2 column(g, n0, t)
-// of the same tile: consumer thread t of each warpgroup calls it when the tile starts, for columns n0 + t (.x) and
-// n0 + t + 128 (.y), so that the global reads are in flight during the tile's K loop and the epilogue reads its per-column
-// values from shared memory with constant offsets.
+// One output tile as the producer decoded it: group g, first row m0 inside the group and first column n0 of the tile, and
+// the group's B batch item, first A row and row count (rows >= m are padding)
+struct TcTile { int g, m0, n0, batch, row0, m; };
+
+// Fragment epilogues (`static constexpr bool kFragment = true`) skip the shared-memory round trip.  The producer writes
+// each tile's TcTile into shared memory next to the tile's first K block, so the consumers neither decode the tile nor
+// read the group tables.  Once that K block has landed (before the tile's first wgmma) consumer thread t of each
+// warpgroup calls
+//   Pre begin(tile, t, r)
+// (r: the thread's first accumulator row, below): it issues the tile's global reads, which are then in flight during the
+// K loop.  Pre has a member `float2 col`, the tile's per-column values for columns n0 + t (.x) and n0 + t + 128 (.y); the
+// body stages them in cols[c] (shared memory, c < BN = 256) so that the epilogue reads them with constant offsets.  Right
+// after the tile's last wgmma has completed, every consumer thread calls
+//   fragment(tile, r, fc, acc, cols, pre)
+// with its own accumulator registers (float, or int in S8 mode; the epilogue may overwrite them): acc[4 i + {0, 1}] are
+// row r, acc[4 i + {2, 3}] row r + 8 (rows inside the group), columns n0 + 8 i + fc + {0, 1}.  The 4 lanes of a quad
+// (lane & 3) hold the same two rows.
 template <class E, class = void> struct EpiFragment { static constexpr bool value = false; };
 template <class E> struct EpiFragment<E, std::enable_if_t<E::kFragment>> { static constexpr bool value = true; };
+template <class E, class = void> struct PreOf { struct type {}; };
+template <class E> struct PreOf<E, std::enable_if_t<EpiFragment<E>::value>> { using type = typename E::Pre; };
 
 struct TcProblem {
   const int* grp_batch;    // [n_groups] B batch item (frame) of each group
@@ -158,6 +167,11 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
     g = last_le(pb.n_groups, mt, pb.tile_start);
     m0 = (mt - pb.tile_start[g]) * TM + (int)rank * TC_BM;
   };
+  // fragment epilogues: the record of the tile whose first K block is in ring slot s (written by the producer before it
+  // arms full[s], read by the consumers before they release the slot)
+  TcTile* recs = reinterpret_cast<TcTile*>(epi_scratch + 4 * BN);
+  static_assert(!EpiFragment<Epi>::value || 4 * BN * 4 + Cfg::kStages * (int)sizeof(TcTile) <= Cfg::kEpiBytes,
+                "fragment epilogue: column buffers and tile records");
 
   if (wg == 0) {
     // ===================== TMA producer =====================
@@ -167,9 +181,11 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
       for (int tile = unit; tile < total_tiles; tile += n_units) {
         int g, m0, n0;
         decode(tile, g, m0, n0);
-        const int arow = pb.grp_row0[g] + m0, batch = pb.grp_batch[g];
+        const int row0 = pb.grp_row0[g], arow = row0 + m0, batch = pb.grp_batch[g];
         for (int kb = 0; kb < KB; ++kb) {
           tc::mbar_wait(&empty[stage], phase ^ 1);
+          if constexpr (EpiFragment<Epi>::value)   // (the arrive below releases this store to the consumers)
+            if (kb == 0) recs[stage] = TcTile{g, m0, n0, batch, row0, pb.grp_m[g]};
           uint8_t* st = smem + stage * Cfg::kStageBytes;
           tc::mbar_expect_tx(&full[stage], Cfg::kStageBytes);
           const int k0 = kb * Cfg::kRowElems;   // (interleaved: 32 channels = one whole row)
@@ -202,17 +218,32 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
     };
     int stage = 0, phase = 0;
     typename Cfg::Acc acc[BN / 2];
+    if constexpr (EpiFragment<Epi>::value) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+    }
     // fragment epilogues: the warpgroup's per-column values of the tile in one of two buffers, used by alternate tiles (a
     // thread rewrites a buffer only after the next tile's barrier, which every thread passes after its epilogue's reads)
     int cbuf = 0;
     static_assert(!EpiFragment<Epi>::value || (BN == 256 && 4 * BN * 4 <= Cfg::kEpiBytes), "fragment epilogue: column buffers");
     for (int tile = unit; tile < total_tiles; tile += n_units) {
       int g, m0, n0;
-      decode(tile, g, m0, n0);
-      float2 col_v;
-      if constexpr (EpiFragment<Epi>::value) col_v = epi.column(g, n0, t);
+      TcTile tl;
+      typename PreOf<Epi>::type pre;
+      if constexpr (EpiFragment<Epi>::value) {
+        tc::mbar_wait(&full[stage], phase);
+        tl = recs[stage];
+        g = tl.g; m0 = tl.m0; n0 = tl.n0;
+        pre = epi.begin(tl, t, m0 + cw * 64 + fr);
+      } else {
+        decode(tile, g, m0, n0);
+      }
+      // fragment epilogues: the tile's first wgmma ignores the accumulators (scale-d 0) instead of a zeroing pass over
+      // them while the tensor pipe waits
+      if constexpr (!EpiFragment<Epi>::value) {
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+      }
       int prev = -1;
       for (int kb = 0; kb < KB; ++kb) {
         tc::mbar_wait(&full[stage], phase);
@@ -223,8 +254,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
         for (int ks = 0; ks < Cfg::kBK / Cfg::kMmaK; ++ks) {
           const uint32_t koff = ks * 32;  // bytes inside the 128-byte swizzle row
           const uint64_t a_hi = tc::smem_desc_sw128(sa + koff), b_hi = tc::smem_desc_sw128(sb + koff);
+          const uint32_t sd = EpiFragment<Epi>::value && kb == 0 && ks == 0 ? 0u : 1u;
           if constexpr (Cfg::kS8) {
-            tc::wgmma_ss_s8<BN>(acc, a_hi, b_hi, 1u);
+            tc::wgmma_ss_s8<BN>(acc, a_hi, b_hi, sd);
           } else if constexpr (Cfg::kIL) {   // lo 64 bytes after hi in the same row; F16X3's product order
             const uint64_t a_lo = tc::smem_desc_sw128(sa + 64 + koff), b_lo = tc::smem_desc_sw128(sb + 64 + koff);
             tc::wgmma_ss<false, BN>(acc, a_lo, b_hi, 1u);
@@ -238,7 +270,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
             tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_lo, 1u);
             tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_hi, 1u);
           } else {
-            tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_hi, 1u);
+            tc::wgmma_ss<Cfg::kTF32, BN>(acc, a_hi, b_hi, sd);
           }
         }
         tc::wgmma_commit();
@@ -255,10 +287,10 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA_hi, const CU
       if constexpr (EpiFragment<Epi>::value) {
         float* cols = epi_scratch + (2 * cw + cbuf) * BN;
         cbuf ^= 1;
-        cols[t] = col_v.x;
-        cols[t + 128] = col_v.y;
+        cols[t] = pre.col.x;
+        cols[t + 128] = pre.col.y;
         tc::named_sync(1 + cw, 128);
-        epi.fragment(g, rbase + fr, pb.grp_m[g], n0, fc, acc, cols);
+        epi.fragment(tl, rbase + fr, fc, acc, cols, pre);
       } else if constexpr (!Cfg::kS8) {
         // ---- epilogue: 32-column blocks through shared memory ----
         const int r = rbase + t;

@@ -16,11 +16,12 @@ namespace dtk {
 // accumulators (converted exactly: C <= XW_S8_MAX_C).
 //
 // A fragment epilogue (tcgemm.cuh): it works on the accumulator registers of all eight consumer warps; the tile's token
-// factors come from shared memory, where the GEMM body staged them (column()).  Per element only u = acc * (1 / |F|) is
+// factors come from shared memory, where the GEMM body staged them (begin()).  Per element only u = acc * (1 / |F|) is
 // formed; the row's positive factor 1 / |d| (and the ReLU) are applied to the two statistics at the end -- multiplication by a positive constant does not change which token holds
 // the maximum.  The statistics -- the maximum, the first token holding it, the second largest value of the multiset -- do
-// not depend on the order the values are folded in: a thread folds its 32 values per (row, key tile) in increasing column
-// order, then the 4 lanes of the quad merge theirs by shuffles.
+// not depend on the order the values are folded in: a thread folds its 32 values per (row, key tile) into the maximum and
+// the second value on min / max alone, the 4 lanes of the quad merge theirs by shuffles, and only then does each lane look
+// for the quad's maximum among its values; the smallest of the four lanes' first columns holding it is the token.
 constexpr int XW_GEMM_BN = 2 * XW_TILE;   // N tile of the coarse GEMM (m64n256 per consumer warpgroup)
 
 template <class Acc>   // float: fp16 pass, int: int8 pass
@@ -30,77 +31,116 @@ struct CoarseEpi {
   const float* rnorms;     // [T][P] token factor: 1 / |F[t][p]| (xw_rnorm_kernel; every norm is >= XW_MIN_NORM on this
                            // path), int8 pass: s_x / |F| (q_fac)
   const float* desc_norm;  // row factor 1 / max(|d|, XW_MIN_NORM) (fp16 pass), desc_norm[row] itself (int8 pass: s_d / |d|)
-  const int* grp_frame;
-  const int* grp_row0;
   const int* grp_map0;
   unsigned long long* key1;
   float* max2;
   int n_tiles, P;
 
-  struct Top2 { float m1, m2; int tok; };
-  static __device__ __forceinline__ void push(Top2& s, float v, int tok) {
-    s.m2 = fmaxf(s.m2, fminf(s.m1, v));
-    s.tok = v > s.m1 ? tok : s.tok;      // strict: tokens come in increasing order, the first one holding the maximum stays
-    s.m1 = fmaxf(s.m1, v);
+  // per tile, read when the tile starts: the token factors of columns n0 + t and n0 + t + 128 (0 past the end of the map),
+  // and for the row this thread writes (r + 8 (q >> 1), below) its row factor and its first map
+  struct Pre { float2 col; float dv; int map0; };
+  __device__ __forceinline__ Pre begin(const TcTile& tl, int t, int r) const {
+    const float* rn = rnorms + (size_t)tl.batch * P;
+    const int c0 = tl.n0 + t, c1 = c0 + XW_TILE;
+    const int rr = r + 8 * ((threadIdx.x & 3) >> 1);
+    Pre p;
+    p.col = make_float2(c0 < P ? __ldg(rn + c0) : 0.f, c1 < P ? __ldg(rn + c1) : 0.f);
+    p.dv = rr < tl.m ? __ldg(desc_norm + tl.row0 + rr) : 0.f;
+    p.map0 = __ldg(grp_map0 + tl.g);
+    return p;
   }
-  static __device__ __forceinline__ void merge(Top2& s, float m1, float m2, int tok) {   // equal maxima -> the smaller token
-    s.m2 = fmaxf(fmaxf(s.m2, m2), fminf(s.m1, m1));
-    const bool take = m1 > s.m1 || (m1 == s.m1 && tok < s.tok);
-    s.tok = take ? tok : s.tok;
-    s.m1 = fmaxf(s.m1, m1);
+  static __device__ __forceinline__ float as_float(Acc a) {
+    if constexpr (kS8) return __int_as_float(a); else return a;
   }
-  // the token factors of columns n0 + t and n0 + t + 128 (0 past the end of the map)
-  __device__ __forceinline__ float2 column(int g, int n0, int t) const {
-    const float* rn = rnorms + (size_t)grp_frame[g] * P;
-    const int c0 = n0 + t, c1 = c0 + XW_TILE;
-    return make_float2(c0 < P ? __ldg(rn + c0) : 0.f, c1 < P ? __ldg(rn + c1) : 0.f);
+  static __device__ __forceinline__ Acc from_float(float v) {
+    if constexpr (kS8) return __float_as_int(v); else return v;
   }
-  // folds key tile kh of the thread's two rows into s[0], s[1]; cols: the tile's token factors.  EDGE: the GEMM tile
-  // reaches past the end of the map
+  // Key tile kh of the thread's two rows, pass 1: forms the values, leaves them in acc as floats (int8 pass: their bits)
+  // and folds their maximum into m1[h] (row r + 8 h).  cols: the tile's token factors.  EDGE: the GEMM tile reaches past
+  // the end of the map
   template <bool EDGE>
-  __device__ __forceinline__ void fold(Top2 (&s)[2], int kh, const float* cols, int n0, int fc,
-                                       const Acc (&acc)[XW_GEMM_BN / 2]) const {
+  __device__ __forceinline__ void fold_max(float (&m1)[2], int kh, const float* cols, int n0, int fc,
+                                           Acc (&acc)[XW_GEMM_BN / 2]) const {
 #pragma unroll
     for (int ii = 0; ii < XW_TILE / 8; ++ii) {   // (constant trip count: acc must stay in registers)
       const int i = kh * XW_TILE / 8 + ii;
       const float2 rnv = tc::lds_f2(tc::smem_u32(cols + fc + 8 * i));
+      const int col = n0 + 8 * i + fc;
+      const bool ok0 = !EDGE || col < P, ok1 = !EDGE || col + 1 < P;   // columns past the end of the map never win
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int col = n0 + 8 * i + fc + j;
-        const bool ok = !EDGE || col < P;                // columns past the end of the map never win
-        const float f = j ? rnv.y : rnv.x;
-        push(s[0], ok ? (float)acc[4 * i + j] * f : -INFINITY, col);
-        push(s[1], ok ? (float)acc[4 * i + 2 + j] * f : -INFINITY, col);
+      for (int h = 0; h < 2; ++h) {
+        const float a = ok0 ? (float)acc[4 * i + 2 * h] * rnv.x : -INFINITY;
+        const float b = ok1 ? (float)acc[4 * i + 2 * h + 1] * rnv.y : -INFINITY;
+        acc[4 * i + 2 * h] = from_float(a);
+        acc[4 * i + 2 * h + 1] = from_float(b);
+        m1[h] = fmaxf(m1[h], fmaxf(a, b));
       }
     }
   }
-  __device__ __forceinline__ void fragment(int g, int r, int m, int n0, int fc, const Acc (&acc)[XW_GEMM_BN / 2],
-                                           const float* cols) const {
+  // Pass 2, once m1 is the quad's maximum of row r + 8 h: among the thread's values of key tile kh, m2 = the largest of
+  // those below m1, and pos records the columns holding m1.  One compare per value; its predicate selects the other two
+  // updates.  Matches come in decreasing column order c = 8 i + j, and each sets pos = pos / 512 + (c + 1) (a
+  // predicated FFMA, kept on the FMA pipe, where a predicated move or add would become an ALU-pipe SEL): the integer
+  // part of pos is 1 + the first column holding m1 (0: none), and pos has a fractional part iff m1 is held twice.
+  // pos < 257, so pos / 512 < 0.51 and the fraction, >= 2^-9 once set, survives the rounding of the sum (ulp <= 2^-15).
+  __device__ __forceinline__ void scan(float m1, int h, int kh, const Acc (&acc)[XW_GEMM_BN / 2], float& pos,
+                                       float& m2) const {
+    pos = 0.f;
+    m2 = -INFINITY;
+#pragma unroll
+    for (int ii = XW_TILE / 8 - 1; ii >= 0; --ii) {
+      const int i = kh * XW_TILE / 8 + ii;
+#pragma unroll
+      for (int j = 1; j >= 0; --j)
+        asm("{\n\t.reg .pred p;\n\t"
+            "setp.eq.f32 p, %2, %3;\n\t"
+            "@p fma.rn.f32 %0, %0, 0f3B000000, %4;\n\t"
+            "@!p max.f32 %1, %1, %2;\n\t}"
+            : "+f"(pos), "+f"(m2)
+            : "f"(as_float(acc[4 * i + 2 * h + j])), "f"(m1), "f"((float)(8 * i + j + 1)));
+    }
+  }
+  __device__ __forceinline__ void fragment(const TcTile& tl, int r, int fc, Acc (&acc)[XW_GEMM_BN / 2], const float* cols,
+                                           const Pre& pre) const {
     // after the quad's merge every lane holds all four results; lane q keeps and writes row r + 8 (q >> 1) of key tile
     // 2 (n0 / 256) + (q & 1)
-    const int q = threadIdx.x & 3;
+    const int q = threadIdx.x & 3, n0 = tl.n0;
     const bool edge = n0 + XW_GEMM_BN > P;
-    Top2 o;
+    float o1, o2;
+    int otok;
 #pragma unroll
     for (int kh = 0; kh < 2; ++kh) {
-      Top2 s[2] = {{-INFINITY, -INFINITY, 0x7fffffff}, {-INFINITY, -INFINITY, 0x7fffffff}};   // rows r, r + 8
-      if (edge) fold<true>(s, kh, cols, n0, fc, acc);
-      else fold<false>(s, kh, cols, n0, fc, acc);
+      float m1[2] = {-INFINITY, -INFINITY};   // rows r, r + 8
+      if (edge) fold_max<true>(m1, kh, cols, n0, fc, acc);
+      else fold_max<false>(m1, kh, cols, n0, fc, acc);
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int sh = 1; sh <= 2; sh <<= 1)
-          merge(s[h], __shfl_xor_sync(0xffffffffu, s[h].m1, sh), __shfl_xor_sync(0xffffffffu, s[h].m2, sh),
-                __shfl_xor_sync(0xffffffffu, s[h].tok, sh));
-      if ((q & 1) == kh) o = (q >> 1) ? s[1] : s[0];
+        for (int sh = 1; sh <= 2; sh <<= 1) m1[h] = fmaxf(m1[h], __shfl_xor_sync(0xffffffffu, m1[h], sh));
+        float pos, m2;
+        scan(m1[h], h, kh, acc, pos, m2);
+        const int ip = (int)pos;   // (truncates)
+        int tok = ip ? n0 + fc + ip - 1 : 0x7fffffff;
+        int cnt = (ip != 0) + ((float)ip != pos);   // 0, 1, or 2 for "at least two"
+#pragma unroll
+        for (int sh = 1; sh <= 2; sh <<= 1) {
+          tok = min(tok, __shfl_xor_sync(0xffffffffu, tok, sh));
+          cnt += __shfl_xor_sync(0xffffffffu, cnt, sh);
+          m2 = fmaxf(m2, __shfl_xor_sync(0xffffffffu, m2, sh));
+        }
+        if ((q & 1) == kh && (q >> 1) == h) {
+          o1 = m1[h];
+          o2 = cnt > 1 ? m1[h] : m2;   // the maximum held twice is also the second value
+          otok = tok;
+        }
+      }
     }
     const int rr = r + 8 * (q >> 1), nt = n0 / XW_TILE + (q & 1);
-    if (rr >= m || nt >= n_tiles) return;   // padding row, or a key tile lying completely past the end of the map
-    const float dv = desc_norm[grp_row0[g] + rr];
-    const float rdn = kS8 ? dv : __fdividef(1.f, fmaxf(dv, XW_MIN_NORM));
-    const size_t off = (size_t)(grp_map0[g] + rr) * n_tiles + nt;
-    key1[off] = ((unsigned long long)__float_as_uint(fmaxf(o.m1 * rdn, 0.f)) << 32) | (unsigned)(0x7fffffff - o.tok);
-    max2[off] = fmaxf(o.m2 * rdn, 0.f);
+    if (rr >= tl.m || nt >= n_tiles) return;   // padding row, or a key tile lying completely past the end of the map
+    const float rdn = kS8 ? pre.dv : __fdividef(1.f, fmaxf(pre.dv, XW_MIN_NORM));
+    const size_t off = (size_t)(pre.map0 + rr) * n_tiles + nt;
+    key1[off] = ((unsigned long long)__float_as_uint(fmaxf(o1 * rdn, 0.f)) << 32) | (unsigned)(0x7fffffff - otok);
+    max2[off] = fmaxf(o2 * rdn, 0.f);
   }
 };
 
@@ -135,11 +175,11 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
   if (desc_q8) {
     DTK_CHECK_ARG(fv.s8() && fv.C % 16 == 0 && fv.C <= XW_S8_MAX_C, "int8 coarse pass: needs the int8 features, C %% 16 == 0 "
                   "and C <= %d", XW_S8_MAX_C);
-    CoarseEpi<int> epi{fv.q_fac, desc_fac, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
+    CoarseEpi<int> epi{fv.q_fac, desc_fac, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
     return tc_launch<TcMode::S8, CoarseEpi<int>, XW_GEMM_BN, true>({desc_q8, nullptr, (uint64_t)desc_rows, 0, fv.q8, nullptr,
                                                                     (uint64_t)fv.T, 0}, pb, max_tiles, epi, st, PROF_XW_COARSE);
   }
-  CoarseEpi<float> epi{rnorms, desc_norm, grp_frame, grp_row0, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
+  CoarseEpi<float> epi{rnorms, desc_norm, grp_map0, xc.key1, xc.max2, cdiv(fv.P, XW_TILE), fv.P};
   return tc_launch<TcMode::F16, CoarseEpi<float>, XW_GEMM_BN, true>({desc_hi, nullptr, (uint64_t)desc_rows, 0, fv.hi, nullptr,
                                                                      (uint64_t)fv.T, 0}, pb, max_tiles, epi, st, PROF_XW_COARSE);
 }
