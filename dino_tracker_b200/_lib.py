@@ -274,11 +274,14 @@ def quantise_s8(x, norms, rows_per_group, stream):
     return q, fac, rho, rho_max
 
 
+S8_MAX_C = 2048   # csrc/xwin.cuh XW_S8_MAX_C: the widest feature the int8 coarse pass takes
+
+
 def quantise_features(tpc, norms, stream):
     """(q8 [T][P][C], fac [T][P], rho_f [T]) of a [T][P][C] feature video: the int8 operands of the anchor phase's coarse
-    pass, or None where that pass cannot run (C not a multiple of 16 or above 1040)."""
+    pass, or None where that pass cannot run (C not a multiple of 16 or above S8_MAX_C)."""
     T, P, C = tpc.shape
-    if C % 16 or C > 1040:
+    if C % 16 or C > S8_MAX_C:
         return None
     q, fac, _, rho_f = quantise_s8(tpc, norms, P, stream)
     return q, fac, rho_f

@@ -182,7 +182,7 @@ __global__ void anchor_scalars_kernel(int T, const int* __restrict__ qlist, int 
                                       const int* __restrict__ grp_row0, const int* __restrict__ grp_map0,
                                       const int* __restrict__ grp_item0, int n_groups, int n_maps, int n_unique, int chunk_row0,
                                       const float* __restrict__ u_norm, const int* __restrict__ u_flag,
-                                      const float* __restrict__ u_rho, const float* __restrict__ rho_f, bool with_eps,
+                                      const float* __restrict__ u_rho, const float* __restrict__ rho_f, float eps_slack, bool with_eps,
                                       int* __restrict__ out_index, int* __restrict__ arow, float* __restrict__ dnorm,
                                       float* __restrict__ desc_eps) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -198,7 +198,7 @@ __global__ void anchor_scalars_kernel(int T, const int* __restrict__ qlist, int 
   arow[j] = r0 < n_unique ? r0 + (j - grp_map0[lo]) : chunk_row0 + j;
   if (u_flag[u]) return;   // sampled per work item: gather_anchor_kernel writes the norm and eps
   dnorm[j] = u_norm[u];
-  if (with_eps) desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[a]);
+  if (with_eps) desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[a], eps_slack);
 }
 
 // descriptors (fp16 hi / lo; with desc_q8: + the int8 row and its factor) of the GATHERED maps of one chunk of anchor work
@@ -213,7 +213,7 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
                                      const __half* __restrict__ u_lo, const int* __restrict__ u_flag,
                                      float* __restrict__ dnorm, __half* __restrict__ desc_hi,
                                      __half* __restrict__ desc_lo, const int8_t* __restrict__ u_q8,
-                                     const float* __restrict__ u_fac, const float* __restrict__ rho_f,
+                                     const float* __restrict__ u_fac, const float* __restrict__ rho_f, float eps_slack,
                                      int8_t* __restrict__ desc_q8, float* __restrict__ desc_fac,
                                      float* __restrict__ desc_eps) {
   const int j = map_lo + blockIdx.x;
@@ -248,7 +248,7 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
   sample_point(tpc, C, P, c, f0, f1, nullptr, dnorm + j, desc_hi + (size_t)j * C, desc_lo + (size_t)j * C);
   if (desc_q8) {
     const float r = quant_desc(desc_hi + (size_t)j * C, desc_lo + (size_t)j * C, C, dnorm + j, desc_q8 + (size_t)j * C, desc_fac + j);
-    if (threadIdx.x == 0) desc_eps[j] = xw_eps_s8(r, rho_f[a]);
+    if (threadIdx.x == 0) desc_eps[j] = xw_eps_s8(r, rho_f[a], eps_slack);
   }
 }
 
@@ -1039,14 +1039,14 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         {
           ProfRange pr(PROF_SAMPLE, sb);
           anchor_scalars_kernel<<<cdiv(cm.used, 256), 256, 0, sb>>>(T, d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, cm.used,
-                                                                   n_unique, x.row0, u_norm, u_flag, u_rho, fv.q_rho, s8, x.out_index,
+                                                                   n_unique, x.row0, u_norm, u_flag, u_rho, fv.q_rho, xw_s8_slack(C), s8, x.out_index,
                                                                    x.arow, x.norm, x.eps);
           DTK_LAUNCHED();
           if (cm.n_gathered > 0) {
             const size_t r0 = (size_t)x.row0;
             gather_anchor_kernel<<<cm.gather_hi - cm.gather_lo, SAMPLE_THREADS, 0, sb>>>(
                 tpc, T, C, P, g->h, g->w, pa, traj, d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, n_unique, cm.gather_lo, fb, u_hi, u_lo, u_flag,
-                                                                    x.norm, u_hi + r0 * C, u_lo + r0 * C, u_q8, u_fac, fv.q_rho,
+                                                                    x.norm, u_hi + r0 * C, u_lo + r0 * C, u_q8, u_fac, fv.q_rho, xw_s8_slack(C),
                                                                     s8 ? u_q8 + r0 * C : nullptr, u_fac + r0, x.eps);
             DTK_LAUNCHED();
           }

@@ -1,6 +1,6 @@
 // DINOv2 ViT feature extractor (SURVEY.md 8a row a1): ImageNet normalisation, 14x14 / stride-7 patch embedding,
-// cls + interpolated position embedding, pre-LN blocks (LayerNorm eps 1e-6, MHA scale 1/8, LayerScale, MLP 4x with
-// exact GELU, or ViT-g/14's SwiGLU MLP), tap = output of block `layer` before the final norm -- or that block's query /
+// cls + interpolated position embedding, pre-LN blocks (LayerNorm eps 1e-6, MHA scale 1/8, LayerScale -- none in DINO v1's
+// 8 x 8-patch ViT-S/8 and ViT-B/8 --, MLP 4x with exact GELU, or ViT-g/14's SwiGLU MLP), tap = output of block `layer` before the final norm -- or that block's query /
 // key / value facet, its qkv Linear output -- cls dropped, written straight into the
 // token-major feature video [T][P][C]   (models/extractor.py:41-85,137-150,224-266; utils.py:32-72; the block arithmetic is
 // facebookresearch/dinov2's -- parity unpinned, see DESIGN.md).
@@ -293,6 +293,32 @@ struct EpiResidual : EpiBase {
   }
 };
 
+// x[r][col] += acc + bias[col]: the residual of a block without LayerScale (DINO v1; the host passes ls = nullptr).  A
+// type of its own, so that the LayerScale launches keep their kernels; the sums are those of EpiResidual with ls = 1.
+struct EpiResidualNoLS : EpiBase {
+  static constexpr bool kCoalesced = true;
+  static constexpr bool kPrefetch = true;
+  float* x; const float* bias; int D;
+  __device__ __forceinline__ float4 fetch(int, int r, int col) const { return *reinterpret_cast<const float4*>(x + (size_t)r * D + col); }
+  __device__ __forceinline__ void vec4(int, int r, int col, float4 v, float4 xv) const {
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col));
+    xv.x += v.x + bb.x; xv.y += v.y + bb.y; xv.z += v.z + bb.z; xv.w += v.w + bb.w;
+    *reinterpret_cast<float4*>(x + (size_t)r * D + col) = xv;
+  }
+  __device__ __forceinline__ void vec4(int g, int r, int col, float4 v) const { vec4(g, r, col, v, fetch(g, r, col)); }
+  __device__ __forceinline__ void operator()(State&, int, int r, int col0, const float (&f)[32], int ncols) const {
+    float* o = x + (size_t)r * D + col0;
+#pragma unroll
+    for (int i = 0; i < 32; i += 4)
+      if (i < ncols) {
+        const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col0 + i));
+        float4 xv = *reinterpret_cast<const float4*>(o + i);
+        xv.x += f[i] + bb.x; xv.y += f[i + 1] + bb.y; xv.z += f[i + 2] + bb.z; xv.w += f[i + 3] + bb.w;
+        *reinterpret_cast<float4*>(o + i) = xv;
+      }
+  }
+};
+
 // 0.5 x (1 + erf(x / sqrt 2)) with erf by Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, two MUFU + 9 FMA-pipe
 // instructions, branch-free): libdevice's erff is ~3x the instructions and made the fc1 epilogue, not its MMAs, pace that
 // GEMM.  The result is rounded to fp16 (relative 4.9e-4) right after.
@@ -539,16 +565,21 @@ static int vit_qkv_fused(const VitShape& s, const TcPlan& pl, const void* y, con
                : tc_launch<TcMode::TF32, EpiQKV16>(op, pb, tiles, eq, st, PROF_VIT_GEMM);
 }
 
-// x[r] += ls * (a[r] . w^T + bias), a [rows][K]: proj (K = D) and fc2 (K = 4 D)
-static int vit_residual(const VitShape& s, const TcPlan& pl, const void* a, const void* w, int K, const float* bias,
-                        const float* ls, float* x, cudaStream_t st) {
-  EpiResidual er{{}, x, bias, ls, s.D};
+// x[r] += ls * (a[r] . w^T + bias), a [rows][K]: proj (K = D) and fc2 (K = 4 D); ls = nullptr: no LayerScale
+template <class Epi>
+static int vit_residual_launch(const VitShape& s, const TcPlan& pl, const void* a, const void* w, int K, const Epi& er,
+                               cudaStream_t st) {
   const TcOperands op = linear_operands(a, s.rows, w);
   const TcProblem pb = pl.problem(1, s.D, K);
   const int tiles = cdiv((int)s.rows, TC_BM);
-  return s.pairs ? tc_launch<TcMode::F16, EpiResidual, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), er, st, PROF_VIT_GEMM)
-       : s.f16 ? tc_launch<TcMode::F16, EpiResidual>(op, pb, tiles, er, st, PROF_VIT_GEMM)
-               : tc_launch<TcMode::TF32, EpiResidual>(op, pb, tiles, er, st, PROF_VIT_GEMM);
+  return s.pairs ? tc_launch<TcMode::F16, Epi, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), er, st, PROF_VIT_GEMM)
+       : s.f16 ? tc_launch<TcMode::F16, Epi>(op, pb, tiles, er, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, Epi>(op, pb, tiles, er, st, PROF_VIT_GEMM);
+}
+static int vit_residual(const VitShape& s, const TcPlan& pl, const void* a, const void* w, int K, const float* bias,
+                        const float* ls, float* x, cudaStream_t st) {
+  if (!ls) return vit_residual_launch(s, pl, a, w, K, EpiResidualNoLS{{}, x, bias, s.D}, st);
+  return vit_residual_launch(s, pl, a, w, K, EpiResidual{{}, x, bias, ls, s.D}, st);
 }
 
 // h = gelu(y . fc1_w^T + bias), y [rows][D] -> h [rows][4 D] (fp16 in fp16 operand mode)
@@ -649,8 +680,7 @@ int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom
   DTK_CHECK_ARG(c->swiglu_hidden >= 0 && c->swiglu_hidden % 8 == 0, "vit_stage: swiglu_hidden must be a multiple of 8");
   DTK_CHECK_ARG(stage != DINOTRK_VIT_SWIGLU || c->swiglu_hidden > 0, "vit_stage: the SwiGLU stage needs swiglu_hidden > 0");
   DTK_CHECK_ARG(stage == DINOTRK_VIT_LAYERNORM || w, "vit_stage: null weight");
-  DTK_CHECK_ARG(stage == DINOTRK_VIT_QKV || stage == DINOTRK_VIT_FC1 || stage == DINOTRK_VIT_SWIGLU || p1,
-                "vit_stage: null second parameter vector");
+  DTK_CHECK_ARG((stage != DINOTRK_VIT_LAYERNORM && stage != DINOTRK_VIT_PATCH) || p1, "vit_stage: null second parameter vector");
   DTK_CHECK_ARG(stage != DINOTRK_VIT_QKV || (out1 && out2), "vit_stage: qkv needs q, k and v^T");
   DTK_CHECK_ARG(workspace && workspace_bytes >= DINOTRK_VIT_STAGE_WORKSPACE_BYTES, "vit_stage: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
@@ -740,6 +770,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   for (int l = 0; l <= c->tap_layer; ++l) {
     const float* const* w = wt->blocks + (size_t)l * 14;
     // w: 0 norm1.w 1 norm1.b 2 qkv.w 3 qkv.b 4 proj.w 5 proj.b 6 ls1 7 norm2.w 8 norm2.b 9 fc1.w 10 fc1.b 11 fc2.w 12 fc2.b 13 ls2
+    // (ls1 / ls2 null: no LayerScale, DINO v1)
     // (the four weight matrices are fp16 arrays in fp16 operand mode; SwiGLU: 9-12 are w12.w, w12.b, w3.w, w3.b)
     if ((rc = vit_layernorm(s, x, w[0], w[1], y, st))) return rc;
     if ((rc = vit_row_plan(s, pl, st))) return rc;

@@ -13,7 +13,7 @@ namespace dtk {
 // per 256-column GEMM tile: key1 = bits(max) << 32 | (0x7fffffff - first token holding it), max2 = second largest value
 // (>= 0).  Values are the same expression as the exact path, relu(acc / max(|d| |F|, 1e-8)), with a fast division (its
 // error is part of XW_EPS).  The int8 pass forms the same statistics of acc * fac_x * fac_d from its exact int32
-// accumulators (converted exactly: C <= XW_S8_MAX_C).
+// accumulators (their conversion to float is exact up to C = 1040; above, eps's slack covers its rounding, xwin.cuh).
 //
 // A fragment epilogue (tcgemm.cuh): it works on the accumulator registers of all eight consumer warps; the tile's token
 // factors come from shared memory, where the GEMM body staged them (begin()).  Per element only u = acc * (1 / |F|) is
@@ -999,12 +999,12 @@ __global__ void xw_tile_prefix_kernel(const int* __restrict__ grp_m, int n_group
   if (lane == 0) tile_start[n_groups] = base;
 }
 
-// eps[row] = xw_eps_s8(rho[row], rho_f[frame]) over the rows of group blockIdx.x
+// eps[row] = xw_eps_s8(rho[row], rho_f[frame], slack) over the rows of group blockIdx.x
 __global__ void xw_eps_kernel(const int* __restrict__ grp_frame, const int* __restrict__ grp_row0, const int* __restrict__ grp_m,
-                              const float* __restrict__ rho, const float* __restrict__ rho_f, float* __restrict__ eps) {
+                              const float* __restrict__ rho, const float* __restrict__ rho_f, float slack, float* __restrict__ eps) {
   const int g = blockIdx.x, r0 = grp_row0[g];
   const float rf = rho_f[grp_frame[g]];
-  for (int r = threadIdx.x; r < grp_m[g]; r += blockDim.x) eps[r0 + r] = xw_eps_s8(rho[r0 + r], rf);
+  for (int r = threadIdx.x; r < grp_m[g]; r += blockDim.x) eps[r0 + r] = xw_eps_s8(rho[r0 + r], rf, slack);
 }
 
 }  // namespace dtk
@@ -1068,7 +1068,7 @@ int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* 
     xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, tile_start);
     DTK_LAUNCHED();
     if (eps) {
-      xw_eps_kernel<<<n_groups, 128, 0, st>>>(grp_frame, grp_row0, grp_m, desc_rho, fv.q_rho, eps);
+      xw_eps_kernel<<<n_groups, 128, 0, st>>>(grp_frame, grp_row0, grp_m, desc_rho, fv.q_rho, xw_s8_slack(fv.C), eps);
       DTK_LAUNCHED();
     }
   }

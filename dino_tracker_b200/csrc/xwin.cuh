@@ -45,19 +45,36 @@ constexpr int XW_TILE = 128;          // tokens per coarse key (half of the coar
 
 // ---- int8 coarse operands.  Per row x (token or descriptor): s = max|x_k| / 127, q = rint(x / s) in [-127, 127],
 // fac = s / max(|x|, XW_MIN_NORM) (the coarse epilogue's factor), rho = |x - s q| / |x| rounded up (0 for x = 0).
-// The coarse value of a map is <q_d, q_x> fac_d fac_x (int32 accumulation: exact while C 127^2 < 2^24).
+// The coarse value of a map is <q_d, q_x> fac_d fac_x (int32 accumulation: exact while C 127^2 < 2^31; its conversion to
+// float, cvt.rn.f32.s32, is exact while C 127^2 < 2^24, i.e. C <= 1040, and above that rounds by <= 2^-24 |<q_d, q_x>|).
 // |<d, x> - <s_d q_d, s_x q_x>| <= |<d - d^, x>| + |<d^, x - x^>| <= (rho_d + (1 + rho_d) rho_x) |d| |x|, so in cosine
-// units |coarse - exact| <= xw_eps_s8(rho_d, rho_F) with rho_F the largest rho_x of the map's frame.  XW_S8_SLACK covers
-// the exact split path's own error (2^-21 + 64 truncating adds x 2^-23, DESIGN.md 3.1) and the epilogue's fp32 roundings.
+// units |coarse - exact| <= xw_eps_s8(rho_d, rho_F, xw_s8_slack(C)) with rho_F the largest rho_x of the map's frame.
+// The slack covers the exact split path's own error -- 2^-21 from the operand split plus one truncating accumulator add
+// (<= 2^-23 of the running magnitude) per wgmma, three wgmma (lo hi, hi lo, hi hi) per 16 channels: 3 ceil(C / 16) adds,
+// DESIGN.md 3.1 -- the epilogue's four fp32 roundings and, above C = 1040, the accumulator's conversion:
+// |<q_d, q_x>| s_d s_x <= |d^| |x^| <= (1 + rho_d)(1 + rho_x) |d| |x|, so <= 2^-24 (1 + rho_d)(1 + rho_F) in cosine units,
+// with rho <= sqrt(C) / 254 (each residual is <= s / 2 and |x| >= 127 s).
+//   C <= 1040: 2^-21 + 195 x 2^-23 + 4 x 2^-24 x 1.27 = 2.4e-5 <= XW_S8_SLACK = 2^-15 = 3.05e-5.
+//   C > 1040:  XW_S8_SLACK + 3 ceil(C / 16) 2^-23: the adds explicitly, and 2^-15 for the rest (2^-21 + 5 x 2^-24 x 1.39
+//              = 8.9e-7 at C = 2048).
 constexpr float XW_S8_SLACK = 3.0518e-5f;   // 2^-15
-constexpr int XW_S8_MAX_C = 1040;           // C 127^2 < 2^24: the int32 -> float conversion of an accumulator is exact
+constexpr int XW_S8_EXACT_C = 1040;         // C 127^2 < 2^24: the conversion is exact and XW_S8_SLACK alone suffices
+// the widest feature the ViT stage writes (dinotrk_vit_forward: dim <= 2048; ViT-g/14: 1536)
+constexpr int XW_S8_MAX_C = 2048;
+// slack of xw_eps_s8 for C channels (see above), rounded up to float; exactly XW_S8_SLACK for C <= XW_S8_EXACT_C
+inline float xw_s8_slack(int C) {
+  if (C <= XW_S8_EXACT_C) return XW_S8_SLACK;
+  const double s = (double)XW_S8_SLACK + 3.0 * (double)((C + 15) / 16) * 0x1p-23;
+  const float f = (float)s;
+  return (double)f < s ? nextafterf(f, INFINITY) : f;
+}
 // rho_F above which the automatic mode runs the fp16 coarse pass: eps ~ 2 rho_F, and 2 eps is the candidate margin.  At
 // 0.03 (twice the largest token residual of Gaussian-like features at C = 1024, 0.0132) the margin stays below ~0.13,
 // under the typical gap between a map's maximum and the next value of another tile; features with outlier channels
 // (max |x| / rms far above Gaussian) exceed it and keep the fp16 pass.
 constexpr float XW_S8_RHO_MAX = 0.03f;
-__device__ __forceinline__ float xw_eps_s8(float rho_d, float rho_f) {
-  return __fadd_ru(__fadd_ru(rho_d, __fmul_ru(__fadd_ru(1.f, rho_d), rho_f)), XW_S8_SLACK);
+__device__ __forceinline__ float xw_eps_s8(float rho_d, float rho_f, float slack) {
+  return __fadd_ru(__fadd_ru(rho_d, __fmul_ru(__fadd_ru(1.f, rho_d), rho_f)), slack);
 }
 
 // One warp quantises row x (element k = ld(k), C % 4 == 0) with fp32 norm `norm` (the exact path's): writes q[C], *fac

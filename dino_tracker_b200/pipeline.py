@@ -16,11 +16,13 @@ from .vit import DinoV2Features
 
 def build_tracker_from_video(video01, vit: DinoV2Features, device="cuda:0", ckpt_path="", delta_channels=None,
                              corr_precision="fp16x3") -> Tracker:
-    """video01: T x 3 x H x W in [0, 1].  Runs the ViT stage in-process and hands its [T][P][C] output to a Tracker."""
+    """video01: T x 3 x H x W in [0, 1].  Runs the ViT stage in-process and hands its [T][P][C] output to a Tracker with
+    the backbone's patch and stride (the token centres: 8-pixel patches put them at 4 + 7 c, 14-pixel ones at 7 + 7 c)."""
     tpc = vit(video01)                                   # [T][P][C] on the GPU
     T, P, C = tpc.shape
     model = Tracker(video=video01.to(device), ckpt_path=ckpt_path, device=device, delta_channels=delta_channels,
-                    corr_precision=corr_precision, dino_embed_video=torch.empty(0), _adopt_tpc=tpc)
+                    corr_precision=corr_precision, dino_embed_video=torch.empty(0), _adopt_tpc=tpc,
+                    dino_patch_size=vit.patch, stride=vit.stride)
     return model
 
 

@@ -9,7 +9,9 @@ DINOv2 state dict (hub key names, so real checkpoints load unchanged), the posit
 interpolated once at load time with the reference's formula, and every frame batch is one
 ``dinotrk_vit_forward`` call that writes token-major features ``[T][P][C]`` directly.  The query / key / value
 facets (the reference's qkv hook, ``models/extractor.py:224-266``) and ViT-g/14's SwiGLU feed-forward run on the same
-call.
+call.  DINO v1's ViT-S/8 and ViT-B/8 (``torch.hub.load('facebookresearch/dino:main', name)`` in the reference) load from
+their hub state dict, whose blocks have no LayerScale; their 8-pixel patch comes from the model name, as the reference's
+``get_patch_size`` derives it (``models/extractor.py:168-169``).
 """
 import ctypes
 import math
@@ -24,7 +26,10 @@ CONFIGS = {  # name: (depth, dim, heads)
     "dinov2_vitb14": (12, 768, 12),
     "dinov2_vitl14": (24, 1024, 16),
     "dinov2_vitg14": (40, 1536, 24),
+    "dino_vits8": (12, 384, 6),
+    "dino_vitb8": (12, 768, 12),
 }
+_LAYERSCALE = ("ls1.gamma", "ls2.gamma")   # absent from DINO v1 blocks: a null table entry (no LayerScale)
 _BLOCK_KEYS = ("norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.bias", "attn.proj.weight",
                "attn.proj.bias", "ls1.gamma", "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias",
                "mlp.fc2.weight", "mlp.fc2.bias", "ls2.gamma")
@@ -42,13 +47,16 @@ def interleave_w12(t):
     return torch.cat((x1, x2), dim=1).reshape(t.shape).contiguous()
 
 
-def interpolate_pos_embed(pos_embed, n_h, n_w):
+def interpolate_pos_embed(pos_embed, n_h, n_w, square_image=None):
     """models/extractor.py:57-85 (DINOv2 passes (w=H_img, h=W_img)): bicubic, +0.1 trick, align_corners=False,
-    recompute_scale_factor=False.  Host-side, once per (model, resolution)."""
+    recompute_scale_factor=False.  Host-side, once per (model, resolution).  The reference returns the table unchanged
+    only when the grid has N tokens AND the frame is square in pixels (``npatch == N and w == h``); ``square_image``
+    passes that second condition (None: taken as n_h == n_w, which agrees whenever the frame is square or the grid is
+    not N tokens)."""
     N = pos_embed.shape[1] - 1
     dim = pos_embed.shape[-1]
     side = int(math.sqrt(N))
-    if n_h * n_w == N and n_h == n_w:
+    if n_h * n_w == N and (n_h == n_w if square_image is None else square_image):
         return pos_embed
     cls_pos = pos_embed[:, 0]
     patch_pos = pos_embed[:, 1:].reshape(1, side, side, dim).permute(0, 3, 1, 2)
@@ -60,24 +68,38 @@ def interpolate_pos_embed(pos_embed, n_h, n_w):
     return torch.cat((cls_pos[:, None], patch_pos), dim=1)
 
 
+def patch_size(model_name):
+    """models/extractor.py:168-169: 8 for a name containing '8' (DINO v1 ViT-S/8, ViT-B/8), else 14."""
+    return 8 if "8" in model_name else 14
+
+
 class DinoV2Features(torch.nn.Module):
     """``VitExtractor`` replacement: ``forward(video01)`` -> token-major features [T][P][C] on the GPU.
 
     ``facet``: 'tokens' (block ``layer``'s output), or 'queries' / 'keys' / 'values' (that block's qkv Linear
     output, the reference's qkv hook, ``models/extractor.py:124-128,224-266``).  A state dict whose blocks carry
-    ``mlp.w12.*`` / ``mlp.w3.*`` (ViT-g/14) runs the SwiGLU feed-forward; its hidden width is read from ``w3``."""
+    ``mlp.w12.*`` / ``mlp.w3.*`` (ViT-g/14) runs the SwiGLU feed-forward; its hidden width is read from ``w3``.  A state
+    dict without ``ls1.gamma`` / ``ls2.gamma`` (DINO v1) runs its blocks without LayerScale.  ``patch`` must match the
+    patch embedding's kernel (``from_name`` takes it from the model name)."""
 
     def __init__(self, state_dict, heads, layer=None, stride=7, patch=14, device="cuda:0", frames_per_call=2,
                  attention="fused", cta_pairs=True, facet="tokens"):
         super().__init__()
         if facet not in FACETS:
             raise ValueError(f"facet {facet} not supported")
+        self.depth = 1 + max(int(k.split(".")[1]) for k in state_dict if k.startswith("blocks."))
+        kernel = tuple(state_dict["patch_embed.proj.weight"].shape[-2:])
+        if kernel != (patch, patch):
+            raise ValueError(f"patch embedding of {kernel} pixels, patch={patch}")
+        self.layerscale = "blocks.0.ls1.gamma" in state_dict
+        for i in range(self.depth):
+            if any((f"blocks.{i}.{k}" in state_dict) != self.layerscale for k in _LAYERSCALE):
+                raise ValueError(f"block {i}: LayerScale weights must be present in every block or in none")
         self._dev = _lib.require_cuda(device)
         self._lib = _lib.load()
         sd = {k: v.detach().to(self._dev, torch.float32).contiguous() for k, v in state_dict.items()}
         self.dim = sd["cls_token"].shape[-1]
         self.heads = heads
-        self.depth = 1 + max(int(k.split(".")[1]) for k in sd if k.startswith("blocks."))
         self.layer = self.depth - 1 if layer is None else layer
         self.stride, self.patch = stride, patch
         self.frames_per_call = frames_per_call
@@ -101,9 +123,11 @@ class DinoV2Features(torch.nn.Module):
             pw = F.pad(pw, (0, mult - pw.shape[1] % mult))
         self._patch_w = pw.to(wdt).contiguous()
         keys = _SWIGLU_KEYS if self.swiglu_hidden else _BLOCK_KEYS
-        self._blocks = [sd[f"blocks.{i}.{k}"].to(wdt).contiguous() if k in mats else sd[f"blocks.{i}.{k}"]
+        self._blocks = [None if k in _LAYERSCALE and not self.layerscale else
+                        sd[f"blocks.{i}.{k}"].to(wdt).contiguous() if k in mats else sd[f"blocks.{i}.{k}"]
                         for i in range(self.depth) for k in keys]
-        self._block_ptrs = (ctypes.c_void_p * len(self._blocks))(*[t.data_ptr() for t in self._blocks])
+        self._block_ptrs = (ctypes.c_void_p * len(self._blocks))(*[t.data_ptr() if t is not None else None
+                                                                    for t in self._blocks])
         self._pos_cache = {}
 
     def _swiglu_hidden(self, sd):
@@ -123,12 +147,12 @@ class DinoV2Features(torch.nn.Module):
     @classmethod
     def from_name(cls, model_name, state_dict, **kw):
         depth, dim, heads = CONFIGS[model_name]
-        return cls(state_dict, heads=heads, **kw)
+        return cls(state_dict, heads=heads, patch=patch_size(model_name), **kw)
 
-    def _pos(self, n_h, n_w):
-        key = (n_h, n_w)
+    def _pos(self, n_h, n_w, square_image):
+        key = (n_h, n_w, square_image)
         if key not in self._pos_cache:
-            pe = interpolate_pos_embed(self._sd["pos_embed"], n_h, n_w)[0]       # (1 + P) x D
+            pe = interpolate_pos_embed(self._sd["pos_embed"], n_h, n_w, square_image)[0]       # (1 + P) x D
             cls_pos = (self._sd["cls_token"][0, 0] + pe[0]).contiguous()
             self._pos_cache[key] = (cls_pos, pe[1:].contiguous())
         return self._pos_cache[key]
@@ -144,7 +168,7 @@ class DinoV2Features(torch.nn.Module):
         cfg = _lib.VitConfig(self.depth, self.dim, self.heads, self.layer, self.patch, self.stride,
                              0 if self.attention == "fused" else 1, 1 if self._f16 else 0, 1 if self.cta_pairs else 0,
                              self.swiglu_hidden, FACETS[self.facet])
-        cls_pos, pos = self._pos(geom.h, geom.w)
+        cls_pos, pos = self._pos(geom.h, geom.w, H == W)
         wt = _lib.VitWeights()
         wt.patch_w, wt.patch_b = self._patch_w.data_ptr(), self._sd["patch_embed.proj.bias"].data_ptr()
         wt.cls_pos, wt.pos = cls_pos.data_ptr(), pos.data_ptr()
@@ -173,10 +197,11 @@ def get_dino_features_video(video, model_name="dinov2_vitb14", facet="tokens", s
                             device="cuda:0", state_dict=None):
     """``utils.py::get_dino_features_video``: T x C x h x w on the CPU like the reference (``utils.py:53,67``), for
     ``facet`` in tokens / queries / keys / values (anything else raises ``ValueError`` as the reference does) and any
-    backbone of ``CONFIGS``.  ``layer=None``: the last block of ``state_dict``.  ``state_dict``: DINOv2 weights with hub
-    key names (the reference downloads them with torch.hub)."""
+    backbone of ``CONFIGS`` (DINOv2 at patch 14, DINO v1 ``dino_vits8`` / ``dino_vitb8`` at patch 8).  ``layer=None``: the
+    last block of ``state_dict``.  ``state_dict``: the backbone's weights with hub key names (the reference downloads
+    them with torch.hub)."""
     if facet not in FACETS:
         raise ValueError(f"facet {facet} not supported")
-    assert state_dict is not None, "pass the DINOv2 state dict (no network access here)"
+    assert state_dict is not None, "pass the backbone's state dict (no network access here)"
     ex = DinoV2Features.from_name(model_name, state_dict, layer=layer, stride=stride, device=device, facet=facet)
     return ex.features_chw(video).cpu()

@@ -55,7 +55,7 @@ typedef struct dinotrk_head_weights {
  * neither): the fp16 split of tpc ([T][P][C] halves each, x = hi + lo) produced by dinotrk_split_fp16; when
  * present the wide correlation groups run on the wgmma tensor cores (3-pass split precision,
  * fp32-faithful), otherwise on the exact-fp32 FFMA GEMM.  C must then be a multiple of 8.
- * q8 / q_fac / q_rho (optional, all or none; C a multiple of 16 and <= 1040): the int8 operands of the anchor phase's
+ * q8 / q_fac / q_rho (optional, all or none; C a multiple of 16 and <= 2048): the int8 operands of the anchor phase's
  * coarse pass, written by dinotrk_quantise_s8 with rows_per_group = h*w (q8 [T][P][C] int8, q_fac [T][P], q_rho [T] =
  * the largest relative residual of each frame).
  * hilo (optional, with hi / lo): the same split interleaved per 32 channels, written by dinotrk_split_hilo; the exact box
@@ -249,7 +249,8 @@ int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, 
 /* The same keys from the int8 pass: values relu(<desc_q8[j], feat->q8[frame][p]> desc_fac[j] feat->q_fac[frame][p])
  * (desc_q8 int8 [desc_rows][C], desc_fac [desc_rows], desc_rho [desc_rows]: dinotrk_quantise_s8 of the descriptors).
  * eps[j] (optional, float [desc_rows], rows of the groups only) receives the per-map bound on |coarse - exact cosine| the
- * plan uses, from desc_rho[j] and feat->q_rho[frame].  feat->q8, q_fac and q_rho are required.  Workspace: as above. */
+ * plan uses, from desc_rho[j], feat->q_rho[frame] and C (its slack grows with C above 1040).  feat->q8, q_fac and q_rho
+ * are required.  Workspace: as above. */
 int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_q8, const float* desc_fac,
                               const float* desc_rho, int desc_rows, const int* grp_frame, const int* grp_row0, const int* grp_m,
                               int n_groups, unsigned long long* key1, float* max2, float* eps, void* workspace,
@@ -354,7 +355,7 @@ int dinotrk_delta_train_backward(const float* frames, int B, int H, int W, const
 typedef struct dinotrk_vit_config {
   int depth, dim, heads;   /* ViT-L/14: 24, 1024, 16; ViT-B/14: 12, 768, 12 (head dim 64) */
   int tap_layer;           /* 0-based block whose output (before the final norm) is returned; 15 in the shipped config */
-  int patch, stride;       /* 14, 7 */
+  int patch, stride;       /* 14, 7 (DINOv2); 8, 7 (DINO v1 ViT-S/8, ViT-B/8) */
   int attn_materialized;   /* 0: fused wgmma attention (fp16 q/k/v/p, scores stay on the SM); 1: TF32 scores through a
                               workspace (tensor-core GEMM -> softmax -> tensor-core GEMM), validation path */
   int gemm_f16;            /* 1: linear layers on the fp16 tensor pipe -- patch_w and the qkv / proj / fc1 / fc2 weight matrices
@@ -374,7 +375,8 @@ typedef struct dinotrk_vit_config {
  * proj.b, ls1.gamma, norm2.w, norm2.b, fc1.w [4D][D], fc1.b, fc2.w [D][4D], fc2.b, ls2.gamma.  With swiglu_hidden = Hd
  * slots 9-12 hold w12.w [2Hd][D], w12.b [2Hd], w3.w [D][Hd], w3.b [D], where the rows of w12 (and its bias) are
  * interleaved in pairs of hidden units: rows 4q .. 4q+3 = x1 rows 2q, 2q+1, then x2 rows 2q, 2q+1 (hub layout: x1 rows
- * 0..Hd-1, x2 rows Hd..2Hd-1).  Every pointer is 16-byte aligned. */
+ * 0..Hd-1, x2 rows Hd..2Hd-1).  A null ls1.gamma / ls2.gamma (slots 6 / 13) means a block without LayerScale (DINO v1:
+ * x += proj(...), x += fc2(...)).  Every other pointer is non-null and every pointer is 16-byte aligned. */
 typedef struct dinotrk_vit_weights {
   const void* patch_w; const float* patch_b; const float* cls_pos; const float* pos;
   const float* const* blocks;
@@ -406,11 +408,12 @@ int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16
  *   QKV        y [rows][D] fp16, qkv_w [3D][D], bias [3D], -  -> q [B*heads][N1][64] fp16 multiplied by
  *              64^-1/2 * log2(e), k [B*heads][N1][64] fp16, vT [B*heads][64][N1p8] fp16 (v transposed, row pitch N1p8 =
  *              N1 rounded up to 8; columns N1..N1p8-1 are not written): dinotrk_vit_attention's inputs
- *   PROJ       y [rows][D] fp16, proj_w [D][D], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (y . proj_w + bias)
+ *   PROJ       y [rows][D] fp16, proj_w [D][D], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (y . proj_w + bias);
+ *              ls = NULL: x += y . proj_w + bias (no LayerScale)
  *   FC1        y [rows][D] fp16, fc1_w [4D][D], bias [4D], -  -> h [rows][4D] fp16 = gelu(y . fc1_w + bias) (exact GELU
  *              with erf to 1.5e-7)
  *   FC2        h [rows][Kh] fp16, fc2_w [D][Kh], bias [D], ls [D]  -> x [rows][D] fp32 += ls * (h . fc2_w + bias), with
- *              Kh = 4D, or Kh = c->swiglu_hidden when that is non-zero (the SwiGLU MLP's w3)
+ *              Kh = 4D, or Kh = c->swiglu_hidden when that is non-zero (the SwiGLU MLP's w3); ls = NULL as for PROJ
  *   SWIGLU     y [rows][D] fp16, w12_w [2Hd][D] (rows interleaved as in dinotrk_vit_weights), bias [2Hd] (interleaved
  *              alike), -  -> h [rows][Hd] fp16 = silu(x1) * x2, Hd = c->swiglu_hidden (> 0); the 2Hd-wide product is
  *              never stored

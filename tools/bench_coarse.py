@@ -4,7 +4,7 @@ shapes one steady-state chunk of BASELINE config 2 gives it.  GPU only.
   python tools/bench_coarse.py [--launches 100] [--windows 5] [--C 1024]
 
 Inputs: seeded feature video T = 50, P = 67 x 121 = 8107 tokens, C = 1024 (--C: another channel count, a multiple of
-16 up to 1040, so that the time per launch can be fitted against the reduction length: the intercept is the cost per tile
+16 up to 2048, so that the time per launch can be fitted against the reduction length: the intercept is the cost per tile
 that does not scale with K); one anchor-phase chunk of 32,750 descriptor rows.  With 256 queries that anchor in every
 frame, every anchor frame holds 256 x 50 = 12,800 work items; the chunk cap of 32,768 maps cut at whole cells (multiples
 of T) is 32,750, and the probe chunk (4,050 items) takes the start of frame 0.  So the first full chunk is frame 0's remaining 8,750 rows, all 12,800 of frame 1 and 11,200 of frame 2.
@@ -83,10 +83,10 @@ def main():
     ap.add_argument("--launches", type=int, default=100, help="launches per timed window (>= 20)")
     ap.add_argument("--windows", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--C", type=int, default=1024, help="feature channels (a multiple of 16, <= 1040)")
+    ap.add_argument("--C", type=int, default=1024, help="feature channels (a multiple of 16, <= 2048)")
     a = ap.parse_args()
     assert a.launches >= 20
-    assert a.C > 0 and a.C % 16 == 0 and a.C <= 1040, "--C: a multiple of 16 up to 1040 (the int8 pass's limits)"
+    assert a.C > 0 and a.C % 16 == 0 and a.C <= 2048, "--C: a multiple of 16 up to 2048 (the int8 pass's limits)"
     C = a.C
     assert torch.cuda.is_available(), "bench_coarse.py needs a CUDA device"
     dev = "cuda:0"
