@@ -42,7 +42,7 @@ struct BBEpi {
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       if (i < ncols) {
-        float v = __fdiv_rn(f[i], fmaxf(__fmul_rn(ns, __ldg(nt + i)), 1e-8f));
+        float v = corr_cos(f[i], ns, __ldg(nt + i));
         unsigned long long k = ((unsigned long long)f2ord(v) << 32) | (unsigned)(0x7fffffff - (col0 + i));
         if (k > s.k1) {
           if (s.k1 != 0ull) { s.v2 = ord2f((unsigned)(s.k1 >> 32)); s.i2 = 0x7fffffff - (int)(s.k1 & 0xffffffffu); }
@@ -99,7 +99,7 @@ __global__ void bb_resolve_kernel(const float* __restrict__ tpc, const float* __
       acc = fmaf(x.x, y.x, acc); acc = fmaf(x.y, y.y, acc); acc = fmaf(x.z, y.z, acc); acc = fmaf(x.w, y.w, acc);
     }
     acc = warp_sum(acc);
-    return __fdiv_rn(acc, fmaxf(__fmul_rn(norms[(size_t)fs * P + r], norms[(size_t)ft * P + col]), 1e-8f));
+    return corr_cos(acc, norms[(size_t)fs * P + r], norms[(size_t)ft * P + col]);
   };
   float e1 = exact(i1);
   if (i2 >= 0 && v1 - v2 < ambiguity) {   // near-tie under tensor-core rounding: decide in exact fp32

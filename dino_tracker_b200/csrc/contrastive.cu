@@ -61,7 +61,7 @@ __global__ void cl_bb_kernel(const float* __restrict__ desc, const float* __rest
   float d = 0.f;
   for (int c = lane; c < C; c += 32) d = fmaf(s[c], u[c], d);
   d = warp_sum(d);
-  if (lane == 0) bb[r] = __fdiv_rn(d, fmaxf(__fmul_rn(dn[r], dn[B + r]), 1e-8f));
+  if (lane == 0) bb[r] = corr_cos(d, dn[r], dn[B + r]);
 }
 
 // fixed-order block reduction (sum or max) of one value per thread

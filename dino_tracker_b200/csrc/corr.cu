@@ -143,7 +143,7 @@ corr_gemm_kernel(const float* __restrict__ tpc, const float* __restrict__ norms,
     for (int j = 0; j < 8; ++j) {
       int c = tx + 16 * j;
       if (c < n_valid) {
-        float v = __fdiv_rn(acc[i][j], fmaxf(__fmul_rn(dnv, fnv[j]), 1e-8f));
+        float v = corr_cos(acc[i][j], dnv, fnv[j]);
         out[c] = fmaxf(v, 0.f);
       }
     }
@@ -226,7 +226,7 @@ corr_stream_kernel(const float* __restrict__ tpc, const float* __restrict__ norm
         for (int q = 0; q < MAXM; ++q) {
           float s = warp_sum(acc[q][r]);
           if (lane == 0 && q < mc && p < P) {
-            float v = __fdiv_rn(s, fmaxf(__fmul_rn(desc_norm[row0 + mb + q], fn), 1e-8f));
+            float v = corr_cos(s, desc_norm[row0 + mb + q], fn);
             maps[(size_t)(map0 + mb + q) * map_stride + p] = fmaxf(v, 0.f);
           }
         }

@@ -23,6 +23,13 @@ __host__ __device__ inline int hilo_row(int C) { return 64 * ((C + 31) / 32); }
 // descriptors' interleaved rows then fill exactly the workspace of their separate halves).
 static inline bool corr_hilo(const FeatView& fv) { return fv.hilo != nullptr && fv.C % 32 == 0; }
 
+// Value of a correlation map entry from its accumulator: acc / max(|d| |F|, clamp), the reference's cosine with its 1e-8
+// clamp (callers apply the ReLU).  Every kernel that forms such a value uses this, so that the exact-window head's values
+// are bit for bit the full-map GEMM's.
+__device__ __forceinline__ float corr_cos(float acc, float dn, float fn, float clamp = 1e-8f) {
+  return __fdiv_rn(acc, fmaxf(__fmul_rn(dn, fn), clamp));
+}
+
 constexpr int CORR_TILE = 256;   // token tile of the tensor-core correlation GEMM (= TC_BN); unit of the tile maxima
 
 // Optional by-products / shortcuts of one launch_corr_maps call (all members may stay zero):

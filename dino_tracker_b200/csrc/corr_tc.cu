@@ -262,10 +262,10 @@ struct CorrEpi {
         // norms rows are only 4-byte aligned (P is odd): scalar broadcast loads
         float4 n4 = make_float4(__ldg(fn + i), __ldg(fn + i + 1), __ldg(fn + i + 2), __ldg(fn + i + 3));
         float4 o;
-        o.x = act(__fdiv_rn(f[i + 0], fmaxf(__fmul_rn(dn, n4.x), eps)));
-        o.y = act(__fdiv_rn(f[i + 1], fmaxf(__fmul_rn(dn, n4.y), eps)));
-        o.z = act(__fdiv_rn(f[i + 2], fmaxf(__fmul_rn(dn, n4.z), eps)));
-        o.w = act(__fdiv_rn(f[i + 3], fmaxf(__fmul_rn(dn, n4.w), eps)));
+        o.x = act(corr_cos(f[i + 0], dn, n4.x, eps));
+        o.y = act(corr_cos(f[i + 1], dn, n4.y, eps));
+        o.z = act(corr_cos(f[i + 2], dn, n4.z, eps));
+        o.w = act(corr_cos(f[i + 3], dn, n4.w, eps));
         *reinterpret_cast<float4*>(out + i) = o;
         // strict >: the first token of the tile holding the maximum (columns are visited in increasing order)
         if (o.x > s.mx) { s.mx = o.x; s.tok = col0 + i; }
@@ -277,7 +277,7 @@ struct CorrEpi {
 #pragma unroll
       for (int i = 0; i < 32; ++i)
         if (i < ncols) {
-          const float o = act(__fdiv_rn(f[i], fmaxf(__fmul_rn(dn, fn[i]), eps)));
+          const float o = act(corr_cos(f[i], dn, fn[i], eps));
           out[i] = o;
           if (o > s.mx) { s.mx = o; s.tok = col0 + i; }
         }

@@ -24,18 +24,11 @@
 
 #include "common.cuh"
 #include "corr.cuh"
+#include "head.cuh"
 
 namespace dtk {
 
 constexpr int HEAD_MAX_W = 128, HEAD_MAX_H = 128;
-
-struct HeadParams {
-  int h, w, P, map_stride;
-  int stride_px, half_patch, radius2;  // pixel geometry: centre = half_patch + stride * index
-  float normW, normH;                  // W - 1, H - 1
-  int out_stride, out_mode;
-  float P1[16], P2[16];                // sums of the positive parts of the normalised 3x3 kernels (logit bound)
-};
 
 __device__ __forceinline__ void cp_async16_head(void* smem, const void* gmem) {
   unsigned s = (unsigned)__cvta_generic_to_shared(smem);
@@ -250,10 +243,10 @@ head_kernel(const float* __restrict__ maps, int n_maps_arg, const int* __restric
       for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          int dr = (r0 + i - arow) * hp.stride_px, dc = (c0 + j - acol) * hp.stride_px;
-          if (r0 + i < h && c0 + j < w && dr * dr + dc * dc <= hp.radius2) {
+          const bool disc = in_disc(hp, r0 + i, c0 + j, arow, acol);
+          if (r0 + i < h && c0 + j < w && disc) {
             float e = expf(acc[i][j] - zmax);
-            float x = (float)(hp.half_patch + (c0 + j) * hp.stride_px), y = (float)(hp.half_patch + (r0 + i) * hp.stride_px);
+            float x = token_px(hp, c0 + j), y = token_px(hp, r0 + i);
             s += e; sx = fmaf(x, e, sx); sy = fmaf(y, e, sy);
             gx += x; gy += y; cnt += 1.f;
           }
@@ -280,24 +273,7 @@ head_kernel(const float* __restrict__ maps, int n_maps_arg, const int* __restric
     if (threadIdx.x == 0) {
       float tot[6];
       for (int q = 0; q < 6; ++q) { float t = 0.f; for (int k = 0; k < nwarps; ++k) t += sm_red[q * 32 + k]; tot[q] = t; }
-      // p_i = e_i / S_all; s = sum p_i over the disc   (softmax then mask, tracker_head.py:84-86)
-      float sp = __fdiv_rn(tot[0], ssum), spx = __fdiv_rn(tot[1], ssum), spy = __fdiv_rn(tot[2], ssum);
-      const bool fallback = sp < 1e-8f;
-      if (fallback) {  // heatmap <- (heatmap + 1/|mask|) * mask  (tracker_head.py:87-94)
-        float u = __fdiv_rn(1.f, tot[5]);
-        sp = fmaf(tot[5], u, sp); spx = fmaf(tot[3], u, spx); spy = fmaf(tot[4], u, spy);
-      }
-      float px = __fdiv_rn(spx, sp), py = __fdiv_rn(spy, sp);
-      // RangeNormalizer((W, H)) dst=(-1,1): x / (W-1); * 2; + (-1)      (data/dataset.py:33-35)
-      float nx = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(px, hp.normW)), -1.f);
-      float ny = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(py, hp.normH)), -1.f);
-      if (hp.out_mode == 0) {  // unnormalize(src=(-1,1)): (v - (-1)) / 2 * (W-1)   (data/dataset.py:50-52)
-        nx = __fmul_rn(__fdiv_rn(__fadd_rn(nx, 1.f), 2.f), hp.normW);
-        ny = __fmul_rn(__fdiv_rn(__fadd_rn(ny, 1.f), 2.f), hp.normH);
-      }
-      size_t oi = (size_t)(out_index ? out_index[map] : map) * hp.out_stride;
-      out[oi] = nx; out[oi + 1] = ny;
-      if (aux) { aux[2 * map] = amax; aux[2 * map + 1] = fallback ? 1 : 0; }
+      head_full_finish(hp, tot, ssum, map, amax, out_index, out, aux);
     }
     __syncthreads();  // lin / sm_hid / sm_red are reused by the next iteration
   }
@@ -308,7 +284,6 @@ head_kernel(const float* __restrict__ maps, int n_maps_arg, const int* __restric
 // ------------------------------------------------------------------------------------------------------
 // Fast path: exact refiner on the 11x11 box around the arg-max + certified absence of the fallback branch.
 constexpr int WIN_THREADS = 128;
-constexpr int WB = 11, WH = 13, WM = 15;  // box, hidden window, input window (side lengths); disc radius <= 5 tokens
 
 __global__ void __launch_bounds__(WIN_THREADS)
 head_window_kernel(const float* __restrict__ maps, int n_maps, HeadParams hp, dinotrk_head_weights wts,
@@ -427,10 +402,9 @@ head_window_kernel(const float* __restrict__ maps, int n_maps, HeadParams hp, di
             for (int kx = 0; kx < 3; ++kx) a = fmaf(wts.w2[o][ky * 3 + kx], hb[ky * WH + kx], a);
         }
         z = a;
-        int dr = (r - arow) * hp.stride_px, dc = (c - acol) * hp.stride_px;
-        indisc = dr * dr + dc * dc <= hp.radius2;
-        px = (float)(hp.half_patch + c * hp.stride_px);
-        py = (float)(hp.half_patch + r * hp.stride_px);
+        indisc = in_disc(hp, r, c, arow, acol);
+        px = token_px(hp, c);
+        py = token_px(hp, r);
       }
     }
     float zmax = warp_max(z);
@@ -451,24 +425,8 @@ head_window_kernel(const float* __restrict__ maps, int n_maps, HeadParams hp, di
       float tot[5];
 #pragma unroll
       for (int q = 0; q < 5; ++q) tot[q] = sm_red[12 + q * 4] + sm_red[13 + q * 4] + sm_red[14 + q * 4] + sm_red[15 + q * 4];
-      // every logit outside the box:  z <= b2 + sum_o P2_o * relu(b1_o + P1_o * mout)   (all terms monotone in m >= 0)
-      float F = wts.b2;
-#pragma unroll
-      for (int o = 0; o < 16; ++o) F = fmaf(hp.P2[o], fmaxf(fmaf(hp.P1[o], mout, wts.b1[o]), 0.f), F);
-      const float rest = ((float)P - tot[4]) * expf(fminf(F - zmax, 80.f));
-      // certified: disc mass >= 2e-8 of (an upper bound of) the whole softmax  ->  the reference does not take the
-      // stability branch and its result is sum(x e) / sum(e) over the disc (the normaliser cancels)
-      const bool certified = tot[1] >= 2e-8f * (tot[0] + rest) && tot[1] > 0.f && isfinite(rest);
-      if (certified) {
-        float px_ = __fdiv_rn(tot[2], tot[1]), py_ = __fdiv_rn(tot[3], tot[1]);
-        float nx = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(px_, hp.normW)), -1.f);
-        float ny = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(py_, hp.normH)), -1.f);
-        if (hp.out_mode == 0) {
-          nx = __fmul_rn(__fdiv_rn(__fadd_rn(nx, 1.f), 2.f), hp.normW);
-          ny = __fmul_rn(__fdiv_rn(__fadd_rn(ny, 1.f), 2.f), hp.normH);
-        }
-        size_t oi = (size_t)(out_index ? out_index[map] : map) * hp.out_stride;
-        out[oi] = nx; out[oi + 1] = ny;
+      if (head_certified(hp, wts, mout, zmax, tot)) {
+        head_store_point(hp, __fdiv_rn(tot[2], tot[1]), __fdiv_rn(tot[3], tot[1]), out_index, out, map);
         if (aux) { aux[2 * map] = amax; aux[2 * map + 1] = 0; }
       } else {
         slow_list[atomicAdd(slow_count, 1)] = map;
@@ -615,10 +573,9 @@ head_tm_kernel(const float* __restrict__ maps, const unsigned long long* __restr
               a = fmaf(wv4.x, hv.x, a); a = fmaf(wv4.y, hv.y, a); a = fmaf(wv4.z, hv.z, a); a = fmaf(wv4.w, hv.w, a);
             }
         z = a;
-        const int dr = (r - arow) * hp.stride_px, dc = (c - acol) * hp.stride_px;
-        indisc = dr * dr + dc * dc <= hp.radius2;
-        px = (float)(hp.half_patch + c * hp.stride_px);
-        py = (float)(hp.half_patch + r * hp.stride_px);
+        indisc = in_disc(hp, r, c, arow, acol);
+        px = token_px(hp, c);
+        py = token_px(hp, r);
       }
     }
     float zmax = warp_max(z);
@@ -639,22 +596,8 @@ head_tm_kernel(const float* __restrict__ maps, const unsigned long long* __restr
       float tot[5];
 #pragma unroll
       for (int q = 0; q < 5; ++q) tot[q] = sm_red[8 + q * 4] + sm_red[9 + q * 4] + sm_red[10 + q * 4] + sm_red[11 + q * 4];
-      // every logit outside the box:  z <= b2 + sum_o P2_o * relu(b1_o + P1_o * mout)   (all terms monotone in m >= 0)
-      float F = wts.b2;
-#pragma unroll
-      for (int o = 0; o < 16; ++o) F = fmaf(hp.P2[o], fmaxf(fmaf(hp.P1[o], mout, wts.b1[o]), 0.f), F);
-      const float rest = ((float)P - tot[4]) * expf(fminf(F - zmax, 80.f));
-      const bool certified = tot[1] >= 2e-8f * (tot[0] + rest) && tot[1] > 0.f && isfinite(rest);
-      if (certified) {
-        float px_ = __fdiv_rn(tot[2], tot[1]), py_ = __fdiv_rn(tot[3], tot[1]);
-        float nx = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(px_, hp.normW)), -1.f);
-        float ny = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(py_, hp.normH)), -1.f);
-        if (hp.out_mode == 0) {
-          nx = __fmul_rn(__fdiv_rn(__fadd_rn(nx, 1.f), 2.f), hp.normW);
-          ny = __fmul_rn(__fdiv_rn(__fadd_rn(ny, 1.f), 2.f), hp.normH);
-        }
-        size_t oi = (size_t)(out_index ? out_index[map] : map) * hp.out_stride;
-        out[oi] = nx; out[oi + 1] = ny;
+      if (head_certified(hp, wts, mout, zmax, tot)) {
+        head_store_point(hp, __fdiv_rn(tot[2], tot[1]), __fdiv_rn(tot[3], tot[1]), out_index, out, map);
         if (aux) { aux[2 * map] = amax; aux[2 * map + 1] = 0; }
       } else {
         slow_list[atomicAdd(slow_count, 1)] = map;
@@ -804,10 +747,10 @@ head_big_kernel(const float* __restrict__ maps, int n_maps_arg, const int* __res
       float s = 0.f, sx = 0.f, sy = 0.f, gx = 0.f, gy = 0.f, cnt = 0.f;
       for (int q = lane; q < box_s * box_s; q += 32) {
         const int r = arow - box_r + q / box_s, c = acol - box_r + q % box_s;
-        const int dr = (r - arow) * hp.stride_px, dc = (c - acol) * hp.stride_px;
-        if (r >= 0 && r < h && c >= 0 && c < w && dr * dr + dc * dc <= hp.radius2) {
+        const bool disc = in_disc(hp, r, c, arow, acol);
+        if (r >= 0 && r < h && c >= 0 && c < w && disc) {
           const float e = expf(sm_box[q] - zmax);
-          const float x = (float)(hp.half_patch + c * hp.stride_px), y = (float)(hp.half_patch + r * hp.stride_px);
+          const float x = token_px(hp, c), y = token_px(hp, r);
           s += e; sx = fmaf(x, e, sx); sy = fmaf(y, e, sy);
           gx += x; gy += y; cnt += 1.f;
         }
@@ -822,22 +765,7 @@ head_big_kernel(const float* __restrict__ maps, int n_maps_arg, const int* __res
           const float mk_ = sm_red[k];
           if (mk_ != -INFINITY) ssum += sm_red[HB_WARPS + k] * expf(mk_ - zmax);
         }
-        float sp = __fdiv_rn(vals[0], ssum), spx = __fdiv_rn(vals[1], ssum), spy = __fdiv_rn(vals[2], ssum);
-        const bool fallback = sp < 1e-8f;
-        if (fallback) {  // heatmap <- (heatmap + 1/|mask|) * mask  (tracker_head.py:87-94)
-          float u = __fdiv_rn(1.f, vals[5]);
-          sp = fmaf(vals[5], u, sp); spx = fmaf(vals[3], u, spx); spy = fmaf(vals[4], u, spy);
-        }
-        float px = __fdiv_rn(spx, sp), py = __fdiv_rn(spy, sp);
-        float nx = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(px, hp.normW)), -1.f);
-        float ny = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(py, hp.normH)), -1.f);
-        if (hp.out_mode == 0) {
-          nx = __fmul_rn(__fdiv_rn(__fadd_rn(nx, 1.f), 2.f), hp.normW);
-          ny = __fmul_rn(__fdiv_rn(__fadd_rn(ny, 1.f), 2.f), hp.normH);
-        }
-        size_t oi = (size_t)(out_index ? out_index[map] : map) * hp.out_stride;
-        out[oi] = nx; out[oi + 1] = ny;
-        if (aux) { aux[2 * map] = amax; aux[2 * map + 1] = fallback ? 1 : 0; }
+        head_full_finish(hp, vals, ssum, map, amax, out_index, out, aux);
       }
     }
     __syncthreads();  // lin / sm_box / sm_red are reused by the next map
@@ -852,20 +780,11 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
                 int ctas_per_sm, int parts) {
   if (n_maps <= 0) return DINOTRK_OK;
   DTK_CHECK_GRID(g, "head");
-  HeadParams hp;
-  hp.h = g.h; hp.w = g.w; hp.P = g.h * g.w; hp.map_stride = map_stride;
-  hp.stride_px = g.stride; hp.half_patch = g.patch / 2; hp.radius2 = g.radius * g.radius;
-  hp.normW = (float)(g.W - 1); hp.normH = (float)(g.H - 1);
-  hp.out_stride = out_stride; hp.out_mode = out_mode;
-  for (int o = 0; o < 16; ++o) {
-    float p1 = 0.f, p2 = 0.f;
-    for (int k = 0; k < 9; ++k) { p1 += hw.w1[o][k] > 0.f ? hw.w1[o][k] : 0.f; p2 += hw.w2[o][k] > 0.f ? hw.w2[o][k] : 0.f; }
-    hp.P1[o] = p1 * (1.f + 1e-6f); hp.P2[o] = p2 * (1.f + 1e-6f);   // rounded up: the bound must stay a bound
-  }
+  const HeadParams hp = make_head_params(g, hw, map_stride, out_stride, out_mode);
   const int sms = num_sms();
   const int lin_elems = (map_stride + 3) & ~3;
   // the window fast path needs the disc inside the 11 x 11 box and a scratch list for the uncertified maps
-  const bool window_ok = scratch != nullptr && g.radius <= 5 * g.stride;
+  const bool window_ok = scratch != nullptr && disc_fits_box(g);
   int* slow_count = scratch;
   int* slow_list = scratch ? scratch + 1 : nullptr;
   if (window_ok && (parts & 1)) {

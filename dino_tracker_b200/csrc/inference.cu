@@ -14,6 +14,7 @@
 
 #include "common.cuh"
 #include "corr.cuh"
+#include "head.cuh"
 #include "sample.cuh"
 #include "xwin.cuh"
 
@@ -932,7 +933,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     }
     std::vector<int> cnt(T);
     // pipeline of the anchor phase: coarse pass + exact window (xwin.cuh) on the tensor path, unless disabled
-    bool use_xw = tensor && g->radius <= 5 * g->stride;
+    bool use_xw = tensor && disc_fits_box(*g);
     int pathsel = g_xw_path;
     if (pathsel < 0) { const char* e = getenv("DTK_XW"); if (e) pathsel = atoi(e) != 0 ? 1 : 0; }
     if (pathsel == 0) use_xw = false;

@@ -20,6 +20,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "head.cuh"
 #include "sample.cuh"
 
 namespace dtk {
@@ -27,11 +28,6 @@ namespace dtk {
 constexpr int TB_THREADS = 512;
 constexpr int TB_WARPS = TB_THREADS / 32;
 constexpr int TB_NRED = 19;          // per hidden channel: dw2[9], dw1[9], db1
-
-struct TrainGeom {
-  int h, w, P, stride, half_patch, radius2, map_stride;
-  float normW, normH;
-};
 
 __device__ __forceinline__ float block_reduce(float v, float* red, bool is_max) {
   v = is_max ? warp_max(v) : warp_sum(v);
@@ -79,10 +75,10 @@ __device__ __forceinline__ float conv3t(const float* __restrict__ src, int r, in
 template <bool kGlobal>
 __global__ void __launch_bounds__(TB_THREADS, 1)
 track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ aux, const float* __restrict__ grad_out,
-                      TrainGeom tg, dinotrk_head_weights wts, float* __restrict__ dcorr, float* __restrict__ grad_w,
+                      HeadParams hp, dinotrk_head_weights wts, float* __restrict__ dcorr, float* __restrict__ grad_w,
                       float* __restrict__ gbuf) {
   extern __shared__ __align__(16) float tb_smem[];
-  const int P = tg.P, h = tg.h, w = tg.w;
+  const int P = hp.P, h = hp.h, w = hp.w;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   float* m = kGlobal ? gbuf + (size_t)b * 5 * P : tb_smem;   // relu(corr)
   float* z = m + P;              // logits, then d/dlogits
@@ -91,7 +87,7 @@ track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ au
   float* dm = dho + P;           // d/dmap
   float* red = kGlobal ? tb_smem : dm + P;   // [TB_WARPS * TB_NRED]
   __shared__ float sc[8];        // px, py, s', count, dot
-  const float* mp = maps + (size_t)b * tg.map_stride;
+  const float* mp = maps + (size_t)b * hp.map_stride;
   const int amax = aux[2 * b], fb = aux[2 * b + 1];
   const int arow = amax / w, acol = amax - arow * w;
 
@@ -120,10 +116,9 @@ track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ au
   // ---- soft-argmax on the disc (warp 0; the disc lies inside the 11 x 11 box around the arg-max) ----
   if (wid == 0) {
     float cnt = 0.f, s = 0.f;
-    for (int q = lane; q < 121; q += 32) {
-      const int r = arow - 5 + q / 11, c = acol - 5 + q % 11;
-      const int dr = (r - arow) * tg.stride, dc = (c - acol) * tg.stride;
-      if (r >= 0 && r < h && c >= 0 && c < w && dr * dr + dc * dc <= tg.radius2) {
+    for (int q = lane; q < WB * WB; q += 32) {
+      const int r = arow - HEAD_BOX_R + q / WB, c = acol - HEAD_BOX_R + q % WB;
+      if (r >= 0 && r < h && c >= 0 && c < w && in_disc(hp, r, c, arow, acol)) {
         cnt += 1.f;
         s += expf(z[r * w + c] - zmax) * inv_se;
       }
@@ -131,27 +126,25 @@ track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ au
     cnt = warp_sum(cnt); s = warp_sum(s);
     const float uni = fb ? 1.f / cnt : 0.f;
     float s2 = 0.f, sx = 0.f, sy = 0.f;
-    for (int q = lane; q < 121; q += 32) {
-      const int r = arow - 5 + q / 11, c = acol - 5 + q % 11;
-      const int dr = (r - arow) * tg.stride, dc = (c - acol) * tg.stride;
-      if (r >= 0 && r < h && c >= 0 && c < w && dr * dr + dc * dc <= tg.radius2) {
+    for (int q = lane; q < WB * WB; q += 32) {
+      const int r = arow - HEAD_BOX_R + q / WB, c = acol - HEAD_BOX_R + q % WB;
+      if (r >= 0 && r < h && c >= 0 && c < w && in_disc(hp, r, c, arow, acol)) {
         const float qv = expf(z[r * w + c] - zmax) * inv_se + uni;
         s2 += qv;
-        sx = fmaf((float)(tg.half_patch + c * tg.stride), qv, sx);
-        sy = fmaf((float)(tg.half_patch + r * tg.stride), qv, sy);
+        sx = fmaf(token_px(hp, c), qv, sx);
+        sy = fmaf(token_px(hp, r), qv, sy);
       }
     }
     s2 = warp_sum(s2); sx = warp_sum(sx); sy = warp_sum(sy);
     const float px = sx / s2, py = sy / s2;
     // out = 2 * point / (W - 1, H - 1) - 1
-    const float dpx = grad_out[2 * b] * 2.f / tg.normW, dpy = grad_out[2 * b + 1] * 2.f / tg.normH;
+    const float dpx = grad_out[2 * b] * 2.f / hp.normW, dpy = grad_out[2 * b + 1] * 2.f / hp.normH;
     float dot = 0.f;
     if (fb) {
-      for (int q = lane; q < 121; q += 32) {
-        const int r = arow - 5 + q / 11, c = acol - 5 + q % 11;
-        const int dr = (r - arow) * tg.stride, dc = (c - acol) * tg.stride;
-        if (r >= 0 && r < h && c >= 0 && c < w && dr * dr + dc * dc <= tg.radius2) {
-          const float dq = (((float)(tg.half_patch + c * tg.stride) - px) * dpx + ((float)(tg.half_patch + r * tg.stride) - py) * dpy) / s2;
+      for (int q = lane; q < WB * WB; q += 32) {
+        const int r = arow - HEAD_BOX_R + q / WB, c = acol - HEAD_BOX_R + q % WB;
+        if (r >= 0 && r < h && c >= 0 && c < w && in_disc(hp, r, c, arow, acol)) {
+          const float dq = ((token_px(hp, c) - px) * dpx + (token_px(hp, r) - py) * dpy) / s2;
           dot = fmaf(expf(z[r * w + c] - zmax) * inv_se, dq, dot);
         }
       }
@@ -165,12 +158,11 @@ track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ au
     float db2 = 0.f;
     for (int p = tid; p < P; p += TB_THREADS) {
       const int r = p / w, c = p - r * w;
-      const int dr = (r - arow) * tg.stride, dc = (c - acol) * tg.stride;
-      const bool in = dr * dr + dc * dc <= tg.radius2;
+      const bool in = in_disc(hp, r, c, arow, acol);
       float g = 0.f;
       if (in || fb) {
         const float pv = expf(z[p] - zmax) * inv_se;
-        const float dq = in ? (((float)(tg.half_patch + c * tg.stride) - px) * dpx + ((float)(tg.half_patch + r * tg.stride) - py) * dpy) / s2 : 0.f;
+        const float dq = in ? ((token_px(hp, c) - px) * dpx + (token_px(hp, r) - py) * dpy) / s2 : 0.f;
         g = pv * (dq - dot);
       }
       db2 += g;
@@ -240,7 +232,7 @@ track_head_bwd_kernel(const float* __restrict__ maps, const int* __restrict__ au
     __syncthreads();
   }
   // ---- through the ReLU of the correlation map ----
-  float* dc = dcorr + (size_t)b * tg.map_stride;
+  float* dc = dcorr + (size_t)b * hp.map_stride;
   for (int p = tid; p < P; p += TB_THREADS) dc[p] = m[p] > 0.f ? dm[p] : 0.f;
 }
 
@@ -372,7 +364,7 @@ int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, 
                 "track_backward: null pointer");
   DTK_CHECK_ARG(B >= 0 && N > 0 && feat->C > 0, "track_backward: bad sizes");
   DTK_CHECK_GRID(*g, "track_backward");
-  DTK_CHECK_ARG(g->radius <= 5 * g->stride, "track_backward: disc radius %d exceeds 5 tokens", g->radius);
+  DTK_CHECK_ARG(disc_fits_box(*g), "track_backward: disc radius %d exceeds 5 tokens", g->radius);
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_track_backward_workspace_bytes(B, feat->C, g), "track_backward: workspace too small");
   if (B == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
@@ -380,10 +372,7 @@ int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, 
   Arena ar(workspace, workspace_bytes);
   float* dcorr = ar.take<float>((size_t)B * dinotrk_map_stride(g));
   float* ddesc = ar.take<float>((size_t)B * C);
-  TrainGeom tg;
-  tg.h = g->h; tg.w = g->w; tg.P = P; tg.stride = g->stride; tg.half_patch = g->patch / 2; tg.radius2 = g->radius * g->radius;
-  tg.map_stride = dinotrk_map_stride(g);
-  tg.normW = (float)(g->W - 1); tg.normH = (float)(g->H - 1);
+  const HeadParams hp = make_head_params(*g, *hw, dinotrk_map_stride(g), 2, 1);
   const bool g1 = head_bwd_global(P), g2 = corr_bwd_global(P);
   float* gbuf1 = g1 ? ar.take<float>((size_t)B * 5 * P) : nullptr;
   float* gbuf2 = g2 ? ar.take<float>((size_t)B * 3 * P) : nullptr;
@@ -401,11 +390,11 @@ int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, 
   }
   NvtxRange nv("dinotrk_track_backward");
   ProfRange pr(PROF_TRAIN_BWD, st);
-  (g1 ? track_head_bwd_kernel<true> : track_head_bwd_kernel<false>)<<<B, TB_THREADS, smem1, st>>>(maps, aux, grad_out, tg, *hw,
+  (g1 ? track_head_bwd_kernel<true> : track_head_bwd_kernel<false>)<<<B, TB_THREADS, smem1, st>>>(maps, aux, grad_out, hp, *hw,
                                                                                               dcorr, grad_w, gbuf1);
   DTK_LAUNCHED();
   (g2 ? track_corr_bwd_kernel<true> : track_corr_bwd_kernel<false>)<<<B, TC_THREADS_BWD, smem2, st>>>(
-      feat->tpc, feat->norms, C, P, tg.map_stride, maps, dcorr, desc, desc_norm, tgt_frame, ddesc, grad_tpc, gbuf2);
+      feat->tpc, feat->norms, C, P, hp.map_stride, maps, dcorr, desc, desc_norm, tgt_frame, ddesc, grad_tpc, gbuf2);
   DTK_LAUNCHED();
   if (grad_tpc) {
     track_sample_bwd_kernel<<<B, SAMPLE_THREADS, 0, st>>>(C, P, g->h, g->w, make_point_affine(*g), points, frames_set, N, 0, ddesc, grad_tpc);

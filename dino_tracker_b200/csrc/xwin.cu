@@ -3,6 +3,7 @@
 
 #include "common.cuh"
 #include "corr.cuh"
+#include "head.cuh"
 #include "tcgemm.cuh"
 #include "xwin.cuh"
 
@@ -561,24 +562,15 @@ int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_h
 // and either the track point or a place in the group's full-map queue.
 constexpr int XH_WARPS = 8;
 constexpr int XH_MP = 18;      // input window pitch (float2 units, even: 16-byte loads of two positions; 4 row groups -> 4 bank quads)
-constexpr int XWM = 15, XWH = 13, XWB = 11;
-constexpr int XH_MWIN = 544;   // floats: the 15 x 15 input window with every value stored twice (XWM * XH_MP * 2 = 540)
-constexpr int XH_PER_WARP = XH_MWIN + XWH * XWH * 16;      // + hidden window [position][8 channel pairs (c, c + 8)]
+constexpr int XH_MWIN = 544;   // floats: the 15 x 15 input window with every value stored twice (WM * XH_MP * 2 = 540)
+constexpr int XH_PER_WARP = XH_MWIN + WH * WH * 16;      // + hidden window [position][8 channel pairs (c, c + 8)]
 constexpr int XH_WTAB = 20 * 16;                           // floats: refiner weights as pairs [w1 k = 0..8 | b1 | w2 k = 0..8 | -][8 pairs]
 constexpr int XH_SMEM = (XH_WTAB + XH_WARPS * XH_PER_WARP) * 4;
-
-struct XhParams {
-  int h, w, P, n_tiles;
-  int stride_px, half_patch, radius2;
-  float normW, normH;
-  int out_stride, out_mode;
-  float P1[16], P2[16];
-};
 
 // Window, refiner and softmax sums of one map (one warp).  INTERIOR: the 15 x 15 window lies inside the token grid (no
 // zero padding anywhere: the per-position bounds tests drop out -- the common case away from the frame border).
 template <bool INTERIOR>
-__device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __restrict__ wtab, float b2w, float2* __restrict__ mm2,
+__device__ __forceinline__ void xw_refine(const HeadParams& hp, const float2* __restrict__ wtab, float b2w, float2* __restrict__ mm2,
                                           float2* __restrict__ hh2, const float (&wv)[8], int arow, int acol, int lane,
                                           float& zmax, float (&tot)[5]) {
   const int h = hp.h, w = hp.w;
@@ -589,7 +581,7 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
   for (int q = 0; q < 8; ++q) {
     const int i = lane + 32 * q;
     const int y = i >> 4, x = i & 15;
-    if (y < XWM && x < XWM) mm2[y * XH_MP + x] = make_float2(wv[q], wv[q]);
+    if (y < WM && x < WM) mm2[y * XH_MP + x] = make_float2(wv[q], wv[q]);
   }
   __syncwarp();
   // ---- refiner on fp32 FMA pairs (f2fma: the lane's two channels share every operand load).  Lane =
@@ -603,7 +595,7 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
 #pragma unroll
     for (int k = 0; k < 9; ++k) w1r[k] = wtab[k * 8 + cp];
     const float2 b1r = wtab[9 * 8 + cp];
-    for (int y = pg; y < XWH; y += 4) {
+    for (int y = pg; y < WH; y += 4) {
       const int r = arow - 6 + y;
       const bool row_in = r >= 0 && r < h;
       const float2* m0 = mm2 + y * XH_MP;
@@ -619,7 +611,7 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
         in2[x] = make_float2(q2.x, q2.y); in2[x + 1] = make_float2(q2.z, q2.w);
       }
 #pragma unroll
-      for (int x = 0; x < XWH; ++x) {
+      for (int x = 0; x < WH; ++x) {
         // three short chains per output (one per input row) instead of one chain of nine dependent FMAs
         float2 a0 = f2fma(w1r[0], in0[x], b1r), a1 = f2mul(w1r[3], in1[x]), a2 = f2mul(w1r[6], in2[x]);
         a0 = f2fma(w1r[1], in0[x + 1], a0); a1 = f2fma(w1r[4], in1[x + 1], a1); a2 = f2fma(w1r[7], in2[x + 1], a2);
@@ -627,7 +619,7 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
         const float2 a = f2add(f2add(a0, a1), a2);
         const int c = acol - 6 + x;
         const bool in = INTERIOR || (row_in && c >= 0 && c < w);
-        hh2[(y * XWH + x) * 8 + cp] = in ? make_float2(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f)) : make_float2(0.f, 0.f);
+        hh2[(y * WH + x) * 8 + cp] = in ? make_float2(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f)) : make_float2(0.f, 0.f);
       }
     }
   }
@@ -640,15 +632,15 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
 #pragma unroll
     for (int yi = 0; yi < 3; ++yi) {
       const int y = pg + 4 * yi;
-      const bool row_ok = y < XWB;                  // (row group 3 has no third row; its lanes still take part in the shuffles)
-      const float2* h0 = hh2 + ((row_ok ? y : 0) * XWH) * 8 + cp;
-      float2 i00 = h0[0], i01 = h0[8], i10 = h0[XWH * 8], i11 = h0[(XWH + 1) * 8];
-      float2 i20 = h0[2 * XWH * 8], i21 = h0[(2 * XWH + 1) * 8];
+      const bool row_ok = y < WB;                  // (row group 3 has no third row; its lanes still take part in the shuffles)
+      const float2* h0 = hh2 + ((row_ok ? y : 0) * WH) * 8 + cp;
+      float2 i00 = h0[0], i01 = h0[8], i10 = h0[WH * 8], i11 = h0[(WH + 1) * 8];
+      float2 i20 = h0[2 * WH * 8], i21 = h0[(2 * WH + 1) * 8];
       float v[12];
       v[11] = 0.f;
 #pragma unroll
-      for (int x = 0; x < XWB; ++x) {
-        const float2 i02 = h0[(x + 2) * 8], i12 = h0[(XWH + x + 2) * 8], i22 = h0[(2 * XWH + x + 2) * 8];
+      for (int x = 0; x < WB; ++x) {
+        const float2 i02 = h0[(x + 2) * 8], i12 = h0[(WH + x + 2) * 8], i22 = h0[(2 * WH + x + 2) * 8];
         float2 a0 = f2mul(w2r[0], i00), a1 = f2mul(w2r[3], i10), a2 = f2mul(w2r[6], i20);
         a0 = f2fma(w2r[1], i01, a0); a1 = f2fma(w2r[4], i11, a1); a2 = f2fma(w2r[7], i21, a2);
         a0 = f2fma(w2r[2], i02, a0); a1 = f2fma(w2r[5], i12, a1); a2 = f2fma(w2r[8], i22, a2);
@@ -673,8 +665,8 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
       const float t0 = (b0 ? w3[2] : w3[0]) + __shfl_xor_sync(0xffffffffu, b0 ? w3[0] : w3[2], 1);
       const float t1 = (b0 ? 0.f : w3[1]) + __shfl_xor_sync(0xffffffffu, b0 ? w3[1] : 0.f, 1);
       const int idx0 = (b2 ? 6 : 0) + (b1 ? 3 : 0) + (b0 ? 2 : 0);
-      if (row_ok && idx0 < XWB) zb[y * XWB + idx0] = t0 + b2w;
-      if (row_ok && !b0) zb[y * XWB + idx0 + 1] = t1 + b2w;
+      if (row_ok && idx0 < WB) zb[y * WB + idx0] = t0 + b2w;
+      if (row_ok && !b0) zb[y * WB + idx0 + 1] = t1 + b2w;
     }
   }
   __syncwarp();
@@ -687,16 +679,15 @@ __device__ __forceinline__ void xw_refine(const XhParams& hp, const float2* __re
   for (int q = 0; q < 4; ++q) {
     const int p = lane + 32 * q;
     valid[q] = false; indisc[q] = false; z[q] = -INFINITY; px[q] = py[q] = 0.f;
-    if (p < XWB * XWB) {
-      const int y = p / XWB, x = p - y * XWB;
+    if (p < WB * WB) {
+      const int y = p / WB, x = p - y * WB;
       const int r = arow - 5 + y, c = acol - 5 + x;
       valid[q] = INTERIOR || (r >= 0 && r < h && c >= 0 && c < w);
       if (valid[q]) {
         z[q] = zb[p];
-        const int dr = (r - arow) * hp.stride_px, dc = (c - acol) * hp.stride_px;
-        indisc[q] = dr * dr + dc * dc <= hp.radius2;
-        px[q] = (float)(hp.half_patch + c * hp.stride_px);
-        py[q] = (float)(hp.half_patch + r * hp.stride_px);
+        indisc[q] = in_disc(hp, r, c, arow, acol);
+        px[q] = token_px(hp, c);
+        py[q] = token_px(hp, r);
       }
     }
     zmax = fmaxf(zmax, z[q]);
@@ -742,7 +733,7 @@ xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __re
     for (int q = 0; q < XW_MAX_CAND; ++q)
       if (ct[q] >= 0) {
         const int tr = ct[q] / w, tcn = ct[q] - tr * w;
-        const float v = fmaxf(__fdiv_rn(__ldg(xr + xw_col(tr - org.x, tcn - org.y)), fmaxf(__fmul_rn(dn, __ldg(fn + ct[q])), 1e-8f)), 0.f);
+        const float v = fmaxf(corr_cos(__ldg(xr + xw_col(tr - org.x, tcn - org.y)), dn, __ldg(fn + ct[q])), 0.f);
         if (v > best || (v == best && ct[q] < amax)) { best = v; amax = ct[q]; }
       }
     const int arow = amax / w, acol = amax - arow * w;
@@ -764,8 +755,8 @@ xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __re
       const int y = i >> 4, x = i & 15;
       const int r = arow - 7 + y, c = acol - 7 + x;
       float v = 0.f;
-      if (y < XWM && x < XWM && r >= 0 && r < h && c >= 0 && c < w) {
-        v = fmaxf(__fdiv_rn(__ldg(xr + xw_col(r - org.x, c - org.y)), fmaxf(__fmul_rn(dn, __ldg(fn + r * w + c)), 1e-8f)), 0.f);
+      if (y < WM && x < WM && r >= 0 && r < h && c >= 0 && c < w) {
+        v = fmaxf(corr_cos(__ldg(xr + xw_col(r - org.x, c - org.y)), dn, __ldg(fn + r * w + c)), 0.f);
         if (!(abs(r - arow) <= 3 && abs(c - acol) <= 3)) mout = fmaxf(mout, v);
       }
       win[(size_t)map * XWIN_PITCH + i] = v;
@@ -778,7 +769,7 @@ xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __re
 // (b) refiner + softmax sums + certificate: one warp per map; the next map's window (8 coalesced loads per lane) and
 // arg-max are in flight while the current map is refined.
 __global__ void __launch_bounds__(XH_WARPS * 32, 2)
-xw_head_kernel(int n_maps, XhParams hp, dinotrk_head_weights wts, const int* __restrict__ cell_group, const int* __restrict__ grp_map0,
+xw_head_kernel(int n_maps, HeadParams hp, dinotrk_head_weights wts, const int* __restrict__ cell_group, const int* __restrict__ grp_map0,
                const int* __restrict__ cell_of, const float* __restrict__ win, const int2* __restrict__ hin,
                const int* __restrict__ out_index, float* __restrict__ out, int* __restrict__ slow_cnt, int* __restrict__ slow_list,
                int n_groups) {
@@ -799,7 +790,7 @@ xw_head_kernel(int n_maps, XhParams hp, dinotrk_head_weights wts, const int* __r
                                  : make_float2(wts.w2[c][k - 10], wts.w2[c + 8][k - 10]);
   }
   __syncthreads();
-  const int h = hp.h, w = hp.w, P = hp.P;
+  const int h = hp.h, w = hp.w;
   const int stride = gridDim.x * XH_WARPS;
 
   int map = blockIdx.x * XH_WARPS + wid;
@@ -835,25 +826,8 @@ xw_head_kernel(int n_maps, XhParams hp, dinotrk_head_weights wts, const int* __r
       for (int q = 0; q < 5; ++q) tot[q] = warp_sum(tot[q]);
     }
     if (lane == 0) {
-      bool certified = false;
-      if (!slow) {
-        // every logit outside the box:  z <= b2 + sum_o P2_o * relu(b1_o + P1_o * mout)   (head.cu, same certificate)
-        float F = wts.b2;
-#pragma unroll
-        for (int o = 0; o < 16; ++o) F = fmaf(hp.P2[o], fmaxf(fmaf(hp.P1[o], mout, wts.b1[o]), 0.f), F);
-        const float rest = ((float)P - tot[4]) * expf(fminf(F - zmax, 80.f));
-        certified = tot[1] >= 2e-8f * (tot[0] + rest) && tot[1] > 0.f && isfinite(rest);
-      }
-      if (certified) {
-        const float px_ = __fdiv_rn(tot[2], tot[1]), py_ = __fdiv_rn(tot[3], tot[1]);
-        float nx = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(px_, hp.normW)), -1.f);
-        float ny = __fadd_rn(__fmul_rn(2.f, __fdiv_rn(py_, hp.normH)), -1.f);
-        if (hp.out_mode == 0) {
-          nx = __fmul_rn(__fdiv_rn(__fadd_rn(nx, 1.f), 2.f), hp.normW);
-          ny = __fmul_rn(__fdiv_rn(__fadd_rn(ny, 1.f), 2.f), hp.normH);
-        }
-        const size_t oi = (size_t)(out_index ? out_index[map] : map) * hp.out_stride;
-        out[oi] = nx; out[oi + 1] = ny;
+      if (!slow && head_certified(hp, wts, mout, zmax, tot)) {
+        head_store_point(hp, __fdiv_rn(tot[2], tot[1]), __fdiv_rn(tot[3], tot[1]), out_index, out, map);
       } else {
         const int g = cell_group[cell_of[map]];
         const int pos = atomicAdd(slow_cnt + g, 1);
@@ -870,17 +844,8 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
                    const float* desc_norm, const int* grp_map0, int n_maps, const int* out_index, float* out, int out_stride,
                    int out_mode, const XwChunk& xc, cudaStream_t st, int n_groups, const float* eps) {
   if (n_maps <= 0) return DINOTRK_OK;
-  DTK_CHECK_ARG(g.radius <= 5 * g.stride, "exact-window path: disc radius %d exceeds 5 tokens", g.radius);
-  XhParams hp;
-  hp.h = g.h; hp.w = g.w; hp.P = g.h * g.w; hp.n_tiles = cdiv(hp.P, XW_TILE);
-  hp.stride_px = g.stride; hp.half_patch = g.patch / 2; hp.radius2 = g.radius * g.radius;
-  hp.normW = (float)(g.W - 1); hp.normH = (float)(g.H - 1);
-  hp.out_stride = out_stride; hp.out_mode = out_mode;
-  for (int o = 0; o < 16; ++o) {
-    float p1 = 0.f, p2 = 0.f;
-    for (int k = 0; k < 9; ++k) { p1 += hw.w1[o][k] > 0.f ? hw.w1[o][k] : 0.f; p2 += hw.w2[o][k] > 0.f ? hw.w2[o][k] : 0.f; }
-    hp.P1[o] = p1 * (1.f + 1e-6f); hp.P2[o] = p2 * (1.f + 1e-6f);
-  }
+  DTK_CHECK_ARG(disc_fits_box(g), "exact-window path: disc radius %d exceeds 5 tokens", g.radius);
+  const HeadParams hp = make_head_params(g, hw, dinotrk_map_stride(&g), out_stride, out_mode);
   const int sms = num_sms();
   int grid = cdiv(n_maps, XH_WARPS);
   if (grid > sms * 2) grid = sms * 2;
@@ -894,8 +859,8 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
   {
     int wgrid = cdiv(n_maps, 8);
     if (wgrid > sms * 8) wgrid = sms * 8;
-    xw_window_kernel<<<wgrid, 256, 0, st>>>(n_maps, g.h, g.w, hp.P, hp.n_tiles, fv.norms, desc_norm, cells.frame, xc.cell_of, xc.box_org,
-                                            xc.stat, xc.cand, xc.key1, xc.max2, xc.xbox, xc.win, xc.hin, eps);
+    xw_window_kernel<<<wgrid, 256, 0, st>>>(n_maps, g.h, g.w, hp.P, cdiv(hp.P, XW_TILE), fv.norms, desc_norm, cells.frame,
+                                            xc.cell_of, xc.box_org, xc.stat, xc.cand, xc.key1, xc.max2, xc.xbox, xc.win, xc.hin, eps);
     DTK_LAUNCHED();
   }
   xw_head_kernel<<<grid, XH_WARPS * 32, XH_SMEM, st>>>(n_maps, hp, hw, cells.group, grp_map0, xc.cell_of, xc.win, xc.hin, out_index,
