@@ -199,6 +199,16 @@ __global__ void bb_plan_kernel(int n_pairs, int P, const int* __restrict__ src, 
   if (i == 0) tile_start[n_pairs] = n_pairs * tiles;
 }
 
+struct BBWs {
+  BBPartial* part; int* row0; int* m; int* tile_start;
+  BBWs(Arena& ar, int n_pairs, int P) {
+    part = ar.take<BBPartial>((size_t)n_pairs * cdiv(P, TC_BN) * P);
+    row0 = ar.take<int>(n_pairs + 1);
+    m = ar.take<int>(n_pairs + 1);
+    tile_start = ar.take<int>(n_pairs + 1);
+  }
+};
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -206,8 +216,7 @@ using namespace dtk;
 extern "C" {
 
 size_t dinotrk_best_buddies_workspace_bytes(int n_pairs, int P) {
-  const int n_tiles = cdiv(P, TC_BN);
-  return align_up((size_t)n_pairs * n_tiles * P * sizeof(BBPartial), 256) + 3 * align_up((size_t)(n_pairs + 1) * 4, 256) + 1024;
+  return align_up(layout_end<BBWs>(n_pairs, P), 256) + 1024;
 }
 
 int dinotrk_best_buddies_pairs(const dinotrk_features* feat, const dinotrk_geom* g, const int* pair_src,
@@ -221,25 +230,22 @@ int dinotrk_best_buddies_pairs(const dinotrk_features* feat, const dinotrk_geom*
   if (n_pairs == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int n_tiles = cdiv(P, TC_BN);
-  Arena ar(workspace, workspace_bytes);
-  BBPartial* part = ar.take<BBPartial>((size_t)n_pairs * n_tiles * P);
-  int* row0 = ar.take<int>(n_pairs + 1);
-  int* m = ar.take<int>(n_pairs + 1);
-  int* tile_start = ar.take<int>(n_pairs + 1);
+  Arena ar(workspace);
+  const BBWs ws(ar, n_pairs, P);
   {
     ProfRange pr(PROF_MISC, st);
-    bb_plan_kernel<<<cdiv(n_pairs, 128), 128, 0, st>>>(n_pairs, P, pair_src, row0, m, tile_start);
+    bb_plan_kernel<<<cdiv(n_pairs, 128), 128, 0, st>>>(n_pairs, P, pair_src, ws.row0, ws.m, ws.tile_start);
     DTK_LAUNCHED();
   }
   // A: the source frames' tokens, B: the target frames (one batch item per frame)
   const TcOperands op{feat->hi, feat->lo, (uint64_t)T * P, 0, feat->hi, feat->lo, (uint64_t)T, 0};
-  const TcProblem pb{pair_tgt, row0, m, tile_start, n_pairs, P, C};
-  BBEpi epi{feat->norms, pair_src, pair_tgt, part, P, n_tiles};
+  const TcProblem pb{pair_tgt, ws.row0, ws.m, ws.tile_start, n_pairs, P, C};
+  BBEpi epi{feat->norms, pair_src, pair_tgt, ws.part, P, n_tiles};
   if (int rc = tc_launch<TcMode::F16X3, BBEpi>(op, pb, n_pairs * cdiv(P, TC_BM), epi, st, PROF_BB)) return rc;
   {
     ProfRange pr(PROF_BB, st);
     size_t warps = (size_t)n_pairs * P;
-    bb_resolve_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(feat->tpc, feat->norms, C, P, pair_src, pair_tgt, part,
+    bb_resolve_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(feat->tpc, feat->norms, C, P, pair_src, pair_tgt, ws.part,
                                                                   n_tiles, n_pairs, 2e-4f, nn_idx, nn_cos);
     DTK_LAUNCHED();
   }

@@ -97,8 +97,8 @@ static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 // bump allocator over a caller-provided workspace
 struct Arena {
   char* base;
-  size_t size, off;
-  Arena(void* p, size_t n) : base((char*)p), size(n), off(0) {}
+  size_t off;
+  explicit Arena(void* p) : base((char*)p), off(0) {}
   template <typename T>
   T* take(size_t count) {
     off = align_up(off, 256);
@@ -106,8 +106,17 @@ struct Arena {
     off += count * sizeof(T);
     return p;
   }
-  bool ok() const { return off <= size; }
 };
+
+// A workspace's layout is a struct whose constructor takes every buffer from an Arena.  Its size function is a dry run of
+// that constructor on a null base, so the size and the carve cannot disagree: this returns where the last buffer ends.
+template <typename Layout, typename... Args>
+static inline size_t layout_end(const Args&... args) {
+  Arena ar(nullptr);
+  const Layout layout(ar, args...);
+  (void)layout;
+  return ar.off;
+}
 
 // element-wise IEEE fp32 operations on pairs (two FFMA / FMUL / FADD: bit for bit what a packed instruction would give)
 __device__ __forceinline__ float2 f2fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }

@@ -439,31 +439,72 @@ static ClPlan cl_plan(int N, int P, int B, const int* grp_src, const int* grp_tg
 }
 
 template <class T>
-static T* upload(Arena& ar, const std::vector<T>& v, cudaStream_t st, int* rc) {
-  T* d = ar.take<T>(v.size() ? v.size() : 1);
-  if (ar.ok() && !v.empty() && cudaMemcpyAsync(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+static void upload(T* d, const std::vector<T>& v, cudaStream_t st, int* rc) {
+  if (!v.empty() && cudaMemcpyAsync(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, st) != cudaSuccess) {
     set_error("bb_contrastive: table upload failed");
     *rc = DINOTRK_ECUDA;
   }
-  return d;
 }
 
-static size_t fwd_bytes(int N, int P, int C, int B, int n_groups) {
-  Arena ar(nullptr, 0);
-  ar.take<__half>((size_t)N * P * C);        // E hi
-  ar.take<__half>((size_t)N * P * C);        // E lo
-  ar.take<float>((size_t)N * P);             // token norms
-  ar.take<float>((size_t)2 * B * C);         // [S; U]
-  ar.take<float>((size_t)2 * B);             // their norms
-  ar.take<char>(corr_tc_workspace_bytes(2 * B, C));
-  ar.take<float>((size_t)N * P);             // scaled token norms
-  ar.take<float>((size_t)2 * B);             // scaled descriptor norms
-  ar.take<unsigned>(1);                      // max |E|
-  ar.take<float>((size_t)2 * B);             // per-row clamp of the scaled norm products
-  for (int i = 0; i < 5; ++i) ar.take<int>(2 * n_groups + 1);
-  ar.take<int>(B > 0 ? B : 1);
-  return ar.off + 256;
-}
+// The plan tables are carved at the bounds the plan can reach from the shapes (the group tables at 2 n_groups + 1).
+struct ClFwdWs {
+  __half* e_hi; __half* e_lo; float* en; float* desc; float* dn; float* split_ws; float* en_s; float* dn_s; unsigned* amax;
+  float* eps_s; int* frame; int* row0; int* m; int* tile_start; int* spare; int* row_grp;
+  ClFwdWs(Arena& ar, int N, int P, int C, int B, int n_groups) {
+    e_hi = ar.take<__half>((size_t)N * P * C);
+    e_lo = ar.take<__half>((size_t)N * P * C);
+    en = ar.take<float>((size_t)N * P);                   // token norms
+    desc = ar.take<float>((size_t)2 * B * C);             // [S; U]
+    dn = ar.take<float>((size_t)2 * B);                   // their norms
+    split_ws = ar.take<float>(corr_tc_workspace_bytes(2 * B, C) / sizeof(float));
+    en_s = ar.take<float>((size_t)N * P);                 // scaled token norms
+    dn_s = ar.take<float>((size_t)2 * B);                 // scaled descriptor norms
+    amax = ar.take<unsigned>(1);                          // max |E|
+    eps_s = ar.take<float>((size_t)2 * B);                // per-row clamp of the scaled norm products
+    frame = ar.take<int>(2 * n_groups + 1);
+    row0 = ar.take<int>(2 * n_groups + 1);
+    m = ar.take<int>(2 * n_groups + 1);
+    tile_start = ar.take<int>(2 * n_groups + 1);
+    spare = ar.take<int>(2 * n_groups + 1);               // unused; part of the size callers allocate
+    row_grp = ar.take<int>(B > 0 ? B : 1);
+  }
+};
+
+struct ClBwdWs {
+  float* en; float* desc; float* dn; float* rcorr; unsigned* amax; float* dbuf;
+  __half *a1_hi, *a1_lo, *b1_hi, *b1_lo, *a2_hi, *a2_lo, *b2_hi, *b2_lo;
+  int *frame, *row0, *m, *tile_start, *row_grp, *row_frame, *frame_k, *frame_rows, *f_batch, *f_row0, *f_m, *f_tiles, *grows;
+  ClBwdWs(Arena& ar, int N, int P, int C, int B, const ClPlan& pl) {
+    const size_t Pp = pad8(P);
+    en = ar.take<float>((size_t)N * P);                   // token norms
+    desc = ar.take<float>((size_t)2 * B * C);             // [S; U]
+    dn = ar.take<float>((size_t)2 * B);                   // norms
+    rcorr = ar.take<float>((size_t)2 * B);                // row corrections
+    amax = ar.take<unsigned>(1);
+    dbuf = ar.take<float>((size_t)2 * B * Pp);            // Deff
+    a1_hi = ar.take<__half>((size_t)2 * B * Pp);
+    a1_lo = ar.take<__half>((size_t)2 * B * Pp);
+    b1_hi = ar.take<__half>((size_t)N * C * Pp);
+    b1_lo = ar.take<__half>((size_t)N * C * Pp);
+    a2_hi = ar.take<__half>((size_t)N * Pp * pl.Kx);
+    a2_lo = ar.take<__half>((size_t)N * Pp * pl.Kx);
+    b2_hi = ar.take<__half>((size_t)N * C * pl.Kx);
+    b2_lo = ar.take<__half>((size_t)N * C * pl.Kx);
+    frame = ar.take<int>(pl.G2 + 1);
+    row0 = ar.take<int>(pl.G2 + 1);
+    m = ar.take<int>(pl.G2 + 1);
+    tile_start = ar.take<int>(pl.G2 + 1);
+    row_grp = ar.take<int>(B > 0 ? B : 1);
+    row_frame = ar.take<int>(2 * (size_t)B + 1);
+    frame_k = ar.take<int>(N);
+    frame_rows = ar.take<int>((size_t)N * pl.Kx);
+    f_batch = ar.take<int>(N + 1);
+    f_row0 = ar.take<int>(N + 1);
+    f_m = ar.take<int>(N + 1);
+    f_tiles = ar.take<int>(N + 1);
+    grows = ar.take<int>(pl.G2 > 0 ? pl.G2 / 2 : 1);   // rows per group
+  }
+};
 
 }  // namespace dtk
 
@@ -474,7 +515,7 @@ extern "C" {
 int dinotrk_bb_contrastive_cos_stride(int P) { return pad8(P); }
 
 size_t dinotrk_bb_contrastive_forward_workspace_bytes(int N, int P, int C, int B, int n_groups) {
-  return fwd_bytes(N, P, C, B, n_groups);
+  return layout_end<ClFwdWs>(N, P, C, B, n_groups) + 256;
 }
 
 int dinotrk_bb_contrastive_forward(const float* E, int N, int P, int C, const float* S, const float* U, int B,
@@ -488,86 +529,52 @@ int dinotrk_bb_contrastive_forward(const float* E, int N, int P, int C, const fl
   if (pl.tiles1 == 0) return DINOTRK_OK;   // every group empty
   cudaStream_t st = (cudaStream_t)stream;
   ProfRange pr(PROF_CONTRASTIVE, st);
-  Arena ar(workspace, workspace_bytes);
-  __half* e_hi = ar.take<__half>((size_t)N * P * C);
-  __half* e_lo = ar.take<__half>((size_t)N * P * C);
-  float* en = ar.take<float>((size_t)N * P);
-  float* desc = ar.take<float>((size_t)2 * B * C);
-  float* dn = ar.take<float>((size_t)2 * B);
-  float* split_ws = ar.take<float>(corr_tc_workspace_bytes(2 * B, C) / sizeof(float));
-  float* en_s = ar.take<float>((size_t)N * P);
-  float* dn_s = ar.take<float>((size_t)2 * B);
-  unsigned* amax = ar.take<unsigned>(1);
-  float* eps_s = ar.take<float>((size_t)2 * B);
+  Arena ar(workspace);
+  const ClFwdWs ws(ar, N, P, C, B, n_groups);
   int rc = DINOTRK_OK;
-  int* d_frame = upload(ar, pl.frame, st, &rc);
-  int* d_row0 = upload(ar, pl.row0, st, &rc);
-  int* d_m = upload(ar, pl.m, st, &rc);
-  int* d_map0 = d_row0;
-  int* d_tiles = upload(ar, pl.tile_start, st, &rc);
-  int* d_row_grp = upload(ar, pl.row_grp, st, &rc);
+  upload(ws.frame, pl.frame, st, &rc);
+  upload(ws.row0, pl.row0, st, &rc);
+  upload(ws.m, pl.m, st, &rc);
+  upload(ws.tile_start, pl.tile_start, st, &rc);
+  upload(ws.row_grp, pl.row_grp, st, &rc);
   if (rc) return rc;
-  DTK_CHECK_ARG(ar.ok(), "bb_contrastive_forward: workspace layout");
-  DTK_CUDA(cudaMemcpyAsync(desc, S, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
-  DTK_CUDA(cudaMemcpyAsync(desc + (size_t)B * C, U, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
+  DTK_CUDA(cudaMemcpyAsync(ws.desc, S, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
+  DTK_CUDA(cudaMemcpyAsync(ws.desc + (size_t)B * C, U, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
   const size_t toks = (size_t)N * P;
-  cl_norms_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(E, toks, C, en);
+  cl_norms_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(E, toks, C, ws.en);
   DTK_LAUNCHED();
-  cl_norms_kernel<<<(unsigned)((2 * (size_t)B * 32 + 255) / 256), 256, 0, st>>>(desc, 2 * (size_t)B, C, dn);
+  cl_norms_kernel<<<(unsigned)((2 * (size_t)B * 32 + 255) / 256), 256, 0, st>>>(ws.desc, 2 * (size_t)B, C, ws.dn);
   DTK_LAUNCHED();
-  cl_bb_kernel<<<(unsigned)(((size_t)B * 32 + 255) / 256), 256, 0, st>>>(desc, dn, B, C, out);
+  cl_bb_kernel<<<(unsigned)(((size_t)B * 32 + 255) / 256), 256, 0, st>>>(ws.desc, ws.dn, B, C, out);
   DTK_LAUNCHED();
   // E is split after the power of two that puts its max |.| in [2^13, 2^14), every descriptor row after its own, and the
   // epilogue's norms and clamp carry the same factors: the cosines do not depend on the inputs' scale, and a row far below
   // the others keeps its precision.
-  DTK_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), st));
-  const size_t nd = (size_t)2 * B * C;
+  DTK_CUDA(cudaMemsetAsync(ws.amax, 0, sizeof(unsigned), st));
   const unsigned ge = (unsigned)std::min<size_t>((toks * C + 255) / 256, (size_t)num_sms() * 16);
-  if ((rc = launch_amax(E, toks * C, amax, ge, st))) return rc;
-  cl_split_rows_kernel<<<ge, 256, 0, st>>>(E, amax, e_hi, e_lo, toks * C);
+  if ((rc = launch_amax(E, toks * C, ws.amax, ge, st))) return rc;
+  cl_split_rows_kernel<<<ge, 256, 0, st>>>(E, ws.amax, ws.e_hi, ws.e_lo, toks * C);
   DTK_LAUNCHED();
-  __half* d_hi = reinterpret_cast<__half*>(split_ws);   // launch_corr_gemm_tc's layout of a ready split
-  __half* d_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(split_ws) + align_up(nd * 2, 256));
-  cl_desc_split_kernel<<<(unsigned)cdiv(2 * B * 32, 256), 256, 0, st>>>(desc, dn, 2 * (size_t)B, C, amax, d_hi, d_lo, dn_s,
-                                                                         eps_s);
+  const DescSplit d(ws.split_ws, 2 * (size_t)B, C);   // launch_corr_gemm_tc's layout of a ready split
+  __half* d_hi = reinterpret_cast<__half*>(d.hi);
+  __half* d_lo = reinterpret_cast<__half*>(d.lo);
+  cl_desc_split_kernel<<<(unsigned)cdiv(2 * B * 32, 256), 256, 0, st>>>(ws.desc, ws.dn, 2 * (size_t)B, C, ws.amax, d_hi, d_lo, ws.dn_s,
+                                                                         ws.eps_s);
   DTK_LAUNCHED();
-  cl_scale_kernel<<<(unsigned)std::min<size_t>((toks + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>(en, amax, en_s, toks);
+  cl_scale_kernel<<<(unsigned)std::min<size_t>((toks + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>(ws.en, ws.amax, ws.en_s, toks);
   DTK_LAUNCHED();
-  if ((rc = launch_corr_gemm_tc(e_hi, e_lo, en_s, N, C, P, desc, 2 * B, dn_s, d_frame, d_row0, d_m, d_map0, d_tiles, pl.G2,
-                                pl.tiles1, cosm, pad8(P), split_ws, st, nullptr, true, TC_BM, false, eps_s)))
+  if ((rc = launch_corr_gemm_tc(ws.e_hi, ws.e_lo, ws.en_s, N, C, P, ws.desc, 2 * B, ws.dn_s, ws.frame, ws.row0, ws.m, ws.row0, ws.tile_start, pl.G2,
+                                pl.tiles1, cosm, pad8(P), ws.split_ws, st, nullptr, true, TC_BM, false, ws.eps_s)))
     return rc;
-  cl_lse_kernel<<<2 * B, CL_THREADS, 0, st>>>(cosm, P, pad8(P), B, 1.f / tau, d_row_grp, out);
+  cl_lse_kernel<<<2 * B, CL_THREADS, 0, st>>>(cosm, P, pad8(P), B, 1.f / tau, ws.row_grp, out);
   DTK_LAUNCHED();
   return DINOTRK_OK;
-}
-
-static size_t bwd_bytes(int N, int P, int C, int B, const ClPlan& pl) {
-  const size_t Pp = pad8(P);
-  Arena ar(nullptr, 0);
-  ar.take<float>((size_t)N * P);                       // token norms
-  ar.take<float>((size_t)2 * B * C);                   // [S; U]
-  ar.take<float>((size_t)2 * B);                       // norms
-  ar.take<float>((size_t)2 * B);                       // row corrections
-  ar.take<unsigned>(1);                                // amax
-  ar.take<float>((size_t)2 * B * Pp);                  // Deff
-  for (int i = 0; i < 2; ++i) ar.take<__half>((size_t)2 * B * Pp);          // A1 hi / lo
-  for (int i = 0; i < 2; ++i) ar.take<__half>((size_t)N * C * Pp);          // B1 hi / lo
-  for (int i = 0; i < 2; ++i) ar.take<__half>((size_t)N * Pp * pl.Kx);      // A2 hi / lo
-  for (int i = 0; i < 2; ++i) ar.take<__half>((size_t)N * C * pl.Kx);       // B2 hi / lo
-  for (int i = 0; i < 4; ++i) ar.take<int>(pl.G2 + 1);
-  ar.take<int>(B > 0 ? B : 1);
-  ar.take<int>(2 * (size_t)B + 1);
-  ar.take<int>(N);
-  ar.take<int>((size_t)N * pl.Kx);
-  for (int i = 0; i < 4; ++i) ar.take<int>(N + 1);
-  ar.take<int>(pl.G2 > 0 ? pl.G2 / 2 : 1);           // rows per group
-  return ar.off + 256;
 }
 
 size_t dinotrk_bb_contrastive_backward_workspace_bytes(int N, int P, int C, int B, const int* grp_src, const int* grp_tgt,
                                                        const int* grp_row0, const int* grp_rows, int n_groups) {
   if (cl_check(N, P, C, B, grp_src, grp_tgt, grp_row0, grp_rows, n_groups, 1.f)) return 0;
-  return bwd_bytes(N, P, C, B, cl_plan(N, P, B, grp_src, grp_tgt, grp_row0, grp_rows, n_groups));
+  return layout_end<ClBwdWs>(N, P, C, B, cl_plan(N, P, B, grp_src, grp_tgt, grp_row0, grp_rows, n_groups)) + 256;
 }
 
 int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const float* S, const float* U, int B,
@@ -580,7 +587,7 @@ int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const f
                     (n_groups == 0 || (g_bbmean && g_cmean)),
                 "bb_contrastive_backward: null pointer");
   ClPlan pl = cl_plan(N, P, B, grp_src, grp_tgt, grp_row0, grp_rows, n_groups);
-  DTK_CHECK_ARG(workspace && workspace_bytes >= bwd_bytes(N, P, C, B, pl), "bb_contrastive_backward: workspace too small");
+  DTK_CHECK_ARG(workspace && workspace_bytes >= layout_end<ClBwdWs>(N, P, C, B, pl) + 256, "bb_contrastive_backward: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   if (pl.tiles1 == 0) {   // every group empty: zero descriptor gradients, nothing into dE
     if (B > 0) {
@@ -591,85 +598,71 @@ int dinotrk_bb_contrastive_backward(const float* E, int N, int P, int C, const f
   }
   ProfRange pr(PROF_CONTRASTIVE, st);
   const int Pp = pad8(P), Kx = pl.Kx;
-  Arena ar(workspace, workspace_bytes);
-  float* en = ar.take<float>((size_t)N * P);
-  float* desc = ar.take<float>((size_t)2 * B * C);
-  float* dn = ar.take<float>((size_t)2 * B);
-  float* rcorr = ar.take<float>((size_t)2 * B);
-  unsigned* amax = ar.take<unsigned>(1);
-  float* dbuf = ar.take<float>((size_t)2 * B * Pp);
-  __half* a1_hi = ar.take<__half>((size_t)2 * B * Pp);
-  __half* a1_lo = ar.take<__half>((size_t)2 * B * Pp);
-  __half* b1_hi = ar.take<__half>((size_t)N * C * Pp);
-  __half* b1_lo = ar.take<__half>((size_t)N * C * Pp);
-  __half* a2_hi = ar.take<__half>((size_t)N * Pp * Kx);
-  __half* a2_lo = ar.take<__half>((size_t)N * Pp * Kx);
-  __half* b2_hi = ar.take<__half>((size_t)N * C * Kx);
-  __half* b2_lo = ar.take<__half>((size_t)N * C * Kx);
+  Arena ar(workspace);
+  const ClBwdWs ws(ar, N, P, C, B, pl);
   int rc = DINOTRK_OK;
-  int* d_frame = upload(ar, pl.frame, st, &rc);
-  int* d_row0 = upload(ar, pl.row0, st, &rc);
-  int* d_m = upload(ar, pl.m, st, &rc);
-  int* d_tiles = upload(ar, pl.tile_start, st, &rc);
-  int* d_row_grp = upload(ar, pl.row_grp, st, &rc);
-  int* d_row_frame = upload(ar, pl.row_frame, st, &rc);
-  int* d_frame_k = upload(ar, pl.frame_k, st, &rc);
-  int* d_frame_rows = upload(ar, pl.frame_rows, st, &rc);
-  int* d_fb = upload(ar, pl.f_batch, st, &rc);
-  int* d_fr0 = upload(ar, pl.f_row0, st, &rc);
-  int* d_fm = upload(ar, pl.f_m, st, &rc);
-  int* d_ft = upload(ar, pl.f_tiles, st, &rc);
+  upload(ws.frame, pl.frame, st, &rc);
+  upload(ws.row0, pl.row0, st, &rc);
+  upload(ws.m, pl.m, st, &rc);
+  upload(ws.tile_start, pl.tile_start, st, &rc);
+  upload(ws.row_grp, pl.row_grp, st, &rc);
+  upload(ws.row_frame, pl.row_frame, st, &rc);
+  upload(ws.frame_k, pl.frame_k, st, &rc);
+  upload(ws.frame_rows, pl.frame_rows, st, &rc);
+  upload(ws.f_batch, pl.f_batch, st, &rc);
+  upload(ws.f_row0, pl.f_row0, st, &rc);
+  upload(ws.f_m, pl.f_m, st, &rc);
+  upload(ws.f_tiles, pl.f_tiles, st, &rc);
   std::vector<int> grows(n_groups);
   for (int g = 0; g < n_groups; ++g) grows[g] = grp_rows[g];
-  int* d_grows = upload(ar, grows, st, &rc);
+  upload(ws.grows, grows, st, &rc);
   if (rc) return rc;
-  DTK_CHECK_ARG(ar.ok(), "bb_contrastive_backward: workspace layout");
-  DTK_CUDA(cudaMemcpyAsync(desc, S, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
-  DTK_CUDA(cudaMemcpyAsync(desc + (size_t)B * C, U, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
-  DTK_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), st));
+  DTK_CUDA(cudaMemcpyAsync(ws.desc, S, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
+  DTK_CUDA(cudaMemcpyAsync(ws.desc + (size_t)B * C, U, (size_t)B * C * 4, cudaMemcpyDeviceToDevice, st));
+  DTK_CUDA(cudaMemsetAsync(ws.amax, 0, sizeof(unsigned), st));
   const size_t toks = (size_t)N * P;
-  cl_norms_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(E, toks, C, en);
+  cl_norms_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(E, toks, C, ws.en);
   DTK_LAUNCHED();
-  cl_norms_kernel<<<(unsigned)((2 * (size_t)B * 32 + 255) / 256), 256, 0, st>>>(desc, 2 * (size_t)B, C, dn);
+  cl_norms_kernel<<<(unsigned)((2 * (size_t)B * 32 + 255) / 256), 256, 0, st>>>(ws.desc, 2 * (size_t)B, C, ws.dn);
   DTK_LAUNCHED();
-  ClGrad gr{cosm, Pp, out, g_st, g_ts, g_cmean, d_row_grp, d_grows, dn, en, d_row_frame, B, P, 1.f / tau};
-  cl_drow_kernel<<<2 * B, CL_THREADS, 0, st>>>(gr, Pp, dbuf, rcorr, amax);
+  ClGrad gr{cosm, Pp, out, g_st, g_ts, g_cmean, ws.row_grp, ws.grows, ws.dn, ws.en, ws.row_frame, B, P, 1.f / tau};
+  cl_drow_kernel<<<2 * B, CL_THREADS, 0, st>>>(gr, Pp, ws.dbuf, ws.rcorr, ws.amax);
   DTK_LAUNCHED();
   {
     const size_t n = (size_t)2 * B * Pp;
     unsigned grid = (unsigned)((n + 255) / 256);
     if (grid > (unsigned)num_sms() * 16) grid = num_sms() * 16;
-    cl_split_rows_kernel<<<grid, 256, 0, st>>>(dbuf, amax, a1_hi, a1_lo, n);
+    cl_split_rows_kernel<<<grid, 256, 0, st>>>(ws.dbuf, ws.amax, ws.a1_hi, ws.a1_lo, n);
     DTK_LAUNCHED();
   }
   const dim3 tb(32, 8);
-  cl_transpose_split_kernel<<<dim3(cdiv(Pp, 32), cdiv(C, 32), N), tb, 0, st>>>(SrcEhatT{E, en, P, C}, Pp, C, Pp, b1_hi, b1_lo);
+  cl_transpose_split_kernel<<<dim3(cdiv(Pp, 32), cdiv(C, 32), N), tb, 0, st>>>(SrcEhatT{E, ws.en, P, C}, Pp, C, Pp, ws.b1_hi, ws.b1_lo);
   DTK_LAUNCHED();
-  cl_transpose_split_kernel<<<dim3(cdiv(Kx, 32), cdiv(Pp, 32), N), tb, 0, st>>>(SrcDT{dbuf, d_frame_rows, amax, Pp, Kx}, Kx, Pp,
-                                                                                  Kx, a2_hi, a2_lo);
+  cl_transpose_split_kernel<<<dim3(cdiv(Kx, 32), cdiv(Pp, 32), N), tb, 0, st>>>(SrcDT{ws.dbuf, ws.frame_rows, ws.amax, Pp, Kx}, Kx, Pp,
+                                                                                  Kx, ws.a2_hi, ws.a2_lo);
   DTK_LAUNCHED();
-  cl_transpose_split_kernel<<<dim3(cdiv(Kx, 32), cdiv(C, 32), N), tb, 0, st>>>(SrcDescT{desc, dn, d_frame_rows, C, Kx}, Kx, C,
-                                                                                 Kx, b2_hi, b2_lo);
+  cl_transpose_split_kernel<<<dim3(cdiv(Kx, 32), cdiv(C, 32), N), tb, 0, st>>>(SrcDescT{ws.desc, ws.dn, ws.frame_rows, C, Kx}, Kx, C,
+                                                                                 Kx, ws.b2_hi, ws.b2_lo);
   DTK_LAUNCHED();
   // GEMM 1: dS / dU over K = P in chains of CL_K_CHUNK, the first chain overwrites; one launch per chain [k0, k0 + kc)
   for (int k0 = 0; k0 < P; k0 += CL_K_CHUNK) {
-    EpiDesc epi{dS, dU, dn, d_row0, amax, B, C, k0 > 0};
-    const TcProblem pb{d_frame, d_row0, d_m, d_tiles, pl.G2, C, std::min(CL_K_CHUNK, P - k0)};
-    if ((rc = tc_launch_bn<TcMode::F16X3>({a1_hi + k0, a1_lo + k0, (uint64_t)2 * B, (uint64_t)Pp, b1_hi + k0, b1_lo + k0,
+    EpiDesc epi{dS, dU, ws.dn, ws.row0, ws.amax, B, C, k0 > 0};
+    const TcProblem pb{ws.frame, ws.row0, ws.m, ws.tile_start, pl.G2, C, std::min(CL_K_CHUNK, P - k0)};
+    if ((rc = tc_launch_bn<TcMode::F16X3>({ws.a1_hi + k0, ws.a1_lo + k0, (uint64_t)2 * B, (uint64_t)Pp, ws.b1_hi + k0, ws.b1_lo + k0,
                                            (uint64_t)N, (uint64_t)Pp}, pb, pl.tiles1, epi, st)))
       return rc;
   }
   cl_row_finish_kernel<<<(unsigned)((2 * (size_t)B * 32 + 255) / 256), 256, 0, st>>>(
-      gr, E, desc, dn, rcorr, out, g_st, g_ts, g_bbmean, d_row_grp, d_grows, B, C, 1.f / tau, dS, dU);
+      gr, E, ws.desc, ws.dn, ws.rcorr, out, g_st, g_ts, g_bbmean, ws.row_grp, ws.grows, B, C, 1.f / tau, dS, dU);
   DTK_LAUNCHED();
   // dE: the norm correction, then GEMM 2 over the frame's rows in chains of CL_K_CHUNK
-  cl_tok_corr_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(gr, E, desc, d_frame_rows, d_frame_k, N, Kx, C, dE);
+  cl_tok_corr_kernel<<<(unsigned)((toks * 32 + 255) / 256), 256, 0, st>>>(gr, E, ws.desc, ws.frame_rows, ws.frame_k, N, Kx, C, dE);
   DTK_LAUNCHED();
   if (pl.tiles2 > 0) {
-    EpiTok epi{dE, en, d_fb, amax, P, C};
+    EpiTok epi{dE, ws.en, ws.f_batch, ws.amax, P, C};
     for (int k0 = 0; k0 < Kx; k0 += CL_K_CHUNK) {
-      const TcProblem pb{d_fb, d_fr0, d_fm, d_ft, N, C, std::min(CL_K_CHUNK, Kx - k0)};
-      if ((rc = tc_launch_bn<TcMode::F16X3>({a2_hi + k0, a2_lo + k0, (uint64_t)N * Pp, (uint64_t)Kx, b2_hi + k0, b2_lo + k0,
+      const TcProblem pb{ws.f_batch, ws.f_row0, ws.f_m, ws.f_tiles, N, C, std::min(CL_K_CHUNK, Kx - k0)};
+      if ((rc = tc_launch_bn<TcMode::F16X3>({ws.a2_hi + k0, ws.a2_lo + k0, (uint64_t)N * Pp, (uint64_t)Kx, ws.b2_hi + k0, ws.b2_lo + k0,
                                              (uint64_t)N, (uint64_t)Kx}, pb, pl.tiles2, epi, st)))
         return rc;
     }

@@ -235,8 +235,6 @@ corr_stream_kernel(const float* __restrict__ tpc, const float* __restrict__ norm
   }
 }
 
-size_t corr_plan_bytes(int n_groups) { return align_up((size_t)(n_groups + 1) * sizeof(int), 256); }
-
 int launch_corr_maps(const FeatView& fv, const float* desc, int desc_rows, const float* desc_norm,
                      const int* grp_frame, const int* grp_row0, const int* grp_m, const int* grp_map0, int n_groups,
                      int total_maps, int max_group_m, float* maps, int map_stride, int* tile_start, float* split_ws,
@@ -313,7 +311,7 @@ extern "C" {
 int dinotrk_map_stride(const dinotrk_geom* g) { return g ? (int)align_up((size_t)g->h * g->w, 4) : 0; }
 
 size_t dinotrk_corr_maps_workspace_bytes(int total_maps, int n_groups, int C) {
-  return corr_plan_bytes(n_groups) + corr_tc_workspace_bytes(total_maps, C) + 1024;
+  return align_up(layout_end<CorrMapsWs>(total_maps, n_groups, C), 256) + 1024;
 }
 
 int dinotrk_corr_maps(const dinotrk_features* feat, const dinotrk_geom* g, const float* desc, const float* desc_norm,
@@ -326,12 +324,11 @@ int dinotrk_corr_maps(const dinotrk_features* feat, const dinotrk_geom* g, const
   DTK_CHECK_ARG((feat->hi == nullptr) == (feat->lo == nullptr), "corr_maps: hi and lo must be given together");
   DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_corr_maps_workspace_bytes(total_maps, n_groups, feat->C),
                 "corr_maps: workspace too small");
-  Arena ar(workspace, workspace_bytes);
-  int* plan = ar.take<int>(n_groups + 1);
-  float* split = ar.take<float>(corr_tc_workspace_bytes(total_maps, feat->C) / 4);
+  Arena ar(workspace);
+  const CorrMapsWs ws(ar, total_maps, n_groups, feat->C);
   // rows of desc = total_maps here (one descriptor row per map is the generic contract)
   return launch_corr_maps(make_view(*feat, *g), desc, total_maps, desc_norm, grp_frame, grp_row0, grp_m, grp_map0,
-                          n_groups, total_maps, max_group_m, maps, dinotrk_map_stride(g), plan, split,
+                          n_groups, total_maps, max_group_m, maps, dinotrk_map_stride(g), ws.plan, ws.split,
                           (cudaStream_t)stream);
 }
 

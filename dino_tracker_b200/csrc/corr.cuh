@@ -51,9 +51,20 @@ struct CorrAssist {
   bool small_tiles = false;   // tensor path: 128-row single-CTA tiles instead of 256-row CTA-pair tiles (many tiny groups)
 };
 
-size_t corr_plan_bytes(int n_groups);
 int corr_tc_tile_rows();   // 256: CTA-pair (two-CTA cluster) kernel, the default; 128: single-CTA kernel (DTK_CORR_PAIRS=0)
 size_t corr_tc_workspace_bytes(int total_rows, int C);
+// The separate-halves split of `rows` descriptor rows of C channels in a split workspace (corr_tc_workspace_bytes): hi rows,
+// then lo rows at the next 256-byte boundary.
+struct DescSplit {
+  char* hi; char* lo;
+  DescSplit(void* ws, size_t rows, int C) : hi(static_cast<char*>(ws)), lo(hi + align_up(rows * C * 2, 256)) {}
+};
+// workspace of launch_corr_maps: the GEMM tile plan of n_groups groups and the split of `rows` descriptor rows
+struct CorrMapsWs {
+  int* plan; float* split;
+  CorrMapsWs(Arena& ar, int rows, int n_groups, int C)
+      : plan(ar.take<int>(n_groups + 1)), split(ar.take<float>(corr_tc_workspace_bytes(rows, C) / 4)) {}
+};
 // desc_rows = number of rows of the desc array (bounds of its tensor map); split_ws: corr_tc_workspace_bytes
 // (only touched when fv.tensor()).
 int launch_corr_maps(const FeatView& fv, const float* desc, int desc_rows, const float* desc_norm,

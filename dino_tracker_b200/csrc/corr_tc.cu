@@ -318,11 +318,10 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
     return pairs ? tc_launch<TcMode::F16X3I, Epi, TC_BN, true>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM)
                  : tc_launch<TcMode::F16X3I, Epi>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM);
   }
-  char* d_hi = reinterpret_cast<char*>(desc_split_ws);
-  char* d_lo = d_hi + align_up((size_t)desc_rows * C * 2, 256);
-  int rc = split_ready ? DINOTRK_OK : launch_split_f16(desc, d_hi, d_lo, (size_t)desc_rows * C, st);
+  const DescSplit d(desc_split_ws, desc_rows, C);
+  int rc = split_ready ? DINOTRK_OK : launch_split_f16(desc, d.hi, d.lo, (size_t)desc_rows * C, st);
   if (rc) return rc;
-  const TcOperands op{d_hi, d_lo, (uint64_t)desc_rows, 0, tpc_hi, tpc_lo, (uint64_t)T, 0};
+  const TcOperands op{d.hi, d.lo, (uint64_t)desc_rows, 0, tpc_hi, tpc_lo, (uint64_t)T, 0};
   auto run = [&](const auto& epi) {
     using Epi = std::decay_t<decltype(epi)>;
     return pairs ? tc_launch<TcMode::F16X3, Epi, TC_BN, true>(op, pb, max_tiles, epi, st, PROF_CORR_GEMM)

@@ -156,6 +156,11 @@ cycle_keep_kernel(const float* __restrict__ start, const float* __restrict__ bac
   if (threadIdx.x == 0) *n_keep = base;
 }
 
+struct CycleMaskWs {
+  int* cnt;   // [T][cdiv(P, CYC_THREADS)] foreground pixels per block
+  CycleMaskWs(Arena& ar, int T, int P) { cnt = ar.take<int>((size_t)T * cdiv(P, CYC_THREADS)); }
+};
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -208,7 +213,7 @@ int dinotrk_randperm_prefix(uint8_t* state, size_t state_bytes, int64_t n, int64
 
 size_t dinotrk_cycle_mask_workspace_bytes(int T, int P) {
   if (T <= 0 || P <= 0) return 0;
-  return align_up((size_t)T * cdiv(P, CYC_THREADS) * sizeof(int), 256) + align_up((size_t)T * sizeof(int), 256);
+  return align_up(layout_end<CycleMaskWs>(T, P), 256);
 }
 
 int dinotrk_cycle_mask_scan(const uint8_t* fg, int T, int P, int* off, int* n_fg, void* workspace, size_t workspace_bytes,
@@ -217,8 +222,8 @@ int dinotrk_cycle_mask_scan(const uint8_t* fg, int T, int P, int* off, int* n_fg
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_cycle_mask_workspace_bytes(T, P), "cycle_mask_scan: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(P, CYC_THREADS);
-  Arena ar(workspace, workspace_bytes);
-  int* cnt = ar.take<int>((size_t)T * nb);
+  Arena ar(workspace);
+  int* cnt = CycleMaskWs(ar, T, P).cnt;
   ProfRange pr(PROF_CYCLE, st);
   cycle_mask_count_kernel<<<dim3(nb, T), CYC_THREADS, 0, st>>>(fg, P, nb, cnt);
   DTK_LAUNCHED();

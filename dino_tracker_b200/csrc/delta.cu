@@ -335,10 +335,24 @@ static size_t delta_max_activation(int B, int H, int W, const int* channels) {
   return best;
 }
 
+// two activation buffers; the tensor-core path adds its fp16 im2col scratch and tile plan
+struct DeltaWs {
+  float* buf0; float* buf1; __half* col_hi = nullptr; __half* col_lo = nullptr; int* cplan = nullptr;
+  DeltaWs(Arena& ar, int B, int H, int W, const int* channels, bool tensor) {
+    const size_t half = delta_max_activation(B, H, W, channels);
+    buf0 = ar.take<float>(half);
+    buf1 = ar.take<float>(half);
+    if (tensor) {
+      const size_t kmax = delta_conv_kmax(channels);
+      col_hi = ar.take<__half>(CONV_TC_ROWS * kmax);
+      col_lo = ar.take<__half>(CONV_TC_ROWS * kmax);
+      cplan = ar.take<int>(16);
+    }
+  }
+};
+
 size_t dinotrk_delta_workspace_bytes(int B, int H, int W, const int* channels) {
-  const size_t kmax = delta_conv_kmax(channels);
-  return 2 * align_up(delta_max_activation(B, H, W, channels) * sizeof(float), 256) +
-         2 * align_up(CONV_TC_ROWS * kmax * 2, 256) + 8192;   // + fp16 im2col scratch of the tensor-core path
+  return align_up(layout_end<DeltaWs>(B, H, W, channels, true), 256) + 7936;
 }
 
 static int delta_refine_impl(const float* frames, int B, int H, int W, const int* channels, const float* const* wgt,
@@ -355,32 +369,22 @@ static int delta_refine_impl(const float* frames, int B, int H, int W, const int
   DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_delta_workspace_bytes(B, H, W, channels),
                 "delta_refine: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  Arena ar(workspace, workspace_bytes);
-  size_t half = delta_max_activation(B, H, W, channels);
-  float* buf0 = ar.take<float>(half);
-  float* buf1 = ar.take<float>(half);
   const bool tensor = wgt_hi != nullptr && wgt_lo != nullptr;
-  __half* col_hi = nullptr; __half* col_lo = nullptr; int* cplan = nullptr;
-  if (tensor) {
-    const size_t kmax = delta_conv_kmax(channels);
-    col_hi = ar.take<__half>(CONV_TC_ROWS * kmax);
-    col_lo = ar.take<__half>(CONV_TC_ROWS * kmax);
-    cplan = ar.take<int>(16);
-    DTK_CHECK_ARG(ar.ok(), "delta_refine: workspace too small for the tensor-core path");
-  }
+  Arena ar(workspace);
+  const DeltaWs ws(ar, B, H, W, channels, tensor);
 
   {
     ProfRange pr(PROF_MISC, st);
-    if (int rc = launch_rgb_to_nhwc4(frames, buf0, B, H * W, st)) return rc;
+    if (int rc = launch_rgb_to_nhwc4(frames, ws.buf0, B, H * W, st)) return rc;
   }
   int ch = H, cw = W, cin = 4;
-  float* cur = buf0;
-  float* oth = buf1;
+  float* cur = ws.buf0;
+  float* oth = ws.buf1;
   const int dil[4] = {1, 1, 1, 2};
   for (int l = 0; l < 4; ++l) {
     ConvShape cs{B, ch, cw, cin, channels[l + 1], dil[l], l < 3 ? 1 : 0};
     int rc = tensor ? launch_conv_tc(cur, (const __half*)wgt_hi[l], (const __half*)wgt_lo[l], bias[l], oth, cs,
-                                     (int)align_up((size_t)25 * cin, 8), col_hi, col_lo, cplan, st)
+                                     (int)align_up((size_t)25 * cin, 8), ws.col_hi, ws.col_lo, ws.cplan, st)
                     : launch_conv(cur, wgt[l], bias[l], oth, cs, st);
     if (rc) return rc;
     std::swap(cur, oth);

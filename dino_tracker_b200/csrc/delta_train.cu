@@ -56,18 +56,14 @@ struct SavedView {
   float* y[4];         // pre-BN conv outputs, NHWC
   double* mean[4];     // per-channel mean used by the forward (batch or running)
   double* invstd[4];   // 1 / sqrt(var + eps)
-};
-
-static size_t saved_view(void* base, const TrainGeom& g, SavedView* v) {
-  Arena ar(base, ~(size_t)0);
-  for (int l = 0; l < 4; ++l) {
-    float* y = ar.take<float>(g.M(l) * g.cout[l]);
-    double* m = ar.take<double>(g.cout[l]);
-    double* s = ar.take<double>(g.cout[l]);
-    if (v) { v->y[l] = y; v->mean[l] = m; v->invstd[l] = s; }
+  SavedView(Arena& ar, const TrainGeom& g) {
+    for (int l = 0; l < 4; ++l) {
+      y[l] = ar.take<float>(g.M(l) * g.cout[l]);
+      mean[l] = ar.take<double>(g.cout[l]);
+      invstd[l] = ar.take<double>(g.cout[l]);
+    }
   }
-  return ar.off;
-}
+};
 
 // ---- BatchNorm ------------------------------------------------------------------------------------------------------
 // Per-channel sums over the M rows of an NHWC [M][C] tensor, in float64, block partials in a fixed order:
@@ -581,42 +577,38 @@ static int max_channels(const int* channels) {
   return c;
 }
 
-struct FwdWs { float* x; __half* col_hi; __half* col_lo; int* plan; double2* part; };
-static size_t fwd_ws(void* base, const TrainGeom& g, const int* channels, FwdWs* w) {
-  Arena ar(base, ~(size_t)0);
-  FwdWs v;
-  v.x = ar.take<float>(max_input_elems(g));
-  v.col_hi = ar.take<__half>(col_elems_of(channels));
-  v.col_lo = ar.take<__half>(col_elems_of(channels));
-  v.plan = ar.take<int>(16);
-  v.part = ar.take<double2>((size_t)BN_MAX_BLOCKS * max_channels(channels));
-  if (w) *w = v;
-  return ar.off;
-}
+struct FwdWs {
+  float* x; __half* col_hi; __half* col_lo; int* plan; double2* part;
+  FwdWs(Arena& ar, const TrainGeom& g, const int* channels) {
+    x = ar.take<float>(max_input_elems(g));
+    col_hi = ar.take<__half>(col_elems_of(channels));
+    col_lo = ar.take<__half>(col_elems_of(channels));
+    plan = ar.take<int>(16);
+    part = ar.take<double2>((size_t)BN_MAX_BLOCKS * max_channels(channels));
+  }
+};
 
-struct BwdWs { float* g; float* x; float* xp; __half* col_hi; __half* col_lo; float* wpart; double* wacc; int* plan; double2* part;
-               double* m_dz; double* m_dzx; unsigned* amax; };
-static size_t bwd_ws(void* base, const TrainGeom& g, const int* channels, BwdWs* w) {
-  Arena ar(base, ~(size_t)0);
-  BwdWs v;
-  const size_t ce = col_elems_of(channels);
-  v.g = ar.take<float>(max_output_elems(g));
-  v.x = ar.take<float>(max_input_elems(g));
-  v.xp = ar.take<float>(max_padded_elems(g));
-  v.col_hi = ar.take<__half>(ce);
-  v.col_lo = ar.take<__half>(ce);
-  v.wpart = ar.take<float>(wgrad_part_elems(g, ce));
-  size_t wmax = 0;
-  for (int l = 0; l < 4; ++l) wmax = (size_t)g.cout[l] * g.Kp[l] > wmax ? (size_t)g.cout[l] * g.Kp[l] : wmax;
-  v.wacc = ar.take<double>(wmax);
-  v.plan = ar.take<int>(4 * WG_MAX_SPLITS + 1);
-  v.part = ar.take<double2>((size_t)BN_MAX_BLOCKS * max_channels(channels));
-  v.m_dz = ar.take<double>(max_channels(channels));
-  v.m_dzx = ar.take<double>(max_channels(channels));
-  v.amax = ar.take<unsigned>(1);
-  if (w) *w = v;
-  return ar.off;
-}
+struct BwdWs {
+  float* g; float* x; float* xp; __half* col_hi; __half* col_lo; float* wpart; double* wacc; int* plan; double2* part;
+  double* m_dz; double* m_dzx; unsigned* amax;
+  BwdWs(Arena& ar, const TrainGeom& tg, const int* channels) {
+    const size_t ce = col_elems_of(channels);
+    g = ar.take<float>(max_output_elems(tg));
+    x = ar.take<float>(max_input_elems(tg));
+    xp = ar.take<float>(max_padded_elems(tg));
+    col_hi = ar.take<__half>(ce);
+    col_lo = ar.take<__half>(ce);
+    wpart = ar.take<float>(wgrad_part_elems(tg, ce));
+    size_t wmax = 0;
+    for (int l = 0; l < 4; ++l) wmax = (size_t)tg.cout[l] * tg.Kp[l] > wmax ? (size_t)tg.cout[l] * tg.Kp[l] : wmax;
+    wacc = ar.take<double>(wmax);
+    plan = ar.take<int>(4 * WG_MAX_SPLITS + 1);
+    part = ar.take<double2>((size_t)BN_MAX_BLOCKS * max_channels(channels));
+    m_dz = ar.take<double>(max_channels(channels));
+    m_dzx = ar.take<double>(max_channels(channels));
+    amax = ar.take<unsigned>(1);
+  }
+};
 
 }  // namespace dtk
 
@@ -626,17 +618,17 @@ extern "C" {
 
 size_t dinotrk_delta_train_saved_bytes(int B, int H, int W, const int* channels) {
   if (!channels || B < 0) return 0;
-  return saved_view(nullptr, train_geom(B, H, W, channels), nullptr);
+  return layout_end<SavedView>(train_geom(B, H, W, channels));
 }
 
 size_t dinotrk_delta_train_forward_workspace_bytes(int B, int H, int W, const int* channels) {
   if (!channels || B < 0) return 0;
-  return fwd_ws(nullptr, train_geom(B, H, W, channels), channels, nullptr);
+  return layout_end<FwdWs>(train_geom(B, H, W, channels), channels);
 }
 
 size_t dinotrk_delta_train_backward_workspace_bytes(int B, int H, int W, const int* channels) {
   if (!channels || B < 0) return 0;
-  return bwd_ws(nullptr, train_geom(B, H, W, channels), channels, nullptr);
+  return layout_end<BwdWs>(train_geom(B, H, W, channels), channels);
 }
 
 static bool all_set(const void* const* a, int from = 0) {
@@ -666,10 +658,9 @@ int dinotrk_delta_train_forward(const float* frames, int B, int H, int W, const 
   if (B == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const TrainGeom g = train_geom(B, H, W, channels);
-  SavedView sv;
-  saved_view(saved, g, &sv);
-  FwdWs ws;
-  fwd_ws(workspace, g, channels, &ws);
+  Arena saved_ar(saved), ar(workspace);
+  const SavedView sv(saved_ar, g);
+  const FwdWs ws(ar, g, channels);
   for (int l = 0; l < 4; ++l) {
     {
       ProfRange pr(PROF_DELTA_BN, st);
@@ -709,10 +700,9 @@ int dinotrk_delta_train_backward(const float* frames, int B, int H, int W, const
   if (B == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const TrainGeom g = train_geom(B, H, W, channels);
-  SavedView sv;
-  saved_view(const_cast<void*>(saved), g, &sv);
-  BwdWs ws;
-  bwd_ws(workspace, g, channels, &ws);
+  Arena saved_ar(const_cast<void*>(saved)), ar(workspace);
+  const SavedView sv(saved_ar, g);
+  const BwdWs ws(ar, g, channels);
   const size_t ce = col_elems_of(channels);
   {
     ProfRange pr(PROF_ALIGN, st);

@@ -472,21 +472,18 @@ int dinotrk_fg_mask(const float* a, int T, int h, int w, int C, int q, const flo
   return dinotrk_mask_upsample(token_mask, T, h, w, H, W, mask, stream);
 }
 
-size_t dinotrk_traj_split_workspace_bytes(int N) {
-  const size_t nb = (size_t)(N > 0 ? (N + SPLIT_THREADS - 1) / SPLIT_THREADS : 1);
-  return align_up((size_t)std::max(N, 1), 256) + 2 * align_up(nb * 4, 256) + 256 + 256;
-}
-
 struct SplitWs {
   uint8_t* cls; int* cnt; int* off; int* counts;
-  SplitWs(void* ws, int N, size_t nb) {
-    Arena ar(ws, (size_t)-1);
+  SplitWs(Arena& ar, int N) {
+    const size_t nb = (size_t)(N > 0 ? cdiv(N, SPLIT_THREADS) : 1);
     cls = ar.take<uint8_t>((size_t)std::max(N, 1));
     cnt = ar.take<int>(nb);
     off = ar.take<int>(nb);
     counts = ar.take<int>(4);
   }
 };
+
+size_t dinotrk_traj_split_workspace_bytes(int N) { return align_up(layout_end<SplitWs>(N), 256) + 256; }
 
 int dinotrk_traj_split_count(const float* traj, int N, int T, const uint8_t* masks, int Tm, int H, int W, int* n_fg,
                              void* workspace, size_t workspace_bytes, void* stream) {
@@ -495,7 +492,8 @@ int dinotrk_traj_split_count(const float* traj, int N, int T, const uint8_t* mas
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_traj_split_workspace_bytes(N), "traj_split_count: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(N, SPLIT_THREADS);
-  SplitWs w(workspace, N, nb);
+  Arena ar(workspace);
+  const SplitWs w(ar, N);
   const int init[4] = {0, 0, N, 0};
   DTK_CUDA(cudaMemcpyAsync(w.counts, init, sizeof(init), cudaMemcpyHostToDevice, st));
   {
@@ -520,7 +518,8 @@ int dinotrk_traj_split_emit(const float* traj, int N, int T, float* fg, float* b
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_traj_split_workspace_bytes(N), "traj_split_emit: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(N, SPLIT_THREADS);
-  SplitWs w(workspace, N, nb);
+  Arena ar(workspace);
+  const SplitWs w(ar, N);
   ProfRange pr(PROF_MISC, st);
   split_emit_kernel<<<nb, SPLIT_THREADS, 0, st>>>(reinterpret_cast<const float2*>(traj), N, T, w.cls, w.off,
                                                    reinterpret_cast<float2*>(fg), reinterpret_cast<float2*>(bg));

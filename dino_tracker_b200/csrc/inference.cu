@@ -543,6 +543,88 @@ static long long g_infer_stats[INFER_STATS] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 // of one per map: int8 loses above ~1/6 extra queued maps.  1/16 leaves a wide margin.
 constexpr int XW_S8_PROBE_QUEUE_DIV = 16;
 
+// workspace of dinotrk_corr_track: the maps, the correlation's plan and split, the head's list of uncertified maps
+struct CorrTrackWs {
+  float* maps; CorrMapsWs corr; int* hscratch;
+  CorrTrackWs(Arena& ar, int total_maps, int n_groups, int C, int map_stride)
+      : maps(ar.take<float>((size_t)total_maps * map_stride)), corr(ar, total_maps, n_groups, C),
+        hscratch(ar.take<int>(total_maps + 1)) {}
+};
+
+struct ChunkBufs {   // everything one chunk in flight owns
+  float* maps; float* desc; float* norm; int* plan; float* split; int* hscratch; unsigned long long* tkeys;
+  ChunkBufs() = default;
+  ChunkBufs(Arena& ar, int C, int N, int P, int ms, int ch, int gcap) {
+    maps = ar.take<float>((size_t)ch * ms);
+    desc = ar.take<float>((size_t)ch * C);
+    norm = ar.take<float>(ch);
+    plan = ar.take<int>(gcap + 1);
+    split = ar.take<float>(corr_tc_workspace_bytes(ch > N ? ch : N, C) / 4);
+    hscratch = ar.take<int>(ch + 1);
+    tkeys = ar.take<unsigned long long>((size_t)ch * cdiv(P, CORR_TILE));
+  }
+};
+
+// One ring slot of the exact-window pipeline: its rows [row0, row0 + ch) of the descriptor table and its per-map arrays
+// (norm: per map; for a gathered map also its row's).
+struct XwSet {
+  int row0; float* norm; int* out_index; int* arow; float* eps; XwChunk xc;
+  XwSet() = default;
+  XwSet(Arena& ar, int row0_, float* u_norm, int P, int ch, int gcap) : row0(row0_), norm(u_norm + row0_) {
+    out_index = ar.take<int>(ch);
+    arow = ar.take<int>(ch);
+    eps = ar.take<float>(ch);
+    xc = XwChunk(ar, ch, (size_t)ch + 2, cdiv(P, XW_TILE), gcap);   // cells have >= 1 row
+  }
+};
+
+// The workspace of dinotrk_infer for chunks of ch maps, gcap groups per chunk and at most max_chunks chunks per phase.
+struct InferWs {
+  float* descA; float* normA;
+  ChunkBufs cb[2];
+  int* out_index_ring[4];   // written by the sampler of chunk k, read by both head kernels of chunk k (the second one late)
+  int* d_groups; int* d_cnt; int* d_qlist;
+  // Descriptor rows of the exact-window GEMMs, one row numbering for every per-row array: rows [0, N T) are the unique
+  // table (row n T + i: trajectory point i of query n), rows N T + k ch + j the gathered map j of ring slot k.  One A
+  // tensor map per operand covers both, so a group reads its rows wherever they are.
+  size_t xw_rows;
+  __half* u_hi; __half* u_lo; int8_t* u_q8; float* u_norm; float* u_fac; int* u_flag; float* u_rho;
+  float* d_rnorms; unsigned* d_minnorm;
+  XwSet xr[XW_RING];
+  int cell_nb;   // cells per trajectory
+  int* d_cells; int* d_tiles;
+  int sg_cap;    // groups of the accumulated full-map queue
+  int* d_cgrp; int* d_splan; int* d_cntA;
+  InferWs(Arena& ar, int T, int C, int N, int P, int ms, int ch, int gcap, size_t max_chunks) {
+    descA = ar.take<float>((size_t)N * C);
+    normA = ar.take<float>(N);
+    for (ChunkBufs& b : cb) b = ChunkBufs(ar, C, N, P, ms, ch, gcap);
+    for (int*& r : out_index_ring) r = ar.take<int>(ch);
+    d_groups = ar.take<int>(max_chunks * 5 * gcap);
+    d_cnt = ar.take<int>(T);
+    d_qlist = ar.take<int>((size_t)T * N);
+    const int n_unique = N * T;
+    xw_rows = (size_t)n_unique + (size_t)XW_RING * ch;
+    u_hi = ar.take<__half>(xw_rows * C);
+    u_lo = ar.take<__half>(xw_rows * C);
+    u_q8 = ar.take<int8_t>(xw_rows * C);
+    u_norm = ar.take<float>(xw_rows);
+    u_fac = ar.take<float>(xw_rows);
+    u_flag = ar.take<int>((size_t)N * T);
+    u_rho = ar.take<float>((size_t)N * T);
+    d_rnorms = ar.take<float>((size_t)T * P);
+    d_minnorm = ar.take<unsigned>(4);
+    for (int k = 0; k < XW_RING; ++k) xr[k] = XwSet(ar, n_unique + k * ch, u_norm, P, ch, gcap);
+    cell_nb = (T + XW_MAX_CELL - 1) / XW_MAX_CELL;
+    d_cells = ar.take<int>((size_t)N * T * cell_nb * 5 + 16);
+    d_tiles = ar.take<int>(max_chunks * (gcap + 1));
+    sg_cap = (int)std::min<size_t>(max_chunks * (size_t)gcap, 16384);
+    d_cgrp = ar.take<int>((size_t)4 * sg_cap);
+    d_splan = ar.take<int>((size_t)sg_cap + 1);
+    d_cntA = ar.take<int>(64);
+  }
+};
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -643,8 +725,7 @@ int dinotrk_infer_set_overlap(int mode) {
 
 size_t dinotrk_corr_track_workspace_bytes(int total_maps, int n_groups, int C, const dinotrk_geom* g) {
   if (!g) return 0;
-  return align_up((size_t)total_maps * dinotrk_map_stride(g) * sizeof(float), 256) + corr_plan_bytes(n_groups) +
-         corr_tc_workspace_bytes(total_maps, C) + align_up((size_t)(total_maps + 1) * 4, 256) + 1024;
+  return align_up(layout_end<CorrTrackWs>(total_maps, n_groups, C, dinotrk_map_stride(g)), 256) + 1024;
 }
 
 int dinotrk_corr_track(const dinotrk_features* feat, const dinotrk_geom* g,
@@ -660,58 +741,23 @@ int dinotrk_corr_track(const dinotrk_features* feat, const dinotrk_geom* g,
   DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_corr_track_workspace_bytes(total_maps, n_groups, C, g),
                 "corr_track: workspace too small");
   if (total_maps == 0) return DINOTRK_OK;
-  Arena ar(workspace, workspace_bytes);
   const int ms = dinotrk_map_stride(g);
-  float* maps = ar.take<float>((size_t)total_maps * ms);
-  int* plan = ar.take<int>(n_groups + 1);
-  float* split = ar.take<float>(corr_tc_workspace_bytes(total_maps, C) / 4);
-  int* hscratch = ar.take<int>(total_maps + 1);
+  Arena ar(workspace);
+  const CorrTrackWs ws(ar, total_maps, n_groups, C, ms);
   cudaStream_t st = (cudaStream_t)stream;
   int rc = launch_corr_maps(make_view(*feat, *g), desc, total_maps, desc_norm, grp_frame, grp_row0, grp_m, grp_map0,
-                            n_groups, total_maps, max_group_m, maps, ms, plan, split, st);
+                            n_groups, total_maps, max_group_m, ws.maps, ms, ws.corr.plan, ws.corr.split, st);
   if (rc) return rc;
-  return launch_head(maps, total_maps, ms, *g, *hw, out_index, out, out_stride, out_mode, nullptr, hscratch, st);
+  return launch_head(ws.maps, total_maps, ms, *g, *hw, out_index, out, out_stride, out_mode, nullptr, ws.hscratch, st);
 }
 
 
 size_t dinotrk_infer_workspace_bytes(int T, int C, const dinotrk_geom* g, int N, int chunk_maps) {
   if (!g) return 0;
-  const size_t ch = infer_chunk_eff(chunk_maps, T), ms = dinotrk_map_stride(g);
-  const int gcap = infer_gcap(T, (int)ch);
-  size_t b = 0;
-  b += align_up((size_t)N * C * 4, 256) + align_up((size_t)N * 4, 256);   // descA, normA
-  size_t c = 0;                                                            // per chunk buffer set (two: pipelining)
-  c += align_up(ch * ms * 4, 256);                                         // maps chunk
-  c += align_up(ch * C * 4, 256) + align_up(ch * 4, 256);                  // descC, normC
-  c += align_up((size_t)(gcap + 1) * 4, 256);                              // GEMM tile plan
-  c += corr_tc_workspace_bytes((int)(ch > (size_t)N ? ch : (size_t)N), C) + 256;  // fp16 split of the descriptors
-  c += align_up((ch + 1) * 4, 256);                                        // head: list of uncertified maps
-  c += align_up(ch * (size_t)cdiv(g->h * g->w, CORR_TILE) * 8, 256);       // tile keys of the chunk's maps
-  b += 2 * c;
-  b += 4 * align_up(ch * 4, 256);                                          // out_index ring
-  b += align_up(infer_max_chunks(T, N, ch) * 5 * gcap * 4, 256);           // group arrays of every chunk of a phase
-  b += align_up((size_t)T * 4, 256) + align_up((size_t)T * N * 4, 256);    // cnt, qlist
-  // exact-window pipeline: the unique descriptors with the rows of a ring of XW_RING chunks behind them, the ring's per-map
-  // arrays (out_index, eps, A row, keys, boxes), the cells of every chunk of the phase, coarse-GEMM tile prefixes, compact
-  // group arrays of the full-map queue
-  const size_t chx = ch;
-  const int nb = (T + XW_MAX_CELL - 1) / XW_MAX_CELL;
-  const size_t max_cells_chunk = chx + 2;                                  // cells have >= 1 row
-  size_t x = 0;
-  x += 3 * align_up(chx * 4, 256);                                         // out_index, eps, A row
-  x += xw_chunk_bytes((int)chx, (int)max_cells_chunk, cdiv(g->h * g->w, XW_TILE), gcap);
-  b += XW_RING * x;
-  const size_t rows = (size_t)N * T + XW_RING * chx;                                      // unique table + the ring's rows
-  b += 2 * align_up(rows * C * 2, 256) + align_up(rows * C, 256) + 2 * align_up(rows * 4, 256);   // hi, lo, int8, norm, factor
-  b += 2 * align_up((size_t)N * T * 4, 256);                                              // flags, residuals of the unique rows
-  b += align_up((size_t)T * g->h * g->w * 4, 256) + 256;                                  // reciprocal token norms, smallest norm
-  b += align_up((size_t)N * T * nb * 20 + 64, 256);                         // cells of all chunks
-  b += align_up(infer_max_chunks(T, N, ch) * (gcap + 1) * 4, 256);         // coarse tile prefixes per chunk
-  {
-    const size_t sg = std::min<size_t>(infer_max_chunks(T, N, ch) * (size_t)gcap, 16384);
-    b += align_up(4 * sg * 4, 256) + align_up((sg + 1) * 4, 256) + align_up(64 * 4, 256);   // queue group arrays + tile plan, phase-A counters
-  }
-  return b + 16384;
+  const int ch = infer_chunk_eff(chunk_maps, T);
+  const size_t end = layout_end<InferWs>(T, C, N, g->h * g->w, dinotrk_map_stride(g), ch, infer_gcap(T, ch),
+                                         infer_max_chunks(T, N, (size_t)ch));
+  return align_up(end, 256) + 25088;
 }
 
 int dinotrk_traj_cos_sims(const float* tpc, int T, int C, const dinotrk_geom* g, const float* traj,
@@ -780,72 +826,11 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   const int gcap = infer_gcap(T, ch);
   const PointAffine pa = make_point_affine(*g);
 
-  Arena ar(workspace, workspace_bytes);
-  float* descA = ar.take<float>((size_t)N * C);
-  float* normA = ar.take<float>(N);
-  struct ChunkBufs {   // everything one chunk in flight owns
-    float* maps; float* desc; float* norm; int* plan; float* split; int* hscratch; unsigned long long* tkeys;
-  } cb[2];
-  int* out_index_ring[4];   // written by the sampler of chunk k, read by both head kernels of chunk k (the second one late)
-  for (int k = 0; k < 2; ++k) {
-    cb[k].maps = ar.take<float>((size_t)ch * ms);
-    cb[k].desc = ar.take<float>((size_t)ch * C);
-    cb[k].norm = ar.take<float>(ch);
-    cb[k].plan = ar.take<int>(gcap + 1);
-    cb[k].split = ar.take<float>(corr_tc_workspace_bytes(ch > N ? ch : N, C) / 4);
-    cb[k].hscratch = ar.take<int>(ch + 1);
-    cb[k].tkeys = ar.take<unsigned long long>((size_t)ch * cdiv(P, CORR_TILE));
-  }
-  for (int k = 0; k < 4; ++k) out_index_ring[k] = ar.take<int>(ch);
   const size_t max_chunks = infer_max_chunks(T, N, (size_t)ch);
-  int* d_groups = ar.take<int>(max_chunks * 5 * gcap);
-  int* d_cnt = ar.take<int>(T);
-  int* d_qlist = ar.take<int>((size_t)T * N);
-  // Descriptor rows of the exact-window GEMMs, one row numbering for every per-row array: rows [0, N T) are the unique
-  // table (row n T + i: trajectory point i of query n), rows N T + k ch + j the gathered map j of ring slot k.  One A
-  // tensor map per operand covers both, so a group reads its rows wherever they are.
-  struct XwSet { int row0; float* norm; int* out_index; int* arow; float* eps; XwChunk xc; } xr[XW_RING];
-  const int n_tiles_map = cdiv(P, XW_TILE);     // coarse keys per map
+  Arena ar(workspace);
+  InferWs ws(ar, T, C, N, P, ms, ch, gcap, max_chunks);
   const int n_unique = N * T;
-  const size_t xw_rows = (size_t)n_unique + (size_t)XW_RING * ch;
-  __half* u_hi = ar.take<__half>(xw_rows * C);
-  __half* u_lo = ar.take<__half>(xw_rows * C);
-  int8_t* u_q8 = ar.take<int8_t>(xw_rows * C);
-  float* u_norm = ar.take<float>(xw_rows);
-  float* u_fac = ar.take<float>(xw_rows);
-  int* u_flag = ar.take<int>((size_t)N * T);
-  float* u_rho = ar.take<float>((size_t)N * T);
-  float* d_rnorms = ar.take<float>((size_t)T * P);
-  unsigned* d_minnorm = ar.take<unsigned>(4);
-  for (int k = 0; k < XW_RING; ++k) {
-    xr[k].row0 = n_unique + k * ch;
-    xr[k].norm = u_norm + xr[k].row0;   // per map; for a gathered map also its row's
-    xr[k].out_index = ar.take<int>(ch);
-    xr[k].arow = ar.take<int>(ch);
-    xr[k].eps = ar.take<float>(ch);
-    XwChunk& x = xr[k].xc;
-    x.key1 = ar.take<unsigned long long>((size_t)ch * n_tiles_map);
-    x.max2 = ar.take<float>((size_t)ch * n_tiles_map);
-    x.cand = ar.take<int>((size_t)ch * XW_MAX_CAND);
-    x.stat = ar.take<int>(ch);
-    x.pinfo = ar.take<int>(ch);
-    x.cell_of = ar.take<int>(ch);
-    x.slow_list = ar.take<int>(ch);
-    x.box_org = ar.take<int2>((size_t)ch + 2);
-    x.xbox = ar.take<float>((size_t)ch * XW_COLS);
-    x.win = ar.take<float>((size_t)ch * 256);
-    x.hin = ar.take<int2>(ch);
-    x.slow_cnt = ar.take<int>(gcap + 2);
-  }
-  const int cell_nb = (T + XW_MAX_CELL - 1) / XW_MAX_CELL;
-  int* d_cells = ar.take<int>((size_t)N * T * cell_nb * 5 + 16);
-  int* d_tiles = ar.take<int>(max_chunks * (gcap + 1));
-  const int sg_cap = (int)std::min<size_t>(max_chunks * (size_t)gcap, 16384);   // groups of the accumulated full-map queue
-  int* d_cgrp = ar.take<int>((size_t)4 * sg_cap);
-  int* d_splan = ar.take<int>((size_t)sg_cap + 1);
-  int* d_cntA = ar.take<int>(64);
-  DTK_CHECK_ARG(ar.ok(), "infer: workspace arena overflow");
-  DTK_CHECK_ARG(xw_rows <= 0x7fffffffu, "infer: %zu descriptor rows exceed the row index", xw_rows);
+  DTK_CHECK_ARG(ws.xw_rows <= 0x7fffffffu, "infer: %zu descriptor rows exceed the row index", ws.xw_rows);
   const bool tensor = fv.tensor();   // tensor-core GEMM: tile keys for the head, fp16 split fused into the samplers
   FeatView fv_split = fv;            // the full-map pipeline's sampler writes the separate halves: F16X3 there
   fv_split.hilo = nullptr;
@@ -857,12 +842,12 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
   auto upload_plan = [&]() -> int {
     DTK_CHECK_ARG(metas.size() <= max_chunks, "infer: chunk plan exceeds its bound (%zu > %zu)", metas.size(), max_chunks);
     if (!plan_host.empty())
-      DTK_CUDA(cudaMemcpyAsync(d_groups, plan_host.data(), plan_host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+      DTK_CUDA(cudaMemcpyAsync(ws.d_groups, plan_host.data(), plan_host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     return DINOTRK_OK;
   };
   struct Grp { const int *f, *r, *m, *map0, *item; };
   auto grp_of = [&](size_t k) {
-    const int* b = d_groups + k * 5 * gcap;
+    const int* b = ws.d_groups + k * 5 * gcap;
     return Grp{b, b + gcap, b + 2 * gcap, b + 3 * gcap, b + 4 * gcap};
   };
 
@@ -873,14 +858,14 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     NvtxRange nv("dinotrk.infer.A.trajectories");
     {
       ProfRange pr(PROF_SAMPLE, st);
-      sample_query_kernel<<<N, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, query_points, descA, normA);
+      sample_query_kernel<<<N, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, query_points, ws.descA, ws.normA);
       DTK_LAUNCHED();
     }
     if (tensor) {   // the query descriptors are reused by every chunk: split them once (layout of desc_rows = N)
       for (int k = 0; k < 2; ++k) {
-        char* a_hi = reinterpret_cast<char*>(cb[k].split);
-        int rc = corr_hilo(fv) ? launch_split_hilo(descA, a_hi, N, C, st)
-                               : launch_split_f16(descA, a_hi, a_hi + align_up((size_t)N * C * 2, 256), (size_t)N * C, st);
+        const DescSplit a(ws.cb[k].split, N, C);
+        int rc = corr_hilo(fv) ? launch_split_hilo(ws.descA, a.hi, N, C, st)
+                               : launch_split_f16(ws.descA, a.hi, a.lo, (size_t)N * C, st);
         if (rc) return rc;
       }
     }
@@ -889,22 +874,22 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     if (rc) return rc;
     for (size_t k = 0; k < metas.size(); ++k) {
       const ChunkMeta& cm = metas[k];
-      const ChunkBufs& b = cb[k & 1];
+      const ChunkBufs& b = ws.cb[k & 1];
       const Grp gp = grp_of(k);
       {
         ProfRange pr(PROF_MISC, st);
-        index_traj_kernel<<<cdiv(cm.used, 256), 256, 0, st>>>(gp.f, gp.r, gp.map0, cm.n_groups, cm.used, T, out_index_ring[k & 3], traj);
+        index_traj_kernel<<<cdiv(cm.used, 256), 256, 0, st>>>(gp.f, gp.r, gp.map0, cm.n_groups, cm.used, T, ws.out_index_ring[k & 3], traj);
         DTK_LAUNCHED();
       }
       CorrAssist as;
       as.tkeys = tensor ? b.tkeys : nullptr; as.zero_word = b.hscratch; as.split_ready = tensor; as.no_thin = cm.no_thin;
-      rc = launch_corr_maps(fv, descA, N, normA, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, ms, b.plan,
+      rc = launch_corr_maps(fv, ws.descA, N, ws.normA, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, ms, b.plan,
                             b.split, st, as);
       if (rc) return rc;
-      rc = launch_head(b.maps, cm.used, ms, *g, *hw, out_index_ring[k & 3], traj, 3, 0, nullptr, b.hscratch, st, as.tkeys, true);
+      rc = launch_head(b.maps, cm.used, ms, *g, *hw, ws.out_index_ring[k & 3], traj, 3, 0, nullptr, b.hscratch, st, as.tkeys, true);
       if (rc) return rc;
       if (k < 16)   // uncertified maps of this chunk: the anchor phase chooses its pipeline from their share
-        DTK_CUDA(cudaMemcpyAsync(d_cntA + k, b.hscratch, sizeof(int), cudaMemcpyDeviceToDevice, st));
+        DTK_CUDA(cudaMemcpyAsync(ws.d_cntA + k, b.hscratch, sizeof(int), cudaMemcpyDeviceToDevice, st));
     }
     n_chunks_A = (int)std::min<size_t>(metas.size(), 16);
     maps_A = (long long)N * T;
@@ -928,7 +913,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     NvtxRange nv("dinotrk.infer.C.anchors");
     {
       ProfRange pr(PROF_ANCHOR_LIST, st);
-      anchor_lists_kernel<<<T, ANCHOR_LIST_THREADS, 0, st>>>(cos_sims, N, T, anchor_th, d_cnt, d_qlist);
+      anchor_lists_kernel<<<T, ANCHOR_LIST_THREADS, 0, st>>>(cos_sims, N, T, anchor_th, ws.d_cnt, ws.d_qlist);
       DTK_LAUNCHED();
     }
     std::vector<int> cnt(T);
@@ -940,13 +925,13 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     XwAsync* xa = use_xw ? xw_async() : nullptr;
     if (!xa) use_xw = false;
     if (xa) {   // reciprocal token norms for the coarse epilogue + the smallest norm of the video (the host reads it below)
-      int rcn = launch_xw_rnorms(fv, d_rnorms, d_minnorm, st);
+      int rcn = launch_xw_rnorms(fv, ws.d_rnorms, ws.d_minnorm, st);
       if (rcn) return rcn;
-      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING + 16, d_minnorm, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING + 16, ws.d_minnorm, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     }
     if (xa && n_chunks_A > 0)
-      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING, d_cntA, (size_t)n_chunks_A * sizeof(int), cudaMemcpyDeviceToHost, st));
-    DTK_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
+      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING, ws.d_cntA, (size_t)n_chunks_A * sizeof(int), cudaMemcpyDeviceToHost, st));
+    DTK_CUDA(cudaMemcpyAsync(cnt.data(), ws.d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
     std::vector<float> rho_f(fv.s8() ? T : 0);
     if (fv.s8()) DTK_CUDA(cudaMemcpyAsync(rho_f.data(), fv.q_rho, (size_t)T * sizeof(float), cudaMemcpyDeviceToHost, st));
     std::vector<int> qlist_h, uflag_h;
@@ -956,13 +941,13 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       const bool q8 = fv.s8() && g_xw_coarse != 0 && C % 16 == 0 && C <= XW_S8_MAX_C;
       {
         ProfRange pr(PROF_SAMPLE, st);
-        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, u_hi, u_lo, u_norm, u_flag,
-                                                               q8 ? u_q8 : nullptr, u_fac, u_rho);
+        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, ws.u_hi, ws.u_lo, ws.u_norm, ws.u_flag,
+                                                               q8 ? ws.u_q8 : nullptr, ws.u_fac, ws.u_rho);
         DTK_LAUNCHED();
       }
       qlist_h.resize((size_t)T * N); uflag_h.resize((size_t)N * T);
-      DTK_CUDA(cudaMemcpyAsync(qlist_h.data(), d_qlist, qlist_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-      DTK_CUDA(cudaMemcpyAsync(uflag_h.data(), u_flag, uflag_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+      DTK_CUDA(cudaMemcpyAsync(qlist_h.data(), ws.d_qlist, qlist_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+      DTK_CUDA(cudaMemcpyAsync(uflag_h.data(), ws.u_flag, uflag_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
     }
     DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: the anchor work lists
     if (use_xw) {   // a token below the split's faithful range (a zero one included) voids the coarse pass's error bound
@@ -1014,9 +999,9 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       planned = true;
       CellPlan cp;
       plan_cells(T, gcap, metas, plan_host, cp);
-      DTK_CHECK_ARG(cp.first.back() * 5 <= (size_t)N * T * cell_nb * 5 + 16, "infer: cell plan exceeds its bound");
-      if (!cp.v.empty()) DTK_CUDA(cudaMemcpyAsync(d_cells, cp.v.data(), cp.v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-      if (!cp.tiles.empty()) DTK_CUDA(cudaMemcpyAsync(d_tiles, cp.tiles.data(), cp.tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+      DTK_CHECK_ARG(cp.first.back() * 5 <= (size_t)N * T * ws.cell_nb * 5 + 16, "infer: cell plan exceeds its bound");
+      if (!cp.v.empty()) DTK_CUDA(cudaMemcpyAsync(ws.d_cells, cp.v.data(), cp.v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+      if (!cp.tiles.empty()) DTK_CUDA(cudaMemcpyAsync(ws.d_tiles, cp.tiles.data(), cp.tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
       InferAsync* ia = infer_async();
       const bool ovl = ia != nullptr && metas.size() > 1;
       cudaStream_t sb = ovl ? ia->aux2 : st;   // sampling stream
@@ -1027,28 +1012,28 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       auto cells_of = [&](size_t k) {
         XwCells c;
         const int n = (int)(cp.first[k + 1] - cp.first[k]);
-        const int* base = d_cells + 5 * cp.first[k];
+        const int* base = ws.d_cells + 5 * cp.first[k];
         c.row0 = base; c.m = base + n; c.frame = base + 2 * n; c.group = base + 3 * n; c.arow = base + 4 * n;
         c.n_cells = n; c.max_m = cp.max_m;
         return c;
       };
       auto enqueue_sample_x = [&](size_t k) -> int {
         const ChunkMeta& cm = metas[k];
-        const XwSet& x = xr[k % XW_RING];
+        const XwSet& x = ws.xr[k % XW_RING];
         const Grp gp = grp_of(k);
         if (ovl && k >= XW_RING) DTK_CUDA(cudaStreamWaitEvent(sb, xa->freed[k % XW_RING], 0));   // chunk k - 4 is through
         {
           ProfRange pr(PROF_SAMPLE, sb);
-          anchor_scalars_kernel<<<cdiv(cm.used, 256), 256, 0, sb>>>(T, d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, cm.used,
-                                                                   n_unique, x.row0, u_norm, u_flag, u_rho, fv.q_rho, xw_s8_slack(C), s8, x.out_index,
+          anchor_scalars_kernel<<<cdiv(cm.used, 256), 256, 0, sb>>>(T, ws.d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, cm.used,
+                                                                   n_unique, x.row0, ws.u_norm, ws.u_flag, ws.u_rho, fv.q_rho, xw_s8_slack(C), s8, x.out_index,
                                                                    x.arow, x.norm, x.eps);
           DTK_LAUNCHED();
           if (cm.n_gathered > 0) {
             const size_t r0 = (size_t)x.row0;
             gather_anchor_kernel<<<cm.gather_hi - cm.gather_lo, SAMPLE_THREADS, 0, sb>>>(
-                tpc, T, C, P, g->h, g->w, pa, traj, d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, n_unique, cm.gather_lo, fb, u_hi, u_lo, u_flag,
-                                                                    x.norm, u_hi + r0 * C, u_lo + r0 * C, u_q8, u_fac, fv.q_rho, xw_s8_slack(C),
-                                                                    s8 ? u_q8 + r0 * C : nullptr, u_fac + r0, x.eps);
+                tpc, T, C, P, g->h, g->w, pa, traj, ws.d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, n_unique, cm.gather_lo, fb, ws.u_hi, ws.u_lo, ws.u_flag,
+                                                                    x.norm, ws.u_hi + r0 * C, ws.u_lo + r0 * C, ws.u_q8, ws.u_fac, fv.q_rho, xw_s8_slack(C),
+                                                                    s8 ? ws.u_q8 + r0 * C : nullptr, ws.u_fac + r0, x.eps);
             DTK_LAUNCHED();
           }
         }
@@ -1056,18 +1041,18 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         return DINOTRK_OK;
       };
       // Full-map queue.  The queued maps of chunk j (the host knows how many once the chunk's head has run) are appended to
-      // ONE compact descriptor array (buffer set cb[0]); the queue is worked off -- split-precision GEMM over all tokens on
+      // ONE compact descriptor array (buffer set ws.cb[0]); the queue is worked off -- split-precision GEMM over all tokens on
       // 128-row tiles + the head kernels of head.cu -- when it is full and at the end of the phase.
       int q_rows = 0, q_groups = 0;
       auto flush = [&]() -> int {
         if (q_rows == 0) return DINOTRK_OK;
-        const ChunkBufs& b = cb[0];
+        const ChunkBufs& b = ws.cb[0];
         CorrAssist as;
         as.tkeys = b.tkeys; as.zero_word = b.hscratch; as.split_ready = true; as.no_thin = true; as.all_wide = true; as.small_tiles = true;
-        int rc2 = launch_corr_maps(fv, nullptr, ch, b.norm, d_cgrp, d_cgrp + sg_cap, d_cgrp + 2 * sg_cap, d_cgrp + 3 * sg_cap, q_groups,
-                                   q_rows, q_rows, b.maps, ms, d_splan, b.split, st, as);
+        int rc2 = launch_corr_maps(fv, nullptr, ch, b.norm, ws.d_cgrp, ws.d_cgrp + ws.sg_cap, ws.d_cgrp + 2 * ws.sg_cap, ws.d_cgrp + 3 * ws.sg_cap, q_groups,
+                                   q_rows, q_rows, b.maps, ms, ws.d_splan, b.split, st, as);
         if (rc2) return rc2;
-        rc2 = launch_head(b.maps, q_rows, ms, *g, *hw, out_index_ring[0], anchors, 2, 0, nullptr, b.hscratch, st, b.tkeys, true);
+        rc2 = launch_head(b.maps, q_rows, ms, *g, *hw, ws.out_index_ring[0], anchors, 2, 0, nullptr, b.hscratch, st, b.tkeys, true);
         q_rows = q_groups = 0;
         return rc2;
       };
@@ -1076,20 +1061,19 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
         const int n_slow = xa->host_cnt[2 * (j % XW_RING)];
         g_infer_stats[4] += xa->host_cnt[2 * (j % XW_RING) + 1];
         const ChunkMeta& cm = metas[j];
-        const XwSet& x = xr[j % XW_RING];
+        const XwSet& x = ws.xr[j % XW_RING];
         const Grp gp = grp_of(j);
         DTK_CHECK_ARG(n_slow >= 0 && n_slow <= cm.used, "infer: corrupt full-map queue (%d of %d)", n_slow, cm.used);
         g_infer_stats[1] += cm.used - n_slow; g_infer_stats[2] += n_slow;
         if (n_slow > 0) {
-          if (q_rows + n_slow > ch || q_groups + cm.n_groups > sg_cap) {
+          if (q_rows + n_slow > ch || q_groups + cm.n_groups > ws.sg_cap) {
             int rc2 = flush();
             if (rc2) return rc2;
           }
-          const ChunkBufs& b = cb[0];
-          char* c_hi = reinterpret_cast<char*>(b.split);
-          char* c_lo = c_hi + align_up((size_t)ch * C * 2, 256);          // layout of a descriptor array of `ch` rows
-          int rc2 = launch_xw_compact(nullptr, u_hi, u_lo, x.arow, x.norm, x.out_index, C, gp.f, gp.map0, cm.n_groups,
-                                      n_slow, x.xc, nullptr, c_hi, c_lo, b.norm, out_index_ring[0], d_cgrp, sg_cap, st, q_rows, q_groups,
+          const ChunkBufs& b = ws.cb[0];
+          const DescSplit c(b.split, ch, C);   // layout of a descriptor array of `ch` rows
+          int rc2 = launch_xw_compact(nullptr, ws.u_hi, ws.u_lo, x.arow, x.norm, x.out_index, C, gp.f, gp.map0, cm.n_groups,
+                                      n_slow, x.xc, nullptr, c.hi, c.lo, b.norm, ws.out_index_ring[0], ws.d_cgrp, ws.sg_cap, st, q_rows, q_groups,
                                       corr_hilo(fv));
           if (rc2) return rc2;
           q_rows += n_slow; q_groups += cm.n_groups;
@@ -1101,17 +1085,17 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       size_t n_finished = 0, k_end = metas.size();
       for (size_t k = 0; k < metas.size(); ++k) {
         const ChunkMeta& cm = metas[k];
-        const XwSet& x = xr[k % XW_RING];
+        const XwSet& x = ws.xr[k % XW_RING];
         const Grp gp = grp_of(k);
         const XwCells cells = cells_of(k);
         if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, xa->sample[k % XW_RING], 0));
         const float* eps = s8 ? x.eps : nullptr;   // (nullptr: the fp16 pass's XW_EPS)
         g_infer_stats[8] += cm.used - cm.n_gathered; g_infer_stats[9] += cm.n_gathered;
-        if ((rc = launch_xw_coarse(fv, u_hi, (int)xw_rows, u_norm, gp.f, gp.r, gp.m, gp.map0, d_tiles + k * (gcap + 1),
-                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, d_rnorms, s8 ? u_q8 : nullptr,
-                                   u_fac))) return rc;
+        if ((rc = launch_xw_coarse(fv, ws.u_hi, (int)ws.xw_rows, ws.u_norm, gp.f, gp.r, gp.m, gp.map0, ws.d_tiles + k * (gcap + 1),
+                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, ws.d_rnorms, s8 ? ws.u_q8 : nullptr,
+                                   ws.u_fac))) return rc;
         if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used, split_min_norm(C), eps))) return rc;
-        if ((rc = launch_xw_gemm(fv, *g, u_hi, u_lo, (int)xw_rows, cells, x.xc, st))) return rc;
+        if ((rc = launch_xw_gemm(fv, *g, ws.u_hi, ws.u_lo, (int)ws.xw_rows, cells, x.xc, st))) return rc;
         if ((rc = launch_xw_head(fv, *g, *hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups,
                                  eps)))
           return rc;
@@ -1167,17 +1151,17 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     }
     auto enqueue_sample = [&](size_t k) -> int {   // descriptors of chunk k (buffer set k & 1)
       const ChunkMeta& cm = metas[k];
-      const ChunkBufs& b = cb[k & 1];
+      const ChunkBufs& b = ws.cb[k & 1];
       const Grp gp = grp_of(k);
       if (ovl && k >= k0 + 2) DTK_CUDA(cudaStreamWaitEvent(sb, ia->gemm[k & 1], 0));   // GEMM k-2 read the descriptors of this set
       {
         ProfRange pr(PROF_SAMPLE, sb);
-        // the split layout of launch_corr_gemm_tc for desc_rows = used: hi rows, then lo rows at the next 256-byte boundary
-        __half* c_hi = tensor ? reinterpret_cast<__half*>(b.split) : nullptr;
-        __half* c_lo = tensor ? reinterpret_cast<__half*>(reinterpret_cast<char*>(b.split) + align_up((size_t)cm.used * C * 2, 256))
-                              : nullptr;
-        sample_anchor_kernel<<<cm.used, SAMPLE_THREADS, 0, sb>>>(tpc, T, C, P, g->h, g->w, pa, traj, d_qlist, N, gp.f, gp.map0,
-                                                                gp.item, cm.n_groups, fb, b.desc, b.norm, out_index_ring[k & 3], c_hi, c_lo);
+        // the split layout of launch_corr_gemm_tc for desc_rows = used
+        const DescSplit c(b.split, cm.used, C);
+        __half* c_hi = tensor ? reinterpret_cast<__half*>(c.hi) : nullptr;
+        __half* c_lo = tensor ? reinterpret_cast<__half*>(c.lo) : nullptr;
+        sample_anchor_kernel<<<cm.used, SAMPLE_THREADS, 0, sb>>>(tpc, T, C, P, g->h, g->w, pa, traj, ws.d_qlist, N, gp.f, gp.map0,
+                                                                gp.item, cm.n_groups, fb, b.desc, b.norm, ws.out_index_ring[k & 3], c_hi, c_lo);
         DTK_LAUNCHED();
       }
       if (ovl) DTK_CUDA(cudaEventRecord(ia->sample[k & 1], sb));
@@ -1186,15 +1170,15 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
     // the full-map head of chunk j (usually an empty list) runs on the GEMM stream between two GEMMs: it needs ~70 KB of
     // shared memory per CTA and could not co-reside with a GEMM anyway
     auto head_full = [&](size_t j) -> int {
-      const ChunkBufs& b = cb[j & 1];
+      const ChunkBufs& b = ws.cb[j & 1];
       if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, ia->head[j & 1], 0));   // fast head of chunk j (its list is complete)
-      return launch_head(b.maps, metas[j].used, ms, *g, *hw, out_index_ring[j & 3], anchors, 2, 0, nullptr, b.hscratch, st,
+      return launch_head(b.maps, metas[j].used, ms, *g, *hw, ws.out_index_ring[j & 3], anchors, 2, 0, nullptr, b.hscratch, st,
                          tensor ? b.tkeys : nullptr, true, 0, 2);
     };
     if (k0 < metas.size() && (rc = enqueue_sample(k0))) return rc;
     for (size_t k = k0; k < metas.size(); ++k) {
       const ChunkMeta& cm = metas[k];
-      const ChunkBufs& b = cb[k & 1];
+      const ChunkBufs& b = ws.cb[k & 1];
       const Grp gp = grp_of(k);
       if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, ia->sample[k & 1], 0));
       if (k >= k0 + 2 && (rc = head_full(k - 2))) return rc;   // last reader of maps / keys / list of this buffer set
@@ -1206,7 +1190,7 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
       if (ovl) DTK_CUDA(cudaEventRecord(ia->gemm[k & 1], st));
       if (k + 1 < metas.size() && (rc = enqueue_sample(k + 1))) return rc;
       if (ovl) DTK_CUDA(cudaStreamWaitEvent(sa, ia->gemm[k & 1], 0));
-      rc = launch_head(b.maps, cm.used, ms, *g, *hw, out_index_ring[k & 3], anchors, 2, 0, nullptr, b.hscratch, sa, as.tkeys, true,
+      rc = launch_head(b.maps, cm.used, ms, *g, *hw, ws.out_index_ring[k & 3], anchors, 2, 0, nullptr, b.hscratch, sa, as.tkeys, true,
                        (ovl && ia->mode >= 2) ? ia->head_ctas_per_sm : 0, 1);
       if (rc) return rc;
       if (ovl) DTK_CUDA(cudaEventRecord(ia->head[k & 1], sa));

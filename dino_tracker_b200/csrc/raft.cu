@@ -568,9 +568,7 @@ extern "C" {
 
 size_t dinotrk_raft_encode_workspace_bytes(int H, int W) {
   if (!raft_shape_ok(H, W)) return 0;
-  Arena ar(nullptr, 0);
-  RaftEncWs ws(ar, (H + 7) / 8 * 8, (W + 7) / 8 * 8);
-  return ar.off + 256;
+  return layout_end<RaftEncWs>((H + 7) / 8 * 8, (W + 7) / 8 * 8) + 256;
 }
 
 int dinotrk_raft_encode(const float* frames, int T, int T_ctx, int H, int W, const dinotrk_raft_weights* w, float* fmap,
@@ -583,7 +581,7 @@ int dinotrk_raft_encode(const float* frames, int T, int T_ctx, int H, int W, con
   cudaStream_t st = (cudaStream_t)stream;
   const int Hp = (H + 7) / 8 * 8, Wp = (W + 7) / 8 * 8, pt = (Hp - H) / 2, pl = (Wp - W) / 2;
   const size_t hw = (size_t)(Hp / 8) * (Wp / 8);
-  Arena ar(workspace, workspace_bytes);
+  Arena ar(workspace);
   RaftEncWs ws(ar, Hp, Wp);
   raft_identity_kernel<<<1, 256, 0, st>>>(ws.ident, 256);
   DTK_LAUNCHED();
@@ -599,9 +597,7 @@ int dinotrk_raft_encode(const float* frames, int T, int T_ctx, int H, int W, con
 
 size_t dinotrk_raft_flow_workspace_bytes(int H, int W, int n_pairs) {
   if (!raft_shape_ok(H, W) || n_pairs <= 0) return 0;
-  Arena ar(nullptr, 0);
-  RaftFlowWs ws(ar, (H + 7) / 8, (W + 7) / 8, n_pairs);
-  return ar.off + 256;
+  return layout_end<RaftFlowWs>((H + 7) / 8, (W + 7) / 8, n_pairs) + 256;
 }
 
 int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_lo, const float* ctx, int T, int T_ctx, int H,
@@ -623,7 +619,7 @@ int dinotrk_raft_flow(const float* fmap, const void* fmap_hi, const void* fmap_l
   const int P = n_pairs;
   const size_t M = (size_t)P * hw;
   DTK_CHECK_ARG(M < (1u << 31) / RAFT_HX, "raft_flow: too many pairs for one call");
-  Arena ar(workspace, workspace_bytes);
+  Arena ar(workspace);
   RaftFlowWs ws(ar, h8, w8, P);
   DTK_CUDA(cudaMemcpyAsync(ws.pairs, pairs, sizeof(int) * 2 * P, cudaMemcpyHostToDevice, st));
 

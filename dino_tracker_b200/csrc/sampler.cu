@@ -144,8 +144,8 @@ static const void* device_view(const void* p) {
 
 struct SamplerWs {
   int* cnt; int* off; int* total;
-  SamplerWs(void* ws, size_t nb) {
-    Arena ar(ws, (size_t)-1);
+  SamplerWs(Arena& ar, int N) {
+    const size_t nb = (size_t)(N > 0 ? cdiv(N, SMP_THREADS) : 1);
     cnt = ar.take<int>(nb);
     off = ar.take<int>(nb);
     total = ar.take<int>(1);
@@ -166,10 +166,7 @@ using namespace dtk;
 
 extern "C" {
 
-size_t dinotrk_sampler_workspace_bytes(int N) {
-  const size_t nb = (size_t)(N > 0 ? cdiv(N, SMP_THREADS) : 1);
-  return 2 * align_up(nb * 4, 256) + 256 + 256;
-}
+size_t dinotrk_sampler_workspace_bytes(int N) { return align_up(layout_end<SamplerWs>(N), 256) + 256; }
 
 int dinotrk_sampler_prepare_count(const float* traj, int N, int T, int* n_valid, void* workspace, size_t workspace_bytes,
                                   void* stream) {
@@ -180,7 +177,8 @@ int dinotrk_sampler_prepare_count(const float* traj, int N, int T, int* n_valid,
   DTK_CHECK_ARG(src, "sampler_prepare_count: trajectories must be in device or pinned host memory");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(N, SMP_THREADS);
-  SamplerWs w(workspace, nb);
+  Arena ar(workspace);
+  const SamplerWs w(ar, N);
   {
     ProfRange pr(PROF_SAMPLER, st);
     sampler_prepare_count_kernel<<<nb, SMP_THREADS, 0, st>>>(src, N, T, w.cnt);
@@ -201,7 +199,8 @@ int dinotrk_sampler_prepare_emit(const float* traj, int N, int T, float* rows, u
   DTK_CHECK_ARG(src && dst && b, "sampler_prepare_emit: buffers must be in device or pinned host memory");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(N, SMP_THREADS);
-  SamplerWs w(workspace, nb);
+  Arena ar(workspace);
+  const SamplerWs w(ar, N);
   ProfRange pr(PROF_SAMPLER, st);
   sampler_prepare_emit_kernel<<<nb, SMP_THREADS, 0, st>>>(src, N, T, w.off, dst, b);
   DTK_LAUNCHED();
@@ -215,7 +214,8 @@ int dinotrk_sampler_count(const uint32_t* bits, int N, int T, const int64_t* fra
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_sampler_workspace_bytes(N), "sampler_count: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(N, SMP_THREADS);
-  SamplerWs w(workspace, nb);
+  Arena ar(workspace);
+  const SamplerWs w(ar, N);
   {
     ProfRange pr(PROF_SAMPLER, st);
     sampler_count_kernel<<<nb, SMP_THREADS, smp_words(T) * 4, st>>>(bits, N, T, frames, n_frames, w.cnt);
@@ -233,7 +233,8 @@ int dinotrk_sampler_select(const uint32_t* bits, int N, int T, const int64_t* fr
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_sampler_workspace_bytes(N), "sampler_select: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = cdiv(N, SMP_THREADS);
-  SamplerWs w(workspace, nb);
+  Arena ar(workspace);
+  const SamplerWs w(ar, N);
   ProfRange pr(PROF_SAMPLER, st);
   sampler_select_kernel<<<cdiv(m, SEL_WARPS), SEL_WARPS * 32, smp_words(T) * 4, st>>>(bits, N, T, frames, n_frames, w.off,
                                                                                       nb, perm, m, row_ids, mat);

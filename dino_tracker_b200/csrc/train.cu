@@ -346,13 +346,23 @@ static bool bwd_smem_fits(const void* kernel, size_t dyn) {
 static bool head_bwd_global(int P) { return !bwd_smem_fits((const void*)track_head_bwd_kernel<false>, head_bwd_smem(P)); }
 static bool corr_bwd_global(int P) { return !bwd_smem_fits((const void*)track_corr_bwd_kernel<false>, corr_bwd_smem(P)); }
 
+// the gradients of the maps and descriptors; the map buffers of a per-map kernel whose shared-memory variant does not fit
+struct TrackBwdWs {
+  float* dcorr; float* ddesc; bool g1, g2; float* gbuf1 = nullptr; float* gbuf2 = nullptr;
+  TrackBwdWs(Arena& ar, int B, int C, const dinotrk_geom& g) {
+    const int P = g.h * g.w;
+    dcorr = ar.take<float>((size_t)B * dinotrk_map_stride(&g));
+    ddesc = ar.take<float>((size_t)B * C);
+    g1 = head_bwd_global(P);
+    g2 = corr_bwd_global(P);
+    if (g1) gbuf1 = ar.take<float>((size_t)B * 5 * P);
+    if (g2) gbuf2 = ar.take<float>((size_t)B * 3 * P);
+  }
+};
+
 size_t dinotrk_track_backward_workspace_bytes(int B, int C, const dinotrk_geom* g) {
   if (!g || B <= 0) return 0;
-  const int P = g->h * g->w;
-  size_t b = align_up((size_t)B * dinotrk_map_stride(g) * sizeof(float), 256) + align_up((size_t)B * C * sizeof(float), 256) + 1024;
-  if (head_bwd_global(P)) b += align_up((size_t)B * 5 * P * sizeof(float), 256);
-  if (corr_bwd_global(P)) b += align_up((size_t)B * 3 * P * sizeof(float), 256);
-  return b;
+  return align_up(layout_end<TrackBwdWs>(B, C, *g), 256) + 1024;
 }
 
 int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, const dinotrk_head_weights* hw,
@@ -369,14 +379,11 @@ int dinotrk_track_backward(const dinotrk_features* feat, const dinotrk_geom* g, 
   if (B == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int P = g->h * g->w, C = feat->C;
-  Arena ar(workspace, workspace_bytes);
-  float* dcorr = ar.take<float>((size_t)B * dinotrk_map_stride(g));
-  float* ddesc = ar.take<float>((size_t)B * C);
+  Arena ar(workspace);
+  const TrackBwdWs ws(ar, B, C, *g);
+  float *dcorr = ws.dcorr, *ddesc = ws.ddesc, *gbuf1 = ws.gbuf1, *gbuf2 = ws.gbuf2;
   const HeadParams hp = make_head_params(*g, *hw, dinotrk_map_stride(g), 2, 1);
-  const bool g1 = head_bwd_global(P), g2 = corr_bwd_global(P);
-  float* gbuf1 = g1 ? ar.take<float>((size_t)B * 5 * P) : nullptr;
-  float* gbuf2 = g2 ? ar.take<float>((size_t)B * 3 * P) : nullptr;
-  DTK_CHECK_ARG(ar.ok(), "track_backward: workspace arena overflow");
+  const bool g1 = ws.g1, g2 = ws.g2;
   const size_t smem1 = g1 ? TB_WARPS * TB_NRED * sizeof(float) : head_bwd_smem(P);
   const size_t smem2 = g2 ? 0 : corr_bwd_smem(P);
   static PerDev<size_t> attr1_dev, attr2_dev;

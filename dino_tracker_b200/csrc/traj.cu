@@ -312,21 +312,18 @@ int dinotrk_flow_masks(const dinotrk_flow_video* fv, float threshold, uint8_t* m
   return DINOTRK_OK;
 }
 
-size_t dinotrk_traj_workspace_bytes(int T, int H, int W) {
-  const size_t P = (size_t)H * W, nb = (P + TRAJ_THREADS - 1) / TRAJ_THREADS;
-  return align_up((size_t)T * P, 256) + align_up(P * 4, 256) + 2 * align_up(nb * 4, 256) + 256;
-}
-
 struct TrajWs {
   uint8_t* occ; int* len; int* cnt; int* off;
-  TrajWs(void* ws, int T, size_t P, size_t nb) {
-    Arena ar(ws, (size_t)-1);
+  TrajWs(Arena& ar, int T, int H, int W) {
+    const size_t P = (size_t)H * W, nb = (P + TRAJ_THREADS - 1) / TRAJ_THREADS;
     occ = ar.take<uint8_t>((size_t)T * P);
     len = ar.take<int>(P);
     cnt = ar.take<int>(nb);
     off = ar.take<int>(nb);
   }
 };
+
+size_t dinotrk_traj_workspace_bytes(int T, int H, int W) { return align_up(layout_end<TrajWs>(T, H, W), 256) + 256; }
 
 int dinotrk_traj_chain(const dinotrk_flow_video* fv, const uint8_t* masks, int s, float threshold, int min_len,
                        const float* direct_fwd, const float* direct_bwd, float direct_threshold, int* n_kept,
@@ -337,7 +334,8 @@ int dinotrk_traj_chain(const dinotrk_flow_video* fv, const uint8_t* masks, int s
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_traj_workspace_bytes(fv->T, fv->H, fv->W), "traj_chain: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const size_t P = (size_t)fv->H * fv->W, nb = (P + TRAJ_THREADS - 1) / TRAJ_THREADS;
-  TrajWs w(workspace, fv->T, P, nb);
+  Arena ar(workspace);
+  const TrajWs w(ar, fv->T, fv->H, fv->W);
   ChainArgs a{fv->fwd, fv->bwd, direct_fwd, direct_bwd, masks, fv->T, fv->H, fv->W, s, min_len, threshold, direct_threshold};
   ProfRange pr(PROF_MISC, st);
   traj_chain_kernel<<<(unsigned)nb, TRAJ_THREADS, 0, st>>>(a, w.occ, w.len, w.cnt);
@@ -350,15 +348,24 @@ int dinotrk_traj_emit(const dinotrk_flow_video* fv, int s, float* out, void* wor
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_traj_workspace_bytes(fv->T, fv->H, fv->W), "traj_emit: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const size_t P = (size_t)fv->H * fv->W, nb = (P + TRAJ_THREADS - 1) / TRAJ_THREADS;
-  TrajWs w(workspace, fv->T, P, nb);
+  Arena ar(workspace);
+  const TrajWs w(ar, fv->T, fv->H, fv->W);
   ProfRange pr(PROF_MISC, st);
   traj_emit_kernel<<<(unsigned)nb, TRAJ_THREADS, 0, st>>>(fv->fwd, fv->T, fv->H, fv->W, s, w.len, w.off, w.occ, out);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
 
+struct NearestWs {
+  float2* posT; unsigned long long* keys;
+  NearestWs(Arena& ar, int M, int T, int gh, int gw) {
+    posT = ar.take<float2>((size_t)M * T);
+    keys = ar.take<unsigned long long>((size_t)T * gh * gw);
+  }
+};
+
 size_t dinotrk_traj_nearest_workspace_bytes(int M, int T, int gh, int gw) {
-  return align_up((size_t)M * T * sizeof(float2), 256) + align_up((size_t)T * gh * gw * 8, 256) + 256;
+  return align_up(layout_end<NearestWs>(M, T, gh, gw), 256) + 256;
 }
 
 int dinotrk_traj_nearest(const float* traj, int M, int T, int gh, int gw, float start, float step, int* nearest,
@@ -366,16 +373,15 @@ int dinotrk_traj_nearest(const float* traj, int M, int T, int gh, int gw, float 
   DTK_CHECK_ARG(traj && nearest && workspace && M > 0 && T > 0 && gh > 0 && gw > 0, "traj_nearest: bad arguments");
   DTK_CHECK_ARG(workspace_bytes >= dinotrk_traj_nearest_workspace_bytes(M, T, gh, gw), "traj_nearest: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  Arena ar(workspace, workspace_bytes);
-  float2* posT = ar.take<float2>((size_t)M * T);
+  Arena ar(workspace);
+  const NearestWs w(ar, M, T, gh, gw);
   const size_t G = (size_t)gh * gw, nk = (size_t)T * G;
-  unsigned long long* keys = ar.take<unsigned long long>(nk);
   ProfRange pr(PROF_MISC, st);
   const size_t nt = (size_t)M * T;
-  traj_transpose_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float2*>(traj), M, T, posT);
+  traj_transpose_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float2*>(traj), M, T, w.posT);
   DTK_LAUNCHED();
   // an all-NaN frame keeps (inf, 0): index 0, as torch.argmin over all-inf distances
-  fill_u64_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(keys, nk, (unsigned long long)0x7f800000u << 32);
+  fill_u64_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(w.keys, nk, (unsigned long long)0x7f800000u << 32);
   DTK_LAUNCHED();
   const int gx = cdiv((int)G, NEAR_THREADS * NEAR_PTS);
   // enough slices of the trajectories to fill the GPU about four times over, none shorter than 4096
@@ -383,9 +389,9 @@ int dinotrk_traj_nearest(const float* traj, int M, int T, int gh, int gw, float 
   slices = max(1, min(slices, cdiv(M, 4096)));
   const int slice = cdiv(cdiv(M, slices), NEAR_THREADS) * NEAR_THREADS;
   slices = cdiv(M, slice);
-  traj_nearest_kernel<<<dim3(gx, T, slices), NEAR_THREADS, 0, st>>>(posT, M, gh, gw, start, step, slice, keys);
+  traj_nearest_kernel<<<dim3(gx, T, slices), NEAR_THREADS, 0, st>>>(w.posT, M, gh, gw, start, step, slice, w.keys);
   DTK_LAUNCHED();
-  key_index_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(keys, nk, nearest);
+  key_index_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(w.keys, nk, nearest);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }

@@ -633,6 +633,23 @@ static int vit_facet(const VitShape& s, const TcPlan& pl, const void* y, const v
                : tc_launch<TcMode::TF32, EpiFacet>(op, pb, tiles, ef, st, PROF_VIT_GEMM);
 }
 
+// the activations of a forward; the MLP hidden buffer is also the patch embedding's im2col
+struct VitWs {
+  float *x, *y, *q, *k, *vT, *hbuf, *S; TcPlan pl;
+  VitWs(Arena& ar, const dinotrk_vit_config& c, const dinotrk_geom& g, int B) {
+    const size_t P = (size_t)g.h * g.w, rows = (size_t)B * (P + 1), D = c.dim, N1p = align_up(P + 1, 4);
+    x = ar.take<float>(rows * D);
+    y = ar.take<float>(rows * D);
+    q = ar.take<float>(rows * D);
+    k = ar.take<float>(rows * D);
+    vT = ar.take<float>((size_t)B * N1p * D);
+    const size_t hid = rows * (c.swiglu_hidden > 0 ? (size_t)c.swiglu_hidden : 4 * D), col = (size_t)B * P * vit_kp(&c);
+    hbuf = ar.take<float>(hid > col ? hid : col);
+    S = ar.take<float>((size_t)c.heads * VIT_ROW_CHUNK * N1p);   // attention scores of one row chunk
+    pl = TcPlan{ar.take<int>(c.heads + 2), ar.take<int>(c.heads + 2), ar.take<int>(c.heads + 2), ar.take<int>(c.heads + 2)};
+  }
+};
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -641,17 +658,7 @@ extern "C" {
 
 size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_geom* g, int B) {
   if (!c || !g) return 0;
-  const size_t P = (size_t)g->h * g->w, N1 = P + 1, D = c->dim;
-  size_t b = 0;
-  const size_t N1p = align_up(N1, 4);
-  b += align_up(B * N1 * D * 4, 256) * 2;                                  // x, y
-  b += align_up(B * N1 * D * 4, 256) * 2 + align_up(B * N1p * D * 4, 256); // q, k, vT
-  const size_t hid_w = c->swiglu_hidden > 0 ? (size_t)c->swiglu_hidden : 4 * D;   // MLP hidden width
-  size_t hid = B * N1 * hid_w * 4, col = B * P * (size_t)vit_kp(c) * 4;
-  b += align_up(hid > col ? hid : col, 256);                               // MLP hidden / im2col (aliased)
-  b += align_up((size_t)c->heads * VIT_ROW_CHUNK * N1p * 4, 256);          // attention scores of one row chunk
-  b += 4 * align_up((size_t)(c->heads + 2) * 4, 256) + 4096;               // plan tables
-  return b;
+  return align_up(layout_end<VitWs>(*c, *g, B), 256) + 4096;
 }
 
 int dinotrk_vit_attention(const void* q16, const void* k16, const void* vT16, int B, int heads, int N1, int N1p,
@@ -685,9 +692,8 @@ int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom
   DTK_CHECK_ARG(workspace && workspace_bytes >= DINOTRK_VIT_STAGE_WORKSPACE_BYTES, "vit_stage: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const VitShape s = vit_shape(c, g, B);
-  Arena ar(workspace, workspace_bytes);
+  Arena ar(workspace);
   TcPlan pl{ar.take<int>(2), ar.take<int>(2), ar.take<int>(2), ar.take<int>(2)};
-  if (!ar.ok()) return DINOTRK_EINVAL;
   if (stage == DINOTRK_VIT_LAYERNORM) return vit_layernorm(s, reinterpret_cast<const float*>(in), p0, p1, out0, st);
   if (stage == DINOTRK_VIT_PATCH) return vit_patch_embed(s, pl, in, w, p0, p1, reinterpret_cast<float*>(out0), st);
   int rc;
@@ -736,18 +742,11 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
                   "vit_forward: qkv weight / bias of the tap block not 16-byte aligned");
   }
   cudaStream_t st = (cudaStream_t)stream;
-  Arena ar(workspace, workspace_bytes);
+  Arena ar(workspace);
+  const VitWs ws(ar, *c, *g, B);
   const size_t rows = (size_t)B * N1;
-  float* x = ar.take<float>(rows * D);
-  float* y = ar.take<float>(rows * D);
-  float* q = ar.take<float>(rows * D);
-  float* k = ar.take<float>(rows * D);
-  float* vT = ar.take<float>((size_t)B * N1p * D);
-  size_t hid = rows * hid_k, col = (size_t)B * P * Kp;
-  float* hbuf = ar.take<float>(hid > col ? hid : col);
-  float* S = ar.take<float>((size_t)heads * VIT_ROW_CHUNK * N1p);
-  TcPlan pl{ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2), ar.take<int>(heads + 2)};
-  DTK_CHECK_ARG(ar.ok(), "vit_forward: workspace arena overflow");
+  float *x = ws.x, *y = ws.y, *q = ws.q, *k = ws.k, *vT = ws.vT, *hbuf = ws.hbuf, *S = ws.S;
+  const TcPlan pl = ws.pl;
   int rc;
   // y and hbuf hold fp16 activations in fp16 operand mode, fp32 ones otherwise
   __half* h16 = reinterpret_cast<__half*>(hbuf);

@@ -933,18 +933,6 @@ int launch_xw_compact(const float* desc, const void* desc_hi, const void* desc_l
   return DINOTRK_OK;
 }
 
-size_t xw_chunk_bytes(int chunk_maps, int max_cells, int n_tiles, int gcap) {
-  const size_t ch = (size_t)chunk_maps;
-  size_t b = 0;
-  b += align_up(ch * n_tiles * 8, 256) + align_up(ch * n_tiles * 4, 256);              // key1, max2
-  b += align_up(ch * XW_MAX_CAND * 4, 256) + 4 * align_up(ch * 4, 256);                // cand, stat, pinfo, cell_of, slow_list
-  b += align_up((size_t)max_cells * 8, 256);                                           // box_org
-  b += align_up(ch * XW_COLS * 4, 256);                                                // xbox
-  b += align_up(ch * 256 * 4, 256) + align_up(ch * 8, 256);                            // win, hin
-  b += align_up((size_t)(gcap + 2) * 4, 256);                                          // slow_cnt
-  return b + 2048;
-}
-
 // tile_start[g] = sum over groups before g of ceil(m / TC2_BM) (one warp; the coarse GEMM's M-tile prefix)
 __global__ void xw_tile_prefix_kernel(const int* __restrict__ grp_m, int n_groups, int* __restrict__ tile_start) {
   const int lane = threadIdx.x;
@@ -964,6 +952,16 @@ __global__ void xw_tile_prefix_kernel(const int* __restrict__ grp_m, int n_group
   if (lane == 0) tile_start[n_groups] = base;
 }
 
+// workspace of the coarse-keys entry points: 1 / |F| of the T P tokens, the GEMM's tile prefix, the smallest token norm
+struct XwKeysWs {
+  float* rnorms; int* tile_start; unsigned* min_bits;
+  XwKeysWs(Arena& ar, size_t tokens, int n_groups) {
+    rnorms = ar.take<float>(tokens);
+    tile_start = ar.take<int>(n_groups + 1);
+    min_bits = ar.take<unsigned>(1);
+  }
+};
+
 // eps[row] = xw_eps_s8(rho[row], rho_f[frame], slack) over the rows of group blockIdx.x
 __global__ void xw_eps_kernel(const int* __restrict__ grp_frame, const int* __restrict__ grp_row0, const int* __restrict__ grp_m,
                               const float* __restrict__ rho, const float* __restrict__ rho_f, float slack, float* __restrict__ eps) {
@@ -979,8 +977,7 @@ using namespace dtk;
 extern "C" {
 
 size_t dinotrk_xw_coarse_keys_workspace_bytes(int T, int n_groups, const dinotrk_geom* g) {
-  const size_t P = g ? (size_t)g->h * g->w : 0;
-  return align_up((size_t)T * P * 4, 256) + align_up((size_t)(n_groups + 1) * 4, 256) + 256 + 1024;
+  return align_up(layout_end<XwKeysWs>((size_t)T * (g ? (size_t)g->h * g->w : 0), n_groups), 256) + 1024;
 }
 
 int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, int desc_rows,
@@ -995,22 +992,20 @@ int dinotrk_xw_coarse_keys(const dinotrk_features* feat, const dinotrk_geom* g, 
   if (n_groups == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const FeatView fv = make_view(*feat, *g);
-  Arena ar(workspace, workspace_bytes);
-  float* rnorms = ar.take<float>((size_t)fv.T * fv.P);
-  int* tile_start = ar.take<int>(n_groups + 1);
-  unsigned* min_bits = ar.take<unsigned>(1);
-  int rc = launch_xw_rnorms(fv, rnorms, min_bits, st);
+  Arena ar(workspace);
+  const XwKeysWs ws(ar, (size_t)fv.T * fv.P, n_groups);
+  int rc = launch_xw_rnorms(fv, ws.rnorms, ws.min_bits, st);
   if (rc) return rc;
   {
     ProfRange pr(PROF_MISC, st);
-    xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, tile_start);
+    xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, ws.tile_start);
     DTK_LAUNCHED();
   }
   XwChunk xc{};
   xc.key1 = key1;
   xc.max2 = max2;
-  return launch_xw_coarse(fv, desc_hi, desc_rows, desc_norm, grp_frame, grp_row0, grp_m, grp_row0, tile_start, n_groups,
-                          desc_rows / TC2_BM + n_groups, xc, st, rnorms);
+  return launch_xw_coarse(fv, desc_hi, desc_rows, desc_norm, grp_frame, grp_row0, grp_m, grp_row0, ws.tile_start, n_groups,
+                          desc_rows / TC2_BM + n_groups, xc, st, ws.rnorms);
 }
 
 int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_q8, const float* desc_fac,
@@ -1026,11 +1021,11 @@ int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* 
   if (n_groups == 0) return DINOTRK_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const FeatView fv = make_view(*feat, *g);
-  Arena ar(workspace, workspace_bytes);
-  int* tile_start = ar.take<int>(n_groups + 1);
+  Arena ar(workspace);
+  const XwKeysWs ws(ar, (size_t)fv.T * fv.P, n_groups);   // rnorms and min_bits unused: the int8 epilogue needs no 1 / |F|
   {
     ProfRange pr(PROF_MISC, st);
-    xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, tile_start);
+    xw_tile_prefix_kernel<<<1, 32, 0, st>>>(grp_m, n_groups, ws.tile_start);
     DTK_LAUNCHED();
     if (eps) {
       xw_eps_kernel<<<n_groups, 128, 0, st>>>(grp_frame, grp_row0, grp_m, desc_rho, fv.q_rho, xw_s8_slack(fv.C), eps);
@@ -1040,7 +1035,7 @@ int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* 
   XwChunk xc{};
   xc.key1 = key1;
   xc.max2 = max2;
-  return launch_xw_coarse(fv, nullptr, desc_rows, nullptr, grp_frame, grp_row0, grp_m, grp_row0, tile_start, n_groups,
+  return launch_xw_coarse(fv, nullptr, desc_rows, nullptr, grp_frame, grp_row0, grp_m, grp_row0, ws.tile_start, n_groups,
                           desc_rows / TC2_BM + n_groups, xc, st, nullptr, desc_q8, desc_fac);
 }
 

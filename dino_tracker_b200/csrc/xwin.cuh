@@ -132,6 +132,22 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
   int2* hin;                  // [maps] (exact first arg-max token or -1, bits of m_out)
   int* slow_cnt;              // [n_groups + 1] per group count of queued maps; [n_groups] = total
   int* slow_list;             // [maps] group g's queue lives at [grp_map0[g], grp_map0[g] + slow_cnt[g])
+  XwChunk() = default;
+  // every buffer of a chunk of `maps` maps, `cells` cells and n_groups groups, n_tiles coarse tiles per map
+  XwChunk(Arena& ar, size_t maps, size_t cells, int n_tiles, int n_groups) {
+    key1 = ar.take<unsigned long long>(maps * n_tiles);
+    max2 = ar.take<float>(maps * n_tiles);
+    cand = ar.take<int>(maps * XW_MAX_CAND);
+    stat = ar.take<int>(maps);
+    pinfo = ar.take<int>(maps);
+    cell_of = ar.take<int>(maps);
+    slow_list = ar.take<int>(maps);
+    box_org = ar.take<int2>(cells);
+    xbox = ar.take<float>(maps * XW_COLS);
+    win = ar.take<float>(maps * 256);
+    hin = ar.take<int2>(maps);
+    slow_cnt = ar.take<int>((size_t)n_groups + 2);
+  }
 };
 
 struct XwCells {          // host-planned, device-resident description of a chunk's cells
@@ -143,7 +159,6 @@ struct XwCells {          // host-planned, device-resident description of a chun
   int n_cells, max_m;
 };
 
-size_t xw_chunk_bytes(int chunk_maps, int max_cells, int n_tiles, int gcap);
 // Coarse GEMM over the chunk's groups (tile_start: prefix of ceil(m / 256) per group, all groups wide): the int8 pass when
 // desc_q8 is given (desc_fac = the rows' factors, fv's int8 features), else fp16 over desc_hi and fv.hi.
 int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, const float* desc_norm, const int* grp_frame,
