@@ -113,8 +113,10 @@ def _best_buddies(features_chw, H, W, stride, patch, dev, rank, world, unordered
 # ---------------------------------------------------------------------------------------------------------------------
 # Peak filter of the best-buddy pairs: preprocessing_dino_bb/compute_dino_bb_nms.py (SURVEY.md 8f-3)
 class PackedFeatures:
-    """Token-major copy of a T x C x h x w feature video on the GPU (+ norms, + fp16 hi / lo halves): what
-    ``compute_bb_nms`` needs of ``dino_emb``; pack once per video."""
+    """Token-major copy of a T x C x h x w feature video on the GPU (+ norms): what ``compute_bb_nms`` needs of
+    ``dino_emb``; pack once per video.  No fp16 hi / lo halves: the peak filter reports map values, so its maps come
+    from the exact-fp32 correlation GEMM.  The split-fp16 tensor-core GEMM accumulates with an error that grows with C
+    (about 9e-6 of a cosine at C = 1024, against 3e-7 in exact fp32)."""
 
     def __init__(self, features_chw, stride=7, patch=14, device="cuda:0"):
         lib = _lib.load()
@@ -126,16 +128,13 @@ class PackedFeatures:
             self.tpc = torch.empty(T, h * w, C, device=self.dev)
             self.norms = torch.empty(T, h * w, device=self.dev)
             _lib.check(lib.dinotrk_pack_features(_lib.ptr(chw), _lib.ptr(self.tpc), _lib.ptr(self.norms), T, C, h * w, _lib.stream_ptr()))
-            self.hi = self.lo = None
-            if C % 8 == 0:
-                self.hi, self.lo = _lib.split_features(self.tpc, self.norms, _lib.stream_ptr())
-        self.feat = _lib.make_features(self.tpc, self.norms, self.hi, self.lo)
+        self.feat = _lib.make_features(self.tpc, self.norms)
 
 
 @torch.no_grad()
 def compute_bb_nms(dino_bb_sf_tf, sf, tf, dino_emb, coords=None, stride=7, box_size=50, iou_thresh=0.2, topk=400):
     """compute_dino_bb_nms.py:50-70.  ``dino_emb``: T x C x h x w features or a ``PackedFeatures``.  For every source point
-    of the pair: its similarity map against frame ``tf`` (the tracker's correlation kernels), then per map the two largest
+    of the pair: its similarity map against frame ``tf`` (the tracker's exact-fp32 correlation kernels), then per map the two largest
     values surviving box NMS among the ``topk`` largest and their ratio r (``dinotrk_bb_nms``).  ``coords`` is accepted for
     signature parity (the token grid is implied by the features)."""
     lib = _lib.load()
