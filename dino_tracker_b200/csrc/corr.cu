@@ -10,6 +10,7 @@
 // The reference instead runs einsum("bc,nchw->bnhw") over all B x N pairs and keeps the diagonal.
 #include "common.cuh"
 #include "corr.cuh"
+#include "tcgemm.cuh"
 
 namespace dtk {
 
@@ -243,7 +244,7 @@ int launch_corr_maps(const FeatView& fv, const float* desc, int desc_rows, const
   unsigned long long* tkeys = fv.tensor() ? assist.tkeys : nullptr;
   // rows per GEMM M tile: 256 (CTA pairs) by default; 128-row single-CTA tiles when no group can fill more than half a
   // pair tile (10-128 points per call: Tracker.forward-sized batches, small query sets) or when the caller asks for them
-  const int tile_rows = fv.tensor() ? ((assist.small_tiles || max_group_m <= 128) ? 128 : corr_tc_tile_rows()) : BM;
+  const int tile_rows = fv.tensor() ? ((assist.small_tiles || max_group_m <= 128) ? TC_BM : TC2_BM) : BM;
   const int n_tiles = cdiv(fv.P, CORR_TILE);
   const float* tpc = fv.tpc;
   const float* norms = fv.norms;

@@ -51,7 +51,6 @@ struct CorrAssist {
   bool small_tiles = false;   // tensor path: 128-row single-CTA tiles instead of 256-row CTA-pair tiles (many tiny groups)
 };
 
-int corr_tc_tile_rows();   // 256: CTA-pair (two-CTA cluster) kernel, the default; 128: single-CTA kernel (DTK_CORR_PAIRS=0)
 size_t corr_tc_workspace_bytes(int total_rows, int C);
 // The separate-halves split of `rows` descriptor rows of C channels in a split workspace (corr_tc_workspace_bytes): hi rows,
 // then lo rows at the next 256-byte boundary.
@@ -75,7 +74,8 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
                         const float* desc, int desc_rows, const float* desc_norm, const int* grp_frame,
                         const int* grp_row0, const int* grp_m, const int* grp_map0, const int* tile_start, int n_groups,
                         int max_tiles, float* maps, int map_stride, float* desc_split_ws, cudaStream_t st,
-                        unsigned long long* tkeys = nullptr, bool split_ready = false, int tile_rows = 0 /* 0: default */,
+                        unsigned long long* tkeys, bool split_ready,
+                        int tile_rows /* TC2_BM: CTA-pair (two-CTA cluster) kernel; TC_BM: single-CTA kernel */,
                         bool relu = true /* false: signed cosines (no tile keys) */,
                         const float* clamp = nullptr /* [desc_rows]: per-row replacement of the norm product's 1e-8 (signed only) */,
                         const void* tpc_hilo = nullptr /* interleaved features (corr_hilo): the F16X3I GEMM; a ready split in
@@ -96,7 +96,6 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
                 const dinotrk_head_weights& hw, const int* out_index, float* out, int out_stride, int out_mode,
                 int* aux, int* scratch /* n_maps + 1 ints, or NULL: full-map kernel for every map */, cudaStream_t st,
                 const unsigned long long* tkeys = nullptr /* tile keys of launch_corr_maps */, bool counter_zeroed = false,
-                int ctas_per_sm = 0 /* > 0: cap of the fast-path grid (co-residency with a GEMM on another stream) */,
                 int parts = 3 /* bit 0: fast path over all maps, bit 1: full-map kernel over the uncertified ones */);
 
 }  // namespace dtk

@@ -285,15 +285,6 @@ struct CorrEpi {
   }
 };
 
-int corr_tc_tile_rows() {
-  static int rows = 0;
-  if (rows == 0) {
-    const char* e = getenv("DTK_CORR_PAIRS");
-    rows = (e && atoi(e) == 0) ? TC_BM : TC2_BM;
-  }
-  return rows;
-}
-
 size_t corr_tc_workspace_bytes(int total_rows, int C) { return 2 * align_up((size_t)total_rows * C * 2, 256); }
 
 // wide groups on tensor cores; tile_start must already hold the plan (corr_plan_kernel).
@@ -307,7 +298,7 @@ int launch_corr_gemm_tc(const void* tpc_hi, const void* tpc_lo, const float* nor
   DTK_CHECK_ARG(C % 8 == 0, "corr (tensor path): C must be a multiple of 8");
   DTK_CHECK_ARG(relu || tkeys == nullptr, "corr (tensor path): tile keys need the ReLU maps");
   DTK_CHECK_ARG(!tpc_hilo || (relu && C % 32 == 0), "corr (tensor path): interleaved operands need C %% 32 == 0 and ReLU maps");
-  const bool pairs = (tile_rows > 0 ? tile_rows : corr_tc_tile_rows()) == TC2_BM;   // tile_start was planned with this M tile
+  const bool pairs = tile_rows == TC2_BM;   // tile_start was planned with this M tile
   const TcProblem pb{grp_frame, grp_row0, grp_m, tile_start, n_groups, P, C};
   if (tpc_hilo) {   // descriptors interleaved like the features: [desc_rows][2 C] at the start of the workspace
     int rc = split_ready ? DINOTRK_OK : launch_split_hilo(desc, desc_split_ws, desc_rows, C, st);

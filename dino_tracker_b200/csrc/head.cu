@@ -777,7 +777,7 @@ __global__ void zero_int_kernel(int* p) { *p = 0; }
 int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geom& g,
                 const dinotrk_head_weights& hw, const int* out_index, float* out, int out_stride, int out_mode,
                 int* aux, int* scratch, cudaStream_t st, const unsigned long long* tkeys, bool counter_zeroed,
-                int ctas_per_sm, int parts) {
+                int parts) {
   if (n_maps <= 0) return DINOTRK_OK;
   DTK_CHECK_GRID(g, "head");
   const HeadParams hp = make_head_params(g, hw, map_stride, out_stride, out_mode);
@@ -800,8 +800,7 @@ int launch_head(const float* maps, int n_maps, int map_stride, const dinotrk_geo
         DTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_tm, head_tm_kernel, TMK_THREADS, 0));
         if (per_sm_tm < 1) per_sm_tm = 1;
       }
-      const int per_sm_use = (ctas_per_sm > 0 && ctas_per_sm < per_sm_tm) ? ctas_per_sm : per_sm_tm;
-      int grid = n_maps < sms * per_sm_use ? n_maps : sms * per_sm_use;
+      int grid = n_maps < sms * per_sm_tm ? n_maps : sms * per_sm_tm;
       ProfRange pr(PROF_HEAD, st);
       head_tm_kernel<<<grid, TMK_THREADS, 0, st>>>(maps, tkeys, cdiv(hp.P, CORR_TILE), n_maps, hp, hw, out_index, out, aux,
                                                    slow_list, slow_count);

@@ -103,9 +103,42 @@ anchor_lists_kernel(const float* __restrict__ cos_sims, int N, int T, float th, 
   if (threadIdx.x == 0) cnt[a] = base;
 }
 
-// descriptors of one chunk of anchor work items.  Group k of the chunk covers items
-// [grp_item0[k], grp_item0[k] + grp_m[k]) of anchor frame grp_frame[k]; item u = (query slot u / T, frame u % T).
-// Source point traj[n][i] lives in frame i; frames_set = [a, i0..e-1] (model_inference.py:138-143).
+// Anchor work item of map j of a chunk, whose group is lo.  Group k of the chunk covers items
+// [grp_item0[k], grp_item0[k] + grp_m[k]) of anchor frame grp_frame[k]; item u = (query slot u / T, frame u % T):
+// anchor frame a, query n = qlist[a][slot], source frame i.
+struct AnchorItem { int a, slot, i, n; };
+__device__ __forceinline__ AnchorItem anchor_item(int j, int lo, int T, const int* __restrict__ qlist, int N,
+                                                  const int* __restrict__ grp_frame, const int* __restrict__ grp_map0,
+                                                  const int* __restrict__ grp_item0) {
+  AnchorItem it;
+  it.a = grp_frame[lo];
+  const int uu = grp_item0[lo] + (j - grp_map0[lo]);
+  it.slot = uu / T; it.i = uu - it.slot * T;
+  it.n = qlist[(size_t)it.a * N + it.slot];
+  return it;
+}
+
+// Trajectory point pt = traj[n][i] (it lives in frame i) sampled from the frame set [a, i0..e-1] at slot i - i0 + 1
+// (model_inference.py:138-143): its corners and the frames of its two slots.  Slot 0 is the anchor frame a; without one
+// (NoAnchor: the unique table, which samples only points that give slot 0 no weight) it is numbered like the others.
+struct NoAnchor {};
+__device__ __forceinline__ int slot_frame(int z, int i0, int a) { return z == 0 ? a : i0 + z - 1; }
+__device__ __forceinline__ int slot_frame(int z, int i0, NoAnchor) { return i0 + z - 1; }
+struct SetSample { TriCorners c; int f0, f1; };
+template <class Anchor>
+__device__ __forceinline__ SetSample frame_set_sample(const float* __restrict__ pt, int i, int T, int frame_batch, int h, int w,
+                                                      const PointAffine& pa, Anchor a) {
+  const int i0 = (i / frame_batch) * frame_batch, e = min(i0 + frame_batch, T);
+  float x = __fadd_rn(__fmul_rn(pa.aw, pt[0]), pa.bw);
+  float y = __fadd_rn(__fmul_rn(pa.ah, pt[1]), pa.bh);
+  SetSample s;
+  s.c = tri_setup(x, y, (float)(i - i0 + 1), e - i0 + 1, h, w);
+  s.f0 = slot_frame(s.c.z0, i0, a);
+  s.f1 = s.c.z1 < 0 ? -1 : slot_frame(s.c.z1, i0, a);
+  return s;
+}
+
+// descriptors of one chunk of anchor work items (see anchor_item)
 __global__ void sample_anchor_kernel(const float* __restrict__ tpc, int T, int C, int P, int h, int w, PointAffine pa,
                                      const float* __restrict__ traj, const int* __restrict__ qlist, int N,
                                      const int* __restrict__ grp_frame, const int* __restrict__ grp_map0,
@@ -113,22 +146,11 @@ __global__ void sample_anchor_kernel(const float* __restrict__ tpc, int T, int C
                                      float* __restrict__ desc, float* __restrict__ dnorm, int* __restrict__ out_index,
                                      __half* __restrict__ desc_hi, __half* __restrict__ desc_lo) {
   const int j = blockIdx.x;
-  const int lo = last_le(n_groups, j, grp_map0);
-  const int a = grp_frame[lo];
-  const int u = grp_item0[lo] + (j - grp_map0[lo]);
-  const int slot = u / T, i = u - slot * T;
-  const int n = qlist[(size_t)a * N + slot];
-  const int i0 = (i / frame_batch) * frame_batch, e = min(i0 + frame_batch, T);
-  const int Nset = e - i0 + 1;
-  const float* pt = traj + ((size_t)n * T + i) * 3;
-  float x = __fadd_rn(__fmul_rn(pa.aw, pt[0]), pa.bw);
-  float y = __fadd_rn(__fmul_rn(pa.ah, pt[1]), pa.bh);
-  TriCorners c = tri_setup(x, y, (float)(i - i0 + 1), Nset, h, w);
-  int f0 = c.z0 == 0 ? a : i0 + c.z0 - 1;
-  int f1 = c.z1 < 0 ? -1 : (c.z1 == 0 ? a : i0 + c.z1 - 1);
-  sample_point(tpc, C, P, c, f0, f1, desc + (size_t)j * C, dnorm + j, desc_hi ? desc_hi + (size_t)j * C : nullptr,
+  const AnchorItem it = anchor_item(j, last_le(n_groups, j, grp_map0), T, qlist, N, grp_frame, grp_map0, grp_item0);
+  const SetSample s = frame_set_sample(traj + ((size_t)it.n * T + it.i) * 3, it.i, T, frame_batch, h, w, pa, it.a);
+  sample_point(tpc, C, P, s.c, s.f0, s.f1, desc + (size_t)j * C, dnorm + j, desc_hi ? desc_hi + (size_t)j * C : nullptr,
                desc_lo ? desc_lo + (size_t)j * C : nullptr);
-  if (threadIdx.x == 0) out_index[j] = (n * T + a) * T + i;
+  if (threadIdx.x == 0) out_index[j] = (it.n * T + it.a) * T + it.i;
 }
 
 // The descriptor of work item (n, i, a) -- trajectory point traj[n][i] sampled from the frame set [a, i0..e-1] at slot
@@ -154,20 +176,13 @@ __global__ void sample_unique_kernel(const float* __restrict__ tpc, int T, int C
                                      __half* __restrict__ u_lo, float* __restrict__ u_norm, int* __restrict__ u_flag,
                                      int8_t* __restrict__ u_q8, float* __restrict__ u_fac, float* __restrict__ u_rho) {
   const int u = blockIdx.x;                 // n * T + i
-  const int i = u % T;
-  const int i0 = (i / frame_batch) * frame_batch, e = min(i0 + frame_batch, T);
-  const float* pt = traj + (size_t)u * 3;
-  float x = __fadd_rn(__fmul_rn(pa.aw, pt[0]), pa.bw);
-  float y = __fadd_rn(__fmul_rn(pa.ah, pt[1]), pa.bh);
-  TriCorners c = tri_setup(x, y, (float)(i - i0 + 1), e - i0 + 1, h, w);
+  const SetSample s = frame_set_sample(traj + (size_t)u * 3, u % T, T, frame_batch, h, w, pa, NoAnchor{});
   bool slot0 = false;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) slot0 = slot0 || (c.z0 == 0 && c.tok[k] >= 0 && c.wxy[k][0] != 0.f);
+  for (int k = 0; k < 4; ++k) slot0 = slot0 || (s.c.z0 == 0 && s.c.tok[k] >= 0 && s.c.wxy[k][0] != 0.f);
   if (threadIdx.x == 0) u_flag[u] = slot0 ? 1 : 0;
   if (slot0) return;                        // depends on the anchor frame: sampled per work item
-  const int f0 = i0 + c.z0 - 1;
-  const int f1 = c.z1 < 0 ? -1 : i0 + c.z1 - 1;
-  sample_point(tpc, C, P, c, f0, f1, nullptr, u_norm + u, u_hi + (size_t)u * C, u_lo + (size_t)u * C);
+  sample_point(tpc, C, P, s.c, s.f0, s.f1, nullptr, u_norm + u, u_hi + (size_t)u * C, u_lo + (size_t)u * C);
   if (u_q8) {   // (+ the int8 row of the coarse pass)
     const float r = quant_desc(u_hi + (size_t)u * C, u_lo + (size_t)u * C, C, u_norm + u, u_q8 + (size_t)u * C, u_fac + u);
     if (threadIdx.x == 0) u_rho[u] = r;
@@ -189,17 +204,14 @@ __global__ void anchor_scalars_kernel(int T, const int* __restrict__ qlist, int 
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_maps) return;
   const int lo = last_le(n_groups, j, grp_map0);
-  const int a = grp_frame[lo];
-  const int uu = grp_item0[lo] + (j - grp_map0[lo]);
-  const int slot = uu / T, i = uu - slot * T;
-  const int n = qlist[(size_t)a * N + slot];
-  const size_t u = (size_t)n * T + i;
-  out_index[j] = (n * T + a) * T + i;
+  const AnchorItem it = anchor_item(j, lo, T, qlist, N, grp_frame, grp_map0, grp_item0);
+  const size_t u = (size_t)it.n * T + it.i;
+  out_index[j] = (it.n * T + it.a) * T + it.i;
   const int r0 = grp_row0[lo];
   arow[j] = r0 < n_unique ? r0 + (j - grp_map0[lo]) : chunk_row0 + j;
   if (u_flag[u]) return;   // sampled per work item: gather_anchor_kernel writes the norm and eps
   dnorm[j] = u_norm[u];
-  if (with_eps) desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[a], eps_slack);
+  if (with_eps) desc_eps[j] = xw_eps_s8(u_rho[u], rho_f[it.a], eps_slack);
 }
 
 // descriptors (fp16 hi / lo; with desc_q8: + the int8 row and its factor) of the GATHERED maps of one chunk of anchor work
@@ -220,11 +232,8 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
   const int j = map_lo + blockIdx.x;
   const int lo = last_le(n_groups, j, grp_map0);
   if (grp_row0[lo] < n_unique) return;   // read in place
-  const int a = grp_frame[lo];
-  const int uu = grp_item0[lo] + (j - grp_map0[lo]);
-  const int slot = uu / T, i = uu - slot * T;
-  const int n = qlist[(size_t)a * N + slot];
-  const size_t u = (size_t)n * T + i;
+  const AnchorItem it = anchor_item(j, lo, T, qlist, N, grp_frame, grp_map0, grp_item0);
+  const size_t u = (size_t)it.n * T + it.i;
   if (!u_flag[u]) {
     const uint4* sh = reinterpret_cast<const uint4*>(u_hi + u * C);
     const uint4* sl = reinterpret_cast<const uint4*>(u_lo + u * C);
@@ -239,17 +248,11 @@ __global__ void gather_anchor_kernel(const float* __restrict__ tpc, int T, int C
     }
     return;
   }
-  const int i0 = (i / frame_batch) * frame_batch, e = min(i0 + frame_batch, T);
-  const float* pt = traj + u * 3;
-  float x = __fadd_rn(__fmul_rn(pa.aw, pt[0]), pa.bw);
-  float y = __fadd_rn(__fmul_rn(pa.ah, pt[1]), pa.bh);
-  TriCorners c = tri_setup(x, y, (float)(i - i0 + 1), e - i0 + 1, h, w);
-  int f0 = c.z0 == 0 ? a : i0 + c.z0 - 1;
-  int f1 = c.z1 < 0 ? -1 : (c.z1 == 0 ? a : i0 + c.z1 - 1);
-  sample_point(tpc, C, P, c, f0, f1, nullptr, dnorm + j, desc_hi + (size_t)j * C, desc_lo + (size_t)j * C);
+  const SetSample s = frame_set_sample(traj + u * 3, it.i, T, frame_batch, h, w, pa, it.a);
+  sample_point(tpc, C, P, s.c, s.f0, s.f1, nullptr, dnorm + j, desc_hi + (size_t)j * C, desc_lo + (size_t)j * C);
   if (desc_q8) {
     const float r = quant_desc(desc_hi + (size_t)j * C, desc_lo + (size_t)j * C, C, dnorm + j, desc_q8 + (size_t)j * C, desc_fac + j);
-    if (threadIdx.x == 0) desc_eps[j] = xw_eps_s8(r, rho_f[a], eps_slack);
+    if (threadIdx.x == 0) desc_eps[j] = xw_eps_s8(r, rho_f[it.a], eps_slack);
   }
 }
 
@@ -472,49 +475,40 @@ static void plan_cells(int T, int gcap, const std::vector<ChunkMeta>& metas, con
   }
 }
 
-// auxiliary stream + events of the phase-C pipeline (one set per process; DTK_OVERLAP=0 disables the overlap)
+// side stream + events of the anchor phase's pipelining (one set per device; see dinotrk_infer_set_overlap)
 struct InferAsync {
-  int mode;                 // 1: sampling overlapped with the GEMMs (default); 2: sampling and the head fast path
-  cudaStream_t aux, aux2;   // head stream, sampling stream
-  cudaEvent_t fork, join, sample[2], gemm[2], head[2];
-  int head_ctas_per_sm;
+  cudaStream_t side;   // sampling stream
+  cudaEvent_t fork, join, sample[2], gemm[2];
 };
-static int g_overlap_mode = -1;   // -1: DTK_OVERLAP or the default (1); see dinotrk_infer_set_overlap
+static int g_overlap_mode = -1;   // -1: the default (1); see dinotrk_infer_set_overlap
 struct InferAsyncSlot { InferAsync ia; int state; };   // state 0: not created, 1: ready, -1: creation failed
 static InferAsync* infer_async() {
   static PerDev<InferAsyncSlot> slots;   // streams and events belong to the device they were created on
+  if (g_overlap_mode == 0) return nullptr;
   InferAsyncSlot& slot = slots.get();
   InferAsync& ia = slot.ia;
-  int& state = slot.state;
-  int mode = g_overlap_mode;
-  if (mode < 0) {
-    const char* e = getenv("DTK_OVERLAP");
-    mode = e ? atoi(e) : 1;
-  }
-  if (mode <= 0) return nullptr;
-  if (state == 0) {
-    state = -1;
-    const char* hc = getenv("DTK_HEAD_OVERLAP_CTAS");
-    ia.head_ctas_per_sm = hc ? atoi(hc) : 2;
-    if (cudaStreamCreateWithFlags(&ia.aux, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
-    if (cudaStreamCreateWithFlags(&ia.aux2, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
-    cudaEvent_t* evs[] = {&ia.fork, &ia.join, &ia.sample[0], &ia.sample[1], &ia.gemm[0], &ia.gemm[1], &ia.head[0], &ia.head[1]};
+  if (slot.state == 0) {
+    slot.state = -1;
+    if (cudaStreamCreateWithFlags(&ia.side, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
+    cudaEvent_t* evs[] = {&ia.fork, &ia.join, &ia.sample[0], &ia.sample[1], &ia.gemm[0], &ia.gemm[1]};
     for (cudaEvent_t* ev : evs)
       if (cudaEventCreateWithFlags(ev, cudaEventDisableTiming) != cudaSuccess) return nullptr;
-    state = 1;
+    slot.state = 1;
   }
-  if (state != 1) return nullptr;
-  ia.mode = mode;
-  return &ia;
+  return slot.state == 1 ? &ia : nullptr;
 }
 
 // events, pinned counters and selection of the exact-window pipeline (one set per device)
 constexpr int XW_RING = 4;
 constexpr int XW_PROBE_MAPS = 4096;   // size of the probe chunk (automatic pipeline choice)
+constexpr int INFER_A_COUNTED = 16;   // trajectory-phase chunks whose uncertified maps the anchor phase's choice reads
+// host_cnt: [XW_RING][2] queue totals / uncertified of the chunks in flight | [INFER_A_COUNTED] trajectory-phase uncertified
+// counts | the video's smallest token norm
+constexpr int XW_CNT_A = 2 * XW_RING, XW_CNT_MINNORM = XW_CNT_A + INFER_A_COUNTED;
 struct XwAsync {
   int state;                                   // 0: not created, 1: ready, -1: failed
   cudaEvent_t sample[XW_RING], done[XW_RING], freed[XW_RING];
-  int* host_cnt;                               // pinned: [XW_RING][2] queue totals / uncertified + [16] phase-A uncertified counts
+  int* host_cnt;                               // pinned (see XW_CNT_*)
 };
 static XwAsync* xw_async() {
   static PerDev<XwAsync> slots;
@@ -526,22 +520,78 @@ static XwAsync* xw_async() {
       if (cudaEventCreateWithFlags(&xa.done[k], cudaEventDisableTiming) != cudaSuccess) return nullptr;
       if (cudaEventCreateWithFlags(&xa.freed[k], cudaEventDisableTiming) != cudaSuccess) return nullptr;
     }
-    if (cudaHostAlloc(&xa.host_cnt, (2 * XW_RING + 16 + 4) * sizeof(int), cudaHostAllocDefault) != cudaSuccess) return nullptr;
+    if (cudaHostAlloc(&xa.host_cnt, (XW_CNT_MINNORM + 4) * sizeof(int), cudaHostAllocDefault) != cudaSuccess) return nullptr;
     xa.state = 1;
   }
   return xa.state == 1 ? &xa : nullptr;
 }
-static int g_xw_path = -1;                     // -1: automatic (DTK_XW or on), 0: full-map path only, 1: exact-window path
+static int g_xw_path = -1;                     // -1: automatic, 0: full-map path only, 1: exact-window path
 static int g_xw_coarse = -1;                   // -1: automatic, 0: fp16 coarse pass, 1: int8 coarse pass
-// anchor-phase maps | on the exact-window path | queued | path used | queued by the certificate | tensor-core contraction |
-// int8 coarse pass | bits of the largest per-frame int8 residual | exact-window maps whose descriptor was read in place from
-// the unique table | those gathered into the chunk's rows
-constexpr int INFER_STATS = 10;
-static long long g_infer_stats[INFER_STATS] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+// Slots of dinotrk_infer_last_stats, named as the keys of _lib.infer_stats(): anchor-phase maps | finished on the
+// exact-window path | re-done on the full-map path | pipeline used | of those re-done, queued by the certificate |
+// tensor-core contraction | int8 coarse pass | bits of the largest per-frame int8 residual | exact-window maps whose
+// descriptor was read in place from the unique table | those gathered into the chunk's rows
+namespace infer_stat {
+enum { anchor_maps, exact_window, full_map, pipeline, full_map_by_certificate, contraction, coarse, coarse_rho_f,
+       desc_in_place, desc_gathered, count };
+}
+static long long g_infer_stats[infer_stat::count] = {};
 // the probe chunk queues more than this fraction of its maps on the int8 coarse pass: the rest of the phase runs the fp16
 // pass.  A queued map costs a full-map split-precision GEMM, ~3 fp16 coarse passes, while the int8 pass saves about half
 // of one per map: int8 loses above ~1/6 extra queued maps.  1/16 leaves a wide margin.
 constexpr int XW_S8_PROBE_QUEUE_DIV = 16;
+
+// Which pipeline the anchor phase runs, and the exact-window pipeline's coarse pass.  Every rule of the choice is here, in
+// the order it is applied: what the call can run (before the host sync), what the video and the trajectory phase showed
+// (after it), and the verdict of the probe chunk.
+struct AnchorChoice {
+  XwAsync* xa = nullptr;   // events and pinned counters of the exact-window pipeline; nullptr: it cannot run
+  bool xw = false;         // the exact-window pipeline: coarse pass + exact window (xwin.cuh)
+  bool probe = false;      // automatic: its first chunk is a probe whose verdict may change the rest of the phase
+  bool s8 = false;         // its coarse pass on int8 tensor cores
+
+  // Before the host sync: the exact-window pipeline needs the tensor-core contraction, the disc inside the window box, not
+  // to be switched off, and its events.
+  AnchorChoice(const FeatView& fv, const dinotrk_geom& g) {
+    if (fv.tensor() && disc_fits_box(g) && g_xw_path != 0) xa = xw_async();
+    xw = xa != nullptr;
+    probe = g_xw_path < 0;
+  }
+  // the int8 rows of the unique table are sampled whenever the int8 coarse pass can still be chosen
+  static bool q8_rows(const FeatView& fv) { return fv.s8() && g_xw_coarse != 0 && fv.C % 16 == 0 && fv.C <= XW_S8_MAX_C; }
+  // After the host sync.  A token below the split's faithful range (a zero one included) voids the coarse pass's error
+  // bound.  Automatic mode: head weights the certificate cannot handle send (almost) every map to the full-map kernels
+  // anyway; the trajectory phase just showed it when more than a quarter of its first chunks' maps went uncertified.
+  void after_sync(int C, int n_counted_A, long long maps_A) {
+    if (!xw) return;
+    float mn;
+    memcpy(&mn, xa->host_cnt + XW_CNT_MINNORM, sizeof(float));
+    if (!(mn >= split_min_norm(C))) xw = false;
+    if (xw && probe && n_counted_A > 0) {
+      long long unc = 0;
+      for (int k = 0; k < n_counted_A; ++k) unc += xa->host_cnt[XW_CNT_A + k];
+      if (unc * 4 > maps_A) xw = false;
+    }
+  }
+  // Once xw is final: int8 when the features carry their int8 operands (forced: required), unless in automatic mode a
+  // frame's residual rho_f makes the bound too loose.
+  int coarse_pass(const FeatView& fv, float rho_max) {
+    DTK_CHECK_ARG(g_xw_coarse != 1 || !xw || fv.s8(), "infer: int8 coarse pass forced without the int8 features");
+    s8 = xw && fv.s8() && g_xw_coarse != 0;
+    DTK_CHECK_ARG(!s8 || (fv.C % 16 == 0 && fv.C <= XW_S8_MAX_C), "infer: int8 coarse pass needs C %% 16 == 0 and C <= %d",
+                  XW_S8_MAX_C);
+    if (g_xw_coarse < 0 && !(rho_max <= XW_S8_RHO_MAX)) s8 = false;
+    return DINOTRK_OK;
+  }
+  // The probe chunk's verdict from its maps queued for the full-map kernels.  More than a quarter queued by the certificate
+  // (refiner weights whose outside-the-box logit bound needs the exact map): the rest of the phase runs the full-map
+  // pipeline (true).  Else, automatic coarse mode, more than 1 / XW_S8_PROBE_QUEUE_DIV queued: the fp16 coarse pass.
+  bool probe_says_full_maps(long long by_certificate, long long queued, int maps) {
+    if (by_certificate * 4 > maps) return true;
+    if (s8 && g_xw_coarse < 0 && queued * XW_S8_PROBE_QUEUE_DIV > maps) s8 = false;
+    return false;
+  }
+};
 
 // workspace of dinotrk_corr_track: the maps, the correlation's plan and split, the head's list of uncertified maps
 struct CorrTrackWs {
@@ -625,6 +675,380 @@ struct InferWs {
   }
 };
 
+// What every phase of one dinotrk_infer call reads, and the host plan of the phase's chunks.
+struct InferCtx {
+  const FeatView& fv; const dinotrk_geom& g; const dinotrk_head_weights& hw;
+  InferWs& ws; cudaStream_t st;
+  int T, C, N, P, ms, ch, gcap, fb;   // fb: frames per batch of the anchor phase's frame sets
+  size_t max_chunks;
+  PointAffine pa;
+  // The chunks of a phase are planned on the host in one go and their group arrays uploaded with ONE copy, so the
+  // per-chunk launches never block the host (a pageable cudaMemcpyAsync per chunk would).
+  std::vector<ChunkMeta> metas;
+  std::vector<int> plan_host;
+  int upload_plan() {
+    DTK_CHECK_ARG(metas.size() <= max_chunks, "infer: chunk plan exceeds its bound (%zu > %zu)", metas.size(), max_chunks);
+    if (!plan_host.empty())
+      DTK_CUDA(cudaMemcpyAsync(ws.d_groups, plan_host.data(), plan_host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    return DINOTRK_OK;
+  }
+  struct Grp { const int *f, *r, *m, *map0, *item; };
+  Grp grp_of(size_t k) const {   // the device group arrays of chunk k
+    const int* b = ws.d_groups + k * 5 * gcap;
+    return Grp{b, b + gcap, b + 2 * gcap, b + 3 * gcap, b + 4 * gcap};
+  }
+};
+
+// ---- phase A: trajectories.  The uncertified maps of the first INFER_A_COUNTED chunks are counted into ws.d_cntA, for the
+// anchor phase's choice; n_counted: how many chunks.
+static int infer_trajectories(InferCtx& c, const float* query_points, float* traj, int& n_counted) {
+  NvtxRange nv("dinotrk.infer.A.trajectories");
+  InferWs& ws = c.ws;
+  const bool tensor = c.fv.tensor();   // tensor-core GEMM: tile keys for the head
+  {
+    ProfRange pr(PROF_SAMPLE, c.st);
+    sample_query_kernel<<<c.N, SAMPLE_THREADS, 0, c.st>>>(c.fv.tpc, c.T, c.C, c.P, c.g.h, c.g.w, c.pa, query_points, ws.descA,
+                                                           ws.normA);
+    DTK_LAUNCHED();
+  }
+  if (tensor) {   // the query descriptors are reused by every chunk: split them once (layout of desc_rows = N)
+    for (int k = 0; k < 2; ++k) {
+      const DescSplit a(ws.cb[k].split, c.N, c.C);
+      int rc = corr_hilo(c.fv) ? launch_split_hilo(ws.descA, a.hi, c.N, c.C, c.st)
+                               : launch_split_f16(ws.descA, a.hi, a.lo, (size_t)c.N * c.C, c.st);
+      if (rc) return rc;
+    }
+  }
+  plan_chunks(0, c.T, c.N, nullptr, c.ch, c.gcap, c.metas, c.plan_host);
+  int rc = c.upload_plan();
+  if (rc) return rc;
+  for (size_t k = 0; k < c.metas.size(); ++k) {
+    const ChunkMeta& cm = c.metas[k];
+    const ChunkBufs& b = ws.cb[k & 1];
+    const InferCtx::Grp gp = c.grp_of(k);
+    {
+      ProfRange pr(PROF_MISC, c.st);
+      index_traj_kernel<<<cdiv(cm.used, 256), 256, 0, c.st>>>(gp.f, gp.r, gp.map0, cm.n_groups, cm.used, c.T,
+                                                              ws.out_index_ring[k & 3], traj);
+      DTK_LAUNCHED();
+    }
+    CorrAssist as;
+    as.tkeys = tensor ? b.tkeys : nullptr; as.zero_word = b.hscratch; as.split_ready = tensor; as.no_thin = cm.no_thin;
+    rc = launch_corr_maps(c.fv, ws.descA, c.N, ws.normA, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, c.ms,
+                          b.plan, b.split, c.st, as);
+    if (rc) return rc;
+    rc = launch_head(b.maps, cm.used, c.ms, c.g, c.hw, ws.out_index_ring[k & 3], traj, 3, 0, nullptr, b.hscratch, c.st, as.tkeys,
+                     true);
+    if (rc) return rc;
+    if (k < INFER_A_COUNTED)
+      DTK_CUDA(cudaMemcpyAsync(ws.d_cntA + k, b.hscratch, sizeof(int), cudaMemcpyDeviceToDevice, c.st));
+  }
+  n_counted = (int)std::min<size_t>(c.metas.size(), INFER_A_COUNTED);
+  return DINOTRK_OK;
+}
+
+// ---- phase C, exact-window pipeline (xwin.cuh): XW_RING chunks in flight, each with its ring slot of per-map arrays and
+// gathered descriptor rows.  The sampling stream sb fills a chunk's scalars and gathered rows; the caller's stream runs its
+// coarse pass, cell plan, exact-window GEMM and head.  The maps the head cannot certify go to the full-map queue: their
+// descriptors are appended to ONE compact array (buffer set ws.cb[0]), which is worked off -- split-precision GEMM over all
+// tokens on 128-row tiles + the head kernels of head.cu -- when it is full and at the end of the phase.
+struct ExactWindow {
+  InferCtx& c;
+  const AnchorChoice& choice;
+  const CellPlan& cp;
+  bool ovl;             // sb is the side stream
+  cudaStream_t sb;
+  const float* traj;
+  float* anchors;
+  int q_rows = 0, q_groups = 0;   // the full-map queue
+
+  XwCells cells_of(size_t k) const {
+    XwCells x;
+    const int n = (int)(cp.first[k + 1] - cp.first[k]);
+    const int* base = c.ws.d_cells + 5 * cp.first[k];
+    x.row0 = base; x.m = base + n; x.frame = base + 2 * n; x.group = base + 3 * n; x.arow = base + 4 * n;
+    x.n_cells = n; x.max_m = cp.max_m;
+    return x;
+  }
+  // the per-map scalars of chunk k and its gathered descriptor rows, on sb
+  int sample(size_t k) {
+    InferWs& ws = c.ws;
+    const ChunkMeta& cm = c.metas[k];
+    const XwSet& x = ws.xr[k % XW_RING];
+    const InferCtx::Grp gp = c.grp_of(k);
+    if (ovl && k >= XW_RING) DTK_CUDA(cudaStreamWaitEvent(sb, choice.xa->freed[k % XW_RING], 0));   // chunk k - 4 is through
+    {
+      ProfRange pr(PROF_SAMPLE, sb);
+      anchor_scalars_kernel<<<cdiv(cm.used, 256), 256, 0, sb>>>(c.T, ws.d_qlist, c.N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups,
+                                                               cm.used, c.N * c.T, x.row0, ws.u_norm, ws.u_flag, ws.u_rho,
+                                                               c.fv.q_rho, xw_s8_slack(c.C), choice.s8, x.out_index, x.arow,
+                                                               x.norm, x.eps);
+      DTK_LAUNCHED();
+      if (cm.n_gathered > 0) {
+        const size_t r0 = (size_t)x.row0;
+        gather_anchor_kernel<<<cm.gather_hi - cm.gather_lo, SAMPLE_THREADS, 0, sb>>>(
+            c.fv.tpc, c.T, c.C, c.P, c.g.h, c.g.w, c.pa, traj, ws.d_qlist, c.N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups,
+            c.N * c.T, cm.gather_lo, c.fb, ws.u_hi, ws.u_lo, ws.u_flag, x.norm, ws.u_hi + r0 * c.C, ws.u_lo + r0 * c.C, ws.u_q8,
+            ws.u_fac, c.fv.q_rho, xw_s8_slack(c.C), choice.s8 ? ws.u_q8 + r0 * c.C : nullptr, ws.u_fac + r0, x.eps);
+        DTK_LAUNCHED();
+      }
+    }
+    if (ovl) DTK_CUDA(cudaEventRecord(choice.xa->sample[k % XW_RING], sb));
+    return DINOTRK_OK;
+  }
+  // works off the full-map queue
+  int flush() {
+    if (q_rows == 0) return DINOTRK_OK;
+    const ChunkBufs& b = c.ws.cb[0];
+    CorrAssist as;
+    as.tkeys = b.tkeys; as.zero_word = b.hscratch; as.split_ready = true; as.no_thin = true; as.all_wide = true; as.small_tiles = true;
+    const int* cg = c.ws.d_cgrp;
+    const int sg = c.ws.sg_cap;
+    int rc = launch_corr_maps(c.fv, nullptr, c.ch, b.norm, cg, cg + sg, cg + 2 * sg, cg + 3 * sg, q_groups, q_rows, q_rows,
+                              b.maps, c.ms, c.ws.d_splan, b.split, c.st, as);
+    if (rc) return rc;
+    rc = launch_head(b.maps, q_rows, c.ms, c.g, c.hw, c.ws.out_index_ring[0], anchors, 2, 0, nullptr, b.hscratch, c.st, b.tkeys,
+                     true);
+    q_rows = q_groups = 0;
+    return rc;
+  }
+  // waits for chunk j's head, counts its maps and appends the ones it queued to the full-map queue
+  int finish(size_t j) {
+    InferWs& ws = c.ws;
+    XwAsync* xa = choice.xa;
+    DTK_CUDA(cudaEventSynchronize(xa->done[j % XW_RING]));
+    const int n_slow = xa->host_cnt[2 * (j % XW_RING)];
+    g_infer_stats[infer_stat::full_map_by_certificate] += xa->host_cnt[2 * (j % XW_RING) + 1];
+    const ChunkMeta& cm = c.metas[j];
+    const XwSet& x = ws.xr[j % XW_RING];
+    const InferCtx::Grp gp = c.grp_of(j);
+    DTK_CHECK_ARG(n_slow >= 0 && n_slow <= cm.used, "infer: corrupt full-map queue (%d of %d)", n_slow, cm.used);
+    g_infer_stats[infer_stat::exact_window] += cm.used - n_slow; g_infer_stats[infer_stat::full_map] += n_slow;
+    if (n_slow > 0) {
+      if (q_rows + n_slow > c.ch || q_groups + cm.n_groups > ws.sg_cap) {
+        int rc = flush();
+        if (rc) return rc;
+      }
+      const ChunkBufs& b = ws.cb[0];
+      const DescSplit d(b.split, c.ch, c.C);   // layout of a descriptor array of `ch` rows
+      int rc = launch_xw_compact(nullptr, ws.u_hi, ws.u_lo, x.arow, x.norm, x.out_index, c.C, gp.f, gp.map0, cm.n_groups, n_slow,
+                                 x.xc, nullptr, d.hi, d.lo, b.norm, ws.out_index_ring[0], ws.d_cgrp, ws.sg_cap, c.st, q_rows,
+                                 q_groups, corr_hilo(c.fv));
+      if (rc) return rc;
+      q_rows += n_slow; q_groups += cm.n_groups;
+    }
+    DTK_CUDA(cudaEventRecord(xa->freed[j % XW_RING], c.st));
+    return DINOTRK_OK;
+  }
+};
+
+// Runs the exact-window pipeline over the planned chunks; done: how many it finished.  With a probe, chunk 0 is finished
+// first, and its verdict may end the pipeline there (the caller then runs the rest on full maps) or move the rest to the
+// fp16 coarse pass.
+static int anchors_exact_window(InferCtx& c, AnchorChoice& choice, const float* traj, float* anchors, size_t& done) {
+  InferWs& ws = c.ws;
+  const cudaStream_t st = c.st;
+  XwAsync* xa = choice.xa;
+  CellPlan cp;
+  plan_cells(c.T, c.gcap, c.metas, c.plan_host, cp);
+  DTK_CHECK_ARG(cp.first.back() * 5 <= (size_t)c.N * c.T * ws.cell_nb * 5 + 16, "infer: cell plan exceeds its bound");
+  if (!cp.v.empty()) DTK_CUDA(cudaMemcpyAsync(ws.d_cells, cp.v.data(), cp.v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (!cp.tiles.empty()) DTK_CUDA(cudaMemcpyAsync(ws.d_tiles, cp.tiles.data(), cp.tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  InferAsync* ia = infer_async();
+  const bool ovl = ia != nullptr && c.metas.size() > 1;
+  ExactWindow pipe{c, choice, cp, ovl, ovl ? ia->side : st, traj, anchors};
+  if (ovl) {
+    DTK_CUDA(cudaEventRecord(ia->fork, st));
+    DTK_CUDA(cudaStreamWaitEvent(pipe.sb, ia->fork, 0));
+  }
+  int rc;
+  if (!c.metas.empty() && (rc = pipe.sample(0))) return rc;
+  size_t n_finished = 0;
+  done = c.metas.size();
+  for (size_t k = 0; k < c.metas.size(); ++k) {
+    const ChunkMeta& cm = c.metas[k];
+    const XwSet& x = ws.xr[k % XW_RING];
+    const InferCtx::Grp gp = c.grp_of(k);
+    const XwCells cells = pipe.cells_of(k);
+    if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, xa->sample[k % XW_RING], 0));
+    const float* eps = choice.s8 ? x.eps : nullptr;   // (nullptr: the fp16 pass's XW_EPS)
+    g_infer_stats[infer_stat::desc_in_place] += cm.used - cm.n_gathered; g_infer_stats[infer_stat::desc_gathered] += cm.n_gathered;
+    if ((rc = launch_xw_coarse(c.fv, ws.u_hi, (int)ws.xw_rows, ws.u_norm, gp.f, gp.r, gp.m, gp.map0, ws.d_tiles + k * (c.gcap + 1),
+                               cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, ws.d_rnorms,
+                               choice.s8 ? ws.u_q8 : nullptr, ws.u_fac))) return rc;
+    if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, c.g, x.xc, st, cm.used, split_min_norm(c.C), eps))) return rc;
+    if ((rc = launch_xw_gemm(c.fv, c.g, ws.u_hi, ws.u_lo, (int)ws.xw_rows, cells, x.xc, st))) return rc;
+    if ((rc = launch_xw_head(c.fv, c.g, c.hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups,
+                             eps)))
+      return rc;
+    DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * (k % XW_RING), x.xc.slow_cnt + cm.n_groups, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    DTK_CUDA(cudaEventRecord(xa->done[k % XW_RING], st));
+    if (k == 0 && choice.probe && c.metas.size() > 1) {   // the probe: wait for it, look at the certificate's verdicts
+      if ((rc = pipe.finish(0))) return rc;
+      n_finished = 1;
+      if (choice.probe_says_full_maps(g_infer_stats[infer_stat::full_map_by_certificate], g_infer_stats[infer_stat::full_map], cm.used)) {
+        done = 1;
+        break;
+      }
+      g_infer_stats[infer_stat::coarse] = choice.s8 ? 1 : 0;
+    }
+    if (k + 1 < c.metas.size() && (rc = pipe.sample(k + 1))) return rc;
+    while (n_finished + 2 <= k)
+      if ((rc = pipe.finish(n_finished++))) return rc;
+  }
+  while (n_finished < done)
+    if ((rc = pipe.finish(n_finished++))) return rc;
+  if ((rc = pipe.flush())) return rc;
+  if (ovl) {
+    DTK_CUDA(cudaEventRecord(ia->join, pipe.sb));
+    DTK_CUDA(cudaStreamWaitEvent(st, ia->join, 0));
+  }
+  return DINOTRK_OK;
+}
+
+// ---- phase C, full-map pipeline over chunks k0.. of the plan: the descriptors of chunk k + 1 are sampled on the side
+// stream (buffer set (k + 1) & 1) while the caller's stream runs the split-precision GEMM over all tokens and the head's
+// fast path of chunk k.  The full-map head of chunk j (usually an empty list) runs two chunks later, between two GEMMs: it
+// needs ~70 KB of shared memory per CTA and could not co-reside with a GEMM anyway.
+static int anchors_full_map(InferCtx& c, size_t k0, const float* traj, float* anchors) {
+  InferWs& ws = c.ws;
+  const cudaStream_t st = c.st;
+  const bool tensor = c.fv.tensor();
+  FeatView fv_split = c.fv;   // the sampler writes the separate halves: F16X3 here
+  fv_split.hilo = nullptr;
+  InferAsync* ia = infer_async();
+  const bool ovl = ia != nullptr && c.metas.size() > k0 + 1;
+  const cudaStream_t sb = ovl ? ia->side : st;   // sampling stream
+  if (ovl) {
+    DTK_CUDA(cudaEventRecord(ia->fork, st));
+    DTK_CUDA(cudaStreamWaitEvent(sb, ia->fork, 0));
+  }
+  auto sample = [&](size_t k) -> int {   // descriptors of chunk k (buffer set k & 1)
+    const ChunkMeta& cm = c.metas[k];
+    const ChunkBufs& b = ws.cb[k & 1];
+    const InferCtx::Grp gp = c.grp_of(k);
+    if (ovl && k >= k0 + 2) DTK_CUDA(cudaStreamWaitEvent(sb, ia->gemm[k & 1], 0));   // GEMM k-2 read the descriptors of this set
+    {
+      ProfRange pr(PROF_SAMPLE, sb);
+      const DescSplit d(b.split, cm.used, c.C);   // the split layout of launch_corr_gemm_tc for desc_rows = used
+      __half* d_hi = tensor ? reinterpret_cast<__half*>(d.hi) : nullptr;
+      __half* d_lo = tensor ? reinterpret_cast<__half*>(d.lo) : nullptr;
+      sample_anchor_kernel<<<cm.used, SAMPLE_THREADS, 0, sb>>>(c.fv.tpc, c.T, c.C, c.P, c.g.h, c.g.w, c.pa, traj, ws.d_qlist, c.N,
+                                                              gp.f, gp.map0, gp.item, cm.n_groups, c.fb, b.desc, b.norm,
+                                                              ws.out_index_ring[k & 3], d_hi, d_lo);
+      DTK_LAUNCHED();
+    }
+    if (ovl) DTK_CUDA(cudaEventRecord(ia->sample[k & 1], sb));
+    return DINOTRK_OK;
+  };
+  auto head_full = [&](size_t j) {   // the last reader of chunk j's maps / keys / list
+    const ChunkBufs& b = ws.cb[j & 1];
+    return launch_head(b.maps, c.metas[j].used, c.ms, c.g, c.hw, ws.out_index_ring[j & 3], anchors, 2, 0, nullptr, b.hscratch,
+                       st, tensor ? b.tkeys : nullptr, true, 2);
+  };
+  int rc;
+  if (k0 < c.metas.size() && (rc = sample(k0))) return rc;
+  for (size_t k = k0; k < c.metas.size(); ++k) {
+    const ChunkMeta& cm = c.metas[k];
+    const ChunkBufs& b = ws.cb[k & 1];
+    const InferCtx::Grp gp = c.grp_of(k);
+    if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, ia->sample[k & 1], 0));
+    if (k >= k0 + 2 && (rc = head_full(k - 2))) return rc;
+    CorrAssist as;
+    as.tkeys = tensor ? b.tkeys : nullptr; as.zero_word = b.hscratch; as.split_ready = tensor; as.no_thin = cm.no_thin;
+    rc = launch_corr_maps(fv_split, b.desc, cm.used, b.norm, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps,
+                          c.ms, b.plan, b.split, st, as);
+    if (rc) return rc;
+    if (ovl) DTK_CUDA(cudaEventRecord(ia->gemm[k & 1], st));
+    if (k + 1 < c.metas.size() && (rc = sample(k + 1))) return rc;
+    rc = launch_head(b.maps, cm.used, c.ms, c.g, c.hw, ws.out_index_ring[k & 3], anchors, 2, 0, nullptr, b.hscratch, st, as.tkeys,
+                     true, 1);
+    if (rc) return rc;
+  }
+  for (size_t j = std::max(k0, c.metas.size() >= 2 ? c.metas.size() - 2 : 0); j < c.metas.size(); ++j)
+    if ((rc = head_full(j))) return rc;
+  return DINOTRK_OK;
+}
+
+// ---- phase C: anchor re-tracking.  The anchor lists, the choice of pipeline around the one host sync, then the exact-window
+// pipeline and, when it does not run or its probe turns it down, the full-map pipeline.
+static int infer_anchors(InferCtx& c, const float* traj, const float* cos_sims, float anchor_th, float* anchors, int n_counted_A) {
+  NvtxRange nv("dinotrk.infer.C.anchors");
+  InferWs& ws = c.ws;
+  const cudaStream_t st = c.st;
+  const int T = c.T, N = c.N;
+  {
+    ProfRange pr(PROF_ANCHOR_LIST, st);
+    anchor_lists_kernel<<<T, ANCHOR_LIST_THREADS, 0, st>>>(cos_sims, N, T, anchor_th, ws.d_cnt, ws.d_qlist);
+    DTK_LAUNCHED();
+  }
+  AnchorChoice choice(c.fv, c.g);
+  XwAsync* xa = choice.xa;
+  if (xa) {   // reciprocal token norms for the coarse epilogue + the smallest norm of the video (the choice reads it)
+    int rc = launch_xw_rnorms(c.fv, ws.d_rnorms, ws.d_minnorm, st);
+    if (rc) return rc;
+    DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + XW_CNT_MINNORM, ws.d_minnorm, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    if (n_counted_A > 0)
+      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + XW_CNT_A, ws.d_cntA, (size_t)n_counted_A * sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
+  std::vector<int> cnt(T);
+  DTK_CUDA(cudaMemcpyAsync(cnt.data(), ws.d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
+  std::vector<float> rho_f(c.fv.s8() ? T : 0);
+  if (c.fv.s8()) DTK_CUDA(cudaMemcpyAsync(rho_f.data(), c.fv.q_rho, (size_t)T * sizeof(float), cudaMemcpyDeviceToHost, st));
+  std::vector<int> qlist_h, uflag_h;
+  if (choice.xw) {
+    // every (query, source frame) descriptor once, before the host waits (it depends on the trajectories only).  The
+    // planner needs the anchor lists and the flags.
+    {
+      ProfRange pr(PROF_SAMPLE, st);
+      sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(c.fv.tpc, T, c.C, c.P, c.g.h, c.g.w, c.pa, traj, c.fb, ws.u_hi, ws.u_lo,
+                                                             ws.u_norm, ws.u_flag, AnchorChoice::q8_rows(c.fv) ? ws.u_q8 : nullptr,
+                                                             ws.u_fac, ws.u_rho);
+      DTK_LAUNCHED();
+    }
+    qlist_h.resize((size_t)T * N); uflag_h.resize((size_t)N * T);
+    DTK_CUDA(cudaMemcpyAsync(qlist_h.data(), ws.d_qlist, qlist_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+    DTK_CUDA(cudaMemcpyAsync(uflag_h.data(), ws.u_flag, uflag_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
+  DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: the anchor work lists
+  choice.after_sync(c.C, n_counted_A, (long long)N * T);
+  long long maps_C = 0;
+  for (int a = 0; a < T; ++a) maps_C += (long long)cnt[a] * T;
+  long long* stats = g_infer_stats;
+  stats[infer_stat::anchor_maps] = maps_C; stats[infer_stat::exact_window] = 0; stats[infer_stat::full_map] = 0;
+  stats[infer_stat::pipeline] = choice.xw ? 1 : 0; stats[infer_stat::full_map_by_certificate] = 0;
+  stats[infer_stat::contraction] = c.fv.tensor() ? 1 : 0; stats[infer_stat::desc_in_place] = 0; stats[infer_stat::desc_gathered] = 0;
+  float rho_max = 0.f;
+  for (float r : rho_f) rho_max = std::max(rho_max, r);
+  int rc = choice.coarse_pass(c.fv, rho_max);
+  if (rc) return rc;
+  unsigned bits;
+  memcpy(&bits, &rho_max, sizeof(bits));
+  stats[infer_stat::coarse] = choice.s8 ? 1 : 0; stats[infer_stat::coarse_rho_f] = bits;
+  // The probe is the same set of work items for every chunk size >= XW_PROBE_MAPS.
+  const int probe_cap = choice.probe ? std::max(T, (XW_PROBE_MAPS / T) * T) : 0;
+  size_t k0 = 0;   // first chunk of the full-map pipeline (> 0 after an exact-window probe)
+  if (choice.xw) {
+    std::vector<unsigned char> qflag(N, 0);   // a query with a flagged source frame is never read in place
+    for (size_t u = 0; u < uflag_h.size(); ++u)
+      if (uflag_h[u]) qflag[u / T] = 1;
+    const AnchorRows rows{qlist_h.data(), qflag.data(), N * T, XW_RING, c.ch};
+    DTK_CHECK_ARG(plan_chunks(1, T, N, cnt.data(), c.ch, c.gcap, c.metas, c.plan_host, T, probe_cap, &rows),
+                  "infer: a chunk of the anchor phase has more than %d groups", c.gcap);
+    if ((rc = c.upload_plan())) return rc;
+    if ((rc = anchors_exact_window(c, choice, traj, anchors, k0))) return rc;
+    if (k0 == c.metas.size()) return DINOTRK_OK;
+    // switched: chunks k0.. on the full-map pipeline.  The same chunks, their rows per chunk again.  (Everything that read
+    // the plan is in the caller's stream by now, so the upload is ordered behind it.)
+    stats[infer_stat::pipeline] = 0; stats[infer_stat::coarse] = 0;
+    plan_chunks(1, T, N, cnt.data(), c.ch, c.gcap, c.metas, c.plan_host, T, probe_cap);
+  } else {
+    plan_chunks(1, T, N, cnt.data(), c.ch, c.gcap, c.metas, c.plan_host);
+  }
+  if ((rc = c.upload_plan())) return rc;
+  return anchors_full_map(c, k0, traj, anchors);
+}
+
 }  // namespace dtk
 
 using namespace dtk;
@@ -645,7 +1069,7 @@ int dinotrk_infer_set_coarse(int mode) {
 
 int dinotrk_infer_last_stats(long long* out, int n) {
   DTK_CHECK_ARG(out && n >= 4, "infer_last_stats: need at least 4 slots");
-  for (int i = 0; i < (n < INFER_STATS ? n : INFER_STATS); ++i) out[i] = g_infer_stats[i];
+  for (int i = 0; i < (n < infer_stat::count ? n : infer_stat::count); ++i) out[i] = g_infer_stats[i];
   return DINOTRK_OK;
 }
 
@@ -718,7 +1142,7 @@ int dinotrk_infer_plan_anchors(int T, int N, const int* anchor_counts, const int
 }
 
 int dinotrk_infer_set_overlap(int mode) {
-  DTK_CHECK_ARG(mode >= -1 && mode <= 2, "infer_set_overlap: mode must be -1 (default / DTK_OVERLAP), 0, 1 or 2");
+  DTK_CHECK_ARG(mode >= -1 && mode <= 1, "infer_set_overlap: mode must be -1 (default), 0 or 1");
   g_overlap_mode = mode;
   return DINOTRK_OK;
 }
@@ -805,7 +1229,6 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
                   float* anchors,
                   uint8_t* occ, void* workspace, size_t workspace_bytes, void* stream) {
   DTK_CHECK_ARG(feat && feat->tpc && feat->norms && g && hw && query_points && traj, "infer: null pointer");
-  const float* tpc = feat->tpc;
   const int T = feat->T, C = feat->C;
   DTK_CHECK_ARG(T > 0 && C > 0 && C % 4 == 0 && N >= 0, "infer: bad sizes");
   DTK_CHECK_GRID(*g, "infer");
@@ -819,393 +1242,27 @@ int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
                 "infer: workspace too small (%zu < %zu)", workspace_bytes,
                 dinotrk_infer_workspace_bytes(T, C, g, N, chunk_maps));
   if (N == 0) return DINOTRK_OK;
-  cudaStream_t st = (cudaStream_t)stream;
   const int P = g->h * g->w, ms = dinotrk_map_stride(g);
   const int ch = infer_chunk_eff(chunk_maps, T);
   const int fb = frame_batch > 0 ? (frame_batch < T ? frame_batch : T) : T;
   const int gcap = infer_gcap(T, ch);
-  const PointAffine pa = make_point_affine(*g);
-
   const size_t max_chunks = infer_max_chunks(T, N, (size_t)ch);
   Arena ar(workspace);
   InferWs ws(ar, T, C, N, P, ms, ch, gcap, max_chunks);
-  const int n_unique = N * T;
   DTK_CHECK_ARG(ws.xw_rows <= 0x7fffffffu, "infer: %zu descriptor rows exceed the row index", ws.xw_rows);
-  const bool tensor = fv.tensor();   // tensor-core GEMM: tile keys for the head, fp16 split fused into the samplers
-  FeatView fv_split = fv;            // the full-map pipeline's sampler writes the separate halves: F16X3 there
-  fv_split.hilo = nullptr;
+  InferCtx c{fv, *g, *hw, ws, (cudaStream_t)stream, T, C, N, P, ms, ch, gcap, fb, max_chunks, make_point_affine(*g)};
 
-  // The chunks of a phase are planned on the host in one go and their group arrays uploaded with ONE copy, so the
-  // per-chunk launches below never block the host (a pageable cudaMemcpyAsync per chunk would).
-  std::vector<ChunkMeta> metas;
-  std::vector<int> plan_host;
-  auto upload_plan = [&]() -> int {
-    DTK_CHECK_ARG(metas.size() <= max_chunks, "infer: chunk plan exceeds its bound (%zu > %zu)", metas.size(), max_chunks);
-    if (!plan_host.empty())
-      DTK_CUDA(cudaMemcpyAsync(ws.d_groups, plan_host.data(), plan_host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    return DINOTRK_OK;
-  };
-  struct Grp { const int *f, *r, *m, *map0, *item; };
-  auto grp_of = [&](size_t k) {
-    const int* b = ws.d_groups + k * 5 * gcap;
-    return Grp{b, b + gcap, b + 2 * gcap, b + 3 * gcap, b + 4 * gcap};
-  };
-
-  int n_chunks_A = 0;
-  long long maps_A = 0;
-  // ---- phase A: trajectories -------------------------------------------------------------------
-  if (start_phase <= 0) {
-    NvtxRange nv("dinotrk.infer.A.trajectories");
-    {
-      ProfRange pr(PROF_SAMPLE, st);
-      sample_query_kernel<<<N, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, query_points, ws.descA, ws.normA);
-      DTK_LAUNCHED();
-    }
-    if (tensor) {   // the query descriptors are reused by every chunk: split them once (layout of desc_rows = N)
-      for (int k = 0; k < 2; ++k) {
-        const DescSplit a(ws.cb[k].split, N, C);
-        int rc = corr_hilo(fv) ? launch_split_hilo(ws.descA, a.hi, N, C, st)
-                               : launch_split_f16(ws.descA, a.hi, a.lo, (size_t)N * C, st);
-        if (rc) return rc;
-      }
-    }
-    plan_chunks(0, T, N, nullptr, ch, gcap, metas, plan_host);
-    int rc = upload_plan();
-    if (rc) return rc;
-    for (size_t k = 0; k < metas.size(); ++k) {
-      const ChunkMeta& cm = metas[k];
-      const ChunkBufs& b = ws.cb[k & 1];
-      const Grp gp = grp_of(k);
-      {
-        ProfRange pr(PROF_MISC, st);
-        index_traj_kernel<<<cdiv(cm.used, 256), 256, 0, st>>>(gp.f, gp.r, gp.map0, cm.n_groups, cm.used, T, ws.out_index_ring[k & 3], traj);
-        DTK_LAUNCHED();
-      }
-      CorrAssist as;
-      as.tkeys = tensor ? b.tkeys : nullptr; as.zero_word = b.hscratch; as.split_ready = tensor; as.no_thin = cm.no_thin;
-      rc = launch_corr_maps(fv, ws.descA, N, ws.normA, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, ms, b.plan,
-                            b.split, st, as);
-      if (rc) return rc;
-      rc = launch_head(b.maps, cm.used, ms, *g, *hw, ws.out_index_ring[k & 3], traj, 3, 0, nullptr, b.hscratch, st, as.tkeys, true);
-      if (rc) return rc;
-      if (k < 16)   // uncertified maps of this chunk: the anchor phase chooses its pipeline from their share
-        DTK_CUDA(cudaMemcpyAsync(ws.d_cntA + k, b.hscratch, sizeof(int), cudaMemcpyDeviceToDevice, st));
-    }
-    n_chunks_A = (int)std::min<size_t>(metas.size(), 16);
-    maps_A = (long long)N * T;
-  }
+  int rc, n_counted_A = 0;
+  if (start_phase <= 0 && (rc = infer_trajectories(c, query_points, traj, n_counted_A))) return rc;
   if (stop_after < 1) return DINOTRK_OK;
-
-  // ---- phase B: cosine similarities along the trajectories --------------------------------------
-  if (start_phase <= 1) {
+  if (start_phase <= 1) {   // ---- phase B: cosine similarities along the trajectories
     NvtxRange nv("dinotrk.infer.B.cos_sims");
-    int rc = dinotrk_traj_cos_sims(tpc, T, C, g, traj, query_points, N, cos_sims, nullptr, 0, stream);
-    if (rc) return rc;
+    if ((rc = dinotrk_traj_cos_sims(feat->tpc, T, C, g, traj, query_points, N, cos_sims, nullptr, 0, stream))) return rc;
   }
   if (stop_after < 2) return DINOTRK_OK;
-
-  // ---- phase C: anchor re-tracking ---------------------------------------------------------------
-  // Three streams: the caller's stream runs the correlation GEMMs back to back; one auxiliary stream samples the
-  // descriptors of chunk k+1, another runs the head of chunk k, both while the GEMM of chunk k+1 owns the tensor cores
-  // (the head kernel is then launched with one CTA per SM so that it fits next to the GEMM's ~200 KB of shared memory;
-  // the rare full-map head launches cannot co-reside and simply wait for the GEMM's CTAs to retire).
-  if (start_phase <= 2) {
-    NvtxRange nv("dinotrk.infer.C.anchors");
-    {
-      ProfRange pr(PROF_ANCHOR_LIST, st);
-      anchor_lists_kernel<<<T, ANCHOR_LIST_THREADS, 0, st>>>(cos_sims, N, T, anchor_th, ws.d_cnt, ws.d_qlist);
-      DTK_LAUNCHED();
-    }
-    std::vector<int> cnt(T);
-    // pipeline of the anchor phase: coarse pass + exact window (xwin.cuh) on the tensor path, unless disabled
-    bool use_xw = tensor && disc_fits_box(*g);
-    int pathsel = g_xw_path;
-    if (pathsel < 0) { const char* e = getenv("DTK_XW"); if (e) pathsel = atoi(e) != 0 ? 1 : 0; }
-    if (pathsel == 0) use_xw = false;
-    XwAsync* xa = use_xw ? xw_async() : nullptr;
-    if (!xa) use_xw = false;
-    if (xa) {   // reciprocal token norms for the coarse epilogue + the smallest norm of the video (the host reads it below)
-      int rcn = launch_xw_rnorms(fv, ws.d_rnorms, ws.d_minnorm, st);
-      if (rcn) return rcn;
-      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING + 16, ws.d_minnorm, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    }
-    if (xa && n_chunks_A > 0)
-      DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * XW_RING, ws.d_cntA, (size_t)n_chunks_A * sizeof(int), cudaMemcpyDeviceToHost, st));
-    DTK_CUDA(cudaMemcpyAsync(cnt.data(), ws.d_cnt, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost, st));
-    std::vector<float> rho_f(fv.s8() ? T : 0);
-    if (fv.s8()) DTK_CUDA(cudaMemcpyAsync(rho_f.data(), fv.q_rho, (size_t)T * sizeof(float), cudaMemcpyDeviceToHost, st));
-    std::vector<int> qlist_h, uflag_h;
-    if (use_xw) {
-      // every (query, source frame) descriptor once, before the host waits (it depends on the trajectories only); with the
-      // int8 rows whenever the int8 coarse pass can still be chosen.  The planner needs the anchor lists and the flags.
-      const bool q8 = fv.s8() && g_xw_coarse != 0 && C % 16 == 0 && C <= XW_S8_MAX_C;
-      {
-        ProfRange pr(PROF_SAMPLE, st);
-        sample_unique_kernel<<<N * T, SAMPLE_THREADS, 0, st>>>(tpc, T, C, P, g->h, g->w, pa, traj, fb, ws.u_hi, ws.u_lo, ws.u_norm, ws.u_flag,
-                                                               q8 ? ws.u_q8 : nullptr, ws.u_fac, ws.u_rho);
-        DTK_LAUNCHED();
-      }
-      qlist_h.resize((size_t)T * N); uflag_h.resize((size_t)N * T);
-      DTK_CUDA(cudaMemcpyAsync(qlist_h.data(), ws.d_qlist, qlist_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-      DTK_CUDA(cudaMemcpyAsync(uflag_h.data(), ws.u_flag, uflag_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-    }
-    DTK_CUDA(cudaStreamSynchronize(st));  // the one host sync: the anchor work lists
-    if (use_xw) {   // a token below the split's faithful range (a zero one included) voids the coarse pass's error bound
-      float mn;
-      memcpy(&mn, xa->host_cnt + 2 * XW_RING + 16, sizeof(float));
-      if (!(mn >= split_min_norm(C))) use_xw = false;
-    }
-    if (use_xw && pathsel < 0 && n_chunks_A > 0) {
-      // head weights the certificate cannot handle send (almost) every map to the full-map kernels anyway: the trajectory
-      // phase just showed it; skip the exact-window attempt then.  (Depends on the weights and the video only.)
-      long long unc = 0;
-      for (int k = 0; k < n_chunks_A; ++k) unc += xa->host_cnt[2 * XW_RING + k];
-      if (unc * 4 > maps_A) use_xw = false;
-    }
-    long long maps_C = 0;
-    for (int a = 0; a < T; ++a) maps_C += (long long)cnt[a] * T;
-    g_infer_stats[0] = maps_C; g_infer_stats[1] = 0; g_infer_stats[2] = 0; g_infer_stats[3] = use_xw ? 1 : 0; g_infer_stats[4] = 0;
-    g_infer_stats[5] = tensor ? 1 : 0; g_infer_stats[8] = 0; g_infer_stats[9] = 0;
-    // coarse pass of the exact-window pipeline (decided once use_xw is final): int8 when the features carry their int8
-    // operands (forced: required), unless a frame's residual makes the bound too loose (automatic mode; below: or the probe
-    // chunk queues too many maps)
-    DTK_CHECK_ARG(g_xw_coarse != 1 || !use_xw || fv.s8(), "infer: int8 coarse pass forced without the int8 features");
-    bool s8 = use_xw && fv.s8() && g_xw_coarse != 0;
-    DTK_CHECK_ARG(!s8 || (C % 16 == 0 && C <= XW_S8_MAX_C), "infer: int8 coarse pass needs C %% 16 == 0 and C <= %d", XW_S8_MAX_C);
-    {
-      float rho_max = 0.f;
-      for (float r : rho_f) rho_max = std::max(rho_max, r);
-      if (g_xw_coarse < 0 && !(rho_max <= XW_S8_RHO_MAX)) s8 = false;
-      unsigned bits;
-      memcpy(&bits, &rho_max, sizeof(bits));
-      g_infer_stats[6] = s8 ? 1 : 0; g_infer_stats[7] = bits;
-    }
-    size_t k0 = 0;            // first chunk of the full-map pipeline (> 0 after an exact-window probe)
-    bool planned = false;
-    if (use_xw) {
-      // automatic mode: the first chunk is a small probe; if the head's certificate sends more than a quarter of it to the
-      // full-map queue (refiner weights whose outside-the-box logit bound needs the exact map), the rest of the phase runs
-      // the full-map pipeline directly.  The probe is the same set of work items for every chunk size >= XW_PROBE_MAPS.
-      const bool probing = pathsel < 0;
-      const int probe_cap = std::max(T, (XW_PROBE_MAPS / T) * T);
-      std::vector<unsigned char> qflag(N, 0);   // a query with a flagged source frame is never read in place
-      for (size_t u = 0; u < uflag_h.size(); ++u)
-        if (uflag_h[u]) qflag[u / T] = 1;
-      const AnchorRows rows{qlist_h.data(), qflag.data(), n_unique, XW_RING, ch};
-      DTK_CHECK_ARG(plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host, T, probing ? probe_cap : 0, &rows),
-                    "infer: a chunk of the anchor phase has more than %d groups", gcap);
-      int rc = upload_plan();
-      if (rc) return rc;
-      planned = true;
-      CellPlan cp;
-      plan_cells(T, gcap, metas, plan_host, cp);
-      DTK_CHECK_ARG(cp.first.back() * 5 <= (size_t)N * T * ws.cell_nb * 5 + 16, "infer: cell plan exceeds its bound");
-      if (!cp.v.empty()) DTK_CUDA(cudaMemcpyAsync(ws.d_cells, cp.v.data(), cp.v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-      if (!cp.tiles.empty()) DTK_CUDA(cudaMemcpyAsync(ws.d_tiles, cp.tiles.data(), cp.tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-      InferAsync* ia = infer_async();
-      const bool ovl = ia != nullptr && metas.size() > 1;
-      cudaStream_t sb = ovl ? ia->aux2 : st;   // sampling stream
-      if (ovl) {
-        DTK_CUDA(cudaEventRecord(ia->fork, st));
-        DTK_CUDA(cudaStreamWaitEvent(sb, ia->fork, 0));
-      }
-      auto cells_of = [&](size_t k) {
-        XwCells c;
-        const int n = (int)(cp.first[k + 1] - cp.first[k]);
-        const int* base = ws.d_cells + 5 * cp.first[k];
-        c.row0 = base; c.m = base + n; c.frame = base + 2 * n; c.group = base + 3 * n; c.arow = base + 4 * n;
-        c.n_cells = n; c.max_m = cp.max_m;
-        return c;
-      };
-      auto enqueue_sample_x = [&](size_t k) -> int {
-        const ChunkMeta& cm = metas[k];
-        const XwSet& x = ws.xr[k % XW_RING];
-        const Grp gp = grp_of(k);
-        if (ovl && k >= XW_RING) DTK_CUDA(cudaStreamWaitEvent(sb, xa->freed[k % XW_RING], 0));   // chunk k - 4 is through
-        {
-          ProfRange pr(PROF_SAMPLE, sb);
-          anchor_scalars_kernel<<<cdiv(cm.used, 256), 256, 0, sb>>>(T, ws.d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, cm.used,
-                                                                   n_unique, x.row0, ws.u_norm, ws.u_flag, ws.u_rho, fv.q_rho, xw_s8_slack(C), s8, x.out_index,
-                                                                   x.arow, x.norm, x.eps);
-          DTK_LAUNCHED();
-          if (cm.n_gathered > 0) {
-            const size_t r0 = (size_t)x.row0;
-            gather_anchor_kernel<<<cm.gather_hi - cm.gather_lo, SAMPLE_THREADS, 0, sb>>>(
-                tpc, T, C, P, g->h, g->w, pa, traj, ws.d_qlist, N, gp.f, gp.r, gp.map0, gp.item, cm.n_groups, n_unique, cm.gather_lo, fb, ws.u_hi, ws.u_lo, ws.u_flag,
-                                                                    x.norm, ws.u_hi + r0 * C, ws.u_lo + r0 * C, ws.u_q8, ws.u_fac, fv.q_rho, xw_s8_slack(C),
-                                                                    s8 ? ws.u_q8 + r0 * C : nullptr, ws.u_fac + r0, x.eps);
-            DTK_LAUNCHED();
-          }
-        }
-        if (ovl) DTK_CUDA(cudaEventRecord(xa->sample[k % XW_RING], sb));
-        return DINOTRK_OK;
-      };
-      // Full-map queue.  The queued maps of chunk j (the host knows how many once the chunk's head has run) are appended to
-      // ONE compact descriptor array (buffer set ws.cb[0]); the queue is worked off -- split-precision GEMM over all tokens on
-      // 128-row tiles + the head kernels of head.cu -- when it is full and at the end of the phase.
-      int q_rows = 0, q_groups = 0;
-      auto flush = [&]() -> int {
-        if (q_rows == 0) return DINOTRK_OK;
-        const ChunkBufs& b = ws.cb[0];
-        CorrAssist as;
-        as.tkeys = b.tkeys; as.zero_word = b.hscratch; as.split_ready = true; as.no_thin = true; as.all_wide = true; as.small_tiles = true;
-        int rc2 = launch_corr_maps(fv, nullptr, ch, b.norm, ws.d_cgrp, ws.d_cgrp + ws.sg_cap, ws.d_cgrp + 2 * ws.sg_cap, ws.d_cgrp + 3 * ws.sg_cap, q_groups,
-                                   q_rows, q_rows, b.maps, ms, ws.d_splan, b.split, st, as);
-        if (rc2) return rc2;
-        rc2 = launch_head(b.maps, q_rows, ms, *g, *hw, ws.out_index_ring[0], anchors, 2, 0, nullptr, b.hscratch, st, b.tkeys, true);
-        q_rows = q_groups = 0;
-        return rc2;
-      };
-      auto finish = [&](size_t j) -> int {
-        DTK_CUDA(cudaEventSynchronize(xa->done[j % XW_RING]));
-        const int n_slow = xa->host_cnt[2 * (j % XW_RING)];
-        g_infer_stats[4] += xa->host_cnt[2 * (j % XW_RING) + 1];
-        const ChunkMeta& cm = metas[j];
-        const XwSet& x = ws.xr[j % XW_RING];
-        const Grp gp = grp_of(j);
-        DTK_CHECK_ARG(n_slow >= 0 && n_slow <= cm.used, "infer: corrupt full-map queue (%d of %d)", n_slow, cm.used);
-        g_infer_stats[1] += cm.used - n_slow; g_infer_stats[2] += n_slow;
-        if (n_slow > 0) {
-          if (q_rows + n_slow > ch || q_groups + cm.n_groups > ws.sg_cap) {
-            int rc2 = flush();
-            if (rc2) return rc2;
-          }
-          const ChunkBufs& b = ws.cb[0];
-          const DescSplit c(b.split, ch, C);   // layout of a descriptor array of `ch` rows
-          int rc2 = launch_xw_compact(nullptr, ws.u_hi, ws.u_lo, x.arow, x.norm, x.out_index, C, gp.f, gp.map0, cm.n_groups,
-                                      n_slow, x.xc, nullptr, c.hi, c.lo, b.norm, ws.out_index_ring[0], ws.d_cgrp, ws.sg_cap, st, q_rows, q_groups,
-                                      corr_hilo(fv));
-          if (rc2) return rc2;
-          q_rows += n_slow; q_groups += cm.n_groups;
-        }
-        DTK_CUDA(cudaEventRecord(xa->freed[j % XW_RING], st));
-        return DINOTRK_OK;
-      };
-      if (!metas.empty() && (rc = enqueue_sample_x(0))) return rc;
-      size_t n_finished = 0, k_end = metas.size();
-      for (size_t k = 0; k < metas.size(); ++k) {
-        const ChunkMeta& cm = metas[k];
-        const XwSet& x = ws.xr[k % XW_RING];
-        const Grp gp = grp_of(k);
-        const XwCells cells = cells_of(k);
-        if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, xa->sample[k % XW_RING], 0));
-        const float* eps = s8 ? x.eps : nullptr;   // (nullptr: the fp16 pass's XW_EPS)
-        g_infer_stats[8] += cm.used - cm.n_gathered; g_infer_stats[9] += cm.n_gathered;
-        if ((rc = launch_xw_coarse(fv, ws.u_hi, (int)ws.xw_rows, ws.u_norm, gp.f, gp.r, gp.m, gp.map0, ws.d_tiles + k * (gcap + 1),
-                                   cm.n_groups, cm.used / TC2_BM_ROWS + cm.n_groups, x.xc, st, ws.d_rnorms, s8 ? ws.u_q8 : nullptr,
-                                   ws.u_fac))) return rc;
-        if ((rc = launch_xw_plan(cells, x.norm, cm.n_groups, *g, x.xc, st, cm.used, split_min_norm(C), eps))) return rc;
-        if ((rc = launch_xw_gemm(fv, *g, ws.u_hi, ws.u_lo, (int)ws.xw_rows, cells, x.xc, st))) return rc;
-        if ((rc = launch_xw_head(fv, *g, *hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups,
-                                 eps)))
-          return rc;
-        DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * (k % XW_RING), x.xc.slow_cnt + cm.n_groups, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-        DTK_CUDA(cudaEventRecord(xa->done[k % XW_RING], st));
-        if (k == 0 && probing && metas.size() > 1) {   // the probe: wait for it, look at the certificate's verdicts
-          if ((rc = finish(0))) return rc;
-          n_finished = 1;
-          if (g_infer_stats[4] * 4 > (long long)cm.used) { k_end = 1; break; }
-          if (s8 && g_xw_coarse < 0 && g_infer_stats[2] * XW_S8_PROBE_QUEUE_DIV > (long long)cm.used) {
-            s8 = false;                   // the rest of the phase on the fp16 coarse pass
-            g_infer_stats[6] = 0;
-          }
-        }
-        if (k + 1 < metas.size() && (rc = enqueue_sample_x(k + 1))) return rc;
-        while (n_finished + 2 <= k)
-          if ((rc = finish(n_finished++))) return rc;
-      }
-      while (n_finished < k_end)
-        if ((rc = finish(n_finished++))) return rc;
-      if ((rc = flush())) return rc;
-      if (ovl) {
-        DTK_CUDA(cudaEventRecord(ia->join, sb));
-        DTK_CUDA(cudaStreamWaitEvent(st, ia->join, 0));
-      }
-      if (k_end == metas.size()) {
-        if (stop_after < 3) return DINOTRK_OK;
-        NvtxRange nvd("dinotrk.infer.D.occlusion");
-        return dinotrk_occlusion(traj, cos_sims, anchors, N, T, anchor_th, cos_th, occ, stream);
-      }
-      // switched: chunks k0.. on the full-map pipeline below.  The same chunks, their rows per chunk again.  (Everything
-      // that read the plan is in the caller's stream by now, so the upload is ordered behind it.)
-      k0 = k_end;
-      g_infer_stats[3] = 0;
-      g_infer_stats[6] = 0;
-      plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host, T, probing ? probe_cap : 0);
-      if ((rc = upload_plan())) return rc;
-    }
-    if (!planned) {
-      plan_chunks(1, T, N, cnt.data(), ch, gcap, metas, plan_host);
-      int rc0 = upload_plan();
-      if (rc0) return rc0;
-    }
-    int rc = DINOTRK_OK;
-    InferAsync* ia = infer_async();
-    const bool ovl = ia != nullptr && metas.size() > k0 + 1;
-    cudaStream_t sa = (ovl && ia->mode >= 2) ? ia->aux : st;    // head stream
-    cudaStream_t sb = ovl ? ia->aux2 : st;   // sampling stream
-    if (ovl) {
-      DTK_CUDA(cudaEventRecord(ia->fork, st));
-      DTK_CUDA(cudaStreamWaitEvent(sa, ia->fork, 0));
-      DTK_CUDA(cudaStreamWaitEvent(sb, ia->fork, 0));
-    }
-    auto enqueue_sample = [&](size_t k) -> int {   // descriptors of chunk k (buffer set k & 1)
-      const ChunkMeta& cm = metas[k];
-      const ChunkBufs& b = ws.cb[k & 1];
-      const Grp gp = grp_of(k);
-      if (ovl && k >= k0 + 2) DTK_CUDA(cudaStreamWaitEvent(sb, ia->gemm[k & 1], 0));   // GEMM k-2 read the descriptors of this set
-      {
-        ProfRange pr(PROF_SAMPLE, sb);
-        // the split layout of launch_corr_gemm_tc for desc_rows = used
-        const DescSplit c(b.split, cm.used, C);
-        __half* c_hi = tensor ? reinterpret_cast<__half*>(c.hi) : nullptr;
-        __half* c_lo = tensor ? reinterpret_cast<__half*>(c.lo) : nullptr;
-        sample_anchor_kernel<<<cm.used, SAMPLE_THREADS, 0, sb>>>(tpc, T, C, P, g->h, g->w, pa, traj, ws.d_qlist, N, gp.f, gp.map0,
-                                                                gp.item, cm.n_groups, fb, b.desc, b.norm, ws.out_index_ring[k & 3], c_hi, c_lo);
-        DTK_LAUNCHED();
-      }
-      if (ovl) DTK_CUDA(cudaEventRecord(ia->sample[k & 1], sb));
-      return DINOTRK_OK;
-    };
-    // the full-map head of chunk j (usually an empty list) runs on the GEMM stream between two GEMMs: it needs ~70 KB of
-    // shared memory per CTA and could not co-reside with a GEMM anyway
-    auto head_full = [&](size_t j) -> int {
-      const ChunkBufs& b = ws.cb[j & 1];
-      if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, ia->head[j & 1], 0));   // fast head of chunk j (its list is complete)
-      return launch_head(b.maps, metas[j].used, ms, *g, *hw, ws.out_index_ring[j & 3], anchors, 2, 0, nullptr, b.hscratch, st,
-                         tensor ? b.tkeys : nullptr, true, 0, 2);
-    };
-    if (k0 < metas.size() && (rc = enqueue_sample(k0))) return rc;
-    for (size_t k = k0; k < metas.size(); ++k) {
-      const ChunkMeta& cm = metas[k];
-      const ChunkBufs& b = ws.cb[k & 1];
-      const Grp gp = grp_of(k);
-      if (ovl) DTK_CUDA(cudaStreamWaitEvent(st, ia->sample[k & 1], 0));
-      if (k >= k0 + 2 && (rc = head_full(k - 2))) return rc;   // last reader of maps / keys / list of this buffer set
-      CorrAssist as;
-      as.tkeys = tensor ? b.tkeys : nullptr; as.zero_word = b.hscratch; as.split_ready = tensor; as.no_thin = cm.no_thin;
-      rc = launch_corr_maps(fv_split, b.desc, cm.used, b.norm, gp.f, gp.r, gp.m, gp.map0, cm.n_groups, cm.used, cm.maxm, b.maps, ms,
-                            b.plan, b.split, st, as);
-      if (rc) return rc;
-      if (ovl) DTK_CUDA(cudaEventRecord(ia->gemm[k & 1], st));
-      if (k + 1 < metas.size() && (rc = enqueue_sample(k + 1))) return rc;
-      if (ovl) DTK_CUDA(cudaStreamWaitEvent(sa, ia->gemm[k & 1], 0));
-      rc = launch_head(b.maps, cm.used, ms, *g, *hw, ws.out_index_ring[k & 3], anchors, 2, 0, nullptr, b.hscratch, sa, as.tkeys, true,
-                       (ovl && ia->mode >= 2) ? ia->head_ctas_per_sm : 0, 1);
-      if (rc) return rc;
-      if (ovl) DTK_CUDA(cudaEventRecord(ia->head[k & 1], sa));
-    }
-    for (size_t j = std::max(k0, metas.size() >= 2 ? metas.size() - 2 : 0); j < metas.size(); ++j)
-      if ((rc = head_full(j))) return rc;
-    if (ovl) {
-      DTK_CUDA(cudaEventRecord(ia->join, sa));
-      DTK_CUDA(cudaStreamWaitEvent(st, ia->join, 0));
-    }
-  }
+  if (start_phase <= 2 && (rc = infer_anchors(c, traj, cos_sims, anchor_th, anchors, n_counted_A))) return rc;
   if (stop_after < 3) return DINOTRK_OK;
-
-  // ---- phase D: occlusion --------------------------------------------------------------------------
-  NvtxRange nvd("dinotrk.infer.D.occlusion");
+  NvtxRange nv("dinotrk.infer.D.occlusion");   // ---- phase D: occlusion
   return dinotrk_occlusion(traj, cos_sims, anchors, N, T, anchor_th, cos_th, occ, stream);
 }
 

@@ -555,8 +555,7 @@ static int vit_qkv_fused(const VitShape& s, const TcPlan& pl, const void* y, con
                          __half* k16, __half* v16, cudaStream_t st) {
   const int D = s.D, N1p8 = (int)align_up((size_t)s.N1, 8);
   EpiQKV16 eq{{}, q16, k16, v16, bias, s.N1, D, s.heads, N1p8, 0.125f * 1.4426950408889634f};  // 1/sqrt(64) * log2(e)
-  static const int epi_direct = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;   // bit 0: q / k thread-per-row too (slower)
-  eq.direct_from = (epi_direct & 1) ? 0 : 2 * D;
+  eq.direct_from = 2 * D;   // v^T rows thread-per-row; q / k that way too measured slower
   const TcOperands op = linear_operands(y, s.rows, w);
   const TcProblem pb = pl.problem(1, 3 * D, D);
   const int tiles = cdiv((int)s.rows, TC_BM);
@@ -590,8 +589,7 @@ static int vit_fc1(const VitShape& s, const TcPlan& pl, const void* y, const voi
   const int tiles = cdiv((int)s.rows, TC_BM);
   if (s.pairs) {
     EpiGelu<__half> eg{{}, reinterpret_cast<__half*>(h), bias, 4 * D};
-    static const int epi_direct2 = getenv("DTK_EPI_DIRECT") ? atoi(getenv("DTK_EPI_DIRECT")) : 2;  // bit 1: fp16 GELU rows written thread-per-row (64 B per thread, whole sectors)
-    eg.all_direct = (epi_direct2 & 2) ? 1 : 0;
+    eg.all_direct = 1;   // fp16 GELU rows written thread-per-row (64 B per thread, whole sectors)
     return tc_launch<TcMode::F16, EpiGelu<__half>, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), eg, st, PROF_VIT_GEMM);
   }
   if (s.f16)

@@ -209,10 +209,10 @@ int dinotrk_infer_plan_anchors(int T, int N, const int* anchor_counts, const int
                                int chunk_maps, int probe, int* groups, int* meta, int max_chunks, int* n_chunks);
 /* Phase 2 pipelining across CUDA streams (process-wide; results are identical in every mode):
  * 0 = everything on the caller's stream; 1 (default) = the descriptor sampling of chunk k+1 runs on an
- * internal side stream under the correlation GEMM of chunk k; 2 = the head's fast path as well;
- * -1 = back to the default / the DTK_OVERLAP environment variable.  All side-stream work is joined back
- * into the caller's stream before dinotrk_infer returns.  The side streams and their events are one set per
- * process (one process per GPU): with mode >= 1 do not run dinotrk_infer from two host threads at once. */
+ * internal side stream under the correlation GEMM of chunk k; -1 = back to the default.  Other modes return
+ * DINOTRK_EINVAL.  All side-stream work is joined back into the caller's stream before dinotrk_infer returns.
+ * The side stream and its events are one set per device: with mode 1 do not run dinotrk_infer from two host
+ * threads at once. */
 int dinotrk_infer_set_overlap(int mode);
 /* Pipeline of the anchor re-tracking phase (process-wide):
  *  1 = coarse pass + exact window: one single-pass fp16 GEMM keeps per map and 128-token tile only (max, its token, second
@@ -222,8 +222,7 @@ int dinotrk_infer_set_overlap(int mode);
  *      or that fail the head's certificate are re-done by pipeline 0; no result depends on a coarse value.
  *  0 = full maps: split-precision GEMM over all tokens into chunk buffers + the head kernels (the round-1 pipeline).
  * -1 (default) = 1 when the feature struct carries fp16 hi / lo halves (tensor path), unless the trajectory phase just
- *      showed that the head's certificate fails for more than a quarter of the maps (ill-conditioned refiner weights);
- *      the DTK_XW environment variable (0 / 1) overrides.
+ *      showed that the head's certificate fails for more than a quarter of the maps (ill-conditioned refiner weights).
  * dinotrk_infer_last_stats (n >= 4 slots): {anchor-phase maps, maps finished by the exact-window path, maps re-done by the
  * full-map path, pipeline used[, of the re-done maps: those queued by the head's certificate rather than by the plan[,
  * contraction: 1 = split fp16 tensor cores, 0 = exact fp32[, coarse pass of pipeline 1: 1 = int8, 0 = fp16 (the pass the

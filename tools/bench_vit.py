@@ -1,5 +1,5 @@
 """ViT-L/14 (stride 7, 854x476, tap at block 15) feature-extraction stage on its own: device time per frame and the
-per-class kernel times.  GPU only.  DTK_FA_POLY=<0|25|37|50> selects the share of FMA-pipe exponentials."""
+per-class kernel times.  GPU only."""
 import argparse
 import json
 import os
@@ -19,7 +19,6 @@ def main():
     from dino_tracker_b200 import _lib
     _lib.load()
     r = bench.stage_timings(a, "cuda:0", _lib, bench.measured_peaks(), vit_only=True)
-    r["vit"]["fa_poly"] = os.environ.get("DTK_FA_POLY", "0")
     print(json.dumps(r["vit"]))
 
 
