@@ -85,6 +85,7 @@ SIGNATURES = {
     "dinotrk_infer_workspace_bytes": (c_size_t, [c_int, c_int, POINTER(Geom), c_int, c_int]),
     "dinotrk_infer_set_overlap": (c_int, [c_int]),
     "dinotrk_infer_set_path": (c_int, [c_int]),
+    "dinotrk_xw_head_set_window_only": (c_int, [c_int]),
     "dinotrk_infer_set_coarse": (c_int, [c_int]),
     "dinotrk_infer_last_stats": (c_int, [POINTER(ctypes.c_longlong), c_int]),
     "dinotrk_infer_max_chunks": (c_size_t, [c_int, c_int, c_int]),

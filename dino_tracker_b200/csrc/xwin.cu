@@ -554,291 +554,340 @@ int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_h
 }
 
 // ====================================================================================================== 4. head
-// One warp per map.  Exact values v = relu(acc / max(|d| |F|, 1e-8)) (the full-map GEMM's epilogue expression) are formed
-// from the raw accumulators of xbox on demand: at the candidates (-> exact first arg-max) and on the 15 x 15 window.  Then
-// the refiner on the window (hidden layer 13 x 13 x 16 in two channel halves, logits on 11 x 11), softmax sums, the
-// certificate of head.cu with   m_out = max(exact window values outside the 7 x 7 core,
-//                                             per tile: (its max token inside the core ? second value : max) + XW_EPS)
-// and either the track point or a place in the group's full-map queue.
+// One kernel, two maps per warp: half-warp hf (lanes 16 hf .. 16 hf + 15) owns map 2 pair + hf, and its lane l is refiner
+// channel l.  Per map:
+//   window   exact values v = relu(acc / max(|d| |F|, 1e-8)) (the full-map GEMM's epilogue expression, corr_cos) formed from
+//            xbox's raw accumulators at the candidates (-> exact first arg-max) and on the 15 x 15 window (lane l: window
+//            column l), which goes to shared memory, with m_out = max(exact window values outside the 7 x 7 core,
+//                                                                  per tile: (its max token inside the core ? second value : max) + eps).
+//            Before the current pair is refined, the warp runs the next pair's arg-max chain: three levels of dependent
+//            loads (state, cell, norm, candidates, eps and tile keys; box origin and frame; the values at the candidates),
+//            which it waits for.  Only the window's 2 x 15 loads per lane (cp.async into shared memory) land while the
+//            current pair is refined.
+//   refiner  lane = channel c.  Hidden row j (13 values of channel c, from three window rows read as broadcasts) stays in
+//            registers and goes at once into the three logit rows it is a tap row of: chain A0 of row j, A1 of row j - 1
+//            (whose A0 + A1 is then complete) and A2 of row j - 2 (whose per-channel logit is then complete).  Every lane
+//            works on every row, and no hidden window is stored.  The 16 channels' contributions to a finished logit row
+//            meet in shared memory, where lane x adds them up in the tree of the pair-lane layout: (c, c + 8) first, then
+//            the pair sums xor 4, xor 2, xor 1.
+//   tail     softmax sums on the 11 x 11 box, the certificate of head.cuh, and either the track point or a place in the
+//            group's full-map queue.
+// Every hidden value, logit and softmax sum is the same sequence of fp32 operations as in the refiner's first form
+// (xw_refine): relu((a0 + a1) + a2) with a0 an FMA chain from b1 and a1, a2 chains from a product, taps in (ky, kx) order.
 constexpr int XH_WARPS = 8;
-constexpr int XH_MP = 18;      // input window pitch (float2 units, even: 16-byte loads of two positions; 4 row groups -> 4 bank quads)
-constexpr int XH_MWIN = 544;   // floats: the 15 x 15 input window with every value stored twice (WM * XH_MP * 2 = 540)
-constexpr int XH_PER_WARP = XH_MWIN + WH * WH * 16;      // + hidden window [position][8 channel pairs (c, c + 8)]
-constexpr int XH_WTAB = 20 * 16;                           // floats: refiner weights as pairs [w1 k = 0..8 | b1 | w2 k = 0..8 | -][8 pairs]
-constexpr int XH_SMEM = (XH_WTAB + XH_WARPS * XH_PER_WARP) * 4;
+constexpr int XH_WP = 16;       // window row pitch (floats): 15 values and a zero
+constexpr int XH_WIN = WM * XH_WP;   // 240 floats per map; 240 = 16 mod 32: the two maps' window rows lie in disjoint banks
+constexpr int XH_RP = 20;       // row pitch of a channel-sum buffer: 8 lanes' 16-byte reads of consecutive rows hit distinct banks
+constexpr int XH_RED = 240;     // one logit row's 11 x 16 channel contributions of one map (11 x 20, padded to 16 mod 32)
+constexpr int XH_ZB = 128;      // the 121 logits of one map
+// per warp: [windows: 2 maps | channel sums: 2 buffers x 2 maps | logits: 2 maps | gathered accumulators: 2 maps |
+// gathered token norms: 2 maps]
+constexpr int XH_RAW = 2 * XH_WIN + 4 * XH_RED + 2 * XH_ZB;
+constexpr int XH_PER_WARP = XH_RAW + 4 * XH_WIN;
+constexpr int XH_SMEM = XH_WARPS * XH_PER_WARP * 4;
+static_assert(XH_WIN % 32 == 16 && XH_RED % 32 == 16 && WB * XH_RP <= XH_RED && WB * WB <= XH_ZB, "head buffer layout");
 
-// Window, refiner and softmax sums of one map (one warp).  INTERIOR: the 15 x 15 window lies inside the token grid (no
-// zero padding anywhere: the per-position bounds tests drop out -- the common case away from the frame border).
+constexpr int XH_KEYS = 4;      // tile keys per lane loaded with the map's first loads (all of them up to 64 tiles)
+
+struct XhGather {       // one map's gathers, lane l of its half-warp
+  int amax;             // exact first arg-max token; -1: no map, or a map the plan queued
+  float dn, mout;       // descriptor norm; the lane's share of m_out from the tile keys
+  unsigned ok;          // bit y: window row y, column l lies inside the token grid
+};
+
+// 4-byte asynchronous copy global -> shared: a gathered value lands without holding a register while the pair before it
+// is refined
+__device__ __forceinline__ void xh_cp4(float* dst, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void xh_cp_wait() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+
+__device__ __forceinline__ void xh_gather(XhGather& gt, int map, int n_maps, int l, int h, int w, int P, int n_tiles,
+                                          const float* __restrict__ norms, const float* __restrict__ desc_norm,
+                                          const int* __restrict__ cell_frame, const int* __restrict__ cell_of,
+                                          const int2* __restrict__ box_org, const int* __restrict__ stat,
+                                          const int* __restrict__ cand, const unsigned long long* __restrict__ key1,
+                                          const float* __restrict__ max2, const float* __restrict__ xbox,
+                                          const float* __restrict__ eps_map, float* __restrict__ racc, float* __restrict__ rfn) {
+  gt.amax = -1;
+  gt.ok = 0;
+  if (map >= n_maps) return;
+  // The chain has three levels of dependent loads; everything that depends only on the map index is issued at the first:
+  // the state, the cell, the norm, the candidates, eps and the tile keys of the first 16 XH_KEYS tiles.
+  const int st = __ldg(stat + map), cell = __ldg(cell_of + map);
+  const float dn = __ldg(desc_norm + map);
+  const int4 cd = __ldg(reinterpret_cast<const int4*>(cand) + map);
+  const float eps = eps_map ? __ldg(eps_map + map) : XW_EPS;
+  const unsigned long long* k1 = key1 + (size_t)map * n_tiles;
+  const float* k2 = max2 + (size_t)map * n_tiles;
+  unsigned long long kk[XH_KEYS];
+  float kv2[XH_KEYS];
+#pragma unroll
+  for (int q = 0; q < XH_KEYS; ++q) {
+    const int t = l + 16 * q;
+    kk[q] = t < n_tiles ? __ldg(k1 + t) : 0ull;
+    kv2[q] = t < n_tiles ? __ldg(k2 + t) : 0.f;
+  }
+  if (st != 0) return;
+  const int2 org = __ldg(box_org + cell);
+  const float* fn = norms + (size_t)__ldg(cell_frame + cell) * P;
+  const float* xr = xbox + (size_t)map * XW_COLS;
+  // exact first arg-max among the candidates (every lane, redundantly: <= 4 loads)
+  const int ct[4] = {cd.x, cd.y, cd.z, cd.w};
+  float best = -1.f;
+  int amax = -1;
+#pragma unroll
+  for (int q = 0; q < XW_MAX_CAND; ++q)
+    if (ct[q] >= 0) {
+      const int tr = ct[q] / w, tcn = ct[q] - tr * w;
+      const float v = fmaxf(corr_cos(__ldg(xr + xw_col(tr - org.x, tcn - org.y)), dn, __ldg(fn + ct[q])), 0.f);
+      if (v > best || (v == best && ct[q] < amax)) { best = v; amax = ct[q]; }
+    }
+  const int arow = amax / w, acol = amax - arow * w;
+  // coarse bound on everything outside the window, from the tile keys
+  float mout = 0.f;
+  auto fold = [&](unsigned long long k, float m2) {
+    const int tk = 0x7fffffff - (int)(k & 0xffffffffu);
+    const int tr = tk / w, tcn = tk - tr * w;
+    const bool in_core = abs(tr - arow) <= 3 && abs(tcn - acol) <= 3;
+    mout = fmaxf(mout, (in_core ? m2 : __uint_as_float((unsigned)(k >> 32))) + eps);
+  };
+#pragma unroll
+  for (int q = 0; q < XH_KEYS; ++q)
+    if (l + 16 * q < n_tiles) fold(kk[q], kv2[q]);
+  for (int t = l + 16 * XH_KEYS; t < n_tiles; t += 16) fold(__ldg(k1 + t), __ldg(k2 + t));
+  // window column l: raw accumulators and token norms to racc / rfn (row y at y XH_WP + l), read when the pair is refined
+  const int c = acol - 7 + l;
+  const bool col_in = l < WM && c >= 0 && c < w;
+  unsigned ok = 0;
+#pragma unroll
+  for (int y = 0; y < WM; ++y) {
+    const int r = arow - 7 + y;
+    if (col_in && r >= 0 && r < h) {
+      xh_cp4(racc + y * XH_WP + l, xr + xw_col(r - org.x, c - org.y));
+      xh_cp4(rfn + y * XH_WP + l, fn + r * w + c);
+      ok |= 1u << y;
+    }
+  }
+  gt.amax = amax;
+  gt.dn = dn;
+  gt.mout = mout;
+  gt.ok = ok;
+}
+
+// Exact window column l into shared memory (zero outside the map) from the lane's gathers; returns its share of m_out.
+__device__ __forceinline__ float xh_window(const XhGather& gt, const float* __restrict__ racc, const float* __restrict__ rfn,
+                                           float* __restrict__ win, int l) {
+  xh_cp_wait();
+  float mout = gt.mout;
+#pragma unroll
+  for (int y = 0; y < WM; ++y) {
+    float v = 0.f;
+    if ((gt.ok >> y) & 1u) {
+      v = fmaxf(corr_cos(racc[y * XH_WP + l], gt.dn, rfn[y * XH_WP + l]), 0.f);
+      if (!(abs(y - 7) <= 3 && abs(l - 7) <= 3)) mout = fmaxf(mout, v);
+    }
+    win[y * XH_WP + l] = v;
+  }
+  return mout;
+}
+
+// k-th tap row (ky) chain of a 3-tap kernel row over three consecutive values: a product, then two FMAs
+__device__ __forceinline__ float xh_tap3(const float* wk, float v0, float v1, float v2) {
+  return __fmaf_rn(wk[2], v2, __fmaf_rn(wk[1], v1, __fmul_rn(wk[0], v0)));
+}
+
+// Hidden row j of channel l, and what it completes: in A0in / Sin the A0 chains of logit row j - 1 and the A0 + A1 sums
+// of row j - 2; out A0out / Sout those of rows j and j - 1; the logits of row j - 2 go to zb.  red: this half's first
+// channel-sum buffer (the second lies 2 XH_RED further; rows alternate between them, so one warp barrier per row suffices).
 template <bool INTERIOR>
-__device__ __forceinline__ void xw_refine(const HeadParams& hp, const float2* __restrict__ wtab, float b2w, float2* __restrict__ mm2,
-                                          float2* __restrict__ hh2, const float (&wv)[8], int arow, int acol, int lane,
-                                          float& zmax, float (&tot)[5]) {
-  const int h = hp.h, w = hp.w;
-  const int cp = lane & 7, pg = lane >> 3;
-  // ---- input window (15 x 15 exact values, zero outside the map; extracted by xw_window_kernel, 16-float rows), every
-  // value as the pair (v, v): the pair FMAs below take it straight from one 64-bit shared-memory load ----
+__device__ __forceinline__ void xh_step(int j, const float (&A0in)[WB], const float (&Sin)[WB], float (&A0out)[WB],
+                                        float (&Sout)[WB], const float* __restrict__ win, float* __restrict__ red,
+                                        float* __restrict__ zb, const float (&w1)[9], float b1, const float (&w2)[9], float b2,
+                                        bool row_in, unsigned cmask, int l) {
+  float in[3][16];
 #pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    const int i = lane + 32 * q;
-    const int y = i >> 4, x = i & 15;
-    if (y < WM && x < WM) mm2[y * XH_MP + x] = make_float2(wv[q], wv[q]);
+  for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float4 v = *reinterpret_cast<const float4*>(win + (j + ky) * XH_WP + 4 * q);
+      in[ky][4 * q] = v.x; in[ky][4 * q + 1] = v.y; in[ky][4 * q + 2] = v.z; in[ky][4 * q + 3] = v.w;
+    }
+  float hr[WH];
+#pragma unroll
+  for (int x = 0; x < WH; ++x) {
+    // three short chains per output (one per input row) instead of one chain of nine dependent FMAs
+    float a0 = __fmaf_rn(w1[0], in[0][x], b1), a1 = __fmul_rn(w1[3], in[1][x]), a2 = __fmul_rn(w1[6], in[2][x]);
+    a0 = __fmaf_rn(w1[1], in[0][x + 1], a0); a1 = __fmaf_rn(w1[4], in[1][x + 1], a1); a2 = __fmaf_rn(w1[7], in[2][x + 1], a2);
+    a0 = __fmaf_rn(w1[2], in[0][x + 2], a0); a1 = __fmaf_rn(w1[5], in[1][x + 2], a1); a2 = __fmaf_rn(w1[8], in[2][x + 2], a2);
+    const float a = __fadd_rn(__fadd_rn(a0, a1), a2);
+    hr[x] = INTERIOR || (row_in && ((cmask >> x) & 1u)) ? fmaxf(a, 0.f) : 0.f;
   }
-  __syncwarp();
-  // ---- refiner on fp32 FMA pairs (f2fma: the lane's two channels share every operand load).  Lane =
-  // (channel pair cp = channels (cp, cp + 8), row group pg).  Hidden layer: the lane's two channels on the rows pg, pg + 4,
-  // ... of the 13 x 13 window, a 3 x 3 input window sliding along the row (weights in registers), stored [position][pair].
-  // Output layer: the SAME lane layout -- the lane forms its two channels' contribution to the logits of box rows pg,
-  // pg + 4, pg + 8 (again sliding along the row: 3 new 64-bit shared-memory words per 9 pair FMAs); the pair is folded
-  // and the 8 pair lanes of a row group are summed by shuffles.
-  {
-    float2 w1r[9];
+  if (j < WB) {
 #pragma unroll
-    for (int k = 0; k < 9; ++k) w1r[k] = wtab[k * 8 + cp];
-    const float2 b1r = wtab[9 * 8 + cp];
-    for (int y = pg; y < WH; y += 4) {
-      const int r = arow - 6 + y;
-      const bool row_in = r >= 0 && r < h;
-      const float2* m0 = mm2 + y * XH_MP;
-      // the three input rows of this hidden row, two positions per 16-byte load (positions 15, 16, 17 of a row are padding)
-      float2 in0[16], in1[16], in2[16];
+    for (int x = 0; x < WB; ++x) A0out[x] = xh_tap3(w2, hr[x], hr[x + 1], hr[x + 2]);
+  }
+  if (j >= 1 && j <= WB) {
 #pragma unroll
-      for (int x = 0; x < 16; x += 2) {
-        const float4 q0 = *reinterpret_cast<const float4*>(m0 + x);
-        const float4 q1 = *reinterpret_cast<const float4*>(m0 + XH_MP + x);
-        const float4 q2 = *reinterpret_cast<const float4*>(m0 + 2 * XH_MP + x);
-        in0[x] = make_float2(q0.x, q0.y); in0[x + 1] = make_float2(q0.z, q0.w);
-        in1[x] = make_float2(q1.x, q1.y); in1[x + 1] = make_float2(q1.z, q1.w);
-        in2[x] = make_float2(q2.x, q2.y); in2[x + 1] = make_float2(q2.z, q2.w);
+    for (int x = 0; x < WB; ++x) Sout[x] = __fadd_rn(A0in[x], xh_tap3(w2 + 3, hr[x], hr[x + 1], hr[x + 2]));
+  }
+  if (j >= 2) {
+    float* rb = red + (j & 1) * (2 * XH_RED);
+#pragma unroll
+    for (int x = 0; x < WB; ++x) rb[x * XH_RP + l] = __fadd_rn(Sin[x], xh_tap3(w2 + 6, hr[x], hr[x + 1], hr[x + 2]));
+    __syncwarp();
+    if (l < WB) {
+      float p[16];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float4 v = *reinterpret_cast<const float4*>(rb + l * XH_RP + 4 * q);
+        p[4 * q] = v.x; p[4 * q + 1] = v.y; p[4 * q + 2] = v.z; p[4 * q + 3] = v.w;
       }
+      float v[8];
 #pragma unroll
-      for (int x = 0; x < WH; ++x) {
-        // three short chains per output (one per input row) instead of one chain of nine dependent FMAs
-        float2 a0 = f2fma(w1r[0], in0[x], b1r), a1 = f2mul(w1r[3], in1[x]), a2 = f2mul(w1r[6], in2[x]);
-        a0 = f2fma(w1r[1], in0[x + 1], a0); a1 = f2fma(w1r[4], in1[x + 1], a1); a2 = f2fma(w1r[7], in2[x + 1], a2);
-        a0 = f2fma(w1r[2], in0[x + 2], a0); a1 = f2fma(w1r[5], in1[x + 2], a1); a2 = f2fma(w1r[8], in2[x + 2], a2);
-        const float2 a = f2add(f2add(a0, a1), a2);
-        const int c = acol - 6 + x;
-        const bool in = INTERIOR || (row_in && c >= 0 && c < w);
-        hh2[(y * WH + x) * 8 + cp] = in ? make_float2(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f)) : make_float2(0.f, 0.f);
-      }
+      for (int i = 0; i < 8; ++i) v[i] = __fadd_rn(p[i], p[i + 8]);
+      const float t = __fadd_rn(__fadd_rn(__fadd_rn(v[0], v[4]), __fadd_rn(v[2], v[6])),
+                                __fadd_rn(__fadd_rn(v[1], v[5]), __fadd_rn(v[3], v[7])));
+      zb[(j - 2) * WB + l] = __fadd_rn(t, b2);
     }
   }
-  __syncwarp();
-  float* zb = reinterpret_cast<float*>(mm2);       // the input window is dead: reuse it for the 121 logits
-  {
-    float2 w2r[9];
+}
+
+// Refiner of one map per half-warp: the 121 logits into zb.  INTERIOR: both maps' 15 x 15 windows lie inside the token
+// grid (no hidden value is forced to zero -- the common case away from the frame border).
+template <bool INTERIOR>
+__device__ __forceinline__ void xh_refine(const float* __restrict__ win, float* __restrict__ red, float* __restrict__ zb,
+                                          const float (&w1)[9], float b1, const float (&w2)[9], float b2, int arow, int acol,
+                                          int h, int w, int l) {
+  unsigned cmask = 0;
 #pragma unroll
-    for (int k = 0; k < 9; ++k) w2r[k] = wtab[(10 + k) * 8 + cp];
+  for (int x = 0; x < WH; ++x) cmask |= (acol - 6 + x >= 0 && acol - 6 + x < w) ? 1u << x : 0u;
+  float A0a[WB], Sa[WB], A0b[WB], Sb[WB];
 #pragma unroll
-    for (int yi = 0; yi < 3; ++yi) {
-      const int y = pg + 4 * yi;
-      const bool row_ok = y < WB;                  // (row group 3 has no third row; its lanes still take part in the shuffles)
-      const float2* h0 = hh2 + ((row_ok ? y : 0) * WH) * 8 + cp;
-      float2 i00 = h0[0], i01 = h0[8], i10 = h0[WH * 8], i11 = h0[(WH + 1) * 8];
-      float2 i20 = h0[2 * WH * 8], i21 = h0[(2 * WH + 1) * 8];
-      float v[12];
-      v[11] = 0.f;
-#pragma unroll
-      for (int x = 0; x < WB; ++x) {
-        const float2 i02 = h0[(x + 2) * 8], i12 = h0[(WH + x + 2) * 8], i22 = h0[(2 * WH + x + 2) * 8];
-        float2 a0 = f2mul(w2r[0], i00), a1 = f2mul(w2r[3], i10), a2 = f2mul(w2r[6], i20);
-        a0 = f2fma(w2r[1], i01, a0); a1 = f2fma(w2r[4], i11, a1); a2 = f2fma(w2r[7], i21, a2);
-        a0 = f2fma(w2r[2], i02, a0); a1 = f2fma(w2r[5], i12, a1); a2 = f2fma(w2r[8], i22, a2);
-        const float2 a = f2add(f2add(a0, a1), a2);
-        v[x] = a.x + a.y;
-        i00 = i01; i01 = i02; i10 = i11; i11 = i12; i20 = i21; i21 = i22;
-      }
-      // sum over the 8 pair lanes as a reduce-scatter (11 shuffles per row instead of 33): every halving step sends the
-      // half of the values the partner will own; afterwards lane cp holds logits 6 b2 + 3 b1 + {2 b0, 1 (b0 = 0 only)}
-      const bool b2 = cp & 4, b1 = cp & 2, b0 = cp & 1;
-      float u[6], w3[3];
-#pragma unroll
-      for (int j = 0; j < 6; ++j) {
-        const float send = b2 ? v[j] : v[j + 6], keep = b2 ? v[j + 6] : v[j];
-        u[j] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-      }
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const float send = b1 ? u[j] : u[j + 3], keep = b1 ? u[j + 3] : u[j];
-        w3[j] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-      }
-      const float t0 = (b0 ? w3[2] : w3[0]) + __shfl_xor_sync(0xffffffffu, b0 ? w3[0] : w3[2], 1);
-      const float t1 = (b0 ? 0.f : w3[1]) + __shfl_xor_sync(0xffffffffu, b0 ? w3[1] : 0.f, 1);
-      const int idx0 = (b2 ? 6 : 0) + (b1 ? 3 : 0) + (b0 ? 2 : 0);
-      if (row_ok && idx0 < WB) zb[y * WB + idx0] = t0 + b2w;
-      if (row_ok && !b0) zb[y * WB + idx0 + 1] = t1 + b2w;
-    }
+  for (int x = 0; x < WB; ++x) { A0a[x] = 0.f; Sa[x] = 0.f; }
+#pragma unroll 1
+  for (int j = 0; j < WH; j += 2) {
+    xh_step<INTERIOR>(j, A0a, Sa, A0b, Sb, win, red, zb, w1, b1, w2, b2, arow - 6 + j >= 0 && arow - 6 + j < h, cmask, l);
+    if (j + 1 < WH)
+      xh_step<INTERIOR>(j + 1, A0b, Sb, A0a, Sa, win, red, zb, w1, b1, w2, b2, arow - 5 + j >= 0 && arow - 5 + j < h, cmask, l);
   }
-  __syncwarp();
-  // ---- softmax sums on the box / the disc (thread = box pixel) ----
-  float z[4];
-  bool valid[4], indisc[4];
-  float px[4], py[4];
+}
+
+// Softmax sums on the box / the disc.  Lane l takes pixels l + 16 k: even k are the pixels l + 32 q lane l of a whole warp
+// would take, odd k lane l + 16's, each in its own accumulator; adding the two is the xor-16 step of warp_sum, and the
+// xor 8 .. 1 steps follow -- the sums of the one-map-per-warp form, bit for bit.
+__device__ __forceinline__ void xh_sums(const HeadParams& hp, const float* __restrict__ zb, int arow, int acol, int l,
+                                        float& zmax, float (&tot)[5]) {
+  float z[8];
+  bool valid[8];
   zmax = -INFINITY;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int p = lane + 32 * q;
-    valid[q] = false; indisc[q] = false; z[q] = -INFINITY; px[q] = py[q] = 0.f;
-    if (p < WB * WB) {
-      const int y = p / WB, x = p - y * WB;
-      const int r = arow - 5 + y, c = acol - 5 + x;
-      valid[q] = INTERIOR || (r >= 0 && r < h && c >= 0 && c < w);
-      if (valid[q]) {
-        z[q] = zb[p];
-        indisc[q] = in_disc(hp, r, c, arow, acol);
-        px[q] = token_px(hp, c);
-        py[q] = token_px(hp, r);
-      }
-    }
-    zmax = fmaxf(zmax, z[q]);
+  for (int k = 0; k < 8; ++k) {
+    const int p = l + 16 * k;
+    const int y = p / WB, x = p - y * WB, r = arow - 5 + y, c = acol - 5 + x;
+    valid[k] = p < WB * WB && r >= 0 && r < hp.h && c >= 0 && c < hp.w;
+    z[k] = valid[k] ? zb[p] : -INFINITY;
+    zmax = fmaxf(zmax, z[k]);
   }
-  zmax = warp_max(zmax);
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const float e = valid[q] ? expf(z[q] - zmax) : 0.f;
-    tot[0] += e;
-    if (indisc[q]) { tot[1] += e; tot[2] = fmaf(px[q], e, tot[2]); tot[3] = fmaf(py[q], e, tot[3]); }
-    tot[4] += valid[q] ? 1.f : 0.f;
+  for (int o = 8; o > 0; o >>= 1) zmax = fmaxf(zmax, __shfl_xor_sync(0xffffffffu, zmax, o));
+  float s[2][5] = {};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const int p = l + 16 * k;
+    const int y = p / WB, x = p - y * WB, r = arow - 5 + y, c = acol - 5 + x;
+    const float e = valid[k] ? expf(z[k] - zmax) : 0.f;
+    float (&t)[5] = s[k & 1];
+    t[0] += e;
+    if (valid[k] && in_disc(hp, r, c, arow, acol)) {
+      t[1] += e; t[2] = fmaf(token_px(hp, c), e, t[2]); t[3] = fmaf(token_px(hp, r), e, t[3]);
+    }
+    t[4] += valid[k] ? 1.f : 0.f;
+  }
+#pragma unroll
+  for (int i = 0; i < 5; ++i) {
+    float v = s[0][i] + s[1][i];
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    tot[i] = v;
   }
 }
 
-// (a) window extraction: one warp per map, no shared memory, many warps per SM -- every load here is a dependent gather
-// (candidates -> box accumulators / token norms), so this part wants parallelism, not registers.  Writes the 15 x 15 exact
-// window as [15][16] floats and hin = (exact first arg-max token or -1 for a map the plan queued, m_out bits).
-constexpr int XWIN_PITCH = 256;
-__global__ void __launch_bounds__(256)
-xw_window_kernel(int n_maps, int h, int w, int P, int n_tiles, const float* __restrict__ norms, const float* __restrict__ desc_norm,
-                 const int* __restrict__ cell_frame, const int* __restrict__ cell_of, const int2* __restrict__ box_org,
-                 const int* __restrict__ stat, const int* __restrict__ cand, const unsigned long long* __restrict__ key1,
-                 const float* __restrict__ max2, const float* __restrict__ xbox, float* __restrict__ win, int2* __restrict__ hin,
-                 const float* __restrict__ eps_map) {
-  const int lane = threadIdx.x & 31;
-  const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-  for (int map = gw; map < n_maps; map += nw) {
-    if (stat[map] != 0) {
-      if (lane == 0) hin[map] = make_int2(-1, 0);
+// REFINE = false: the window part alone (arg-max, window, m_out; m_out goes to the map's output x), which only
+// tools/bench_xw_head.py --split runs, to time the two parts of the kernel apart
+template <bool REFINE>
+__global__ void __launch_bounds__(XH_WARPS * 32, 2)
+xw_head_kernel(int n_maps, HeadParams hp, dinotrk_head_weights wts, int n_tiles, const float* __restrict__ norms,
+               const float* __restrict__ desc_norm, const int* __restrict__ cell_frame, const int* __restrict__ cell_group,
+               const int* __restrict__ cell_of, const int2* __restrict__ box_org, const int* __restrict__ stat,
+               const int* __restrict__ cand, const unsigned long long* __restrict__ key1, const float* __restrict__ max2,
+               const float* __restrict__ xbox, const float* __restrict__ eps_map, const int* __restrict__ grp_map0,
+               const int* __restrict__ out_index, float* __restrict__ out, int* __restrict__ slow_cnt,
+               int* __restrict__ slow_list, int n_groups) {
+  extern __shared__ __align__(16) float xh_smem[];
+  // (the warp index through a shuffle: the compiler then knows that everything derived from it -- the pair index, the
+  // loop trip count, the branches on the pair's state -- is warp-uniform and keeps the shuffles plain SHFLs)
+  const int lane = threadIdx.x & 31, wid = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int hf = lane >> 4, l = lane & 15;
+  float* ws = xh_smem + wid * XH_PER_WARP;
+  float* win = ws + hf * XH_WIN;
+  float* red = ws + 2 * XH_WIN + hf * XH_RED;
+  float* zb = ws + 2 * XH_WIN + 4 * XH_RED + hf * XH_ZB;
+  float* racc = ws + XH_RAW + hf * XH_WIN;
+  float* rfn = racc + 2 * XH_WIN;
+  float w1[9], w2[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) { w1[k] = wts.w1[l][k]; w2[k] = wts.w2[l][k]; }
+  const float b1 = wts.b1[l];
+  const int h = hp.h, w = hp.w;
+  const int n_pairs = (n_maps + 1) >> 1, stride = gridDim.x * XH_WARPS;
+
+  int pair = blockIdx.x * XH_WARPS + wid;
+  XhGather gt;
+  if (pair < n_pairs)
+    xh_gather(gt, 2 * pair + hf, n_maps, l, h, w, hp.P, n_tiles, norms, desc_norm, cell_frame, cell_of, box_org, stat, cand,
+              key1, max2, xbox, eps_map, racc, rfn);
+  for (; pair < n_pairs; pair += stride) {
+    const int map = 2 * pair + hf, amax = gt.amax;
+    const bool exact = amax >= 0;
+    const int arow = exact ? amax / w : 7, acol = exact ? amax - arow * w : 7;
+    float mout = xh_window(gt, racc, rfn, win, l);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) mout = fmaxf(mout, __shfl_xor_sync(0xffffffffu, mout, o));
+    const bool any = __any_sync(0xffffffffu, exact);
+    const bool interior = __all_sync(0xffffffffu, !exact || (arow >= 7 && arow + 7 < h && acol >= 7 && acol + 7 < w));
+    if (pair + stride < n_pairs)   // the next pair's arg-max chain; its window's loads land while this pair is refined
+      xh_gather(gt, 2 * (pair + stride) + hf, n_maps, l, h, w, hp.P, n_tiles, norms, desc_norm, cell_frame, cell_of, box_org,
+                stat, cand, key1, max2, xbox, eps_map, racc, rfn);
+    __syncwarp();
+    if constexpr (!REFINE) {
+      if (l == 0 && exact) out[(size_t)(out_index ? out_index[map] : map) * hp.out_stride] = mout;
       continue;
     }
-    const int cell = cell_of[map];
-    const int2 org = box_org[cell];
-    const float* fn = norms + (size_t)cell_frame[cell] * P;
-    const float* xr = xbox + (size_t)map * XW_COLS;
-    const float dn = desc_norm[map];
-    // exact first arg-max among the candidates (every lane, redundantly: <= 4 loads)
-    const int4 cd = __ldg(reinterpret_cast<const int4*>(cand) + map);
-    const int ct[4] = {cd.x, cd.y, cd.z, cd.w};
-    float best = -1.f;
-    int amax = -1;
-#pragma unroll
-    for (int q = 0; q < XW_MAX_CAND; ++q)
-      if (ct[q] >= 0) {
-        const int tr = ct[q] / w, tcn = ct[q] - tr * w;
-        const float v = fmaxf(corr_cos(__ldg(xr + xw_col(tr - org.x, tcn - org.y)), dn, __ldg(fn + ct[q])), 0.f);
-        if (v > best || (v == best && ct[q] < amax)) { best = v; amax = ct[q]; }
-      }
-    const int arow = amax / w, acol = amax - arow * w;
-    // coarse bound on everything outside the window, from the tile keys
-    const float eps = eps_map ? eps_map[map] : XW_EPS;
-    float mout = 0.f;
-    for (int t = lane; t < n_tiles; t += 32) {
-      const unsigned long long k = __ldg(key1 + (size_t)map * n_tiles + t);
-      const int tk = 0x7fffffff - (int)(k & 0xffffffffu);
-      const int tr = tk / w, tcn = tk - tr * w;
-      const bool in_core = abs(tr - arow) <= 3 && abs(tcn - acol) <= 3;
-      const float b = in_core ? __ldg(max2 + (size_t)map * n_tiles + t) : __uint_as_float((unsigned)(k >> 32));
-      mout = fmaxf(mout, b + eps);
-    }
-    // exact window + exact part of m_out
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const int i = lane + 32 * q;
-      const int y = i >> 4, x = i & 15;
-      const int r = arow - 7 + y, c = acol - 7 + x;
-      float v = 0.f;
-      if (y < WM && x < WM && r >= 0 && r < h && c >= 0 && c < w) {
-        v = fmaxf(corr_cos(__ldg(xr + xw_col(r - org.x, c - org.y)), dn, __ldg(fn + r * w + c)), 0.f);
-        if (!(abs(r - arow) <= 3 && abs(c - acol) <= 3)) mout = fmaxf(mout, v);
-      }
-      win[(size_t)map * XWIN_PITCH + i] = v;
-    }
-    mout = warp_max(mout);
-    if (lane == 0) hin[map] = make_int2(amax, __float_as_int(mout));
-  }
-}
-
-// (b) refiner + softmax sums + certificate: one warp per map; the next map's window (8 coalesced loads per lane) and
-// arg-max are in flight while the current map is refined.
-__global__ void __launch_bounds__(XH_WARPS * 32, 2)
-xw_head_kernel(int n_maps, HeadParams hp, dinotrk_head_weights wts, const int* __restrict__ cell_group, const int* __restrict__ grp_map0,
-               const int* __restrict__ cell_of, const float* __restrict__ win, const int2* __restrict__ hin,
-               const int* __restrict__ out_index, float* __restrict__ out, int* __restrict__ slow_cnt, int* __restrict__ slow_list,
-               int n_groups) {
-  extern __shared__ __align__(16) float xh_smem[];     // [weights table: 320] then per warp [input window pairs: 544 | hidden window: 2704]
-  // (the warp index through a shuffle: the compiler then knows that everything derived from it -- the map index, the
-  // loop trip count, the branches on the map's state -- is warp-uniform and keeps the shuffles below plain SHFLs instead
-  // of wrapping each in a WARPSYNC.COLLECTIVE sequence)
-  const int lane = threadIdx.x & 31, wid = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  float2* wtab = reinterpret_cast<float2*>(xh_smem);
-  float2* mm = reinterpret_cast<float2*>(xh_smem + XH_WTAB + wid * XH_PER_WARP);
-  float2* hh_ = reinterpret_cast<float2*>(xh_smem + XH_WTAB + wid * XH_PER_WARP + XH_MWIN);
-  // refiner weights as channel pairs (c, c + 8) in shared memory: a lane-indexed read of the constant bank serialises over
-  // its 8 distinct addresses in the address-divergence unit (55 % busy in the capture before this table existed)
-  if (threadIdx.x < 19 * 8) {
-    const int k = threadIdx.x >> 3, c = threadIdx.x & 7;
-    wtab[threadIdx.x] = k < 9    ? make_float2(wts.w1[c][k], wts.w1[c + 8][k])
-                        : k == 9 ? make_float2(wts.b1[c], wts.b1[c + 8])
-                                 : make_float2(wts.w2[c][k - 10], wts.w2[c + 8][k - 10]);
-  }
-  __syncthreads();
-  const int h = hp.h, w = hp.w;
-  const int stride = gridDim.x * XH_WARPS;
-
-  int map = blockIdx.x * XH_WARPS + wid;
-  float wnext[8];
-  int2 hnext = make_int2(-1, 0);
-  if (map < n_maps) {
-    hnext = __ldg(hin + map);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) wnext[q] = __ldg(win + (size_t)map * XWIN_PITCH + lane + 32 * q);
-  }
-  for (; map < n_maps; map += stride) {
-    float wv[8];
-#pragma unroll
-    for (int q = 0; q < 8; ++q) wv[q] = wnext[q];
-    const int2 hcur = hnext;
-    if (map + stride < n_maps) {
-      hnext = __ldg(hin + map + stride);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) wnext[q] = __ldg(win + (size_t)(map + stride) * XWIN_PITCH + lane + 32 * q);
-    }
-    const bool slow = hcur.x < 0;
-    const int amax = hcur.x;
-    const float mout = __int_as_float(hcur.y);
     float zmax = 0.f;
     float tot[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    if (!slow) {
-      const int arow = amax / w, acol = amax - arow * w;
-      if (arow >= 7 && arow + 7 < h && acol >= 7 && acol + 7 < w)
-        xw_refine<true>(hp, wtab, wts.b2, mm, hh_, wv, arow, acol, lane, zmax, tot);
-      else
-        xw_refine<false>(hp, wtab, wts.b2, mm, hh_, wv, arow, acol, lane, zmax, tot);
-#pragma unroll
-      for (int q = 0; q < 5; ++q) tot[q] = warp_sum(tot[q]);
+    if (any) {
+      if (interior) xh_refine<true>(win, red, zb, w1, b1, w2, wts.b2, arow, acol, h, w, l);
+      else xh_refine<false>(win, red, zb, w1, b1, w2, wts.b2, arow, acol, h, w, l);
+      __syncwarp();
+      xh_sums(hp, zb, arow, acol, l, zmax, tot);
     }
-    if (lane == 0) {
-      if (!slow && head_certified(hp, wts, mout, zmax, tot)) {
+    if (l == 0 && map < n_maps) {
+      if (exact && head_certified(hp, wts, mout, zmax, tot)) {
         head_store_point(hp, __fdiv_rn(tot[2], tot[1]), __fdiv_rn(tot[3], tot[1]), out_index, out, map);
       } else {
         const int g = cell_group[cell_of[map]];
         const int pos = atomicAdd(slow_cnt + g, 1);
         slow_list[grp_map0[g] + pos] = map;
         atomicAdd(slow_cnt + n_groups, 1);
-        if (!slow) atomicAdd(slow_cnt + n_groups + 1, 1);   // (statistics: queued by the certificate, not by the plan)
+        if (exact) atomicAdd(slow_cnt + n_groups + 1, 1);   // (statistics: queued by the certificate, not by the plan)
       }
     }
     __syncwarp();
   }
 }
+
+static int g_xw_head_window_only = 0;   // dinotrk_xw_head_set_window_only
 
 int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head_weights& hw, const XwCells& cells,
                    const float* desc_norm, const int* grp_map0, int n_maps, const int* out_index, float* out, int out_stride,
@@ -847,24 +896,20 @@ int launch_xw_head(const FeatView& fv, const dinotrk_geom& g, const dinotrk_head
   DTK_CHECK_ARG(disc_fits_box(g), "exact-window path: disc radius %d exceeds 5 tokens", g.radius);
   const HeadParams hp = make_head_params(g, hw, dinotrk_map_stride(&g), out_stride, out_mode);
   const int sms = num_sms();
-  int grid = cdiv(n_maps, XH_WARPS);
+  int grid = cdiv(cdiv(n_maps, 2), XH_WARPS);
   if (grid > sms * 2) grid = sms * 2;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
-    DTK_CUDA(cudaFuncSetAttribute(xw_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XH_SMEM));
+    DTK_CUDA(cudaFuncSetAttribute(xw_head_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, XH_SMEM));
+    DTK_CUDA(cudaFuncSetAttribute(xw_head_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, XH_SMEM));
     attr = true;
   }
   ProfRange pr(PROF_XW_HEAD, st);
-  {
-    int wgrid = cdiv(n_maps, 8);
-    if (wgrid > sms * 8) wgrid = sms * 8;
-    xw_window_kernel<<<wgrid, 256, 0, st>>>(n_maps, g.h, g.w, hp.P, cdiv(hp.P, XW_TILE), fv.norms, desc_norm, cells.frame,
-                                            xc.cell_of, xc.box_org, xc.stat, xc.cand, xc.key1, xc.max2, xc.xbox, xc.win, xc.hin, eps);
-    DTK_LAUNCHED();
-  }
-  xw_head_kernel<<<grid, XH_WARPS * 32, XH_SMEM, st>>>(n_maps, hp, hw, cells.group, grp_map0, xc.cell_of, xc.win, xc.hin, out_index,
-                                                 out, xc.slow_cnt, xc.slow_list, n_groups);
+  (g_xw_head_window_only ? xw_head_kernel<false> : xw_head_kernel<true>)<<<grid, XH_WARPS * 32, XH_SMEM, st>>>(n_maps, hp, hw, cdiv(hp.P, XW_TILE), fv.norms, desc_norm, cells.frame,
+                                                       cells.group, xc.cell_of, xc.box_org, xc.stat, xc.cand, xc.key1, xc.max2,
+                                                       xc.xbox, eps, grp_map0, out_index, out, xc.slow_cnt, xc.slow_list,
+                                                       n_groups);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -1037,6 +1082,12 @@ int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* 
   xc.max2 = max2;
   return launch_xw_coarse(fv, nullptr, desc_rows, nullptr, grp_frame, grp_row0, grp_m, grp_row0, ws.tile_start, n_groups,
                           desc_rows / TC2_BM + n_groups, xc, st, nullptr, desc_q8, desc_fac);
+}
+
+int dinotrk_xw_head_set_window_only(int on) {
+  DTK_CHECK_ARG(on == 0 || on == 1, "xw_head_set_window_only: 0 or 1");
+  g_xw_head_window_only = on;
+  return DINOTRK_OK;
 }
 
 int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,

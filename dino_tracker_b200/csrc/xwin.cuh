@@ -17,9 +17,10 @@
 //   3. exact GEMM    per cell, the fp32-faithful split-precision contraction (lo*hi + hi*lo + hi*hi, same operation
 //                    sequence as the full-map GEMM) of the cell's descriptors against the box's 441 tokens only:
 //                    5.4 % of the map.  Raw accumulators go to a [map][448] buffer (1.8 KB per map instead of 32 KB).
-//   4. head          two kernels, one warp per map each: (a) exact arg-max among the candidates + the exact 15 x 15 window
-//                    + m_out (dependent gathers: many warps per SM), (b) refiner, softmax sums on the 11 x 11 box, certificate
-//                    with the bound from (1); writes the track point.
+//   4. head          one kernel, two maps per warp (a half-warp each, lane = refiner channel): exact arg-max among the
+//                    candidates, the exact 15 x 15 window built in shared memory and m_out; the refiner one hidden row at a
+//                    time, kept in registers; softmax sums on the 11 x 11 box, certificate with the bound from (1); writes
+//                    the track point.  The next pair's window loads land while a pair is refined.
 //   Maps that are ambiguous, do not fit their cell's box or fail the certificate are queued and re-done by the full-map
 //   path (split-precision GEMM over all tokens + head kernels of head.cu) -- results never depend on the coarse values.
 #pragma once
@@ -128,8 +129,6 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
   int* cell_of;               // [maps] cell index
   int2* box_org;              // [cells] (first box row, first box column); y = INT_MIN: skip the cell
   float* xbox;                // [maps][XW_COLS] raw split-precision accumulators of the box tokens
-  float* win;                 // [maps][256] exact 15 x 15 windows ([15][16] floats, zero outside the map)
-  int2* hin;                  // [maps] (exact first arg-max token or -1, bits of m_out)
   int* slow_cnt;              // [n_groups + 1] per group count of queued maps; [n_groups] = total
   int* slow_list;             // [maps] group g's queue lives at [grp_map0[g], grp_map0[g] + slow_cnt[g])
   XwChunk() = default;
@@ -144,8 +143,6 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
     slow_list = ar.take<int>(maps);
     box_org = ar.take<int2>(cells);
     xbox = ar.take<float>(maps * XW_COLS);
-    win = ar.take<float>(maps * 256);
-    hin = ar.take<int2>(maps);
     slow_cnt = ar.take<int>((size_t)n_groups + 2);
   }
 };

@@ -230,6 +230,10 @@ int dinotrk_infer_set_overlap(int mode);
  * whose descriptor the GEMMs read in place from the unique (query, source frame) table, maps whose descriptor was gathered
  * into the chunk's rows]]]]]} of the last dinotrk_infer call that ran the anchor phase. */
 int dinotrk_infer_set_path(int path);
+/* Timing aid for the exact-window head (tools/bench_xw_head.py --split): 1 = run only its window part (exact arg-max,
+ * 15 x 15 window, m_out) and write no track points -- the results of dinotrk_infer are then NOT valid; 0 (default) = the
+ * whole head. */
+int dinotrk_xw_head_set_window_only(int on);
 /* Coarse pass of pipeline 1:  1 = int8 (feat->q8 required),  0 = fp16 over feat->hi,
  * -1 (default) = int8 when feat->q8 is given and every frame's q_rho is <= 0.03, unless the probe chunk queues more than
  *      1/16 of its maps to pipeline 0; fp16 otherwise.  No result depends on the choice. */
