@@ -17,7 +17,8 @@ from .pipeline import build_tracker_from_video, track_video, save_dino_embed_vid
 from .benchmark import infer_query_frames, save_predictions, run_videos  # noqa: F401
 from .trajectories import extract_trajectories, save_trajectories  # noqa: F401
 from .best_buddies import of_filter, run_of_filter  # noqa: F401
+from .trainer import DinoTrackerTrainer  # noqa: F401
 
-__all__ = ["extract_trajectories", "save_trajectories", "of_filter", "run_of_filter", "preprocess_best_buddies",
+__all__ = ["DinoTrackerTrainer", "extract_trajectories", "save_trajectories", "of_filter", "run_of_filter", "preprocess_best_buddies",
            "infer_query_frames", "save_predictions", "run_videos", "DinoV2Features", "get_dino_features_video", "build_tracker_from_video", "track_video", "save_dino_embed_video","Tracker", "ModelInference", "RangeNormalizer", "generate_trajectory_input", "generate_trajectory",
            "generate_trajectories"]

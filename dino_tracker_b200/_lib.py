@@ -174,6 +174,9 @@ SIGNATURES = {
     "dinotrk_cycle_select": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, _P, _P, _P]),
     "dinotrk_cycle_unnorm": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P]),
     "dinotrk_cycle_keep": (c_int, [_P, _P, c_int, c_int, c_int, c_float, _P, _P, _P, _P]),
+    "dinotrk_emb_reg_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dinotrk_emb_reg_forward": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P, c_size_t, _P]),
+    "dinotrk_emb_reg_backward": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "dinotrk_raft_encode_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dinotrk_raft_encode": (c_int, [_P, c_int, c_int, c_int, c_int, POINTER(RaftWeights), _P, _P, _P, c_size_t, _P]),
     "dinotrk_raft_flow_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),

@@ -56,7 +56,7 @@ enum ProfClass {
   PROF_PACK, PROF_CONV, PROF_BLUR, PROF_ALIGN, PROF_MISC, PROF_BB, PROF_VIT_GEMM, PROF_VIT_ATTN, PROF_VIT_MISC, PROF_HEAD_FULL,
   PROF_XW_COARSE, PROF_XW_PLAN, PROF_XW_GEMM, PROF_XW_HEAD, PROF_TRAIN_BWD,
   PROF_DELTA_TRAIN_CONV, PROF_DELTA_BN, PROF_DELTA_DGRAD, PROF_DELTA_WGRAD, PROF_FG_MASK, PROF_CONTRASTIVE,
-  PROF_SAMPLER, PROF_CYCLE, PROF_COUNT
+  PROF_SAMPLER, PROF_CYCLE, PROF_EMB_REG, PROF_COUNT
 };
 extern bool g_prof_on;
 void prof_begin(int cls, cudaStream_t st);

@@ -127,7 +127,7 @@ static const char* kProfNames[PROF_COUNT] = {"sample", "corr_gemm", "corr_stream
                                               "best_buddies", "vit_gemm", "vit_attn", "vit_misc", "head_full",
                                               "xw_coarse_gemm", "xw_plan", "xw_exact_gemm", "xw_head", "train_backward",
                                               "delta_train_conv", "delta_bn", "delta_dgrad", "delta_wgrad",
-                                              "fg_mask", "contrastive", "sampler", "cycle"};
+                                              "fg_mask", "contrastive", "sampler", "cycle", "emb_reg"};
 int dinotrk_profile_classes(void) { return PROF_COUNT; }
 const char* dinotrk_profile_class_name(int cls) { return (cls >= 0 && cls < PROF_COUNT) ? kProfNames[cls] : ""; }
 void dinotrk_profile_enable(int on) { dtk::g_prof_on = on != 0; }

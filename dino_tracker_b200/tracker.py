@@ -7,7 +7,7 @@ in the CUDA kernels; this file only owns tensors and forwards calls.  With gradi
 ``dino_tracker.py:405-429``) ``forward`` builds a graph: delta-DINO as torch ops, the tracker as one autograd node
 with hand-written forward and backward kernels (``train.py``, ``csrc/train.cu``); the cycle-consistency methods
 (``models/tracker.py:182-301``) run all pairs as one batch (``cycle.py``).  The losses / optimiser loop of
-``dino_tracker.py`` stay with the reference's trainer.
+``dino_tracker.py`` are ``trainer.py``'s.
 
 Internal layout: features are kept token-major ``[T][P][C]`` (see include/dinotrk.h);
 ``refined_features`` / ``dino_embed_video`` expose zero-copy ``T x C x h x w`` views of them.

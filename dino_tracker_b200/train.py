@@ -253,6 +253,61 @@ def sample_points(tracker, emb_chw, pts):
     return SampleFunction.apply(emb_chw.permute(0, 2, 3, 1).reshape(T, h * w, C), pts, tracker)
 
 
+def token_rows(emb_chw):
+    """N x C x h x w -> [N][P][C], as ``track_points`` reads the frame set.  A view (no copy) where the embeddings are
+    token-major in memory, as the training forward's are."""
+    N, C, h, w = emb_chw.shape
+    return emb_chw.permute(0, 2, 3, 1).reshape(N, h * w, C)
+
+
+class RegularisersFunction(torch.autograd.Function):
+    """(norm_reg, angle_reg) = (mean_p |a/b - 1|, mean_p |d/(a b) - 1|) of the refined embeddings E and the raw DINO
+    embeddings R, both token-major [n][P][C] (``get_emb_norm_regularization_loss`` / ``get_emb_angle_regularization_loss``
+    of dino_tracker.py:136-146).  Forward ``dinotrk_emb_reg_forward``, backward ``dinotrk_emb_reg_backward``: the upstream
+    gradients stay on the device, so the backward never waits for the host.  R is a constant (the raw features)."""
+
+    @staticmethod
+    def forward(ctx, E, R):
+        if R.requires_grad:
+            raise ValueError("RegularisersFunction: the raw embeddings R are constants and must not require grad")
+        lib = _lib.load()
+        dev = E.device
+        E_, R_ = E.detach().contiguous(), R.detach().contiguous()
+        n, P, C = E_.shape
+        assert R_.shape == E_.shape and E_.dtype == R_.dtype == torch.float32
+        with torch.cuda.device(dev):
+            out = torch.empty(2, device=dev, dtype=torch.float32)
+            aux = torch.empty(n * P, 3, device=dev, dtype=torch.float32)
+            ws_bytes = lib.dinotrk_emb_reg_workspace_bytes(n, P)
+            ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+            _lib.check(lib.dinotrk_emb_reg_forward(_lib.ptr(E_), _lib.ptr(R_), n, P, C, _lib.ptr(out), _lib.ptr(aux),
+                                                   _lib.ptr(ws), ws_bytes, _lib.stream_ptr()), "emb_reg_forward")
+        ctx.save_for_backward(E_, R_, aux)
+        return out[0], out[1]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_norm, g_angle):
+        lib = _lib.load()
+        E, R, aux = ctx.saved_tensors
+        n, P, C = E.shape
+        dev = E.device
+        with torch.cuda.device(dev):
+            zero = torch.zeros((), device=dev, dtype=torch.float32)
+            g_n = zero if g_norm is None else g_norm.detach().float().contiguous()
+            g_a = zero if g_angle is None else g_angle.detach().float().contiguous()
+            dE = torch.empty_like(E)
+            _lib.check(lib.dinotrk_emb_reg_backward(_lib.ptr(E), _lib.ptr(R), n, P, C, _lib.ptr(aux), _lib.ptr(g_n), _lib.ptr(g_a),
+                                                    _lib.ptr(dE), _lib.stream_ptr()), "emb_reg_backward")
+        return dE, None
+
+
+def emb_regularisers(model):
+    """(norm_reg, angle_reg) of the last training forward's ``model.frame_embeddings`` / ``model.raw_embeddings`` as one
+    node: the two regularisers of dino_tracker.py:136-146 with a graph to the refined embeddings."""
+    return RegularisersFunction.apply(token_rows(model.frame_embeddings), token_rows(model.raw_embeddings))
+
+
 def track_points(tracker, emb_chw, inp):
     """``Tracker.get_point_predictions`` (models/tracker.py:175-180) with a graph: emb_chw N x C x h x w (the frame set's
     embeddings, may require grad), inp as in ``Tracker.forward``.  Returns B x 2 in [-1, 1]."""
@@ -260,7 +315,7 @@ def track_points(tracker, emb_chw, inp):
     N, C, h, w = emb_chw.shape
     if src_pts.shape[0] == 0:                      # nothing to track (e.g. an empty cycle-consistency draw)
         return emb_chw.new_zeros(0, 2)
-    emb_tpc = emb_chw.permute(0, 2, 3, 1).reshape(N, h * w, C)
+    emb_tpc = token_rows(emb_chw)
     head = tracker.tracker_head.cnn_refiner
     pts = torch.cat([src_pts.to(tracker._dev, torch.float32)[:, :2], src_idx.to(tracker._dev).to(torch.float32)[:, None]], dim=1)
     return TrackFunction.apply(emb_tpc, head[0].normalized_weight_graph(), head[0].bias, head[2].normalized_weight_graph(),

@@ -616,6 +616,22 @@ int dinotrk_cycle_unnorm(const float* there_out, const int* rows, int R, int H, 
 int dinotrk_cycle_keep(const float* start, const float* back_out, int R, int H, int W, float thresh, int* keep_rows,
                        float* cycle_px, int* n_keep, void* stream);
 
+/* ---- embedding regularisers (dino_tracker.py:136-146, models/utils.py:79-84) --------------------------------------- */
+/* E (refined) and R (raw DINO) embeddings of the frame set, token-major [n][P][C] fp32, C a multiple of 4, both 16-byte
+ * aligned.  Per token a = |E_p|, b = |R_p|, d = E_p . R_p.
+ *   forward: out [2] = (mean_p |a / b - 1|, mean_p |d / (a b) - 1|) over all n P tokens (no eps, as the reference) and
+ *            aux [n P][3] = (a, b, d) for the backward.  Fixed per-block partials, then one fixed-order final sum: two runs
+ *            give the same bits.  Workspace of dinotrk_emb_reg_workspace_bytes(n, P) bytes (0 on invalid shapes).
+ *   backward: g_norm, g_angle are DEVICE pointers to the upstream gradients of out[0], out[1] (no sync).  OVERWRITES
+ *            dE [n][P][C] = g_norm / (nP) s1 E / (a b) + g_angle / (nP) s2 (R / (a b) - cos E / a^2) with
+ *            s1 = sgn(a / b - 1), s2 = sgn(cos - 1) and sgn(0) = 0 (torch's abs backward).  R gets no gradient.
+ * Argument errors (C % 4 != 0 among them) return DINOTRK_EINVAL before any launch.  Profile class "emb_reg". */
+size_t dinotrk_emb_reg_workspace_bytes(int n, int P);
+int dinotrk_emb_reg_forward(const float* E, const float* R, int n, int P, int C, float* out, float* aux, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int dinotrk_emb_reg_backward(const float* E, const float* R, int n, int P, int C, const float* aux, const float* g_norm,
+                             const float* g_angle, float* dE, void* stream);
+
 /* ---- RAFT-large optical flow (torchvision models/optical_flow/raft.py raft_large, eval mode) ---------------------- */
 /* Weights: one entry per convolution in torchvision's parameter order.  w_hi / w_lo are the fp16 split
  * (dinotrk_split_fp16) of the K-major matrix [Np][Kp]: row n = output channel, k = (ky * kw + kx) * C_in + ci with the

@@ -1,17 +1,21 @@
 """The time of one whole training iteration (dino_tracker.py:405-435 after iteration 5000: the cycle term and both
-contrastive terms active) at train.yaml's shape, with two sampler routes alternated in the same process:
-  (a) ``oracle``: the plain-torch sampler of data/dataset.py (oracle/sampler.py), the route the reference's trainer runs;
-  (b) ``library``: dino_tracker_b200.sampler.DinoTrackerSampler.
+contrastive terms active) at train.yaml's shape: ``DinoTrackerTrainer.iteration`` (dino_tracker_b200/trainer.py), three
+routes alternated in the same process:
+  (a) ``trainer``: the trainer as it ships (library sampler, the regulariser node);
+  (b) ``trainer_torch_reg``: the trainer with the reference's torch regulariser expressions in place of the node;
+  (c) ``oracle_sampler``: the trainer with the plain-torch sampler of data/dataset.py (oracle/sampler.py), the sampler
+      the reference's trainer runs.
+Then the two regularisers on their own on the frame set's embeddings (4 x 1024 x 67 x 121, token-major as the training
+forward leaves them): the node's forward and backward against the torch expressions' forward and backward.
 
-    python tools/bench_train_iter.py [--steps 20] [--warmup 3] [--out DIR]
+    python tools/bench_train_iter.py [--steps 20] [--warmup 3] [--reg-reps 50] [--out DIR]
 
 Set-up: 50 frames of 476 x 854, C = 1024 seeded features, the shipped delta-DINO widths, Adam + LambdaLR as
 ``train_setup`` builds them, trajectories chained from smooth flows (as tools/bench_fg_mask.py builds them, about 1M)
-split by a planted mask, and a best-buddies dict for every ordered frame pair.  The loop body is restated with the
-library's Tracker and contrastive losses (the reference is not importable here); the norm and angle regularisers are the
-reference's torch expressions.  Per route: the median ms per iteration, the median CUDA-event ms of each phase, and the
-peak device memory above the set-up's.  The card's name, power limit and SM clock are read in the same run.  Prints one
-JSON line (and writes it to DIR/bench_train_iter.json with --out).
+split by a planted mask, and a best-buddies dict for every ordered frame pair.  Per route: the median ms per iteration
+and the peak device memory above the set-up's; per regulariser implementation the median CUDA-event ms of forward and
+backward.  The card's name, power limit and SM clock are read in the same run.  Prints one JSON line (and writes it to
+DIR/bench_train_iter.json with --out).
 """
 import argparse
 import json
@@ -31,7 +35,6 @@ CFG = {"lr_delta_dino": 0.01, "lr_cnn_refiner": 0.01, "scheduler_gamma": 0.999, 
        "lambda_cl_ref_bb": 0.00005, "cl_n_frames": 4, "cl_points_per_pair": 256, "cl_fg_points_ratio": 0.7, "cl_temp": 0.1,
        "cl_div_dino_bb": 700, "cl_div_ref_bb": 900, "bb_amb_sig_a": 27, "bb_amb_sig_b": -5.7, "dino_patch_size": 14,
        "train_batch_size": 512, "batch_n_frames": 4, "fg_traj_ratio": 0.5}
-PHASES = ("sampler", "forward", "cycle", "refined_loss", "dino_bb_loss", "regularisers", "backward", "optimiser")
 
 
 def card():
@@ -86,84 +89,121 @@ def setup(dev):
     return model, opt, sched, tr, fg, bg, (W, H, T)
 
 
+def torch_regularisers(model):
+    """dino_tracker.py:136-146 as the reference evaluates them."""
+    emb, raw = model.frame_embeddings, model.raw_embeddings
+    norm_reg = (emb.norm(dim=1) / raw.norm(dim=1) - 1).abs().mean()
+    angle_reg = (torch.einsum("bchw,bchw->bhw", emb, raw) / (emb.norm(dim=1) * raw.norm(dim=1)) - 1).abs().mean()
+    return norm_reg, angle_reg
+
+
+def trainer_for(tr_stub, T, workdir):
+    """A DinoTrackerTrainer over the set-up's masks and best buddies (its data folder holds only T placeholder frames:
+    the trainer reads the frame count from it)."""
+    from PIL import Image
+    from dino_tracker_b200.trainer import DinoTrackerTrainer
+    os.makedirs(os.path.join(workdir, "video"))
+    for t in range(T):
+        Image.new("RGB", (1, 1)).save(os.path.join(workdir, "video", f"{t:05d}.png"))
+    cfg = dict(CFG, video_resw=854, video_resh=476)
+    tr = DinoTrackerTrainer(cfg, workdir, device="cuda:0")
+    tr.fg_masks, tr.dino_bb_pairs = tr_stub.fg_masks, tr_stub.dino_bb_pairs
+    return tr
+
+
+def time_regularisers(reps):
+    """ms (median of reps) of the node's and the torch expressions' forward and backward on 4 x 1024 x 67 x 121."""
+    from oracle import synth
+    from dino_tracker_b200.train import RegularisersFunction, token_rows
+    n, C, h, w = 4, 1024, 67, 121
+    raw = synth.random_features(n, C, h, w, seed=410).cuda().permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+    emb = (raw * 1.05 + 0.01 * torch.randn_like(raw)).requires_grad_(True)
+    g = torch.ones((), device="cuda:0")
+
+    def node():
+        return RegularisersFunction.apply(token_rows(emb), token_rows(raw))
+
+    def ref():
+        class M:
+            frame_embeddings, raw_embeddings = emb, raw
+        return torch_regularisers(M)
+    out = {}
+    for name, fn in (("node", node), ("torch", ref)):
+        fwd, bwd = [], []
+        for r in range(reps + 3):
+            emb.grad = None
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+            ev[0].record()
+            a, b = fn()
+            ev[1].record()
+            torch.autograd.backward([a, b], [g, g])
+            ev[2].record()
+            torch.cuda.synchronize()
+            if r >= 3:
+                fwd.append(ev[0].elapsed_time(ev[1]))
+                bwd.append(ev[1].elapsed_time(ev[2]))
+        out[name] = {"forward_ms": round(statistics.median(fwd), 4), "backward_ms": round(statistics.median(bwd), 4)}
+    # what the node must move at least: forward reads E and R, backward reads both and writes dE
+    nbytes = n * C * h * w * 4
+    out["min_bytes"] = {"forward": 2 * nbytes, "backward": 3 * nbytes}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--reg-reps", type=int, default=50)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train_iter needs a CUDA device")
-    from dino_tracker_b200 import contrastive as c
+    import tempfile
     from dino_tracker_b200 import sampler as sm
     from oracle import sampler as osm
     dev = "cuda:0"
     info = card()
-    model, opt, sched, tr, fg, bg, shapes = setup(dev)
+    model, opt, sched, stub, fg, bg, shapes = setup(dev)
     rn = osm.RangeNormalizer(shapes=shapes, device=dev)
-    huber = torch.nn.HuberLoss(delta=1 / 32, reduction="none")
     kw = dict(batch_size=CFG["train_batch_size"], range_normalizer=rn, dst_range=(-1, 1), fg_trajectories=fg,
               bg_trajectories=bg, fg_traj_ratio=CFG["fg_traj_ratio"], num_frames=CFG["batch_n_frames"])
-    samplers = {"oracle": osm.DinoTrackerSampler(**kw), "library": sm.DinoTrackerSampler(**kw)}
+    library, oracle_sampler = sm.DinoTrackerSampler(**kw), osm.DinoTrackerSampler(**kw)
+    with tempfile.TemporaryDirectory() as workdir:
+        tr = trainer_for(stub, shapes[2], workdir)
+    node_reg = tr.regularisers
+    routes = {"trainer": (library, node_reg), "trainer_torch_reg": (library, torch_regularisers),
+              "oracle_sampler": (oracle_sampler, node_reg)}
     torch.cuda.synchronize()
     base = torch.cuda.memory_allocated()
 
-    def iteration(sampler):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(len(PHASES) + 1)]
-        torch.cuda.empty_cache()
-        opt.zero_grad()
+    def iteration(sampler, regularisers):
+        tr.regularisers = regularisers
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
         ev[0].record()
-        sample = sampler()
-        labels = sample["t2_points_normalized"][:, :-1]
-        inputs = (sample["t1_points"], sample["source_frame_indices"], sample["target_frame_indices"], sample["frames_set_t"])
+        terms = tr.iteration(6000, model, sampler, opt, sched)
         ev[1].record()
-        loss = huber(model(inputs), labels).mean()
-        ev[2].record()
-        cyc = model.get_cycle_consistent_preds(inputs[-1], tr.fg_masks)
-        wgt = CFG["cyc_gamma"] ** cyc["cycle_consistency_dists"]
-        st = wgt[:, None] * huber(cyc["source_target_coords"], cyc["target_coords"][:, :2])
-        ts = wgt[:, None] * huber(cyc["target_source_coords"], cyc["source_coords"][:, :2])
-        loss = loss + CFG["lambda_cyc"] * (st.mean() + ts.mean()) / 2
-        ev[3].record()
-        ref_l = c.get_refined_bb_contrastive_loss(tr, model, inputs[-1], model.frame_embeddings,
-                                                  batch_size=CFG["cl_n_frames"], points_per_pair=CFG["cl_points_per_pair"],
-                                                  fg_points_ratio=CFG["cl_fg_points_ratio"], temp=CFG["cl_temp"],
-                                                  cl_div=CFG["cl_div_ref_bb"])
-        loss = loss + CFG["lambda_cl_ref_bb"] * ref_l
-        ev[4].record()
-        dino_l = c.get_dino_bb_contrastive_loss(tr, model, inputs[-1])
-        ev[5].record()
-        emb, raw = model.frame_embeddings, model.raw_embeddings
-        norm_reg = (emb.norm(dim=1) / raw.norm(dim=1) - 1).abs().mean()
-        angle_reg = (torch.einsum("bchw,bchw->bhw", emb, raw) / (emb.norm(dim=1) * raw.norm(dim=1)) - 1).abs().mean()
-        loss = loss + CFG["lambda_cl_dino_bb"] * dino_l + CFG["lambda_emb_norm"] * norm_reg + CFG["lambda_angle"] * angle_reg
-        ev[6].record()
-        loss.backward()
-        ev[7].record()
-        opt.step()
-        sched.step()
-        ev[8].record()
-        loss.item()
+        terms.tolist()
         torch.cuda.synchronize()
-        return ev[0].elapsed_time(ev[-1]), [ev[i].elapsed_time(ev[i + 1]) for i in range(len(PHASES))]
+        return ev[0].elapsed_time(ev[1])
 
-    res = {r: {"total": [], "phases": [], "peak": 0} for r in samplers}
+    res = {r: {"total": [], "peak": 0} for r in routes}
     for it in range(args.warmup + args.steps):
-        for route, s in samplers.items():
+        for route, (s, reg) in routes.items():
             torch.cuda.synchronize()
             torch.cuda.reset_peak_memory_stats()
-            total, phases = iteration(s)
+            total = iteration(s, reg)
             if it >= args.warmup:
                 res[route]["total"].append(total)
-                res[route]["phases"].append(phases)
                 res[route]["peak"] = max(res[route]["peak"], torch.cuda.max_memory_allocated() - base)
     out = {"what": "train_iteration", "T": shapes[2], "H": shapes[1], "W": shapes[0], "C": 1024, "batch": CFG["train_batch_size"],
            "n_fg": fg.shape[0], "n_bg": bg.shape[0], "steps": args.steps, "warmup": args.warmup, "card": info}
     for route, r in res.items():
         out[route] = {"ms_median": round(statistics.median(r["total"]), 2),
                       "ms_min": round(min(r["total"]), 2), "ms_max": round(max(r["total"]), 2),
-                      "phases_ms_median": {p: round(statistics.median(x[i] for x in r["phases"]), 3) for i, p in enumerate(PHASES)},
                       "peak_extra_gib": round(r["peak"] / 2 ** 30, 3)}
+    del model, opt, sched, library, oracle_sampler, tr
+    torch.cuda.empty_cache()
+    out["regularisers"] = time_regularisers(args.reg_reps)
     out["card_after"] = card()
     print(json.dumps(out), flush=True)
     if args.out:
