@@ -95,6 +95,7 @@ SIGNATURES = {
     "dinotrk_xw_coarse_keys_i8": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, _P, c_int, _P, _P, _P, c_int, _P, _P, _P, _P,
                                           c_size_t, _P]),
     "dinotrk_xw_box_gemm": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P]),
+    "dinotrk_xw_box_gemm_ext": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, c_int, _P, _P, _P, _P, _P, c_int, c_int, _P, _P]),
     "dinotrk_infer_plan": (c_int, [c_int, c_int, c_int, _P, c_int, _P, _P, c_int, _P]),
     "dinotrk_infer_anchor_gcap": (c_int, [c_int, c_int]),
     "dinotrk_infer_plan_anchors": (c_int, [c_int, c_int, _P, _P, _P, c_int, c_int, _P, _P, c_int, _P]),
@@ -351,13 +352,15 @@ def profile_collect():
 
 def infer_stats():
     """{anchor-phase maps, finished by the exact-window path, re-done by the full-map path, pipeline, contraction, coarse pass,
-    exact-window maps whose descriptor was read in place / gathered} of the last infer."""
-    a = (ctypes.c_longlong * 10)()
-    check(load().dinotrk_infer_last_stats(a, 10), "infer_last_stats")
+    exact-window maps whose descriptor was read in place / gathered, cells of the exact box GEMM and the tokens of their
+    tight extents} of the last infer."""
+    a = (ctypes.c_longlong * 12)()
+    check(load().dinotrk_infer_last_stats(a, 12), "infer_last_stats")
     rho_f = struct.unpack("<f", struct.pack("<I", int(a[7])))[0]
     return {"anchor_maps": int(a[0]), "exact_window": int(a[1]), "full_map": int(a[2]), "pipeline": "exact-window" if a[3] else "full-map",
             "full_map_by_certificate": int(a[4]), "contraction": "fp16x3" if a[5] else "fp32",
-            "coarse": "int8" if a[6] else "fp16", "coarse_rho_f": rho_f, "desc_in_place": int(a[8]), "desc_gathered": int(a[9])}
+            "coarse": "int8" if a[6] else "fp16", "coarse_rho_f": rho_f, "desc_in_place": int(a[8]), "desc_gathered": int(a[9]),
+            "exact_box_cells": int(a[10]), "exact_box_tokens": int(a[11])}
 
 
 def launch_count():

@@ -502,9 +502,9 @@ static InferAsync* infer_async() {
 constexpr int XW_RING = 4;
 constexpr int XW_PROBE_MAPS = 4096;   // size of the probe chunk (automatic pipeline choice)
 constexpr int INFER_A_COUNTED = 16;   // trajectory-phase chunks whose uncertified maps the anchor phase's choice reads
-// host_cnt: [XW_RING][2] queue totals / uncertified of the chunks in flight | [INFER_A_COUNTED] trajectory-phase uncertified
-// counts | the video's smallest token norm
-constexpr int XW_CNT_A = 2 * XW_RING, XW_CNT_MINNORM = XW_CNT_A + INFER_A_COUNTED;
+// host_cnt: [XW_RING][XW_CNT_CHUNK] queue total / uncertified / extent tokens / box-GEMM cells of the chunks in flight |
+// [INFER_A_COUNTED] trajectory-phase uncertified counts | the video's smallest token norm
+constexpr int XW_CNT_CHUNK = 4, XW_CNT_A = XW_CNT_CHUNK * XW_RING, XW_CNT_MINNORM = XW_CNT_A + INFER_A_COUNTED;
 struct XwAsync {
   int state;                                   // 0: not created, 1: ready, -1: failed
   cudaEvent_t sample[XW_RING], done[XW_RING], freed[XW_RING];
@@ -530,10 +530,11 @@ static int g_xw_coarse = -1;                   // -1: automatic, 0: fp16 coarse 
 // Slots of dinotrk_infer_last_stats, named as the keys of _lib.infer_stats(): anchor-phase maps | finished on the
 // exact-window path | re-done on the full-map path | pipeline used | of those re-done, queued by the certificate |
 // tensor-core contraction | int8 coarse pass | bits of the largest per-frame int8 residual | exact-window maps whose
-// descriptor was read in place from the unique table | those gathered into the chunk's rows
+// descriptor was read in place from the unique table | those gathered into the chunk's rows | cells the exact box GEMM
+// ran on | the tokens of their extents (xwin.cuh, XwChunk::box_ext)
 namespace infer_stat {
 enum { anchor_maps, exact_window, full_map, pipeline, full_map_by_certificate, contraction, coarse, coarse_rho_f,
-       desc_in_place, desc_gathered, count };
+       desc_in_place, desc_gathered, exact_box_cells, exact_box_tokens, count };
 }
 static long long g_infer_stats[infer_stat::count] = {};
 // the probe chunk queues more than this fraction of its maps on the int8 coarse pass: the rest of the phase runs the fp16
@@ -817,8 +818,10 @@ struct ExactWindow {
     InferWs& ws = c.ws;
     XwAsync* xa = choice.xa;
     DTK_CUDA(cudaEventSynchronize(xa->done[j % XW_RING]));
-    const int n_slow = xa->host_cnt[2 * (j % XW_RING)];
-    g_infer_stats[infer_stat::full_map_by_certificate] += xa->host_cnt[2 * (j % XW_RING) + 1];
+    const int* cnt = xa->host_cnt + XW_CNT_CHUNK * (j % XW_RING);
+    const int n_slow = cnt[0];
+    g_infer_stats[infer_stat::full_map_by_certificate] += cnt[1];
+    g_infer_stats[infer_stat::exact_box_tokens] += cnt[2]; g_infer_stats[infer_stat::exact_box_cells] += cnt[3];
     const ChunkMeta& cm = c.metas[j];
     const XwSet& x = ws.xr[j % XW_RING];
     const InferCtx::Grp gp = c.grp_of(j);
@@ -881,7 +884,8 @@ static int anchors_exact_window(InferCtx& c, AnchorChoice& choice, const float* 
     if ((rc = launch_xw_head(c.fv, c.g, c.hw, cells, x.norm, gp.map0, cm.used, x.out_index, anchors, 2, 0, x.xc, st, cm.n_groups,
                              eps)))
       return rc;
-    DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + 2 * (k % XW_RING), x.xc.slow_cnt + cm.n_groups, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    DTK_CUDA(cudaMemcpyAsync(xa->host_cnt + XW_CNT_CHUNK * (k % XW_RING), x.xc.slow_cnt + cm.n_groups, XW_CNT_CHUNK * sizeof(int),
+                             cudaMemcpyDeviceToHost, st));
     DTK_CUDA(cudaEventRecord(xa->done[k % XW_RING], st));
     if (k == 0 && choice.probe && c.metas.size() > 1) {   // the probe: wait for it, look at the certificate's verdicts
       if ((rc = pipe.finish(0))) return rc;
@@ -1018,6 +1022,7 @@ static int infer_anchors(InferCtx& c, const float* traj, const float* cos_sims, 
   stats[infer_stat::anchor_maps] = maps_C; stats[infer_stat::exact_window] = 0; stats[infer_stat::full_map] = 0;
   stats[infer_stat::pipeline] = choice.xw ? 1 : 0; stats[infer_stat::full_map_by_certificate] = 0;
   stats[infer_stat::contraction] = c.fv.tensor() ? 1 : 0; stats[infer_stat::desc_in_place] = 0; stats[infer_stat::desc_gathered] = 0;
+  stats[infer_stat::exact_box_cells] = 0; stats[infer_stat::exact_box_tokens] = 0;
   float rho_max = 0.f;
   for (float r : rho_f) rho_max = std::max(rho_max, r);
   int rc = choice.coarse_pass(c.fv, rho_max);

@@ -190,7 +190,8 @@ int launch_xw_coarse(const FeatView& fv, const void* desc_hi, int desc_rows, con
 //     SECOND value is also within 2 eps: an arg-max candidate whose token is unknown).  Writes the candidate tokens and
 //     pinfo[map] = coarse arg-max token, or -1 - token if the map is ambiguous.
 // (b) one warp per CELL: the lower medians of the unambiguous maps' coarse arg-max row / column give the box centre; a map
-//     fits if every candidate lies within +-XW_SLACK of it.
+//     fits if every candidate lies within +-XW_SLACK of it.  The cell's extent (box_ext) is the union of its fitting maps'
+//     candidate windows: the only box tokens the head reads.  Its tokens and the cell are counted into box_cnt[0] / [1].
 //     KPL = cdiv(n_tiles, 32) keys per lane, tile t = lane + 32 q: candidates are ranked in tile order for any KPL.
 constexpr int PLAN_WARPS = 8;
 template <int KPL>
@@ -201,7 +202,7 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, 
   const int lane = threadIdx.x & 31;
   const int gw = blockIdx.x * PLAN_WARPS + (threadIdx.x >> 5), nw = gridDim.x * PLAN_WARPS;
   if (gw == 0)   // zero the queue counters of this chunk (n_groups per-group counts + the total + the uncertified count)
-    for (int i = lane; i <= n_groups + 1; i += 32) slow_cnt[i] = 0;
+    for (int i = lane; i <= n_groups + 3; i += 32) slow_cnt[i] = 0;
   for (int map = gw; map < n_maps; map += nw) {
     const unsigned long long* k1 = key1 + (size_t)map * n_tiles;
     const float* k2 = max2 + (size_t)map * n_tiles;
@@ -243,7 +244,7 @@ xw_cand_kernel(int n_maps, const float* __restrict__ desc_norm, float min_norm, 
 
 __global__ void __launch_bounds__(PLAN_WARPS * 32)
 xw_cell_kernel(XwCells cells, int w, const int* __restrict__ cand, const int* __restrict__ pinfo, int* __restrict__ stat,
-               int* __restrict__ cell_of, int2* __restrict__ box_org) {
+               int* __restrict__ cell_of, int2* __restrict__ box_org, int4* __restrict__ box_ext, int* __restrict__ box_cnt) {
   __shared__ short s_r[PLAN_WARPS][XW_MAX_CELL], s_c[PLAN_WARPS][XW_MAX_CELL];
   __shared__ unsigned char s_ok[PLAN_WARPS][XW_MAX_CELL];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -284,10 +285,12 @@ xw_cell_kernel(XwCells cells, int w, const int* __restrict__ cand, const int* __
         med_c = max(med_c, __shfl_xor_sync(0xffffffffu, med_c, o));
       }
     }
-    int n_fit = 0;
+    // the fitting maps' candidates span rows [lo_r, hi_r] and columns [lo_c, hi_c]
+    int n_fit = 0, lo_r = INT_MAX, hi_r = INT_MIN, lo_c = INT_MAX, hi_c = INT_MIN;
     for (int r = lane; r < m; r += 32) {
       const int map = row0 + r;
       bool fit = s_ok[wid][r] != 0;
+      int mr0 = INT_MAX, mr1 = INT_MIN, mc0 = INT_MAX, mc1 = INT_MIN;
       if (fit) {
         const int4 cd = __ldg(reinterpret_cast<const int4*>(cand) + map);
         const int ct[4] = {cd.x, cd.y, cd.z, cd.w};
@@ -296,15 +299,29 @@ xw_cell_kernel(XwCells cells, int w, const int* __restrict__ cand, const int* __
           if (ct[q] >= 0) {
             const int tr = ct[q] / w, tc_ = ct[q] - tr * w;
             fit = fit && abs(tr - med_r) <= XW_SLACK && abs(tc_ - med_c) <= XW_SLACK;
+            mr0 = min(mr0, tr); mr1 = max(mr1, tr); mc0 = min(mc0, tc_); mc1 = max(mc1, tc_);
           }
       }
       stat[map] = fit ? 0 : 1;
       n_fit += fit ? 1 : 0;
+      if (fit) { lo_r = min(lo_r, mr0); hi_r = max(hi_r, mr1); lo_c = min(lo_c, mc0); hi_c = max(hi_c, mc1); }
     }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) n_fit += __shfl_xor_sync(0xffffffffu, n_fit, o);
-    if (lane == 0)
-      box_org[cell] = n_fit > 0 ? make_int2(med_r - XW_BOX / 2, med_c - XW_BOX / 2) : make_int2(0, INT_MIN);
+    for (int o = 16; o > 0; o >>= 1) {
+      n_fit += __shfl_xor_sync(0xffffffffu, n_fit, o);
+      lo_r = min(lo_r, __shfl_xor_sync(0xffffffffu, lo_r, o)); hi_r = max(hi_r, __shfl_xor_sync(0xffffffffu, hi_r, o));
+      lo_c = min(lo_c, __shfl_xor_sync(0xffffffffu, lo_c, o)); hi_c = max(hi_c, __shfl_xor_sync(0xffffffffu, hi_c, o));
+    }
+    if (lane == 0) {
+      const int org_r = med_r - XW_BOX / 2, org_c = med_c - XW_BOX / 2;
+      box_org[cell] = n_fit > 0 ? make_int2(org_r, org_c) : make_int2(0, INT_MIN);
+      if (n_fit > 0) {   // every candidate lies within +-XW_SLACK of the centre: the extent lies inside the 21 x 21 box
+        const int4 e = make_int4(lo_r - WM / 2 - org_r, lo_c - WM / 2 - org_c, hi_r - lo_r + WM, hi_c - lo_c + WM);
+        box_ext[cell] = e;
+        atomicAdd(box_cnt, e.z * e.w);
+        atomicAdd(box_cnt + 1, 1);
+      }
+    }
     __syncwarp();
   }
 }
@@ -325,31 +342,48 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
   DTK_LAUNCHED();
   grid = cdiv(cells.n_cells, PLAN_WARPS);
   if (grid > num_sms() * 8) grid = num_sms() * 8;
-  xw_cell_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(cells, g.w, xc.cand, xc.pinfo, xc.stat, xc.cell_of, xc.box_org);
+  xw_cell_kernel<<<grid, PLAN_WARPS * 32, 0, st>>>(cells, g.w, xc.cand, xc.pinfo, xc.stat, xc.cell_of, xc.box_org, xc.box_ext,
+                                                   xc.slow_cnt + n_groups + 2);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
 
 // ====================================================================================================== 3. exact box GEMM
 // Persistent, warp-specialised (same roles as tc_gemm_kernel).  The cell's DESCRIPTORS are the wgmma M operand (64 rows per
-// consumer warpgroup) and the BOX TOKENS the N operand, in two parts: box rows 0-11 (252 tokens, m64n256k16) and rows 12-20
-// (189 tokens, m64n192k16), 448 columns for 441 tokens.  Large-N shapes read the fewest shared-memory operand bytes per FMA,
-// and shared-memory bandwidth is what bounds this kernel (DESIGN.md 4.3).  Two layouts:
-//   MB = 64   every cell of the call has <= 64 maps: both consumer warpgroups work on the same cell, warpgroup 1 on part 0
-//             and warpgroup 2 on part 1.  A ring stage holds the descriptor K-block and both parts, so the descriptors are
-//             loaded once per cell and each warpgroup drains its pipeline once per cell.
+// consumer warpgroup) and the tokens of its tight extent (XwChunk::box_ext: bh x bw tokens, 15..21 each) the N operand, in
+// PARTS of whole extent rows, at most XW_PART_TOK = 128 tokens each (m64n128k16; the columns past a part's tokens are
+// computed and never stored): rp = floor(128 / bw) rows per part at most (8 for bw <= 16, 6 at bw = 21), the rows shared
+// out evenly.  A cell whose maps agree (15 x 15 or 16 x 16 tokens) is two parts; the whole 21 x 21 box is four.  A stage
+// of a 128-token part is small, so the ring holds five or six stages: a stage's time is set by how many fills are in
+// flight, not by its bytes (DESIGN.md 4.3).  Two layouts:
+//   MB = 64   every cell of the call has <= 64 maps: the parts go in pairs (their count is rounded up to even), warpgroup 1
+//             on the first and warpgroup 2 on the second of a pair.  A ring stage holds the descriptor K-block and both
+//             parts of the pair, so the descriptors are loaded once per pair and each warpgroup drains its pipeline once
+//             per pair.
 //   MB = 128  cells of up to 128 maps: warpgroup 1 takes descriptor rows 0-63 and warpgroup 2 rows 64-127 of the same part;
-//             the two parts run one after the other, a stage holding the descriptor K-block and one part.
+//             the parts run one after the other, a stage holding the descriptor K-block and one part.
 // K blocks of 32 channels.  Split precision: lo*hi + hi*lo + hi*hi per K step of 16, K ascending -- the full-map GEMM's
-// sequence of products.  The descriptor K-block is two tiles (hi, lo) of 64-byte-swizzled rows.  The box rows arrive as 4-D
-// TMA boxes {channels, 21 columns, 12 or 9 rows, 1 frame} of the feature video, zero-filled outside the token grid, in one
-// of two row layouts (HILO):
+// sequence of products, whatever the extent and its parts.  The descriptor K-block is two tiles (hi, lo) of
+// 64-byte-swizzled rows.  A part's tokens arrive as one 4-D TMA box {channels, bw columns, rows, 1 frame} of the feature
+// video, zero-filled outside the token grid, landing at the start of the part's 1024-byte-aligned slot (part token (y, x)
+// in slot row y bw + x).  The box's shape changes from cell to cell, so the kernel takes a table of tensor maps, one per
+// (bw, rows) (XwTokMaps).  Token rows come in one of two layouts (HILO):
 //   false  the separate hi and lo halves [T][h][w][C]: two boxes of 64-byte rows (32 channels) per part and K block.
 //   true   the interleaved split [T][h][w][ceil(C / 32)][64] (FeatView::hilo): one box of 128-byte rows [hi 32 | lo 32] in
 //          the 128-byte swizzle; a K step reads hi 0 / 32 and lo 64 / 96 bytes into the row.  Same bytes in half as many
 //          rows: the TMA's cost per row, not the MMA, bounds the 64-byte layout (DESIGN.md 4.3).
-// A MB = 64 stage is 64 KiB in either layout (three fit), a MB = 128 stage 48 KiB (four).
-// Epilogue: straight from the accumulator fragment to xbox[map][token] (a quad holds 8 consecutive tokens of one map).
+// A MB = 64 stage is 40 KiB in either layout (five fit), a MB = 128 stage 32 KiB (six).
+// Epilogue: straight from the accumulator fragment to xbox[map][xw_col(row, column)] of the 21 x 21 box (a quad holds 8
+// consecutive part tokens of one map, which may straddle an extent row).
+constexpr int XW_EXT_MIN = WM;                          // smallest extent side: one candidate's window
+constexpr int XW_NW = XW_BOX - XW_EXT_MIN + 1;          // extent widths 15 .. 21
+constexpr int XW_PART_TOK = 128;                        // tokens of a part at most: its wgmma N
+constexpr int XW_PART_ROWS = XW_PART_TOK / XW_EXT_MIN;  // rows of a part at most (8)
+
+// the token boxes' tensor maps: [hi or the interleaved split, lo][bw - XW_EXT_MIN][rows - 1]
+template <bool HILO>
+struct XwTokMaps { CUtensorMap m[HILO ? 1 : 2][XW_NW][XW_PART_ROWS]; };
+
 template <int MB, bool HILO>
 struct XwCfg {
   static constexpr int kBK = 32;                                  // channels per K block
@@ -357,29 +391,48 @@ struct XwCfg {
   static constexpr int kTokRow = HILO ? 2 * kRow : kRow;          // bytes per token row of one TMA box
   static constexpr int kBoxes = HILO ? 1 : 2;                     // token boxes per part and K block
   static constexpr int kDescBytes = MB * kRow;                    // one operand half (hi or lo) of the descriptor K-block
-  static constexpr int kTok0Bytes = XW_N0 * kTokRow, kTok1Bytes = XW_N1 * kTokRow;   // one token box's slot
-  static constexpr int kTok0Tx = XW_ROWS0 * XW_BOX * kTokRow, kTok1Tx = XW_ROWS1 * XW_BOX * kTokRow;   // bytes a box lands
-  // stage: [desc hi | desc lo | part 0 boxes (| part 1 boxes, MB = 64)]; with MB = 128 either part uses the part 0 slots.
-  // Every token box starts 1024-byte aligned (the 128-byte swizzle's atom).
+  static constexpr int kSlotBytes = XW_PART_TOK * kTokRow;        // one token box's slot
+  static constexpr int kParts = MB == 64 ? 2 : 1;                 // parts per stage
+  // stage: [desc hi | desc lo | part boxes (| the second part's boxes, MB = 64)].  Every token box starts 1024-byte
+  // aligned (the 128-byte swizzle's atom).
   static constexpr int kTokOff = 2 * kDescBytes;
-  static constexpr int kStageBytes = kTokOff + kBoxes * (MB == 64 ? kTok0Bytes + kTok1Bytes : kTok0Bytes);
-  static constexpr int kStages = MB == 64 ? 3 : 4;
+  static constexpr int kStageBytes = kTokOff + kParts * kBoxes * kSlotBytes;
+  static constexpr int kStages = MB == 64 ? 5 : 6;
   static constexpr int kSmem = kStages * kStageBytes + 1024 + 256;
   static_assert(kStages * kStageBytes + 1024 + 256 <= 227 * 1024, "shared-memory ring too large");
-  static_assert(kTokOff % 1024 == 0 && kTok0Bytes % 1024 == 0 && kTok1Bytes % 1024 == 0 && kStageBytes % 1024 == 0,
+  static_assert(kTokOff % 1024 == 0 && kSlotBytes % 1024 == 0 && kStageBytes % 1024 == 0,
                 "token boxes must start 1024-byte aligned");
 };
 
+// A cell's extent and its parts.  Null box_ext: the whole 21 x 21 box.  An extent outside the box skips the cell.
+template <int MB>
+struct XwExt {
+  int y, x, bh, bw, n;   // first box row / column, rows, columns, parts
+  __device__ __forceinline__ XwExt(const int4* __restrict__ box_ext, int cell) {
+    const int4 e = box_ext ? __ldg(box_ext + cell) : make_int4(0, 0, XW_BOX, XW_BOX);
+    y = e.x; x = e.y; bh = e.z; bw = e.w;
+    const int rp = XW_PART_TOK / max(bw, 1);
+    n = ok() ? (bh + rp - 1) / rp : 0;
+    if (MB == 64) n += n & 1;   // whole pairs
+  }
+  __device__ __forceinline__ bool ok() const {
+    return y >= 0 && x >= 0 && bh >= XW_EXT_MIN && bw >= XW_EXT_MIN && y + bh <= XW_BOX && x + bw <= XW_BOX;
+  }
+  // part i: rows bh / n, one more for the first bh % n parts (so <= ceil(bh / n) <= rp rows, >= 1 since n <= 8 < bh)
+  __device__ __forceinline__ int rows(int i) const { return bh / n + (i < bh % n ? 1 : 0); }
+  __device__ __forceinline__ int row(int i) const { return y + i * (bh / n) + min(i, bh % n); }   // its first box row
+};
+
 // One part of a cell on one consumer warpgroup: the K loop over the ring, then rows [r0, r0 + 64) of the cell x the part's
-// tokens into xbox.  d_off / t_off: byte offsets of the warpgroup's descriptor rows / the part's token box(es) in a stage,
-// t_half: distance from a token box's hi half to its lo half (separate halves only).
-template <int MB, bool HILO, int N>
+// ntok tokens (rows of bw, from box column col0 = xw_col(first row, first column)) into xbox.  d_off / t_off: byte offsets
+// of the warpgroup's descriptor rows / the part's token box(es) in a stage, t_half: distance from a token box's hi half to
+// its lo half (separate halves only).
+template <int MB, bool HILO>
 __device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t* empty, int& stage, int& phase, int KB,
                                         uint32_t d_off, uint32_t t_off, uint32_t t_half, float* __restrict__ xbox, int map0,
-                                        int r0, int m) {
+                                        int r0, int m, int ntok, int bw, int col0) {
   using Cfg = XwCfg<MB, HILO>;
-  constexpr int kTok = (N == XW_N0 ? XW_ROWS0 : XW_ROWS1) * XW_BOX;   // tokens of the part
-  constexpr int kCol0 = N == XW_N0 ? 0 : XW_ROWS0 * XW_BOX;           // its first column in xbox
+  constexpr int N = XW_PART_TOK;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = threadIdx.x & 127;
   float acc[N / 2];
 #pragma unroll
@@ -409,29 +462,31 @@ __device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t*
   tc::wgmma_wait<0>();
   tc::reg_fence(acc);
   if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
-  // fragment rows are maps, columns box tokens: acc[4 i + 2 h + {0, 1}] = map r0 + fr + 8 h, tokens 8 i + fc + {0, 1}
+  // fragment rows are maps, columns part tokens: acc[4 i + 2 h + {0, 1}] = map r0 + fr + 8 h, tokens 8 i + fc + {0, 1}.
+  // Token j = 8 i + fc is (y, x) = (j / bw, j % bw), followed as i steps: 8 < bw, so x wraps at most once per step.
   const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = r0 + fr + 8 * h;
     if (r >= m) continue;
-    float* dst = xbox + (size_t)(map0 + r) * XW_COLS + kCol0;
+    float* dst = xbox + (size_t)(map0 + r) * XW_COLS + col0;
+    int y = 0, x = fc;
 #pragma unroll
     for (int i = 0; i < N / 8; ++i) {
       const int j = 8 * i + fc;
-      if (j + 1 < kTok) *reinterpret_cast<float2*>(dst + j) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-      else if (j < kTok) dst[j] = acc[4 * i + 2 * h];
+      if (j < ntok) dst[y * XW_BOX + x] = acc[4 * i + 2 * h];
+      if (j + 1 < ntok) dst[x + 1 == bw ? (y + 1) * XW_BOX : y * XW_BOX + x + 1] = acc[4 * i + 2 * h + 1];
+      x += 8;
+      if (x >= bw) { x -= bw; ++y; }
     }
   }
 }
 
-// tm0 / tm1: token boxes of part 0 / 1 ([0] hi or the interleaved split, [1] lo; [1] unused with HILO)
 template <int MB, bool HILO>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant__ CUtensorMap tmD_lo,
-               const __grid_constant__ CUtensorMap tm0_hi, const __grid_constant__ CUtensorMap tm0_lo,
-               const __grid_constant__ CUtensorMap tm1_hi, const __grid_constant__ CUtensorMap tm1_lo, XwCells cells,
-               const int2* __restrict__ box_org, float* __restrict__ xbox, int K) {
+               const __grid_constant__ XwTokMaps<HILO> tok, XwCells cells, const int2* __restrict__ box_org,
+               const int4* __restrict__ box_ext, float* __restrict__ xbox, int K) {
   using Cfg = XwCfg<MB, HILO>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -442,10 +497,7 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
   const int KB = (K + Cfg::kBK - 1) / Cfg::kBK;
 
   if (threadIdx.x == 0) {
-    tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo); tc::prefetch_tmap(&tm0_hi);
-    if (!HILO) tc::prefetch_tmap(&tm0_lo);
-    tc::prefetch_tmap(&tm1_hi);
-    if (!HILO) tc::prefetch_tmap(&tm1_lo);
+    tc::prefetch_tmap(&tmD_hi); tc::prefetch_tmap(&tmD_lo);
     for (int s = 0; s < Cfg::kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 2); }   // 2 consumer warpgroups
     tc::mbar_fence_init();
   }
@@ -459,25 +511,22 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
       for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
         const int2 org = box_org[cell];
         if (org.y == INT_MIN) continue;            // every map of the cell takes the full-map path
-        const int drow = cells.arow[cell], frame = cells.frame[cell];
-        for (int part = 0; part < (MB == 64 ? 1 : 2); ++part) {
+        const XwExt<MB> e(box_ext, cell);
+        const int drow = cells.arow[cell], frame = cells.frame[cell], col = org.y + e.x;   // first grid column
+        const int wi = e.bw - XW_EXT_MIN;
+        for (int p0 = 0; p0 < e.n; p0 += Cfg::kParts) {
+          int tok_rows = 0;   // token rows of the stage's box(es)
+          for (int q = 0; q < Cfg::kParts; ++q) tok_rows += e.rows(p0 + q) * e.bw;
           for (int kb = 0; kb < KB; ++kb) {
             const int k0 = kb * Cfg::kBK, kt = HILO ? 2 * k0 : k0;   // channel / token-row element of the K block
             tc::mbar_wait(&empty[stage], phase ^ 1);
             uint8_t* st = smem + stage * Cfg::kStageBytes;
-            uint8_t* s0 = st + Cfg::kTokOff;
-            if constexpr (MB == 64) {   // the descriptors and both parts
-              tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + Cfg::kBoxes * (Cfg::kTok0Tx + Cfg::kTok1Tx));
-              uint8_t* s1 = s0 + Cfg::kBoxes * Cfg::kTok0Bytes;
-              tc::tma_load_4d(&tm0_hi, &full[stage], s0, kt, org.y, org.x, frame);
-              if (!HILO) tc::tma_load_4d(&tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, kt, org.y, org.x, frame);
-              tc::tma_load_4d(&tm1_hi, &full[stage], s1, kt, org.y, org.x + XW_ROWS0, frame);
-              if (!HILO) tc::tma_load_4d(&tm1_lo, &full[stage], s1 + Cfg::kTok1Bytes, kt, org.y, org.x + XW_ROWS0, frame);
-            } else {                    // the descriptors and part `part`
-              tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + Cfg::kBoxes * (part ? Cfg::kTok1Tx : Cfg::kTok0Tx));
-              const int by = org.x + (part ? XW_ROWS0 : 0);
-              tc::tma_load_4d(part ? &tm1_hi : &tm0_hi, &full[stage], s0, kt, org.y, by, frame);
-              if (!HILO) tc::tma_load_4d(part ? &tm1_lo : &tm0_lo, &full[stage], s0 + Cfg::kTok0Bytes, kt, org.y, by, frame);
+            tc::mbar_expect_tx(&full[stage], 2 * Cfg::kDescBytes + Cfg::kBoxes * tok_rows * Cfg::kTokRow);
+            for (int q = 0; q < Cfg::kParts; ++q) {
+              uint8_t* s = st + Cfg::kTokOff + q * Cfg::kBoxes * Cfg::kSlotBytes;
+              const int ri = e.rows(p0 + q) - 1, row = org.x + e.row(p0 + q);
+              tc::tma_load_4d(&tok.m[0][wi][ri], &full[stage], s, kt, col, row, frame);
+              if constexpr (!HILO) tc::tma_load_4d(&tok.m[1][wi][ri], &full[stage], s + Cfg::kSlotBytes, kt, col, row, frame);
             }
             tc::tma_load_2d(&tmD_hi, &full[stage], st, k0, drow);
             tc::tma_load_2d(&tmD_lo, &full[stage], st + Cfg::kDescBytes, k0, drow);
@@ -493,24 +542,56 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
     int stage = 0, phase = 0;
     for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
       if (box_org[cell].y == INT_MIN) continue;
+      const XwExt<MB> e(box_ext, cell);
       const int m = cells.m[cell], map0 = cells.row0[cell];
-      if constexpr (MB == 64) {   // warpgroup 1: part 0, warpgroup 2: part 1, all 64 descriptor rows
-        if (cw == 0)
-          xw_part<MB, HILO, XW_N0>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 0, m);
-        else
-          xw_part<MB, HILO, XW_N1>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff + Cfg::kBoxes * Cfg::kTok0Bytes,
-                                   Cfg::kTok1Bytes, xbox, map0, 0, m);
-      } else {                    // warpgroup cw: descriptor rows [64 cw, 64 cw + 64) of both parts
-        const uint32_t d_off = cw * 64 * Cfg::kRow;
-        xw_part<MB, HILO, XW_N0>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
-        xw_part<MB, HILO, XW_N1>(smem, full, empty, stage, phase, KB, d_off, Cfg::kTokOff, Cfg::kTok0Bytes, xbox, map0, 64 * cw, m);
+      for (int p0 = 0; p0 < e.n; p0 += Cfg::kParts) {
+        if constexpr (MB == 64) {   // warpgroup cw: part p0 + cw of the pair, all 64 descriptor rows
+          const int p = p0 + cw;
+          xw_part<MB, HILO>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff + cw * Cfg::kBoxes * Cfg::kSlotBytes,
+                            Cfg::kSlotBytes, xbox, map0, 0, m, e.rows(p) * e.bw, e.bw, xw_col(e.row(p), e.x));
+        } else {                    // warpgroup cw: descriptor rows [64 cw, 64 cw + 64) of part p0
+          xw_part<MB, HILO>(smem, full, empty, stage, phase, KB, cw * 64 * Cfg::kRow, Cfg::kTokOff, Cfg::kSlotBytes, xbox,
+                            map0, 64 * cw, m, e.rows(p0) * e.bw, e.bw, xw_col(e.row(p0), e.x));
+        }
       }
     }
   }
 }
 
+// The token boxes' tensor maps of a feature view, encoded once per (tensor, shape) and kept for the following launches
+// (a chunk's launch would otherwise encode up to 112 maps).  One entry per device: it is rebuilt when the features change.
+template <bool HILO>
+static int xw_tok_maps(const FeatView& fv, const dinotrk_geom& g, const XwTokMaps<HILO>*& out) {
+  struct Entry { const void* base[2]; uint64_t dims[4]; bool valid; XwTokMaps<HILO> maps; };
+  static PerDev<Entry> cache;
+  Entry& e = cache.get();
+  const void* base[2] = {HILO ? fv.hilo : fv.hi, HILO ? nullptr : fv.lo};
+  const uint64_t row = HILO ? (uint64_t)hilo_row(fv.C) : (uint64_t)fv.C;   // fp16 elements per token row
+  const uint64_t dims[4] = {row, (uint64_t)g.w, (uint64_t)g.h, (uint64_t)fv.T};
+  if (!e.valid || memcmp(e.base, base, sizeof(base)) != 0 || memcmp(e.dims, dims, sizeof(dims)) != 0) {
+    e.valid = false;
+    const uint64_t strides[3] = {row * 2, (uint64_t)g.w * row * 2, (uint64_t)fv.P * row * 2};
+    constexpr int BK = XwCfg<64, HILO>::kBK;
+    const uint32_t ib = HILO ? 2 * BK : BK, tsw = HILO ? 128 : 2 * BK;
+    for (int o = 0; o < (HILO ? 1 : 2); ++o)
+      for (int wi = 0; wi < XW_NW; ++wi)
+        for (int ri = 0; ri < XW_PART_ROWS; ++ri) {
+          const uint32_t box[4] = {ib, (uint32_t)(XW_EXT_MIN + wi), (uint32_t)(1 + ri), 1};
+          if (int rc = make_tmap_4d(&e.maps.m[o][wi][ri], base[o], dims, strides, box, TMAP_F16, tsw)) return rc;
+        }
+    memcpy(e.base, base, sizeof(base));
+    memcpy(e.dims, dims, sizeof(dims));
+    e.valid = true;
+  }
+  out = &e.maps;
+  return DINOTRK_OK;
+}
+
 template <int MB, bool HILO>
-static int run_xw_gemm(const CUtensorMap (&tm)[6], const XwCells& cells, const XwChunk& xc, int C, cudaStream_t st) {
+static int run_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const CUtensorMap (&tmD)[2], const XwCells& cells,
+                       const XwChunk& xc, cudaStream_t st) {
+  const XwTokMaps<HILO>* tok;
+  if (int rc = xw_tok_maps<HILO>(fv, g, tok)) return rc;
   static PerDev<bool> attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
@@ -520,8 +601,8 @@ static int run_xw_gemm(const CUtensorMap (&tm)[6], const XwCells& cells, const X
   const int sms = num_sms();
   const int grid = cells.n_cells < sms ? cells.n_cells : sms;
   ProfRange pr(PROF_XW_GEMM, st);
-  xw_gemm_kernel<MB, HILO><<<grid, TC_THREADS, XwCfg<MB, HILO>::kSmem, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], cells,
-                                                                              xc.box_org, xc.xbox, C);
+  xw_gemm_kernel<MB, HILO><<<grid, TC_THREADS, XwCfg<MB, HILO>::kSmem, st>>>(tmD[0], tmD[1], *tok, cells, xc.box_org, xc.box_ext,
+                                                                              xc.xbox, fv.C);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
@@ -532,25 +613,12 @@ int launch_xw_gemm(const FeatView& fv, const dinotrk_geom& g, const void* desc_h
   DTK_CHECK_ARG(fv.C % 8 == 0 && cells.max_m <= XW_MAX_CELL, "exact-window GEMM: bad sizes");
   const bool small = cells.max_m <= 64, hilo = fv.hilo != nullptr;
   constexpr int BK = XwCfg<64, false>::kBK, SW = 2 * BK;   // 32-channel K blocks; descriptors in 64-byte swizzle
-  CUtensorMap tm[6];   // desc hi, desc lo, part 0 [hi | hilo], part 0 lo, part 1 [hi | hilo], part 1 lo
+  CUtensorMap tmD[2];   // desc hi, desc lo
   int rc;
-  if ((rc = make_tmap_2d(&tm[0], desc_hi, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
-  if ((rc = make_tmap_2d(&tm[1], desc_lo, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
-  const uint64_t row = hilo ? (uint64_t)hilo_row(fv.C) : (uint64_t)fv.C;   // fp16 elements per token row
-  const uint64_t dims[4] = {row, (uint64_t)g.w, (uint64_t)g.h, (uint64_t)fv.T};
-  const uint64_t strides[3] = {row * 2, (uint64_t)g.w * row * 2, (uint64_t)fv.P * row * 2};
-  const uint32_t ib = hilo ? 2 * BK : BK, tsw = hilo ? 128 : SW;
-  const uint32_t box0[4] = {ib, XW_BOX, XW_ROWS0, 1}, box1[4] = {ib, XW_BOX, XW_ROWS1, 1};
-  if ((rc = make_tmap_4d(&tm[2], hilo ? fv.hilo : fv.hi, dims, strides, box0, TMAP_F16, tsw))) return rc;
-  if ((rc = make_tmap_4d(&tm[4], hilo ? fv.hilo : fv.hi, dims, strides, box1, TMAP_F16, tsw))) return rc;
-  if (hilo) {
-    tm[3] = tm[2];
-    tm[5] = tm[4];
-    return small ? run_xw_gemm<64, true>(tm, cells, xc, fv.C, st) : run_xw_gemm<128, true>(tm, cells, xc, fv.C, st);
-  }
-  if ((rc = make_tmap_4d(&tm[3], fv.lo, dims, strides, box0, TMAP_F16, tsw))) return rc;
-  if ((rc = make_tmap_4d(&tm[5], fv.lo, dims, strides, box1, TMAP_F16, tsw))) return rc;
-  return small ? run_xw_gemm<64, false>(tm, cells, xc, fv.C, st) : run_xw_gemm<128, false>(tm, cells, xc, fv.C, st);
+  if ((rc = make_tmap_2d(&tmD[0], desc_hi, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
+  if ((rc = make_tmap_2d(&tmD[1], desc_lo, desc_rows, fv.C, small ? 64 : 128, BK, TMAP_F16, 0, SW))) return rc;
+  if (hilo) return small ? run_xw_gemm<64, true>(fv, g, tmD, cells, xc, st) : run_xw_gemm<128, true>(fv, g, tmD, cells, xc, st);
+  return small ? run_xw_gemm<64, false>(fv, g, tmD, cells, xc, st) : run_xw_gemm<128, false>(fv, g, tmD, cells, xc, st);
 }
 
 // ====================================================================================================== 4. head
@@ -1090,20 +1158,29 @@ int dinotrk_xw_head_set_window_only(int on) {
   return DINOTRK_OK;
 }
 
-int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
-                        int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
-                        int n_cells, int max_m, float* xbox, void* stream) {
+int dinotrk_xw_box_gemm_ext(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
+                            int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
+                            const int* box_ext, int n_cells, int max_m, float* xbox, void* stream) {
   DTK_CHECK_ARG(feat && feat->hi && feat->lo && g && desc_hi && desc_lo && cell_row0 && cell_m && cell_frame && box_org && xbox,
                 "xw_box_gemm: null pointer (the fp16 split of the features is required)");
   DTK_CHECK_ARG(feat->T > 0 && feat->C > 0 && feat->C % 8 == 0 && desc_rows > 0 && n_cells >= 0 && max_m > 0 &&
                 max_m <= XW_MAX_CELL, "xw_box_gemm: bad sizes (C must be a multiple of 8, cells of 1..%d rows)", XW_MAX_CELL);
   DTK_CHECK_ARG(reinterpret_cast<uintptr_t>(box_org) % 8 == 0, "xw_box_gemm: box_org must be 8-byte aligned");
+  DTK_CHECK_ARG(reinterpret_cast<uintptr_t>(box_ext) % 16 == 0, "xw_box_gemm: box_ext must be 16-byte aligned");
   const FeatView fv = make_view(*feat, *g);
   const XwCells cells{cell_row0, cell_row0, cell_m, cell_frame, nullptr, n_cells, max_m};
   XwChunk xc{};
   xc.box_org = reinterpret_cast<int2*>(const_cast<int*>(box_org));
+  xc.box_ext = reinterpret_cast<int4*>(const_cast<int*>(box_ext));
   xc.xbox = xbox;
   return launch_xw_gemm(fv, *g, desc_hi, desc_lo, desc_rows, cells, xc, (cudaStream_t)stream);
+}
+
+int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
+                        int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
+                        int n_cells, int max_m, float* xbox, void* stream) {
+  return dinotrk_xw_box_gemm_ext(feat, g, desc_hi, desc_lo, desc_rows, cell_row0, cell_m, cell_frame, box_org, nullptr, n_cells,
+                                 max_m, xbox, stream);
 }
 
 }  // extern "C"

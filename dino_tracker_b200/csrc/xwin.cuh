@@ -15,8 +15,10 @@
 //                    anchor frame) pair: their arg-maxes cluster around the query's position in the anchor frame, so one
 //                    21 x 21 token box around the cell's median arg-max holds every map's window.
 //   3. exact GEMM    per cell, the fp32-faithful split-precision contraction (lo*hi + hi*lo + hi*hi, same operation
-//                    sequence as the full-map GEMM) of the cell's descriptors against the box's 441 tokens only:
-//                    5.4 % of the map.  Raw accumulators go to a [map][448] buffer (1.8 KB per map instead of 32 KB).
+//                    sequence as the full-map GEMM) of the cell's descriptors against the tokens of its tight extent
+//                    only: the union of its fitting maps' candidate windows, 225 to 441 of the box's tokens (2.8 to 5.4 %
+//                    of the map).  Raw accumulators go to a [map][448] buffer laid out as the whole box (1.8 KB per map
+//                    instead of 32 KB); the head reads nothing outside the extent.
 //   4. head          one kernel, two maps per warp (a half-warp each, lane = refiner channel): exact arg-max among the
 //                    candidates, the exact 15 x 15 window built in shared memory and m_out; the refiner one hidden row at a
 //                    time, kept in registers; softmax sums on the 11 x 11 box, certificate with the bound from (1); writes
@@ -34,8 +36,6 @@ namespace dtk {
 constexpr float XW_EPS = 1.1e-3f;     // bound on |coarse - exact| in cosine units (2^-10 + accumulation, rounded up)
 constexpr int XW_BOX = 21;            // box side (tokens); windows of maps whose arg-max lies within +-3 of the centre fit
 constexpr int XW_SLACK = 3;
-constexpr int XW_ROWS0 = 12, XW_ROWS1 = XW_BOX - XW_ROWS0;       // box rows of the two wgmma N parts (252 and 189 tokens)
-constexpr int XW_N0 = 256, XW_N1 = 192;                          // their wgmma N (448 columns for 441 tokens)
 constexpr int XW_COLS = 448;                                     // accumulator row pitch per map (441 box tokens, row-major)
 constexpr int XW_MAX_CELL = 128;      // maps (source frames) per cell = wgmma M rows (64 or 128)
 constexpr int XW_MAX_CAND = 4;
@@ -128,8 +128,11 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
   int* stat;                  // [maps] 0: exact-window path, 1: full-map path
   int* cell_of;               // [maps] cell index
   int2* box_org;              // [cells] (first box row, first box column); y = INT_MIN: skip the cell
+  int4* box_ext;              // [cells] tight extent {first row, first column, rows, columns} relative to box_org: the union
+                              // of the fitting maps' candidate windows, rows and columns in [15, 21] (set when box_org is)
   float* xbox;                // [maps][XW_COLS] raw split-precision accumulators of the box tokens
-  int* slow_cnt;              // [n_groups + 1] per group count of queued maps; [n_groups] = total
+  int* slow_cnt;              // [n_groups + 4] per group count of queued maps; [n_groups] = total, [n_groups + 1] = of
+                              // those queued by the certificate, [n_groups + 2] = extent tokens, [n_groups + 3] = cells
   int* slow_list;             // [maps] group g's queue lives at [grp_map0[g], grp_map0[g] + slow_cnt[g])
   XwChunk() = default;
   // every buffer of a chunk of `maps` maps, `cells` cells and n_groups groups, n_tiles coarse tiles per map
@@ -142,8 +145,9 @@ struct XwChunk {          // device buffers of one chunk in flight (all sized fo
     cell_of = ar.take<int>(maps);
     slow_list = ar.take<int>(maps);
     box_org = ar.take<int2>(cells);
+    box_ext = ar.take<int4>(cells);
     xbox = ar.take<float>(maps * XW_COLS);
-    slow_cnt = ar.take<int>((size_t)n_groups + 2);
+    slow_cnt = ar.take<int>((size_t)n_groups + 4);
   }
 };
 

@@ -228,7 +228,9 @@ int dinotrk_infer_set_overlap(int mode);
  * contraction: 1 = split fp16 tensor cores, 0 = exact fp32[, coarse pass of pipeline 1: 1 = int8, 0 = fp16 (the pass the
  * phase finished with)[, bits of the float max over frames of feat->q_rho, 0 without int8 operands[, maps of pipeline 1
  * whose descriptor the GEMMs read in place from the unique (query, source frame) table, maps whose descriptor was gathered
- * into the chunk's rows]]]]]} of the last dinotrk_infer call that ran the anchor phase. */
+ * into the chunk's rows[, cells the exact box GEMM of pipeline 1 ran on, the tokens of those cells' tight extents (the union
+ * of their maps' 15 x 15 candidate windows; 225 to 441 per cell)]]]]]]} of the last dinotrk_infer call that ran the anchor
+ * phase. */
 int dinotrk_infer_set_path(int path);
 /* Timing aid for the exact-window head (tools/bench_xw_head.py --split): 1 = run only its window part (exact arg-max,
  * 15 x 15 window, m_out) and write no track points -- the results of dinotrk_infer are then NOT valid; 0 (default) = the
@@ -269,6 +271,13 @@ int dinotrk_xw_coarse_keys_i8(const dinotrk_features* feat, const dinotrk_geom* 
 int dinotrk_xw_box_gemm(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
                         int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
                         int n_cells, int max_m, float* xbox, void* stream);
+/* The same on each cell's tight extent: box_ext[k] = {first row, first column, rows, columns} relative to box_org[k] (int32
+ * [n_cells][4], 16-byte aligned; rows and columns in 15..21, inside the 21 x 21 box; a cell whose extent is not is
+ * skipped).  Writes the accumulators of the extent's tokens only, at their 21 x 21 box columns, by the same sequence of
+ * products as the whole box; every other column is not written.  box_ext = NULL: the whole box (dinotrk_xw_box_gemm). */
+int dinotrk_xw_box_gemm_ext(const dinotrk_features* feat, const dinotrk_geom* g, const void* desc_hi, const void* desc_lo,
+                            int desc_rows, const int* cell_row0, const int* cell_m, const int* cell_frame, const int* box_org,
+                            const int* box_ext, int n_cells, int max_m, float* xbox, void* stream);
 int dinotrk_infer(const dinotrk_features* feat, const dinotrk_geom* g,
                   const dinotrk_head_weights* hw, const float* query_points, int N,
                   float anchor_th, float cos_th, int frame_batch, int start_phase, int stop_after,
