@@ -373,12 +373,14 @@ int launch_xw_plan(const XwCells& cells, const float* desc_norm, int n_groups, c
 //          the 128-byte swizzle; a K step reads hi 0 / 32 and lo 64 / 96 bytes into the row.  Same bytes in half as many
 //          rows: the TMA's cost per row, not the MMA, bounds the 64-byte layout (DESIGN.md 4.3).
 // A MB = 64 stage is 40 KiB in either layout (five fit), a MB = 128 stage 32 KiB (six).
-// Epilogue: straight from the accumulator fragment to xbox[map][xw_col(row, column)] of the 21 x 21 box (a quad holds 8
-// consecutive part tokens of one map, which may straddle an extent row).
+// Epilogue: from the accumulator fragment through a per-warp shared-memory tile (16 maps x 32 part tokens) to
+// xbox[map][xw_col(row, column)] of the 21 x 21 box, one map's consecutive tokens per warp store.
 constexpr int XW_EXT_MIN = WM;                          // smallest extent side: one candidate's window
 constexpr int XW_NW = XW_BOX - XW_EXT_MIN + 1;          // extent widths 15 .. 21
 constexpr int XW_PART_TOK = 128;                        // tokens of a part at most: its wgmma N
 constexpr int XW_PART_ROWS = XW_PART_TOK / XW_EXT_MIN;  // rows of a part at most (8)
+constexpr int XW_EPI_ROWS = 16;                         // maps of one consumer warp's fragment rows
+constexpr int XW_EPI_PITCH = 40;                        // floats per staged map row: the quads' 8-byte writes are conflict-free
 
 // the token boxes' tensor maps: [hi or the interleaved split, lo][bw - XW_EXT_MIN][rows - 1]
 template <bool HILO>
@@ -398,8 +400,12 @@ struct XwCfg {
   static constexpr int kTokOff = 2 * kDescBytes;
   static constexpr int kStageBytes = kTokOff + kParts * kBoxes * kSlotBytes;
   static constexpr int kStages = MB == 64 ? 5 : 6;
-  static constexpr int kSmem = kStages * kStageBytes + 1024 + 256;
-  static_assert(kStages * kStageBytes + 1024 + 256 <= 227 * 1024, "shared-memory ring too large");
+  // after the ring and its barriers: one epilogue staging tile per consumer warp (its 16 maps x 32 part tokens)
+  static constexpr int kBarBytes = 256;
+  static constexpr int kEpiBytes = 8 * XW_EPI_ROWS * XW_EPI_PITCH * 4;
+  static constexpr int kSmem = kStages * kStageBytes + 1024 + kBarBytes + kEpiBytes;
+  static_assert(2 * kStages * 8 <= kBarBytes, "barriers");
+  static_assert(kSmem <= 227 * 1024, "shared-memory ring too large");
   static_assert(kTokOff % 1024 == 0 && kSlotBytes % 1024 == 0 && kStageBytes % 1024 == 0,
                 "token boxes must start 1024-byte aligned");
 };
@@ -408,6 +414,7 @@ struct XwCfg {
 template <int MB>
 struct XwExt {
   int y, x, bh, bw, n;   // first box row / column, rows, columns, parts
+  XwExt() = default;
   __device__ __forceinline__ XwExt(const int4* __restrict__ box_ext, int cell) {
     const int4 e = box_ext ? __ldg(box_ext + cell) : make_int4(0, 0, XW_BOX, XW_BOX);
     y = e.x; x = e.y; bh = e.z; bw = e.w;
@@ -428,7 +435,7 @@ struct XwExt {
 // of the warpgroup's descriptor rows / the part's token box(es) in a stage, t_half: distance from a token box's hi half to
 // its lo half (separate halves only).
 template <int MB, bool HILO>
-__device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t* empty, int& stage, int& phase, int KB,
+__device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t* empty, float* epi, int& stage, int& phase, int KB,
                                         uint32_t d_off, uint32_t t_off, uint32_t t_half, float* __restrict__ xbox, int map0,
                                         int r0, int m, int ntok, int bw, int col0) {
   using Cfg = XwCfg<MB, HILO>;
@@ -462,23 +469,29 @@ __device__ __forceinline__ void xw_part(uint8_t* smem, uint64_t* full, uint64_t*
   tc::wgmma_wait<0>();
   tc::reg_fence(acc);
   if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
-  // fragment rows are maps, columns part tokens: acc[4 i + 2 h + {0, 1}] = map r0 + fr + 8 h, tokens 8 i + fc + {0, 1}.
-  // Token j = 8 i + fc is (y, x) = (j / bw, j % bw), followed as i steps: 8 < bw, so x wraps at most once per step.
-  const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+  // Fragment rows are maps, columns part tokens: acc[4 i + 2 h + {0, 1}] = map rw + fr + 8 h, tokens 8 i + fc + {0, 1}
+  // (rw = the warp's first row).  Stored straight from the fragment, every warp store would write 4 lanes' values of 8
+  // maps, half of each 32-byte sector; the partial sectors held a part's epilogue at about a quarter of a cell's time
+  // with the ring idle (DESIGN.md 4.3).  So each warp passes its 16 maps through shared memory 32 tokens at a time, and
+  // lane l stores token 32 q + l of one map per store: runs of bw consecutive floats.
+  const int rw = r0 + (warp & 3) * 16, fr = lane >> 2, fc = 2 * (lane & 3);
+  float* buf = epi + (warp & 7) * XW_EPI_ROWS * XW_EPI_PITCH;
+  float* dst = xbox + (size_t)(map0 + rw) * XW_COLS + col0;
+  const int nr = min(m - rw, XW_EPI_ROWS);   // the warp's maps (<= 0: none)
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = r0 + fr + 8 * h;
-    if (r >= m) continue;
-    float* dst = xbox + (size_t)(map0 + r) * XW_COLS + col0;
-    int y = 0, x = fc;
+  for (int q = 0; q < N / 32; ++q) {
+    if (32 * q >= ntok || nr <= 0) break;
 #pragma unroll
-    for (int i = 0; i < N / 8; ++i) {
-      const int j = 8 * i + fc;
-      if (j < ntok) dst[y * XW_BOX + x] = acc[4 * i + 2 * h];
-      if (j + 1 < ntok) dst[x + 1 == bw ? (y + 1) * XW_BOX : y * XW_BOX + x + 1] = acc[4 * i + 2 * h + 1];
-      x += 8;
-      if (x >= bw) { x -= bw; ++y; }
-    }
+    for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(buf + (fr + 8 * h) * XW_EPI_PITCH + 8 * ii + fc) =
+            make_float2(acc[4 * (4 * q + ii) + 2 * h], acc[4 * (4 * q + ii) + 2 * h + 1]);
+    __syncwarp();
+    const int j = 32 * q + lane, y = j / bw, off = y * XW_BOX + (j - y * bw);
+    if (j < ntok)
+      for (int k = 0; k < nr; ++k) dst[(size_t)k * XW_COLS + off] = buf[k * XW_EPI_PITCH + lane];
+    __syncwarp();
   }
 }
 
@@ -492,6 +505,7 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);   // [kStages]
   uint64_t* empty = full + Cfg::kStages;                                                    // [kStages]
+  float* epi = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kBarBytes);
 
   const int warp = threadIdx.x >> 5, wg = threadIdx.x >> 7;
   const int KB = (K + Cfg::kBK - 1) / Cfg::kBK;
@@ -540,20 +554,30 @@ xw_gemm_kernel(const __grid_constant__ CUtensorMap tmD_hi, const __grid_constant
     tc::regs_alloc<232>();
     const int cw = wg - 1;
     int stage = 0, phase = 0;
+    // a cell's description is loaded one cell ahead: its loads land while the cell before it runs, not between the two
+    struct Meta { bool skip; XwExt<MB> e; int m, map0; };
+    auto meta = [&](int cell) {
+      return Meta{box_org[cell].y == INT_MIN, XwExt<MB>(box_ext, cell), cells.m[cell], cells.row0[cell]};
+    };
+    Meta cur;
+    if (blockIdx.x < cells.n_cells) cur = meta(blockIdx.x);
     for (int cell = blockIdx.x; cell < cells.n_cells; cell += gridDim.x) {
-      if (box_org[cell].y == INT_MIN) continue;
-      const XwExt<MB> e(box_ext, cell);
-      const int m = cells.m[cell], map0 = cells.row0[cell];
-      for (int p0 = 0; p0 < e.n; p0 += Cfg::kParts) {
-        if constexpr (MB == 64) {   // warpgroup cw: part p0 + cw of the pair, all 64 descriptor rows
-          const int p = p0 + cw;
-          xw_part<MB, HILO>(smem, full, empty, stage, phase, KB, 0, Cfg::kTokOff + cw * Cfg::kBoxes * Cfg::kSlotBytes,
-                            Cfg::kSlotBytes, xbox, map0, 0, m, e.rows(p) * e.bw, e.bw, xw_col(e.row(p), e.x));
-        } else {                    // warpgroup cw: descriptor rows [64 cw, 64 cw + 64) of part p0
-          xw_part<MB, HILO>(smem, full, empty, stage, phase, KB, cw * 64 * Cfg::kRow, Cfg::kTokOff, Cfg::kSlotBytes, xbox,
-                            map0, 64 * cw, m, e.rows(p0) * e.bw, e.bw, xw_col(e.row(p0), e.x));
+      Meta nxt;
+      if (cell + gridDim.x < cells.n_cells) nxt = meta(cell + gridDim.x);
+      const XwExt<MB>& e = cur.e;
+      const int m = cur.m, map0 = cur.map0;
+      if (!cur.skip)
+        for (int p0 = 0; p0 < e.n; p0 += Cfg::kParts) {
+          if constexpr (MB == 64) {   // warpgroup cw: part p0 + cw of the pair, all 64 descriptor rows
+            const int p = p0 + cw;
+            xw_part<MB, HILO>(smem, full, empty, epi, stage, phase, KB, 0, Cfg::kTokOff + cw * Cfg::kBoxes * Cfg::kSlotBytes,
+                              Cfg::kSlotBytes, xbox, map0, 0, m, e.rows(p) * e.bw, e.bw, xw_col(e.row(p), e.x));
+          } else {                    // warpgroup cw: descriptor rows [64 cw, 64 cw + 64) of part p0
+            xw_part<MB, HILO>(smem, full, empty, epi, stage, phase, KB, cw * 64 * Cfg::kRow, Cfg::kTokOff, Cfg::kSlotBytes,
+                              xbox, map0, 64 * cw, m, e.rows(p0) * e.bw, e.bw, xw_col(e.row(p0), e.x));
+          }
         }
-      }
+      cur = nxt;
     }
   }
 }
