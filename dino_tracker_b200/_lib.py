@@ -35,7 +35,8 @@ class VitConfig(Structure):
 
 class VitWeights(Structure):
     _fields_ = [("patch_w", c_void_p), ("patch_b", c_void_p), ("cls_pos", c_void_p), ("pos", c_void_p),
-                ("blocks", POINTER(c_void_p))]
+                ("blocks", POINTER(c_void_p)), ("registers", c_void_p), ("rope", c_void_p), ("n_registers", c_int),
+                ("ln_eps", c_float)]
 
 
 class FlowVideo(Structure):
@@ -106,10 +107,13 @@ SIGNATURES = {
     "dinotrk_delta_refine": (c_int, [_P, c_int, c_int, c_int, POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p), _P,
                                      _P, _P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
     "dinotrk_vit_workspace_bytes": (c_size_t, [POINTER(VitConfig), POINTER(Geom), c_int]),
+    "dinotrk_vit_workspace_bytes_ext": (c_size_t, [POINTER(VitConfig), POINTER(VitWeights), POINTER(Geom), c_int]),
     "dinotrk_vit_attention": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "dinotrk_vit_attention_f16": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "dinotrk_vit_stage": (c_int, [c_int, POINTER(VitConfig), POINTER(Geom), c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t,
                                   _P]),
+    "dinotrk_vit_stage_ext": (c_int, [c_int, POINTER(VitConfig), POINTER(VitWeights), POINTER(Geom), c_int, _P, _P, _P, _P, _P, _P,
+                                      _P, _P, c_size_t, _P]),
     "dinotrk_vit_forward": (c_int, [_P, c_int, POINTER(Geom), POINTER(VitConfig), POINTER(VitWeights), _P, _P, c_size_t, _P]),
     "dinotrk_best_buddies_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dinotrk_best_buddies_pairs": (c_int, [POINTER(Features), POINTER(Geom), _P, _P, c_int, _P, _P, _P, c_size_t, _P]),

@@ -11,6 +11,11 @@
 // the residual stream stays fp32.  Attention is the fused kernel of flash.cuh (scores never leave the SM).
 // Validation path (attn_materialized = 1): TF32 GEMMs, attention scores materialised per (frame, row chunk) in a workspace
 // (tensor-core GEMM -> row softmax -> tensor-core GEMM).
+//
+// DINOv3 and DINOv2 with registers (dinotrk_vit_weights' appended fields): R register rows after cls, so every frame has
+// pre = 1 + R prefix rows ahead of its patches (N1 = P + pre); DINOv3 has no position table but a rotary position
+// embedding on q and k of the patch rows, applied in the qkv epilogue (EpiQKV16Rope / EpiQKVRope), and LayerNorm eps 1e-5.
+// The new layouts run on epilogue types of their own, so the one-cls-row DINOv2 / DINO v1 launches keep their kernels.
 #include "common.cuh"
 #include "corr.cuh"
 #include "tcgemm.cuh"
@@ -47,15 +52,18 @@ __global__ void vit_im2col_kernel(const float* __restrict__ frames, OutT* __rest
   }
 }
 
-__global__ void vit_cls_kernel(float* __restrict__ x, const float* __restrict__ cls_pos, int N1, int D) {
+// the pre = 1 + R prefix rows of frame b: x[b][0] = cls_pos, x[b][1 + i] = registers[i] (no position: DINOv2 adds pos[0]
+// to cls only, DINOv3 has none)
+__global__ void vit_cls_kernel(float* __restrict__ x, const float* __restrict__ cls_pos, const float* __restrict__ registers,
+                               int pre, int N1, int D) {
   const int b = blockIdx.x;
-  for (int i = threadIdx.x; i < D; i += blockDim.x) x[(size_t)b * N1 * D + i] = cls_pos[i];
+  for (int i = threadIdx.x; i < pre * D; i += blockDim.x) x[(size_t)b * N1 * D + i] = i < D ? cls_pos[i] : registers[i - D];
 }
 
 // warp per row, D <= 2048
 template <typename OutT>
 __global__ void vit_layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gw, const float* __restrict__ gb,
-                                     OutT* __restrict__ y, size_t rows, int D) {
+                                     OutT* __restrict__ y, size_t rows, int D, float eps) {
   const size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -78,7 +86,7 @@ __global__ void vit_layernorm_kernel(const float* __restrict__ x, const float* _
       q += (a * a + b * b) + (c * c + d * d);
     }
   }
-  const float rstd = rsqrtf(warp_sum(q) / (float)D + 1e-6f);
+  const float rstd = rsqrtf(warp_sum(q) / (float)D + eps);
   OutT* yr = y + row * D;
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
@@ -123,8 +131,8 @@ __global__ void vit_softmax_kernel(float* __restrict__ s, int n, int ld, size_t 
   for (int i = threadIdx.x; i < n; i += blockDim.x) p[i] = row[i] * inv;
 }
 
-// x[b][1 + p][:] -> tpc[b][p][:]
-__global__ void vit_tap_kernel(const float* __restrict__ x, float* __restrict__ tpc, int B, int P, int D) {
+// x[b][pre + p][:] -> tpc[b][p][:]
+__global__ void vit_tap_kernel(const float* __restrict__ x, float* __restrict__ tpc, int B, int P, int pre, int D) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // float4 index
   const int n4 = D >> 2;
   size_t total = (size_t)B * P * n4;
@@ -132,7 +140,7 @@ __global__ void vit_tap_kernel(const float* __restrict__ x, float* __restrict__ 
   size_t row = i / n4;
   int c = (int)(i - row * n4);
   size_t b = row / P, p = row - b * P;
-  reinterpret_cast<float4*>(tpc)[i] = reinterpret_cast<const float4*>(x)[((b * (P + 1) + 1 + p)) * n4 + c];
+  reinterpret_cast<float4*>(tpc)[i] = reinterpret_cast<const float4*>(x)[((b * (P + pre) + pre + p)) * n4 + c];
 }
 
 // ---------------------------------------------------------------------------------------------- epilogues
@@ -176,6 +184,39 @@ struct EpiPatch : EpiBase {
       }
   }
 };
+
+// tokens after pre = 1 + R prefix rows: x[b][pre + p][col] = acc + bias[col] (+ pos[p][col] unless pos is null: DINOv3)
+struct EpiPatchPrefix : EpiPatch {
+  int pre;
+  __device__ __forceinline__ float4 pos4(int p, int col) const {
+    return pos ? __ldg(reinterpret_cast<const float4*>(pos + (size_t)p * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  __device__ __forceinline__ void vec4(int, int r, int col, float4 v) const {
+    const int b = fast_div(r, P), p = r - b * P;
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col)), pp = pos4(p, col);
+    *reinterpret_cast<float4*>(x + ((size_t)b * (P + pre) + pre + p) * D + col) =
+        make_float4(v.x + bb.x + pp.x, v.y + bb.y + pp.y, v.z + bb.z + pp.z, v.w + bb.w + pp.w);
+  }
+  __device__ __forceinline__ void operator()(State&, int, int r, int col0, const float (&f)[32], int ncols) const {
+    const int b = r / P, p = r - b * P;
+    float* o = x + ((size_t)b * (P + pre) + pre + p) * D + col0;
+#pragma unroll
+    for (int i = 0; i < 32; i += 4)
+      if (i < ncols) {
+        const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col0 + i)), pp = pos4(p, col0 + i);
+        *reinterpret_cast<float4*>(o + i) = make_float4(f[i] + bb.x + pp.x, f[i + 1] + bb.y + pp.y, f[i + 2] + bb.z + pp.z, f[i + 3] + bb.w + pp.w);
+      }
+  }
+};
+
+// DINOv3's rotary position embedding of one (j, j + 32) pair of a head, which the host's row permutation of the q / k
+// weights (and q bias) puts in adjacent columns (2j, 2j + 1); (c, s) = (cos, sin) of the pair's angle for this token.
+// q . k is unchanged by the same permutation of both, so attention needs nothing else.
+__device__ __forceinline__ void rope_pair(float& a, float& b, float2 cs) {
+  const float a0 = a;
+  a = __fmaf_rn(a0, cs.x, -__fmul_rn(b, cs.y));
+  b = __fmaf_rn(b, cs.x, __fmul_rn(a0, cs.y));
+}
 
 // qkv: scatter to q [b][hd][n][64] (scaled 1/8), k [b][hd][n][64], vT [b][hd][64][n]
 struct EpiQKV : EpiBase {
@@ -233,6 +274,63 @@ struct EpiQKV16 : EpiBase {
 #pragma unroll
       for (int i = 0; i < 32; ++i) if (i < ncols) o[(size_t)i * N1p] = __float2half_rn(f[i] + __ldg(bias + col0 + i));
     }
+  }
+};
+
+// EpiQKV with the rotary embedding on q and k of the patch rows n >= pre; rope [P][32] (cos, sin) per token and pair,
+// applied to acc + bias before the q scale
+struct EpiQKVRope : EpiQKV {
+  const float2* rope; int pre;
+  __device__ __forceinline__ void operator()(State& st, int g, int r, int col0, const float (&f)[32], int ncols) const {
+    if (col0 >= 2 * D) { EpiQKV::operator()(st, g, r, col0, f, ncols); return; }
+    const int b = r / N1, n = r - b * N1;
+    const int which = col0 / D, c = col0 - which * D, hd = c / HD, e0 = c - hd * HD;
+    float* o = (which == 0 ? q : k) + (((size_t)b * heads + hd) * N1 + n) * HD + e0;
+    const float sc = which == 0 ? 0.125f : 1.f;
+    const float2* cs = rope + (size_t)(n - pre) * 32 + (e0 >> 1);
+#pragma unroll
+    for (int i = 0; i < 32; i += 2)
+      if (i < ncols) {
+        float a = f[i] + __ldg(bias + col0 + i), bv = f[i + 1] + __ldg(bias + col0 + i + 1);
+        if (n >= pre) rope_pair(a, bv, __ldg(cs + i / 2));
+        o[i] = a * sc;
+        o[i + 1] = bv * sc;
+      }
+  }
+};
+
+// EpiQKV16 with the rotary embedding on q and k of the patch rows n >= pre (as EpiQKVRope, before the q scale and the
+// fp16 rounding)
+struct EpiQKV16Rope : EpiQKV16 {
+  const float2* rope; int pre;
+  __device__ __forceinline__ void vec4(int, int r, int col, float4 v) const {
+    const int b = fast_div(r, N1), n = r - b * N1;
+    const int which = (col >= D) + (col >= 2 * D), c = col - which * D, hd = c / HD, e0 = c - hd * HD;
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col));
+    const float sc = which == 0 ? qscale : 1.f;
+    float a0 = v.x + bb.x, b0 = v.y + bb.y, a1 = v.z + bb.z, b1 = v.w + bb.w;
+    if (n >= pre) {   // pairs e0 / 2 and e0 / 2 + 1: one 16-byte load (e0 % 4 == 0)
+      const float4 cs = __ldg(reinterpret_cast<const float4*>(rope + (size_t)(n - pre) * 32 + (e0 >> 1)));
+      rope_pair(a0, b0, make_float2(cs.x, cs.y));
+      rope_pair(a1, b1, make_float2(cs.z, cs.w));
+    }
+    __half* o = (which == 0 ? q : k) + (((size_t)b * heads + hd) * N1 + n) * HD + e0;
+    *reinterpret_cast<uint2*>(o) = pack_half4(a0 * sc, b0 * sc, a1 * sc, b1 * sc);
+  }
+  __device__ __forceinline__ void operator()(State& st, int g, int r, int col0, const float (&f)[32], int ncols) const {
+    if (col0 >= 2 * D) { EpiQKV16::operator()(st, g, r, col0, f, ncols); return; }
+    const int b = r / N1, n = r - b * N1;
+    const int which = col0 / D, c = col0 - which * D, hd = c / HD, e0 = c - hd * HD;
+    __half* o = (which == 0 ? q : k) + (((size_t)b * heads + hd) * N1 + n) * HD + e0;
+    const float sc = which == 0 ? qscale : 1.f;
+    const float2* cs = rope + (size_t)(n - pre) * 32 + (e0 >> 1);
+#pragma unroll
+    for (int i = 0; i < 32; i += 2)
+      if (i < ncols) {
+        float a = f[i] + __ldg(bias + col0 + i), bv = f[i + 1] + __ldg(bias + col0 + i + 1);
+        if (n >= pre) rope_pair(a, bv, __ldg(cs + i / 2));
+        *reinterpret_cast<__half2*>(o + i) = __floats2half2_rn(a * sc, bv * sc);
+      }
   }
 };
 
@@ -464,6 +562,29 @@ struct EpiFacet : EpiBase {
   }
 };
 
+// EpiFacet after pre = 1 + R prefix rows: out[b][n - pre][col] for n >= pre
+struct EpiFacetPrefix : EpiFacet {
+  int pre;
+  __device__ __forceinline__ void vec4(int, int r, int col, float4 v) const {
+    const int b = fast_div(r, N1), n = r - b * N1;
+    if (n < pre) return;
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col));
+    *reinterpret_cast<float4*>(out + ((size_t)b * (N1 - pre) + n - pre) * D + col) =
+        make_float4(v.x + bb.x, v.y + bb.y, v.z + bb.z, v.w + bb.w);
+  }
+  __device__ __forceinline__ void operator()(State&, int, int r, int col0, const float (&f)[32], int ncols) const {
+    const int b = r / N1, n = r - b * N1;
+    if (n < pre) return;
+    float* o = out + ((size_t)b * (N1 - pre) + n - pre) * D + col0;
+#pragma unroll
+    for (int i = 0; i < 32; i += 4)
+      if (i < ncols) {
+        const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col0 + i));
+        *reinterpret_cast<float4*>(o + i) = make_float4(f[i] + bb.x, f[i + 1] + bb.y, f[i + 2] + bb.z, f[i + 3] + bb.w);
+      }
+  }
+};
+
 // group tables for the GEMMs: one group of `rows` rows, or `heads` groups (attention)
 static int plan(const TcPlan& pl, int n_groups, int rows, int row_stride, int row_base, int batch_base, cudaStream_t st,
                 int tile_rows = TC_BM) {
@@ -505,9 +626,16 @@ static int launch_flash(const __half* q16, const __half* k16, const __half* v16,
 // run on the tile plan of vit_row_plan (one group of all B * N1 rows); the forward makes it once per block half.
 struct VitShape {
   int B, P, N1, D, heads, Kp;
+  int pre;            // prefix rows per frame: cls + R registers (N1 = P + pre)
   size_t rows;        // B * N1
   bool f16, pairs;    // fp16 operands (else fp32 / TF32); linear layers on CTA pairs (fp16 only)
+  float eps;          // LayerNorm eps
+  const float2* rope; // [P][32] (cos, sin) of the rotary embedding, or null (no rotation)
 };
+
+// what dinotrk_vit_weights' appended fields say about the token layout; wt = null: one cls row, eps 1e-6, no RoPE
+static int vit_prefix(const dinotrk_vit_weights* wt) { return 1 + (wt ? wt->n_registers : 0); }
+static float vit_eps(const dinotrk_vit_weights* wt) { return wt && wt->ln_eps > 0.f ? wt->ln_eps : 1e-6f; }
 
 // row length of the im2col matrix / patch weight: 16-byte multiple of the operand type
 static int vit_kp(const dinotrk_vit_config* c) {
@@ -515,9 +643,11 @@ static int vit_kp(const dinotrk_vit_config* c) {
   return (int)align_up((size_t)3 * c->patch * c->patch, f16 ? 8 : 4);
 }
 
-static VitShape vit_shape(const dinotrk_vit_config* c, const dinotrk_geom* g, int B) {
+static VitShape vit_shape(const dinotrk_vit_config* c, const dinotrk_vit_weights* wt, const dinotrk_geom* g, int B) {
   VitShape s;
-  s.B = B; s.P = g->h * g->w; s.N1 = s.P + 1; s.D = c->dim; s.heads = c->heads; s.Kp = vit_kp(c);
+  s.B = B; s.P = g->h * g->w; s.pre = vit_prefix(wt); s.N1 = s.P + s.pre; s.D = c->dim; s.heads = c->heads; s.Kp = vit_kp(c);
+  s.eps = vit_eps(wt);
+  s.rope = wt ? reinterpret_cast<const float2*>(wt->rope) : nullptr;
   s.rows = (size_t)B * s.N1;
   s.f16 = c->gemm_f16 != 0 && c->attn_materialized == 0;
   s.pairs = s.f16 && c->gemm_pair != 0;
@@ -528,40 +658,50 @@ static int vit_row_plan(const VitShape& s, const TcPlan& pl, cudaStream_t st) {
   return plan(pl, 1, (int)s.rows, 0, 0, 0, st, s.pairs ? TC2_BM : TC_BM);
 }
 
-// y = LayerNorm(x) (eps 1e-6), x [rows][D] fp32 -> y [rows][D] (fp16 in fp16 operand mode)
+// y = LayerNorm(x) (eps s.eps), x [rows][D] fp32 -> y [rows][D] (fp16 in fp16 operand mode)
 static int vit_layernorm(const VitShape& s, const float* x, const float* gw, const float* gb, void* y, cudaStream_t st) {
   ProfRange pr(PROF_VIT_MISC, st);
   const unsigned grid = (unsigned)((s.rows + 7) / 8);
-  if (s.f16) vit_layernorm_kernel<__half><<<grid, 256, 0, st>>>(x, gw, gb, reinterpret_cast<__half*>(y), s.rows, s.D);
-  else vit_layernorm_kernel<float><<<grid, 256, 0, st>>>(x, gw, gb, reinterpret_cast<float*>(y), s.rows, s.D);
+  if (s.f16) vit_layernorm_kernel<__half><<<grid, 256, 0, st>>>(x, gw, gb, reinterpret_cast<__half*>(y), s.rows, s.D, s.eps);
+  else vit_layernorm_kernel<float><<<grid, 256, 0, st>>>(x, gw, gb, reinterpret_cast<float*>(y), s.rows, s.D, s.eps);
   DTK_LAUNCHED();
   return DINOTRK_OK;
 }
 
-// x[b][1 + p] = cols[b P + p] . patch_w + bias + pos[p]; cols [B P][Kp] (makes its own 128-row tile plan)
-static int vit_patch_embed(const VitShape& s, const TcPlan& pl, const void* cols, const void* w, const float* bias,
-                           const float* pos, float* x, cudaStream_t st) {
+// x[b][pre + p] = cols[b P + p] . patch_w + bias (+ pos[p] when pos); cols [B P][Kp] (makes its own 128-row tile plan)
+template <class Epi>
+static int vit_patch_launch(const VitShape& s, const TcPlan& pl, const void* cols, const void* w, const Epi& ep, cudaStream_t st) {
   int rc;
   if ((rc = plan(pl, 1, s.B * s.P, 0, 0, 0, st))) return rc;
-  EpiPatch ep{{}, x, bias, pos, s.P, s.D};
   const TcOperands op = linear_operands(cols, (uint64_t)s.B * s.P, w);
   const int tiles = cdiv(s.B * s.P, TC_BM);
-  return s.f16 ? tc_launch<TcMode::F16, EpiPatch>(op, pl.problem(1, s.D, s.Kp), tiles, ep, st, PROF_VIT_GEMM)
-               : tc_launch<TcMode::TF32, EpiPatch>(op, pl.problem(1, s.D, s.Kp), tiles, ep, st, PROF_VIT_GEMM);
+  return s.f16 ? tc_launch<TcMode::F16, Epi>(op, pl.problem(1, s.D, s.Kp), tiles, ep, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, Epi>(op, pl.problem(1, s.D, s.Kp), tiles, ep, st, PROF_VIT_GEMM);
+}
+static int vit_patch_embed(const VitShape& s, const TcPlan& pl, const void* cols, const void* w, const float* bias,
+                           const float* pos, float* x, cudaStream_t st) {
+  if (s.pre == 1 && pos) return vit_patch_launch(s, pl, cols, w, EpiPatch{{}, x, bias, pos, s.P, s.D}, st);
+  return vit_patch_launch(s, pl, cols, w, EpiPatchPrefix{{{}, x, bias, pos, s.P, s.D}, s.pre}, st);
 }
 
-// qkv for the fused attention: y [rows][D] . qkv_w^T + bias -> fp16 q (scaled by 64^-1/2 log2 e), k, v^T (pitch align8(N1))
+// qkv for the fused attention: y [rows][D] . qkv_w^T + bias -> fp16 q (scaled by 64^-1/2 log2 e), k, v^T (pitch align8(N1));
+// with s.rope, q and k of the patch rows rotated first
+template <class Epi>
+static int vit_qkv_launch(const VitShape& s, const TcPlan& pl, const void* y, const void* w, const Epi& eq, cudaStream_t st) {
+  const TcOperands op = linear_operands(y, s.rows, w);
+  const TcProblem pb = pl.problem(1, 3 * s.D, s.D);
+  const int tiles = cdiv((int)s.rows, TC_BM);
+  return s.pairs ? tc_launch<TcMode::F16, Epi, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), eq, st, PROF_VIT_GEMM)
+       : s.f16 ? tc_launch<TcMode::F16, Epi>(op, pb, tiles, eq, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, Epi>(op, pb, tiles, eq, st, PROF_VIT_GEMM);
+}
 static int vit_qkv_fused(const VitShape& s, const TcPlan& pl, const void* y, const void* w, const float* bias, __half* q16,
                          __half* k16, __half* v16, cudaStream_t st) {
   const int D = s.D, N1p8 = (int)align_up((size_t)s.N1, 8);
   EpiQKV16 eq{{}, q16, k16, v16, bias, s.N1, D, s.heads, N1p8, 0.125f * 1.4426950408889634f};  // 1/sqrt(64) * log2(e)
   eq.direct_from = 2 * D;   // v^T rows thread-per-row; q / k that way too measured slower
-  const TcOperands op = linear_operands(y, s.rows, w);
-  const TcProblem pb = pl.problem(1, 3 * D, D);
-  const int tiles = cdiv((int)s.rows, TC_BM);
-  return s.pairs ? tc_launch<TcMode::F16, EpiQKV16, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), eq, st, PROF_VIT_GEMM)
-       : s.f16 ? tc_launch<TcMode::F16, EpiQKV16>(op, pb, tiles, eq, st, PROF_VIT_GEMM)
-               : tc_launch<TcMode::TF32, EpiQKV16>(op, pb, tiles, eq, st, PROF_VIT_GEMM);
+  if (!s.rope) return vit_qkv_launch(s, pl, y, w, eq, st);
+  return vit_qkv_launch(s, pl, y, w, EpiQKV16Rope{eq, s.rope, s.pre}, st);
 }
 
 // x[r] += ls * (a[r] . w^T + bias), a [rows][K]: proj (K = D) and fc2 (K = 4 D); ls = nullptr: no LayerScale
@@ -620,22 +760,28 @@ static int vit_swiglu(const VitShape& s, const TcPlan& pl, const void* y, const 
 // facet f of the tap block: out_tpc [B][P][D] = (y . qkv_w[(f-1) D : f D]^T + qkv_b[(f-1) D : f D]) without the cls rows.
 // The weight slice starts (f-1) D^2 elements into qkv_w; the caller checks that it and the bias slice are 16-byte aligned
 // (the TMA base and the epilogue's float4 bias reads).
-static int vit_facet(const VitShape& s, const TcPlan& pl, const void* y, const void* w_slice, const float* bias_slice,
-                     float* out_tpc, cudaStream_t st) {
-  const EpiFacet ef{{}, out_tpc, bias_slice, s.N1, s.D};
+template <class Epi>
+static int vit_facet_launch(const VitShape& s, const TcPlan& pl, const void* y, const void* w_slice, const Epi& ef,
+                            cudaStream_t st) {
   const TcOperands op = linear_operands(y, s.rows, w_slice);
   const TcProblem pb = pl.problem(1, s.D, s.D);
   const int tiles = cdiv((int)s.rows, TC_BM);
-  return s.pairs ? tc_launch<TcMode::F16, EpiFacet, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), ef, st, PROF_VIT_GEMM)
-       : s.f16 ? tc_launch<TcMode::F16, EpiFacet>(op, pb, tiles, ef, st, PROF_VIT_GEMM)
-               : tc_launch<TcMode::TF32, EpiFacet>(op, pb, tiles, ef, st, PROF_VIT_GEMM);
+  return s.pairs ? tc_launch<TcMode::F16, Epi, TC_BN, true>(op, pb, cdiv((int)s.rows, TC2_BM), ef, st, PROF_VIT_GEMM)
+       : s.f16 ? tc_launch<TcMode::F16, Epi>(op, pb, tiles, ef, st, PROF_VIT_GEMM)
+               : tc_launch<TcMode::TF32, Epi>(op, pb, tiles, ef, st, PROF_VIT_GEMM);
+}
+static int vit_facet(const VitShape& s, const TcPlan& pl, const void* y, const void* w_slice, const float* bias_slice,
+                     float* out_tpc, cudaStream_t st) {
+  const EpiFacet ef{{}, out_tpc, bias_slice, s.N1, s.D};
+  if (s.pre == 1) return vit_facet_launch(s, pl, y, w_slice, ef, st);
+  return vit_facet_launch(s, pl, y, w_slice, EpiFacetPrefix{ef, s.pre}, st);
 }
 
 // the activations of a forward; the MLP hidden buffer is also the patch embedding's im2col
 struct VitWs {
   float *x, *y, *q, *k, *vT, *hbuf, *S; TcPlan pl;
-  VitWs(Arena& ar, const dinotrk_vit_config& c, const dinotrk_geom& g, int B) {
-    const size_t P = (size_t)g.h * g.w, rows = (size_t)B * (P + 1), D = c.dim, N1p = align_up(P + 1, 4);
+  VitWs(Arena& ar, const dinotrk_vit_config& c, const dinotrk_geom& g, int B, int pre) {
+    const size_t P = (size_t)g.h * g.w, rows = (size_t)B * (P + pre), D = c.dim, N1p = align_up(P + pre, 4);
     x = ar.take<float>(rows * D);
     y = ar.take<float>(rows * D);
     q = ar.take<float>(rows * D);
@@ -654,9 +800,13 @@ using namespace dtk;
 
 extern "C" {
 
-size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_geom* g, int B) {
+size_t dinotrk_vit_workspace_bytes_ext(const dinotrk_vit_config* c, const dinotrk_vit_weights* wt, const dinotrk_geom* g, int B) {
   if (!c || !g) return 0;
-  return align_up(layout_end<VitWs>(*c, *g, B), 256) + 4096;
+  return align_up(layout_end<VitWs>(*c, *g, B, vit_prefix(wt)), 256) + 4096;
+}
+
+size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_geom* g, int B) {
+  return dinotrk_vit_workspace_bytes_ext(c, nullptr, g, B);
 }
 
 int dinotrk_vit_attention(const void* q16, const void* k16, const void* vT16, int B, int heads, int N1, int N1p,
@@ -675,21 +825,24 @@ int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16
                       reinterpret_cast<const __half*>(vT16), B, heads, N1, N1p, heads * HD, out16, true, (cudaStream_t)stream);
 }
 
-int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom* g, int B, const void* in, const void* w,
-                      const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
-                      size_t workspace_bytes, void* stream) {
+int dinotrk_vit_stage_ext(int stage, const dinotrk_vit_config* c, const dinotrk_vit_weights* wt, const dinotrk_geom* g, int B,
+                          const void* in, const void* w, const float* p0, const float* p1, void* out0, void* out1, void* out2,
+                          void* workspace, size_t workspace_bytes, void* stream) {
   DTK_CHECK_ARG(c && g && in && p0 && out0, "vit_stage: null pointer");
+  DTK_CHECK_ARG(!wt || wt->n_registers >= 0, "vit_stage: negative register count");
+  const bool rope = wt && wt->rope;
   DTK_CHECK_ARG(stage >= DINOTRK_VIT_LAYERNORM && stage <= DINOTRK_VIT_SWIGLU, "vit_stage: unknown stage %d", stage);
   DTK_CHECK_ARG(c->gemm_f16 != 0 && c->attn_materialized == 0, "vit_stage: fp16 operand mode only");
   DTK_CHECK_ARG(B > 0 && c->dim == c->heads * HD && c->dim <= 2048, "vit_stage: dim must be heads x 64 (<= 2048)");
   DTK_CHECK_ARG(c->swiglu_hidden >= 0 && c->swiglu_hidden % 8 == 0, "vit_stage: swiglu_hidden must be a multiple of 8");
   DTK_CHECK_ARG(stage != DINOTRK_VIT_SWIGLU || c->swiglu_hidden > 0, "vit_stage: the SwiGLU stage needs swiglu_hidden > 0");
   DTK_CHECK_ARG(stage == DINOTRK_VIT_LAYERNORM || w, "vit_stage: null weight");
-  DTK_CHECK_ARG((stage != DINOTRK_VIT_LAYERNORM && stage != DINOTRK_VIT_PATCH) || p1, "vit_stage: null second parameter vector");
+  DTK_CHECK_ARG(stage != DINOTRK_VIT_LAYERNORM || p1, "vit_stage: null LayerNorm bias");
+  DTK_CHECK_ARG(stage != DINOTRK_VIT_PATCH || p1 || rope, "vit_stage: null position table (only a RoPE model has none)");
   DTK_CHECK_ARG(stage != DINOTRK_VIT_QKV || (out1 && out2), "vit_stage: qkv needs q, k and v^T");
   DTK_CHECK_ARG(workspace && workspace_bytes >= DINOTRK_VIT_STAGE_WORKSPACE_BYTES, "vit_stage: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  const VitShape s = vit_shape(c, g, B);
+  const VitShape s = vit_shape(c, wt, g, B);
   Arena ar(workspace);
   TcPlan pl{ar.take<int>(2), ar.take<int>(2), ar.take<int>(2), ar.take<int>(2)};
   if (stage == DINOTRK_VIT_LAYERNORM) return vit_layernorm(s, reinterpret_cast<const float*>(in), p0, p1, out0, st);
@@ -708,23 +861,31 @@ int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom
   }
 }
 
+int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom* g, int B, const void* in, const void* w,
+                      const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  return dinotrk_vit_stage_ext(stage, c, nullptr, g, B, in, w, p0, p1, out0, out1, out2, workspace, workspace_bytes, stream);
+}
+
 int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const dinotrk_vit_config* c,
                         const dinotrk_vit_weights* wt, float* out_tpc, void* workspace, size_t workspace_bytes,
                         void* stream) {
   NvtxRange nvtx_range("dinotrk.vit_forward");
-  DTK_CHECK_ARG(frames && g && c && wt && out_tpc && wt->blocks, "vit_forward: null pointer");
-  const int D = c->dim, heads = c->heads, P = g->h * g->w, N1 = P + 1, Kp = vit_kp(c);
+  DTK_CHECK_ARG(frames && g && c && wt && out_tpc && wt->blocks && wt->cls_pos, "vit_forward: null pointer");
+  DTK_CHECK_ARG(wt->n_registers >= 0 && (wt->n_registers == 0 || wt->registers), "vit_forward: register rows missing");
+  DTK_CHECK_ARG(wt->pos || wt->rope, "vit_forward: a model without a position table needs the RoPE table");
+  const int D = c->dim, heads = c->heads, P = g->h * g->w, pre = vit_prefix(wt), N1 = P + pre, Kp = vit_kp(c);
   DTK_CHECK_ARG(D == heads * HD && D % 64 == 0 && D <= 2048, "vit_forward: dim must be heads x 64 (<= 2048)");
   DTK_CHECK_ARG(c->tap_layer >= 0 && c->tap_layer < c->depth, "vit_forward: tap layer out of range");
   DTK_CHECK_ARG(c->swiglu_hidden >= 0 && c->swiglu_hidden % 8 == 0, "vit_forward: swiglu_hidden must be a multiple of 8");
   DTK_CHECK_ARG(c->facet >= 0 && c->facet <= 3, "vit_forward: facet must be 0 (tokens), 1 (queries), 2 (keys) or 3 (values)");
   const int Hd = c->swiglu_hidden, hid_k = Hd ? Hd : 4 * D;   // MLP hidden width: the K of fc2 / w3
   const int N1p = (int)align_up((size_t)N1, 4);   // row pitch of the score / v^T arrays (TMA strides are 16-byte multiples)
-  DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_vit_workspace_bytes(c, g, B), "vit_forward: workspace too small");
+  DTK_CHECK_ARG(workspace && workspace_bytes >= dinotrk_vit_workspace_bytes_ext(c, wt, g, B), "vit_forward: workspace too small");
   // fp16 operand mode (default): LayerNorm / GELU / attention write fp16 activations, weights are fp16 (11-bit
   // significand like TF32, twice the tensor rate, half the operand traffic).  The validation path
   // (attn_materialized) keeps every operand fp32 / TF32.
-  const VitShape s = vit_shape(c, g, B);
+  const VitShape s = vit_shape(c, wt, g, B);
   const bool f16 = s.f16;
   // facet > 0: the features are the tap block's qkv Linear output (what the reference's qkv hook records), rows
   // [(f-1) D, f D) of qkv.w and qkv.b -- one N = D GEMM after that block's LayerNorm 1, written straight into out_tpc;
@@ -741,7 +902,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   }
   cudaStream_t st = (cudaStream_t)stream;
   Arena ar(workspace);
-  const VitWs ws(ar, *c, *g, B);
+  const VitWs ws(ar, *c, *g, B, pre);
   const size_t rows = (size_t)B * N1;
   float *x = ws.x, *y = ws.y, *q = ws.q, *k = ws.k, *vT = ws.vT, *hbuf = ws.hbuf, *S = ws.S;
   const TcPlan pl = ws.pl;
@@ -756,10 +917,10 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
     else vit_im2col_kernel<float><<<B * P, 128, 0, st>>>(frames, hbuf, B, g->H, g->W, g->h, g->w, c->patch, c->stride, Kp);
     DTK_LAUNCHED();
   }
-  if ((rc = vit_patch_embed(s, pl, hbuf, wt->patch_w, wt->patch_b, wt->pos, x, st))) return rc;
+  if ((rc = vit_patch_embed(s, pl, hbuf, wt->patch_w, wt->patch_b, wt->rope ? nullptr : wt->pos, x, st))) return rc;
   {
     ProfRange pr(PROF_VIT_MISC, st);
-    vit_cls_kernel<<<B, 256, 0, st>>>(x, wt->cls_pos, N1, D);
+    vit_cls_kernel<<<B, 256, 0, st>>>(x, wt->cls_pos, wt->registers, pre, N1, D);
     DTK_LAUNCHED();
   }
 
@@ -780,8 +941,11 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
       if ((rc = vit_qkv_fused(s, pl, y, w[2], w[3], q16, k16, v16, st))) return rc;
       if ((rc = launch_flash(q16, k16, v16, B, heads, N1, (int)align_up((size_t)N1, 8), D, y, f16, st))) return rc;
     } else {
-      if ((rc = tc_launch<TcMode::TF32, EpiQKV>(linear_operands(y, rows, w[2]), pl.problem(1, 3 * D, D), all_tiles,
-                                                EpiQKV{{}, q, k, vT, w[3], N1, D, heads, N1p}, st, PROF_VIT_GEMM))) return rc;
+      const EpiQKV eq{{}, q, k, vT, w[3], N1, D, heads, N1p};
+      const TcOperands op = linear_operands(y, rows, w[2]);
+      if ((rc = s.rope ? tc_launch<TcMode::TF32, EpiQKVRope>(op, pl.problem(1, 3 * D, D), all_tiles, EpiQKVRope{eq, s.rope, pre}, st,
+                                                           PROF_VIT_GEMM)
+                       : tc_launch<TcMode::TF32, EpiQKV>(op, pl.problem(1, 3 * D, D), all_tiles, eq, st, PROF_VIT_GEMM))) return rc;
       // attention, per frame and chunk of query rows: S = q k^T (all heads) -> softmax -> y = S v
       for (int b = 0; b < B; ++b) {
         for (int c0 = 0; c0 < N1; c0 += VIT_ROW_CHUNK) {
@@ -823,7 +987,7 @@ int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const
   {
     ProfRange pr(PROF_VIT_MISC, st);
     size_t tot = (size_t)B * P * (D / 4);
-    vit_tap_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(x, out_tpc, B, P, D);
+    vit_tap_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(x, out_tpc, B, P, pre, D);
     DTK_LAUNCHED();
   }
   return DINOTRK_OK;

@@ -250,6 +250,7 @@ class DeltaDINO(nn.Module):
             return self.forward_graph(x.float(), vit_features.shape[-2:])
         B, C, h, w = vit_features.shape
         geom = _lib.make_geom(x.shape[-2], x.shape[-1], 14, self.vit_stride, 35)
+        geom.h, geom.w = h, w   # the backbone's grid: patch-14 alignment, but 16-pixel patches have fewer columns
         zeros = torch.zeros(B, h * w, C, device=vit_features.device, dtype=torch.float32)
         res, _ = self.refine_tpc(x.float().contiguous(), zeros, geom)
         return res.view(B, h, w, C).permute(0, 3, 1, 2)

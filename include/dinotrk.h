@@ -388,14 +388,29 @@ typedef struct dinotrk_vit_config {
  * slots 9-12 hold w12.w [2Hd][D], w12.b [2Hd], w3.w [D][Hd], w3.b [D], where the rows of w12 (and its bias) are
  * interleaved in pairs of hidden units: rows 4q .. 4q+3 = x1 rows 2q, 2q+1, then x2 rows 2q, 2q+1 (hub layout: x1 rows
  * 0..Hd-1, x2 rows Hd..2Hd-1).  A null ls1.gamma / ls2.gamma (slots 6 / 13) means a block without LayerScale (DINO v1:
- * x += proj(...), x += fc2(...)).  Every other pointer is non-null and every pointer is 16-byte aligned. */
+ * x += proj(...), x += fc2(...)).  Every other pointer is non-null and every pointer is 16-byte aligned.
+ * Appended (zero-initialised: DINOv2 / DINO v1 as above):
+ *   registers, n_registers: R register tokens [R][dim], rows 1..R of every frame between cls and the patches, without
+ *     position (DINOv3, DINOv2 *_reg: R = 4), so every frame has N1 = h*w + 1 + R rows; cls_pos is then the bare cls
+ *     token for DINOv3.
+ *   rope: [h*w][32][2] fp32 (cos, sin) of the rotary position embedding (DINOv3): pair j of every head of q and k of patch
+ *     p turns by the angle of rope[p][j].  The pair is head dims (j, j + 32), which the caller puts in adjacent columns
+ *     (2j, 2j + 1) by permuting each head's q and k rows of qkv.w (and of qkv.b) alike; q . k is unchanged by that.
+ *     Non-null: pos is not read (may be null) and cls / register rows are not rotated.
+ *   ln_eps: LayerNorm eps; 0 = 1e-6 (DINOv2, DINO v1), DINOv3: 1e-5. */
 typedef struct dinotrk_vit_weights {
   const void* patch_w; const float* patch_b; const float* cls_pos; const float* pos;
   const float* const* blocks;
+  const float* registers; const float* rope;
+  int n_registers;
+  float ln_eps;
 } dinotrk_vit_weights;
 size_t dinotrk_vit_workspace_bytes(const dinotrk_vit_config* c, const dinotrk_geom* g, int B);
+/* The workspace of a model with wt->n_registers register rows (the other one is for wt = NULL: none). */
+size_t dinotrk_vit_workspace_bytes_ext(const dinotrk_vit_config* c, const dinotrk_vit_weights* wt, const dinotrk_geom* g, int B);
 /* frames [B][3][H][W] RGB in [0,1] -> out_tpc [B][h*w][dim] (token-major features of block tap_layer: its output, or
- * its query / key / value facet), cls token dropped.  The workspace holds the MLP hidden activations at the config's
+ * its query / key / value facet), cls and register tokens dropped.  The queries and keys facets are the qkv Linear output
+ * before RoPE.  The workspace holds the MLP hidden activations at the config's
  * width (4 dim, or swiglu_hidden). */
 int dinotrk_vit_forward(const float* frames, int B, const dinotrk_geom* g, const dinotrk_vit_config* c,
                         const dinotrk_vit_weights* wt, float* out_tpc, void* workspace,
@@ -441,6 +456,13 @@ int dinotrk_vit_attention_f16(const void* q16, const void* k16, const void* vT16
 int dinotrk_vit_stage(int stage, const dinotrk_vit_config* c, const dinotrk_geom* g, int B, const void* in, const void* w,
                       const float* p0, const float* p1, void* out0, void* out1, void* out2, void* workspace,
                       size_t workspace_bytes, void* stream);
+/* dinotrk_vit_stage for the token layout of wt's appended fields (its other fields are not read; wt = NULL is
+ * dinotrk_vit_stage): N1 = g->h * g->w + 1 + wt->n_registers; LAYERNORM with eps wt->ln_eps; PATCH writes rows
+ * 1 + R .. N1 - 1 of each frame, pos (p1) may be NULL when wt->rope is set; QKV rotates q and k of rows n >= 1 + R with
+ * wt->rope (the weight rows permuted as dinotrk_vit_weights says) before the q scale and the fp16 rounding. */
+int dinotrk_vit_stage_ext(int stage, const dinotrk_vit_config* c, const dinotrk_vit_weights* wt, const dinotrk_geom* g, int B,
+                          const void* in, const void* w, const float* p0, const float* p1, void* out0, void* out1, void* out2,
+                          void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- best buddies (preprocessing_dino_bb/extract_dino_best_buddies.py:12-54) ------------------------ */
 /* For every ordered pair k (source frame pair_src[k], target frame pair_tgt[k]; device int32[n_pairs]):
